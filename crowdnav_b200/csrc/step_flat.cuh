@@ -16,7 +16,8 @@
 // shared-memory LP code of orca_device.cuh), followed by a 4-step scan.
 // The queue is per BLOCK (WARPQ = false: one warp runs the pass for the whole block, the others wait at a barrier;
 // fewest instructions, best when the launch fills the chip) or per WARP (WARPQ = true: no block barrier, every warp runs
-// the pass for its own 1-2 solves; best for launches that leave the SMs mostly empty). cs::launch() picks by grid size.
+// the pass for its own 1-2 solves; best for launches that leave the SMs mostly empty). cs::launch() picks by grid size
+// for the single-step kernel; the multi-step kernel always runs the block queue.
 // Two finer splits of the pass were tried, both bit-identical, both slower, neither kept: (a) projections on (i, j) lanes +
 // register-resident speculative sub-problems (orca_spec.cuh: lp3_project_pair / lp3_sub_spec, host-fuzzed); (b) four lane
 // levels with early-exit code (projections, lp1 candidates, lp2 scans, outer scan; 10 lanes per item). More lanes
@@ -27,8 +28,14 @@
 // loop), so a launch advances its envs n steps with the state in REGISTERS: one load of the state, n x (solve, collision,
 // ladder, bookkeeping, install of the prefetched next scene when an episode ends), one store. That removes the launch gap
 // and the load/store stage from every step but the first. Results are bit-identical to n x crowdsim_step.
+// Its workload is many such launches in flight at once (independent batches on parallel streams), which fills the chip, so
+// it is built for issue throughput: the block lp3 queue (one pass covers the 5-6 items of a block instead of one pass per
+// warp in ~3 of its 4 warps), a step loop that ends when no env of the BLOCK has anything left to do (__syncthreads_or:
+// the lp3 pass has block barriers), and the robot lane's own state (RobotRec) in shared memory rather than in registers
+// that every lane of the warp would pay for.
 //
-// The multi-step kernel writes its memory effects once, at the end of the launch, from the registers; rare events (an
+// The multi-step kernel writes its memory effects once, at the end of the launch, from the registers and the robot lanes'
+// shared-memory records; rare events (an
 // episode's result row, parking, slot hand-over) are written when they happen. The single-step kernel stores as it goes.
 #pragma once
 #include "crowdsim_common.cuh"
@@ -42,11 +49,13 @@ namespace cs {
 // step_kernel.cu). STAGE is a profiling aid (scripts/latency_probe.cu instantiates cut-down variants to
 // attribute latency); the library only instantiates the full kernel (STAGE = 99).
 // Register budget of the single-step kernel: 6 resident blocks per SM (<= 80 registers), which pays off when a launch
-// fills the chip; the multi-step kernel serves launches that leave the chip mostly empty and carries ~35 registers of
-// state across steps: 4 blocks per SM (<= 128 registers). Both budgets are -D knobs for A/B builds; they have not been
-// re-tuned on H100.
-// CS_FLAT_STRAIGHT_LINES (multi-step kernel): the M line constructions unconditionally and branch-free so that their chains
-// interleave; 0 = the branchy form of the single-step kernel.
+// fills the chip. Multi-step kernel: 5 blocks per SM (<= 96 registers; N = 5 compiles to 91 with no spills). Measured on an
+// H100 80GB (bench.py, 16 batches in flight, 700 W power limit, 1980 MHz): 5 blocks per SM ran 6 % faster than 4; 6 blocks
+// per SM (80 registers, 20 B of spills) another 5 % faster, but 17 % slower with one batch in flight, where a launch lasts
+// as long as one warp's dependent chains. Both budgets are -D knobs for A/B builds.
+// CS_FLAT_STRAIGHT_LINES = 1 (multi-step kernel): the M line constructions unconditionally and branch-free so that their
+// chains interleave. Off (default): the branchy form of the single-step kernel; it needs fewer registers (91 against 96
+// plus spills at this budget) and measured 3 % faster with 16 batches in flight (same H100 runs).
 // ROT: the robot is a unicycle (CROWDSIM_ROBOT_EXTERNAL_ROT, agent.py:115-135). A template parameter so that the double
 // precision cos / sin / fmod code (12 % of the round-1 kernel's SASS) is only present in the kernels that execute it.
 #ifndef CS_FLAT_WPB
@@ -56,19 +65,30 @@ namespace cs {
 #define CS_FLAT_MINBLOCKS 6
 #endif
 #ifndef CS_FLAT_STRAIGHT_LINES
-#define CS_FLAT_STRAIGHT_LINES 1
+#define CS_FLAT_STRAIGHT_LINES 0
 #endif
 #ifndef CS_FLAT_MINBLOCKS_MULTI
-#define CS_FLAT_MINBLOCKS_MULTI 4
+#define CS_FLAT_MINBLOCKS_MULTI 5
 #endif
 
-template <int N, int STAGE = 99, bool ROT = false, bool MULTI = false, bool WARPQ = MULTI>
+// What only an env's robot lane carries: the global time, the episode accumulators, the parked-and-waiting flag and, in the
+// multi-step kernel, the outputs of the env's last live step and what the launch changed. The single-step kernel keeps it
+// in registers; the multi-step kernel keeps one record per env of the block in shared memory, so that the other lanes of
+// the warp do not pay registers for it across the n steps.
+struct RobotRec {
+    double gtime, ep_ret, ep_mds, o_reward, o_dmin;
+    double2 o_act;
+    int ep_t, ep_tc, ep_c, o_info;
+    uint8_t want, o_done, any_live, dirty_ep, new_case;
+};
+
+template <int N, int STAGE = 99, bool ROT = false, bool MULTI = false, bool WARPQ = false>
 __global__ void __launch_bounds__(32 * CS_FLAT_WPB, (MULTI ? CS_FLAT_MINBLOCKS_MULTI : CS_FLAT_MINBLOCKS) * 4 / CS_FLAT_WPB)
 step_flat_kernel(const __grid_constant__ StepArgs A)
 {
     static_assert(STAGE == 99 || !MULTI, "stage cut-offs exist for the single-step kernel only");
     static_assert(!(ROT && MULTI), "a unicycle robot needs an external action every step");
-    static_assert(WARPQ || !MULTI, "the multi-step kernel has no block barrier: warps run ahead of each other");
+    static_assert(!(WARPQ && MULTI), "the multi-step kernel runs the block queue: its step loop exits block-uniformly");
     if constexpr (STAGE == 0) return;
     using namespace orca;
     constexpr int L = N + 1, M = N, EPW = 32 / L, WPB = CS_FLAT_WPB;
@@ -80,6 +100,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     __shared__ float s_r2[3][T];                            // per-thread sub-problem result (x, y, ok)
     __shared__ float s_res[2][T];
     __shared__ int s_qcount;
+    __shared__ RobotRec s_rr[MULTI ? WPB : 1][EPW + 1];    // multi-step: [warp][env] (le <= EPW on every lane)
 
     const KParams &k = A.k;
     const int tid = threadIdx.x, lane = tid & 31, wib = tid >> 5;
@@ -91,37 +112,39 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     const bool env_ok = (le < EPW) && (e < A.B);
     const size_t hi = (size_t)e * N + a;                    // my element of the [B][N][2] arrays (human lanes)
     if (!WARPQ && tid == 0) s_qcount = 0;
+    RobotRec reg_rr = {};
+    RobotRec &rr = MULTI ? s_rr[MULTI ? wib : 0][le] : reg_rr;     // read and written by the robot lane of a valid env only
 
     // ---- all global loads of the launch are issued up front, unconditionally for valid envs, so that they overlap into ONE
     // DRAM round trip ----
     // (idle lanes get a goal 5 m away: a zero goal vector would drag the warp through the f64 sqrt / division slow paths)
     double2 pos = make_double2(0, 0), vel = pos, goal = make_double2(3, 4), attr = make_double2(0.3, 1.0);
-    double theta = 0, gtime = 0; double2 ext = make_double2(0, 0);
-    uint8_t act_flag = 1, slot_state = 0, want_flag = 0;
-    int ep_t = 0, ep_tc = 0, ep_c = -1; double ep_ret = 0, ep_mds = 0;
+    double theta = 0; double2 ext = make_double2(0, 0);
+    uint8_t act_flag = 1, slot_state = 0;
     if (env_ok) {
         if (A.st.active) act_flag = A.st.active[e];
         if (!is_robot) {
             pos = ld2(A.st.h_pos, hi); vel = ld2(A.st.h_vel, hi); goal = ld2(A.st.h_goal, hi); attr = ld2(A.st.h_attr, hi);
         } else {
             pos = ld2(A.st.r_pos, e); vel = ld2(A.st.r_vel, e); goal = ld2(A.st.r_goal, e); attr = ld2(A.st.r_attr, e);
-            gtime = A.st.g_time[e];
+            RobotRec r0 = {}; r0.ep_c = -1;
+            r0.gtime = A.st.g_time[e];
             if (ROT) theta = A.st.r_theta[e];
-            if (k.robot_policy != CROWDSIM_ROBOT_ORCA) ext = ld2(A.io.action, e);
-            if (A.has_ep) { ep_t = A.ep.ep_steps[e]; ep_ret = A.ep.ep_return[e]; ep_tc = A.ep.ep_too_close[e]; ep_mds = A.ep.ep_min_dist_sum[e]; ep_c = A.ep.ep_case[e]; }
-            if (A.has_ar) { if (!MULTI) slot_state = ld_relaxed_u8(A.ar.n_state + e); want_flag = A.ar.want[e]; }
+            if (!MULTI && k.robot_policy != CROWDSIM_ROBOT_ORCA) ext = ld2(A.io.action, e);     // (multi-step: always ORCA)
+            if (A.has_ep) { r0.ep_t = A.ep.ep_steps[e]; r0.ep_ret = A.ep.ep_return[e]; r0.ep_tc = A.ep.ep_too_close[e]; r0.ep_mds = A.ep.ep_min_dist_sum[e]; r0.ep_c = A.ep.ep_case[e]; }
+            if (A.has_ar) { if (!MULTI) slot_state = ld_relaxed_u8(A.ar.n_state + e); r0.want = A.ar.want[e]; }
+            rr = r0;
         }
     }
     if constexpr (STAGE == 1) {            // loads + stores only
         const bool live1 = env_ok && (act_flag != 0);
         if (live1 && !is_robot) { st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, make_double2(vel.x + goal.x * 0, vel.y + attr.x * 0)); }
-        if (live1 && is_robot) { st2(A.st.r_pos, e, pos); A.st.g_time[e] = gtime + ext.x * 0 + theta * 0; }
+        if (live1 && is_robot) { st2(A.st.r_pos, e, pos); A.st.g_time[e] = rr.gtime + ext.x * 0 + theta * 0; }
         return;
     }
 
-    // what this launch changed (decides the stores at the end)
-    bool dirty_kin = false, dirty_scene = false, dirty_ep = false, any_live = false, new_case = false;
-    double o_reward = 0, o_dmin = 0; double2 o_act = make_double2(0, 0); int o_done = 0, o_info = 0;
+    // what this launch changed on this lane (decides the stores at the end; the robot lane's other flags are in rr)
+    bool dirty_kin = false, dirty_scene = false;
     const double dt = k.time_step;
 
     const int n_steps = MULTI ? A.n_steps : 1;
@@ -129,14 +152,15 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     for (int s = 0; s < n_steps; ++s) {
     const bool live = env_ok && (act_flag != 0);
     if constexpr (MULTI) {
-        // nothing left to do for this warp: every env is frozen and none is waiting for a scene
-        if (__ballot_sync(CS_FULL, live || (is_robot && env_ok && want_flag != 0 && A.has_ar)) == 0u) break;
+        // nothing left to do for this block: every env is frozen and none is waiting for a scene. Block-uniform, because the
+        // step's linearProgram3 pass has block barriers that every thread must reach.
+        if (!__syncthreads_or(live || (is_robot && env_ok && A.has_ar && rr.want != 0))) break;
     }
     // float32 view of myself for the other lanes of my env (rvo2 boundary casts, orca.py:100-110)
     const float fpx = (float)pos.x, fpy = (float)pos.y, fvx = (float)vel.x, fvy = (float)vel.y;
     const float frh = (float)(attr.x + 0.01 + k.human_safety_space);     // my radius as seen by a human observer
     const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
-    const bool solves = live && (!is_robot || k.robot_policy == CROWDSIM_ROBOT_ORCA);
+    const bool solves = live && (MULTI || !is_robot || k.robot_policy == CROWDSIM_ROBOT_ORCA);
 
     // ---- orca.py:113-115 preferred velocity (float64) ----
     const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
@@ -186,7 +210,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     // ---- ORCA lines in rank order, in registers ----
     RegLines<M> R; bool valid[M];
     if constexpr (CS_FLAT_STRAIGHT_LINES && MULTI) {
-        // multi-step kernel (1-2 warps per scheduler: a launch lasts as long as one warp's dependent chains): all M constructions
+        // for launches that leave 1-2 warps per scheduler (a launch lasts as long as one warp's dependent chains): all M constructions
         // unconditionally and branch-free, so that their chains interleave; absent positions get a far-away dummy neighbour (no
         // special values) and are zeroed afterwards, the rare overlapping lines (0.09 %) are repaired behind a warp vote.
         V2 qp[M], qv[M]; float qr[M]; bool ov[M]; bool any_ov = false;
@@ -292,10 +316,11 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                 __syncwarp();
             }
             if (need3) nv = mk(s_res[0][slot], s_res[1][slot]);
-            __syncwarp();                                        // the queue is reused by the next step (MULTI)
+            __syncwarp();
         }
     } else {
-        __syncthreads();                                         // s_qcount = 0 visible
+        // s_qcount = 0 visible (multi-step kernel: the barrier at the top of the step loop)
+        if constexpr (!MULTI) __syncthreads();
         int slot = -1;
         if (need3) {
             slot = atomicAdd(&s_qcount, 1);
@@ -341,6 +366,8 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                 __syncthreads();
             }
             if (need3) nv = mk(s_res[0][slot], s_res[1][slot]);
+            // the queue is reused by the next step; every thread read cnt before the pass's first barrier
+            if (MULTI && tid == 0) s_qcount = 0;
         }
     }
 
@@ -351,7 +378,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     // ---- robot velocity of this step, broadcast inside the env ----
     double ax = 0, ay = 0, rvx = 0, rvy = 0;
     if (is_robot) {
-        if (k.robot_policy == CROWDSIM_ROBOT_ORCA) { ax = (double)nv.x; ay = (double)nv.y; rvx = ax; rvy = ay; }
+        if (MULTI || k.robot_policy == CROWDSIM_ROBOT_ORCA) { ax = (double)nv.x; ay = (double)nv.y; rvx = ax; rvy = ay; }
         else if (ROT) { ax = ext.x; ay = ext.y; rvx = ax * cos(ay + theta); rvy = ax * sin(ay + theta); }      // crowd_sim.py:340-341
         else { ax = ext.x; ay = ext.y; rvx = ax; rvy = ay; }
     }
@@ -386,6 +413,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             else { const double th = theta + ay; npx = pos.x + cos(th) * ax * dt; npy = pos.y + sin(th) * ax * dt; nvx = nvy = 0; }
             const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
             double reward; int info;
+            const double gtime = rr.gtime;
             if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
             else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
             else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
@@ -396,23 +424,27 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                 theta = nth; nvx = ax * cos(nth); nvy = ax * sin(nth);
             }
             pos = make_double2(npx, npy); vel = make_double2(nvx, nvy);
-            gtime = gtime + dt;
-            if constexpr (MULTI) { o_act = vel; o_reward = reward; o_dmin = dmin; o_done = done ? 1 : 0; o_info = info; any_live = true; dirty_kin = true; }
+            const double ntime = gtime + dt;
+            rr.gtime = ntime;
+            if constexpr (MULTI) { rr.o_act = vel; rr.o_reward = reward; rr.o_dmin = dmin; rr.o_done = done ? 1 : 0; rr.o_info = info; rr.any_live = 1; dirty_kin = true; }
             else {                                           // single step: nothing to carry, state and outputs leave at once
-                st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = gtime; if (ROT) A.st.r_theta[e] = theta;
+                st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = ntime; if (ROT) A.st.r_theta[e] = theta;
                 if (A.io.action_out) st2(A.io.action_out, e, vel);
                 A.io.reward[e] = reward; A.io.dmin[e] = dmin; A.io.done[e] = done ? 1 : 0; A.io.info[e] = (uint8_t)info;
             }
             if (A.has_ep) {
                 const crowdsim_episodes &ep = A.ep;
+                int ep_t = rr.ep_t, ep_tc = rr.ep_tc; double ep_ret = rr.ep_ret, ep_mds = rr.ep_mds;
                 const double disc = (ep_t < ep.discount_len) ? ep.discount[ep_t] : 0.0;
                 ep_ret = ep_ret + disc * reward; ep_t += 1;
                 if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; if constexpr (!MULTI) { ep.ep_too_close[e] = ep_tc; ep.ep_min_dist_sum[e] = ep_mds; } }
-                if constexpr (MULTI) dirty_ep = true; else { ep.ep_return[e] = ep_ret; ep.ep_steps[e] = ep_t; }
+                rr.ep_t = ep_t; rr.ep_tc = ep_tc; rr.ep_ret = ep_ret; rr.ep_mds = ep_mds;
+                if constexpr (MULTI) rr.dirty_ep = 1; else { ep.ep_return[e] = ep_ret; ep.ep_steps[e] = ep_t; }
                 if (done) {
+                    const int ep_c = rr.ep_c;
                     if (ep_c >= 0) {
                         ep.res_info[ep_c] = (uint8_t)info; ep.res_steps[ep_c] = ep_t;
-                        ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : gtime;
+                        ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
                         if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
                     }
@@ -423,13 +455,14 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         if (A.has_ar) {
             // consumer side of the auto-reset protocol (include/crowdsim_b200.h): an env that just finished, or is parked
             // waiting, looks at its next-scene slot; a slot the generator publishes later is picked up by a later step
-            const bool finished = live && done, parked = !live && want_flag != 0;
+            const bool finished = live && done, parked = !live && rr.want != 0;
             if (finished || parked) {
                 const uint8_t sst = MULTI ? ld_relaxed_u8(A.ar.n_state + e) : slot_state;
                 if (sst == CROWDSIM_SLOT_READY) install = 1;
                 else {
                     act_flag = 0; A.st.active[e] = 0;                             // park: nothing to install (yet)
-                    want_flag = (sst == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1; A.ar.want[e] = want_flag;
+                    const uint8_t want = (sst == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1;
+                    rr.want = want; A.ar.want[e] = want;
                 }
             }
         }
@@ -453,10 +486,10 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             } else {                                         // crowd_sim.py:262,274 + fresh episode accumulators
                 pos = make_double2(0.0, -A.ar.circle_radius); goal = make_double2(0.0, A.ar.circle_radius);
                 vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
-                theta = CS_PI / 2; gtime = 0.0;
+                theta = CS_PI / 2; rr.gtime = 0.0;
                 if (!ROT && A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
-                if (A.has_ep) { ep_t = 0; ep_ret = 0.0; ep_tc = 0; ep_mds = 0.0; ep_c = __ldcg(A.ar.n_case + e); dirty_ep = true; new_case = true; }
-                act_flag = 1; A.st.active[e] = 1; want_flag = 0; A.ar.want[e] = 0;
+                if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
+                act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
             }
             dirty_kin = true; dirty_scene = true;
         }
@@ -487,15 +520,15 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             }
             if (dirty_scene) { st2(A.st.h_goal, hi, goal); st2(A.st.h_attr, hi, attr); }
         } else {
-            if (dirty_kin) { st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = gtime; if (ROT) A.st.r_theta[e] = theta; }
+            if (dirty_kin) { st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = rr.gtime; if (ROT) A.st.r_theta[e] = theta; }
             if (dirty_scene) { st2(A.st.r_goal, e, goal); st2(A.st.r_attr, e, attr); }
-            if (any_live) {                                  // outputs of the env's last live step
-                if (A.io.action_out) st2(A.io.action_out, e, o_act);
-                A.io.reward[e] = o_reward; A.io.dmin[e] = o_dmin; A.io.done[e] = (uint8_t)o_done; A.io.info[e] = (uint8_t)o_info;
+            if (rr.any_live) {                               // outputs of the env's last live step
+                if (A.io.action_out) st2(A.io.action_out, e, rr.o_act);
+                A.io.reward[e] = rr.o_reward; A.io.dmin[e] = rr.o_dmin; A.io.done[e] = rr.o_done; A.io.info[e] = (uint8_t)rr.o_info;
             }
-            if (A.has_ep && dirty_ep) {
-                A.ep.ep_steps[e] = ep_t; A.ep.ep_return[e] = ep_ret; A.ep.ep_too_close[e] = ep_tc; A.ep.ep_min_dist_sum[e] = ep_mds;
-                if (new_case) A.ep.ep_case[e] = ep_c;
+            if (A.has_ep && rr.dirty_ep) {
+                A.ep.ep_steps[e] = rr.ep_t; A.ep.ep_return[e] = rr.ep_ret; A.ep.ep_too_close[e] = rr.ep_tc; A.ep.ep_min_dist_sum[e] = rr.ep_mds;
+                if (rr.new_case) A.ep.ep_case[e] = rr.ep_c;
             }
         }
     }

@@ -363,9 +363,11 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         if (multi) A.n_steps = n_steps;
         // linearProgram3 queue of the single-step kernel: per warp when the launch leaves SMs mostly empty (latency-bound: no
         // block barrier), per block when the chip is full (issue-bound: one warp runs the pass for the whole block).
-        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both.
+        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both. The multi-step kernel always
+        // uses the block queue: its launches are meant to run many at a time (independent batches on parallel streams), which
+        // fills the chip however small each grid is.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        #define CS_FLAT_LAUNCH(NN) do { if (multi) step_flat_kernel<NN, 99, false, true, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
+        #define CS_FLAT_LAUNCH(NN) do { if (multi) step_flat_kernel<NN, 99, false, true, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
                                         else if (rot) step_flat_kernel<NN, 99, true, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
                                         else if (warpq) step_flat_kernel<NN, 99, false, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
                                         else step_flat_kernel<NN, 99, false, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
