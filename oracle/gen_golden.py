@@ -16,9 +16,11 @@ What is recorded (floats as repr() strings, exact round trip):
   occupancy_maps.json  MultiHumanRL.build_occupancy_maps on scene / lookahead / random human states
   policy_decisions.json  per-action values and greedy actions of the reference's CADRL / LSTM-RL policies
   network_ports.json  the reference's value-network modules run with the weights of crowdnav_b200.policy's seeded ports
+  boundary_steps.json  one reference step on every constructed boundary scene (tests/boundary_scenes.py) and
+                 get_human_times on the arrival-edge scenes
 
 usage: python oracle/gen_golden.py [--quick]
-       python oracle/gen_golden.py --only NAME     one generator of ONLY (the non-default parameter profiles)
+       python oracle/gen_golden.py --only NAME     one generator of ONLY (the non-default parameter profiles, boundary)
 """
 import configparser
 import gzip
@@ -48,7 +50,7 @@ import gym  # noqa: E402
 import crowd_sim  # noqa: E402,F401  (registers CrowdSim-v0)
 from crowd_sim.envs.utils.robot import Robot  # noqa: E402
 from crowd_sim.envs.utils.info import Timeout, ReachGoal, Danger, Collision, Nothing  # noqa: E402
-from crowd_sim.envs.utils.action import ActionXY  # noqa: E402
+from crowd_sim.envs.utils.action import ActionXY, ActionRot  # noqa: E402
 from crowd_sim.envs.utils.state import JointState  # noqa: E402
 from crowd_sim.envs.policy.orca import ORCA  # noqa: E402
 from crowd_nav.utils.explorer import Explorer  # noqa: E402
@@ -512,8 +514,80 @@ def run_envcfg():
               record_traj=(0, 5))
 
 
-# generators of the non-default profiles; each writes only its own fixtures (--only NAME)
+BOUNDARY_N = (1, 2, 3, 5, 9)     # every RVO2 simulation of these scenes holds <= 10 agents: the kd-tree is one leaf
+
+
+def _set_orca_constants(env, vals):
+    """The ORCA constants and safety spaces of a parameter point on every agent's ORCA policy (orca.py:61-64 hard-codes
+    (10, 10, 5, 5); the robot's safety_space is train.py's knob, the humans' the same attribute on their policies)."""
+    for agent, safety in [(env.robot, vals['robot_safety_space'])] + [(h, vals['human_safety_space']) for h in env.humans]:
+        pol = agent.policy
+        pol.neighbor_dist, pol.max_neighbors = vals['neighbor_dist'], vals['max_neighbors']
+        pol.time_horizon = pol.time_horizon_obst = vals['time_horizon']
+        pol.safety_space = safety
+        pol.sim = None
+
+
+def _boundary_env(N, vis, b, s):
+    """A reference env holding exactly the scene: reset() builds the agents, set() overwrites their states."""
+    env, robot, _ = make_env(human_num=N, robot_visible=bool(vis), profile=b.prof)
+    env.reset('test', 0)
+    r = s.robot
+    robot.set(r[0], r[1], r[4], r[5], r[2], r[3], r[8], r[6], r[7])
+    for h, row in zip(env.humans, s.padded(N)):
+        h.set(row[0], row[1], row[4], row[5], row[2], row[3], 0, row[6], row[7])
+    env.global_time = s.g_time
+    env.human_times = [0] * N
+    _set_orca_constants(env, dict(test_util.profile(b.prof), **b.over))
+    return env, robot
+
+
+def run_boundary():
+    """The reference's own CrowdSim.step (ORCA.predict for the humans and, for ORCA batches, the robot) on every constructed
+    boundary scene of tests/boundary_scenes.py with N in BOUNDARY_N, robot visible and not, holonomic ORCA / external and
+    unicycle external robots; and get_human_times on the arrival-edge scenes. Recorded per step like traj_*.json, plus the
+    scene's batch and label; `action` is the raw action ((vx, vy) or (v, r))."""
+    import boundary_scenes as bs
+    rows, times = [], []
+    for N in BOUNDARY_N:
+        for policy in ('orca', 'external_xy', 'external_rot'):
+            for vis in (0, 1):
+                for b in bs.batches(N, policy, vis):
+                    for s in b.scenes:
+                        env, robot = _boundary_env(N, vis, b, s)
+                        pre, t0 = scene(env), env.global_time
+                        ob = [h.get_observable_state() for h in env.humans]
+                        if policy == 'orca':
+                            action = robot.act(ob)
+                        elif policy == 'external_rot':
+                            robot.kinematics = 'unicycle'            # agent.py:110-135 with (v, r) actions
+                            action = ActionRot(*s.action)
+                        else:
+                            action = ActionXY(*s.action)
+                        _, reward, done, info = env.step(action)
+                        rows.append({'N': N, 'policy': policy, 'vis': vis, 'batch': b.name, 'label': s.label,
+                                     'pre': pre, 'g_time': R(t0), 'action': [R(x) for x in action],
+                                     'reward': R(reward), 'done': bool(done), 'info': INFO_CODE[type(info)],
+                                     'dmin': R(info.min_dist) if isinstance(info, Danger) else None,
+                                     'post': scene(env), 'global_time': R(env.global_time)})
+    b = bs.Batch('h1', 2, 'orca', 0, bs.family_h1())
+    for s in b.scenes:
+        s.g_time = 10.0
+        env, robot = _boundary_env(2, 0, b, s)
+        assert robot.reached_destination()
+        pre = scene(env)
+        ht = env.get_human_times()
+        times.append({'label': s.label, 'N': 2, 'scene': pre, 'global_time': R(10.0), 'human_times': [R(t) for t in ht],
+                      'global_time_after': R(env.global_time), 'final_robot': [R(robot.px), R(robot.py)],
+                      'final_humans': [[R(h.px), R(h.py)] for h in env.humans]})
+    with gzip.open(os.path.join(OUT, 'boundary_steps.json.gz'), 'wt') as f:
+        json.dump({'steps': rows, 'human_times': times}, f, separators=(',', ':'))
+    print('boundary steps', len(rows), 'human_times rows', len(times))
+
+
+# generators of the non-default profiles and the boundary scenes; each writes only its own fixtures (--only NAME)
 ONLY = {
+    'boundary': run_boundary,
     'il_safety': run_il_safety,
     'envcfg': run_envcfg,
     'resets_envcfg': run_resets_envcfg,

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from util import (SUITES, NON_DEFAULT, ORCA_TIGHT, PROFILE_SUITES, load_golden, scene_arrays, fill_host_state, pre_step_times,
-                  profile, profile_env, profile_params, reset_kw)
+                  profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits)
 
 pytestmark = pytest.mark.gpu
 
@@ -16,19 +16,15 @@ STATE_FIELDS = ('h_pos', 'h_vel', 'h_goal', 'h_attr', 'r_pos', 'r_vel', 'r_goal'
 
 
 def _assert_state_equal(env, host, fields=STATE_FIELDS, what=''):
+    """Bit patterns, not values: -0.0 and +0.0 differ."""
     dev = env.state.to_host()
     for f in fields:
-        a, b = dev[f], getattr(host, f)
-        assert np.array_equal(a, b), '%s: field %s differs in %d entries (max abs %.3g)' % (
-            what, f, int((a != b).sum()), float(np.abs(a - b).max()))
+        assert_same_bits(dev[f], getattr(host, f), '%s: field %s' % (what, f))
 
 
 def _assert_io_equal(env, io, what=''):
-    assert np.array_equal(env.done.cpu().numpy(), io.done), what + ' done'
-    assert np.array_equal(env.info.cpu().numpy(), io.info), what + ' info'
-    assert np.array_equal(env.reward.cpu().numpy(), io.reward), what + ' reward'
-    assert np.array_equal(env.dmin.cpu().numpy(), io.dmin), what + ' dmin'
-    assert np.array_equal(env.action_out.cpu().numpy(), io.action_out), what + ' action_out'
+    for f in ('done', 'info', 'reward', 'dmin', 'action_out'):
+        assert_same_bits(getattr(env, f).cpu().numpy(), getattr(io, f), '%s %s' % (what, f))
 
 
 def _random_host_state(oracle, B, N, seed, spread=4.5):
@@ -111,9 +107,9 @@ def test_step_random_scenes_bit_exact(cuda_env, oracle, N, vis, policy, generic)
             # CUDA's double cos/sin are not glibc's: compare with a tolerance, then resynchronise the states
             dev = env.state.to_host()
             for f in ('h_pos', 'h_vel'):
-                assert np.array_equal(dev[f], getattr(host, f))
+                assert same_bits(dev[f], getattr(host, f))
             assert np.allclose(dev['r_pos'], host.r_pos, rtol=0, atol=1e-12) and np.allclose(dev['r_theta'], host.r_theta, rtol=0, atol=1e-12)
-            assert np.array_equal(env.info.cpu().numpy(), io.info)
+            assert same_bits(env.info.cpu().numpy(), io.info)
             env.state.load_host(host)
         else:
             _assert_state_equal(env, host, what='N=%d step %d' % (N, t))
@@ -206,7 +202,7 @@ def test_reset_matches_oracle(cuda_env, oracle):
         torch.cuda.synchronize()
         dev = env.state.to_host()
         for f in ('h_attr', 'r_pos', 'r_goal', 'r_attr', 'r_vel', 'h_vel', 'g_time', 'r_theta'):
-            assert np.array_equal(dev[f], getattr(host, f)), f
+            assert same_bits(dev[f], getattr(host, f)), f
         for f in ('h_pos', 'h_goal'):
             # px = 4*cos(angle) + noise: CUDA's cos/sin are within 1-2 ulp of glibc's, i.e. <= ~2e-15 absolute on
             # |4 cos| <= 4 (cancellation against the noise term makes a relative/ulp bound meaningless)
@@ -216,7 +212,7 @@ def test_reset_matches_oracle(cuda_env, oracle):
             frac_exact = float((dev[f] == getattr(host, f)).mean())
             print('%s N=%d %s: %.1f%% of coordinates bit-identical, max abs diff %.2e' % (rule, N, f, 100 * frac_exact, d))
         if rule == 'square_crossing':        # no cos/sin on this path: bit-exact
-            assert np.array_equal(dev['h_pos'], host.h_pos) and np.array_equal(dev['h_goal'], host.h_goal)
+            assert same_bits(dev['h_pos'], host.h_pos) and same_bits(dev['h_goal'], host.h_goal)
     print('worst abs difference of initial coordinates:', worst)
 
 
@@ -239,16 +235,16 @@ def test_reset_mask_and_active(cuda_env, oracle):
     env.state.active.zero_()
     env.reset_seeds(torch.arange(B) + 5000, mask=torch.from_numpy(mask))
     after = env.state.to_host()
-    assert np.array_equal(after['h_pos'][mask == 0], before['h_pos'][mask == 0])
-    assert not np.array_equal(after['h_pos'][mask == 1], before['h_pos'][mask == 1])
-    assert np.array_equal(after['active'], mask)
+    assert same_bits(after['h_pos'][mask == 0], before['h_pos'][mask == 0])
+    assert not same_bits(after['h_pos'][mask == 1], before['h_pos'][mask == 1])
+    assert same_bits(after['active'], mask)
     # frozen envs are not touched by a step
     snap = env.state.to_host()
     env.step()
     torch.cuda.synchronize()
     now = env.state.to_host()
     for f in STATE_FIELDS:
-        assert np.array_equal(now[f][mask == 0], snap[f][mask == 0]), f
+        assert same_bits(now[f][mask == 0], snap[f][mask == 0]), f
     assert (now['g_time'][mask == 1] == 0.25).all()
 
 
@@ -261,10 +257,10 @@ def test_orca_act_matches_oracle(cuda_env, oracle):
         snap = env.state.to_host()
         act = env.orca_act().cpu().numpy()
         ref = oracle.orca_act(oracle.default_params(robot_visible=vis), host)
-        assert np.array_equal(act, ref)
+        assert same_bits(act, ref)
         now = env.state.to_host()
         for f in STATE_FIELDS:
-            assert np.array_equal(now[f], snap[f])
+            assert same_bits(now[f], snap[f])
 
 
 def test_pack_and_lookahead_match_oracle_and_reference(cuda_env, oracle):
@@ -281,7 +277,7 @@ def test_pack_and_lookahead_match_oracle_and_reference(cuda_env, oracle):
     states = states.cpu().numpy(); reward = reward.cpu().numpy()
     o_packed = oracle.pack_joint(host)
     o_states, o_reward = oracle.lookahead_pack(oracle.default_params(robot_policy=0), host, actions)
-    assert np.array_equal(reward, o_reward)
+    assert same_bits(reward, o_reward)
     assert np.abs(packed - o_packed).max() < 1e-5 and np.abs(states - o_states).max() < 1e-5
     for e, r in enumerate(rows):      # the reference's own torch rotate / onestep_lookahead outputs
         ref_cur = np.array([[float(v) for v in row] for row in r['rotated_current']], dtype=np.float32)
@@ -296,7 +292,7 @@ def test_pack_and_lookahead_match_oracle_and_reference(cuda_env, oracle):
     env.state.load_host(host)
     states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
     o_states, o_reward = oracle.lookahead_pack(oracle.default_params(robot_visible=1, robot_policy=0), host, actions)
-    assert np.array_equal(reward.cpu().numpy(), o_reward)
+    assert same_bits(reward.cpu().numpy(), o_reward)
     assert np.abs(states.cpu().numpy() - o_states).max() < 1e-4
 
 
@@ -348,15 +344,15 @@ def test_autoreset_install_bit_exact(cuda_env, oracle):
             oracle.step(prm, host, io, hep, har)
             torch.cuda.synchronize()
             d = env.autoreset.to_host()
-            assert np.array_equal(d['n_state'], har.n_state) and np.array_equal(d['want'], har.want), it
-            assert np.array_equal(env.state.active.cpu().numpy(), host.active), it
+            assert same_bits(d['n_state'], har.n_state) and same_bits(d['want'], har.want), it
+            assert same_bits(env.state.active.cpu().numpy(), host.active), it
             if it % 25 == 0:
                 _assert_state_equal(env, host, what='autoreset N=%d it=%d' % (N, it))
             it += 1
         assert int(counter[0]) >= k
         _assert_state_equal(env, host, what='autoreset final')
         for f in ('res_info', 'res_steps', 'res_time', 'res_return', 'res_too_close', 'res_min_dist_sum', 'res_final_rpos'):
-            assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
+            assert same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
 
 
 @pytest.mark.parametrize('slots,suite', [(64, 'circle5_invisible'), (500, 'circle5_invisible'), (48, 'mixed5_invisible')])
@@ -408,7 +404,7 @@ def test_case_queue_hands_out_cases_in_slot_order(cuda_env, oracle):
         return host
     env.reset_seeds(rule=rule, use_queue=True)
     torch.cuda.synchronize()
-    assert np.array_equal(ep.ep_case.cpu().numpy(), np.arange(B)) and int(env._case_counter.item()) == B
+    assert same_bits(ep.ep_case.cpu().numpy(), np.arange(B)) and int(env._case_counter.item()) == B
     _assert_state_equal(env, oracle_scenes(np.arange(B)), fields=('h_pos', 'h_goal', 'h_attr'), what='queue reset')
 
     mask = np.arange(B) % 3 == 0
@@ -416,18 +412,18 @@ def test_case_queue_hands_out_cases_in_slot_order(cuda_env, oracle):
     torch.cuda.synchronize()
     m = int(mask.sum())
     want = np.arange(B); want[mask] = B + np.arange(m)
-    assert np.array_equal(ep.ep_case.cpu().numpy(), want) and int(env._case_counter.item()) == B + m
+    assert same_bits(ep.ep_case.cpu().numpy(), want) and int(env._case_counter.item()) == B + m
 
     env.prefetch()                                           # every slot EMPTY: the queue runs out at slot k - (B + m)
     torch.cuda.synchronize()
     ar = env.autoreset.to_host()
     cases = B + m + np.arange(B)
     ready = cases < k
-    assert np.array_equal(ar['n_state'], np.where(ready, _abi.SLOT_READY, _abi.SLOT_EXHAUSTED))
-    assert np.array_equal(ar['n_case'][ready], cases[ready]) and int(env._case_counter.item()) == B + m + B
+    assert same_bits(ar['n_state'], np.where(ready, _abi.SLOT_READY, _abi.SLOT_EXHAUSTED))
+    assert same_bits(ar['n_case'][ready], cases[ready]) and int(env._case_counter.item()) == B + m + B
     host = oracle_scenes(cases[ready])
     for f, g in (('n_h_pos', 'h_pos'), ('n_h_goal', 'h_goal'), ('n_h_attr', 'h_attr')):
-        assert np.array_equal(ar[f][ready], getattr(host, g)), f
+        assert same_bits(ar[f][ready], getattr(host, g)), f
 
     def run():
         e = cuda_env(512, 5)
@@ -447,7 +443,7 @@ def test_case_queue_hands_out_cases_in_slot_order(cuda_env, oracle):
     for f in ('ep_case', 'ep_steps', 'ep_return', 'res_info', 'res_steps', 'res_time', 'res_return', 'res_final_rpos'):
         assert torch.equal(getattr(a.episodes, f), getattr(b.episodes, f)), f
     for f, x in a.autoreset.to_host().items():
-        assert np.array_equal(x, b.autoreset.to_host()[f]), f
+        assert same_bits(x, b.autoreset.to_host()[f]), f
     for f in ('reward', 'dmin', 'done', 'info'):
         assert torch.equal(getattr(a, f), getattr(b, f)), f
 
@@ -532,18 +528,18 @@ def test_step_n_autoreset_bit_exact(cuda_env, oracle, N, n):
             oracle.step(prm, host, io, hep, har)
         torch.cuda.synchronize()
         d = env.autoreset.to_host()
-        assert np.array_equal(d['n_state'], har.n_state) and np.array_equal(d['want'], har.want), it
-        assert np.array_equal(env.state.active.cpu().numpy(), host.active), it
+        assert same_bits(d['n_state'], har.n_state) and same_bits(d['want'], har.want), it
+        assert same_bits(env.state.active.cpu().numpy(), host.active), it
         if it % 10 == 0:
             _assert_state_equal(env, host, what='step_n autoreset N=%d it=%d' % (N, it))
             for f in ('ep_case', 'ep_steps', 'ep_return', 'ep_too_close', 'ep_min_dist_sum'):
-                assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), (f, it)
+                assert same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f)), (f, it)
         it += 1
     assert int(counter[0]) >= k
     _assert_state_equal(env, host, what='step_n autoreset final')
     _assert_io_equal(env, io, what='step_n autoreset final')
     for f in ('res_info', 'res_steps', 'res_time', 'res_return', 'res_too_close', 'res_min_dist_sum', 'res_final_rpos'):
-        assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
+        assert same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
 
 
 def test_step_n_generic_and_external_fall_back_to_launch_loops(cuda_env, oracle):
@@ -585,7 +581,7 @@ def test_human_times_match_reference(cuda_env, oracle):
         assert ht[0].tolist() == [float(t) for t in r['human_times']], (r['tag'], r['case'])
         assert float(gt[0]) == float(r['global_time_after'])
         want = np.array([[float(x) for x in r['final_robot']]] + [[float(x) for x in h] for h in r['final_humans']])
-        assert np.array_equal(fp[0].cpu().numpy(), want), (r['tag'], r['case'])
+        assert same_bits(fp[0].cpu().numpy(), want), (r['tag'], r['case'])
         _assert_state_equal(env, host, what='human_times leaves the state alone')
 
 
@@ -613,12 +609,12 @@ def test_onestep_lookahead_is_a_step_without_update(cuda_env, oracle, N, vis, po
     import copy
     stepped = copy.deepcopy(host)
     oracle.step(prm, stepped, io)
-    assert np.array_equal(npos.cpu().numpy(), stepped.h_pos) and np.array_equal(nvel.cpu().numpy(), stepped.h_vel)
-    assert np.array_equal(info.cpu().numpy(), io.info) and np.array_equal(done.cpu().numpy(), io.done)
+    assert same_bits(npos.cpu().numpy(), stepped.h_pos) and same_bits(nvel.cpu().numpy(), stepped.h_vel)
+    assert same_bits(info.cpu().numpy(), io.info) and same_bits(done.cpu().numpy(), io.done)
     if policy == 'external_rot':
         assert np.allclose(rew.cpu().numpy(), io.reward, rtol=0, atol=1e-12)
     else:
-        assert np.array_equal(rew.cpu().numpy(), io.reward) and np.array_equal(env.dmin.cpu().numpy(), io.dmin)
+        assert same_bits(rew.cpu().numpy(), io.reward) and same_bits(env.dmin.cpu().numpy(), io.dmin)
 
 
 def test_lookahead_humans_matches_oracle(cuda_env, oracle):
@@ -632,7 +628,7 @@ def test_lookahead_humans_matches_oracle(cuda_env, oracle):
         npos, nvel = env.lookahead_humans()
         torch.cuda.synchronize()
         o_pos, o_vel = oracle.lookahead_humans(oracle.default_params(robot_visible=vis, robot_policy=0), host)
-        assert np.array_equal(npos.cpu().numpy(), o_pos) and np.array_equal(nvel.cpu().numpy(), o_vel), (N, vis)
+        assert same_bits(npos.cpu().numpy(), o_pos) and same_bits(nvel.cpu().numpy(), o_vel), (N, vis)
         _assert_state_equal(env, host, what='state untouched')
 
 
@@ -646,7 +642,7 @@ def test_occupancy_maps_match_reference_and_oracle(cuda_env, oracle):
         env = cuda_env(1, h.shape[0])
         pos = torch.from_numpy(h[None, :, 0:2].copy()).to(env.device); vel = torch.from_numpy(h[None, :, 2:4].copy()).to(env.device)
         got = env.occupancy_maps(pos, vel, r['cell_num'], float(r['cell_size']), r['channels'])[0].cpu().numpy()
-        assert np.array_equal(got != 0, ref != 0), r['tag']
+        assert same_bits(got != 0, ref != 0), r['tag']
         assert np.abs(got - ref).max() <= 1e-6, r['tag']
     rng = np.random.RandomState(3)
     for N in (2, 5, 20):
@@ -700,9 +696,9 @@ def _run_steps(cuda_env, oracle, prof, B, N, vis, policy, generic, steps, seed):
         if policy == 'external_rot':             # CUDA's double cos/sin: tolerance on the robot pose, then resynchronise
             dev = env.state.to_host()
             for f in ('h_pos', 'h_vel', 'g_time'):
-                assert np.array_equal(dev[f], getattr(host, f)), (what, t, f)
+                assert same_bits(dev[f], getattr(host, f)), (what, t, f)
             assert np.allclose(dev['r_pos'], host.r_pos, rtol=0, atol=1e-12) and np.allclose(dev['r_theta'], host.r_theta, rtol=0, atol=1e-12)
-            assert np.array_equal(env.info.cpu().numpy(), io.info), (what, t)
+            assert same_bits(env.info.cpu().numpy(), io.info), (what, t)
             env.state.load_host(host)
         else:
             _assert_state_equal(env, host, what='%s step %d' % (what, t))
@@ -775,7 +771,7 @@ def test_profile_step_n_autoreset_bit_exact(cuda_env, oracle, prof):
     oracle.reset(host, None, ep=hep, **q)
     env = profile_env(cuda_env, prof, B, N)
     ep = env.track_episodes(k)
-    assert ep.discount.numel() == hep.discount.size and np.array_equal(ep.discount.cpu().numpy(), hep.discount)
+    assert ep.discount.numel() == hep.discount.size and same_bits(ep.discount.cpu().numpy(), hep.discount)
     env.enable_autoreset()
     env.state.load_host(host)
     ep.ep_case.copy_(torch.from_numpy(hep.ep_case))
@@ -789,15 +785,15 @@ def test_profile_step_n_autoreset_bit_exact(cuda_env, oracle, prof):
             oracle.step(prm, host, io, hep, har)
         torch.cuda.synchronize()
         d = env.autoreset.to_host()
-        assert np.array_equal(d['n_state'], har.n_state) and np.array_equal(d['want'], har.want), it
-        assert np.array_equal(env.state.active.cpu().numpy(), host.active), it
+        assert same_bits(d['n_state'], har.n_state) and same_bits(d['want'], har.want), it
+        assert same_bits(env.state.active.cpu().numpy(), host.active), it
         if it % 10 == 0:
             _assert_state_equal(env, host, what='%s step_n autoreset it=%d' % (prof, it))
         it += 1
     assert int(counter[0]) >= k
     _assert_state_equal(env, host, what='%s step_n autoreset final' % prof)
     for f in ('res_info', 'res_steps', 'res_time', 'res_return', 'res_too_close', 'res_min_dist_sum', 'res_final_rpos'):
-        assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
+        assert same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
 
 
 @pytest.mark.parametrize('prof', NON_DEFAULT)
@@ -817,24 +813,24 @@ def test_profile_orca_act_and_lookahead_kernels(cuda_env, oracle, prof):
         for generic in (0, 1):
             lib.crowdsim_debug_force_generic(generic)
             act = env.orca_act().cpu().numpy()
-            assert np.array_equal(act, ref), (prof, N, vis, generic)
+            assert same_bits(act, ref), (prof, N, vis, generic)
         lib.crowdsim_debug_force_generic(0)
         prm = profile_params(oracle, prof, robot_visible=vis, robot_policy=_abi.ROBOT_EXTERNAL_XY)
         npos, nvel = env.lookahead_humans()
         o_pos, o_vel = oracle.lookahead_humans(prm, host)
-        assert np.array_equal(npos.cpu().numpy(), o_pos) and np.array_equal(nvel.cpu().numpy(), o_vel), (prof, N)
+        assert same_bits(npos.cpu().numpy(), o_pos) and same_bits(nvel.cpu().numpy(), o_vel), (prof, N)
         io = oracle.HostStepIO(B)
         io.action[...] = rng.uniform(-1, 1, (B, 2))
         (lpos, lvel, _), rew, done, info = env.onestep_lookahead(torch.from_numpy(io.action).to(env.device))
         torch.cuda.synchronize()
         stepped = host.copy()
         oracle.step(prm, stepped, io)
-        assert np.array_equal(lpos.cpu().numpy(), stepped.h_pos) and np.array_equal(lvel.cpu().numpy(), stepped.h_vel)
-        assert np.array_equal(rew.cpu().numpy(), io.reward) and np.array_equal(env.dmin.cpu().numpy(), io.dmin), (prof, N)
-        assert np.array_equal(info.cpu().numpy(), io.info) and np.array_equal(done.cpu().numpy(), io.done)
+        assert same_bits(lpos.cpu().numpy(), stepped.h_pos) and same_bits(lvel.cpu().numpy(), stepped.h_vel)
+        assert same_bits(rew.cpu().numpy(), io.reward) and same_bits(env.dmin.cpu().numpy(), io.dmin), (prof, N)
+        assert same_bits(info.cpu().numpy(), io.info) and same_bits(done.cpu().numpy(), io.done)
         states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
         o_states, o_reward = oracle.lookahead_pack(prm, host, actions)
-        assert np.array_equal(reward.cpu().numpy(), o_reward), (prof, N)
+        assert same_bits(reward.cpu().numpy(), o_reward), (prof, N)
         assert np.abs(states.cpu().numpy() - o_states).max() < 1e-5
         _assert_state_equal(env, host, what='%s N=%d: the lookahead kernels leave the state alone' % (prof, N))
 
@@ -854,7 +850,7 @@ def test_profile_lookahead_pack_matches_reference(cuda_env, oracle):
     states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
     states = states.cpu().numpy(); reward = reward.cpu().numpy()
     o_states, o_reward = oracle.lookahead_pack(profile_params(oracle, prof, robot_policy=0), host, actions)
-    assert np.array_equal(reward, o_reward)
+    assert same_bits(reward, o_reward)
     assert np.abs(states - o_states).max() < 1e-5
     for e, r in enumerate(rows):
         for k, la in enumerate(r['lookahead']):
@@ -879,7 +875,7 @@ def test_profile_reset_and_prefetch_match_oracle_and_reference(cuda_env, oracle)
         torch.cuda.synchronize()
         dev = env.state.to_host()
         for f in ('h_attr', 'r_pos', 'r_goal', 'r_attr', 'r_vel', 'h_vel', 'g_time', 'r_theta'):
-            assert np.array_equal(dev[f], getattr(host, f)), (rule, N, f)
+            assert same_bits(dev[f], getattr(host, f)), (rule, N, f)
         for f in ('h_pos', 'h_goal'):
             tol = 0.0 if rule == 'square_crossing' else 5e-15
             assert np.abs(dev[f] - getattr(host, f)).max() <= tol, (rule, N, f)
@@ -890,8 +886,8 @@ def test_profile_reset_and_prefetch_match_oracle_and_reference(cuda_env, oracle)
         env.prefetch()
         torch.cuda.synchronize()
         ar = env.autoreset.to_host()
-        assert (ar['n_state'] == _abi.SLOT_READY).all() and np.array_equal(ar['n_case'], np.arange(B))
-        assert np.array_equal(ar['n_h_attr'], host.h_attr)
+        assert (ar['n_state'] == _abi.SLOT_READY).all() and same_bits(ar['n_case'], np.arange(B))
+        assert same_bits(ar['n_h_attr'], host.h_attr)
         for f, g in (('n_h_pos', 'h_pos'), ('n_h_goal', 'h_goal')):
             tol = 0.0 if rule == 'square_crossing' else 5e-15
             assert np.abs(ar[f] - getattr(host, g)).max() <= tol, (rule, N, f)
@@ -987,6 +983,6 @@ def test_profile_human_times(cuda_env, oracle):
         assert ht == [float(t) for t in r['human_times']], (r['tag'], r['case'])
         assert gt == float(r['global_time_after'])
         want = np.array([[float(x) for x in r['final_robot']]] + [[float(x) for x in h] for h in r['final_humans']])
-        assert np.array_equal(fp, want), (r['tag'], r['case'])
+        assert same_bits(fp, want), (r['tag'], r['case'])
         for prof, (ht2, gt2, fp2) in results.items():
-            assert ht2 == ht and gt2 == gt and np.array_equal(fp2, fp), (r['tag'], r['case'], prof)
+            assert ht2 == ht and gt2 == gt and same_bits(fp2, fp), (r['tag'], r['case'], prof)

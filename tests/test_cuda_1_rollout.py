@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import SUITES, PROFILE_SUITES, load_golden, fill_host_state, profile_env
+from util import SUITES, PROFILE_SUITES, load_golden, fill_host_state, profile_env, same_bits
 
 pytestmark = pytest.mark.gpu
 
@@ -241,12 +241,12 @@ def test_host_stepper_matches_oracle(cuda_env, oracle, obs, N, transfer):
         io.action[...] = act
         oracle.step(prm_ext, host, io)
         if obs == 'f64':
-            assert np.array_equal(ob[0].numpy(), host.h_pos) and np.array_equal(ob[1].numpy(), host.h_vel), t
+            assert same_bits(ob[0].numpy(), host.h_pos) and same_bits(ob[1].numpy(), host.h_vel), t
         else:
-            assert np.array_equal(ob[0].numpy(), np.concatenate([host.h_pos, host.h_vel], axis=-1).astype(np.float32)), t
-        assert np.array_equal(rew.numpy(), io.reward) and np.array_equal(done.numpy(), io.done) and np.array_equal(info.numpy(), io.info)
+            assert same_bits(ob[0].numpy(), np.concatenate([host.h_pos, host.h_vel], axis=-1).astype(np.float32)), t
+        assert same_bits(rew.numpy(), io.reward) and same_bits(done.numpy(), io.done) and same_bits(info.numpy(), io.info)
         act = oracle.orca_act(oracle.default_params(), host)
-        assert np.array_equal(stepper.h_next_action.numpy(), act), t
+        assert same_bits(stepper.h_next_action.numpy(), act), t
 
 
 def test_host_stepper_batches_in_flight(cuda_env, oracle):
@@ -271,10 +271,10 @@ def test_host_stepper_batches_in_flight(cuda_env, oracle):
             (h_pos, h_vel), rew, done, info = steppers[q].wait()
             ios[q].action[...] = acts[q]
             oracle.step(prm_ext, hosts[q], ios[q])
-            assert np.array_equal(h_pos.numpy(), hosts[q].h_pos) and np.array_equal(h_vel.numpy(), hosts[q].h_vel), (t, q)
-            assert np.array_equal(rew.numpy(), ios[q].reward) and np.array_equal(info.numpy(), ios[q].info), (t, q)
+            assert same_bits(h_pos.numpy(), hosts[q].h_pos) and same_bits(h_vel.numpy(), hosts[q].h_vel), (t, q)
+            assert same_bits(rew.numpy(), ios[q].reward) and same_bits(info.numpy(), ios[q].info), (t, q)
             acts[q] = oracle.orca_act(oracle.default_params(), hosts[q])
-            assert np.array_equal(steppers[q].h_next_action.numpy(), acts[q]), (t, q)
+            assert same_bits(steppers[q].h_next_action.numpy(), acts[q]), (t, q)
             steppers[q].h_action.copy_(steppers[q].h_next_action); steppers[q].launch()
     for q in range(P):
         steppers[q].wait()
@@ -303,8 +303,8 @@ def test_host_stepper_group_native_round_robin(cuda_env, oracle):
             io.action[...] = oracle.orca_act(oracle.default_params(), hosts[q])
             oracle.step(prm_ext, hosts[q], io)
         (h_pos, h_vel), rew, done, info = results[q]
-        assert np.array_equal(h_pos.numpy(), hosts[q].h_pos) and np.array_equal(h_vel.numpy(), hosts[q].h_vel), q
-        assert np.array_equal(rew.numpy(), io.reward) and np.array_equal(info.numpy(), io.info), q
+        assert same_bits(h_pos.numpy(), hosts[q].h_pos) and same_bits(h_vel.numpy(), hosts[q].h_vel), q
+        assert same_bits(rew.numpy(), io.reward) and same_bits(info.numpy(), io.info), q
 
 
 def test_host_stepper_with_autoreset_streams_the_test_suite(cuda_env):

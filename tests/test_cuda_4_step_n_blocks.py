@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+from util import assert_same_bits
+
 pytestmark = pytest.mark.gpu
 
 STATE_FIELDS = ('h_pos', 'h_vel', 'h_goal', 'h_attr', 'r_pos', 'r_vel', 'r_goal', 'r_attr', 'g_time')
@@ -64,12 +66,12 @@ def test_step_n_frozen_parked_and_live_warps_share_blocks(cuda_env, oracle, N, n
         assert np.array_equal(env.state.active.cpu().numpy(), host.active), it
         dev = env.state.to_host()
         for f in STATE_FIELDS:
-            assert np.array_equal(dev[f], getattr(host, f)), (f, it)
+            assert_same_bits(dev[f], getattr(host, f), '%s it=%d' % (f, it))
         for f in EP_FIELDS:
-            assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), (f, it)
+            assert_same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f), '%s it=%d' % (f, it))
         it += 1
     assert not host.active.any() and not har.want.any() and int(counter[0]) >= k
     for f in RES_FIELDS:
-        assert np.array_equal(getattr(ep, f).cpu().numpy(), getattr(hep, f)), f
+        assert_same_bits(getattr(ep, f).cpu().numpy(), getattr(hep, f), f)
     for f in ('done', 'info', 'reward', 'dmin', 'action_out'):
-        assert np.array_equal(getattr(env, f).cpu().numpy(), getattr(io, f)), f
+        assert_same_bits(getattr(env, f).cpu().numpy(), getattr(io, f), f)

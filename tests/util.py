@@ -138,6 +138,36 @@ def fill_host_state(po, scenes, N):
     return st
 
 
+def same_bits(a, b):
+    """True when two arrays hold the same bit patterns (np.array_equal would take -0.0 == +0.0 and never NaN == NaN).
+    Floating-point arrays must also have the same dtype; integer and boolean arrays compare by value."""
+    a = np.ascontiguousarray(a); b = np.ascontiguousarray(b)
+    if a.shape != b.shape:
+        return False
+    if a.dtype.kind != 'f' and b.dtype.kind != 'f':
+        return np.array_equal(a, b)
+    if a.dtype != b.dtype:
+        return False
+    if a.dtype.kind == 'f':
+        u = {2: np.uint16, 4: np.uint32, 8: np.uint64}[a.dtype.itemsize]
+        return np.array_equal(a.view(u), b.view(u))
+    return np.array_equal(a, b)
+
+
+def assert_same_bits(a, b, what=''):
+    a = np.ascontiguousarray(a); b = np.ascontiguousarray(b)
+    assert a.shape == b.shape and a.dtype == b.dtype, '%s: %s %s vs %s %s' % (what, a.shape, a.dtype, b.shape, b.dtype)
+    if not same_bits(a, b):
+        if a.dtype.kind == 'f':
+            u = {2: np.uint16, 4: np.uint32, 8: np.uint64}[a.dtype.itemsize]
+            bad = a.view(u) != b.view(u)
+        else:
+            bad = a != b
+        i = np.argwhere(bad)[0]
+        raise AssertionError('%s: %d entries differ in their bits, first at %s: %r vs %r' % (
+            what, int(bad.sum()), tuple(int(x) for x in i), a[tuple(i)], b[tuple(i)]))
+
+
 def ulp_diff(a, b):
     """Elementwise distance in float64 ulps (for values of equal sign / finite)."""
     a = np.ascontiguousarray(a, dtype=np.float64); b = np.ascontiguousarray(b, dtype=np.float64)
