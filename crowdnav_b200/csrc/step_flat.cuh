@@ -1,4 +1,4 @@
-// step_flat.cuh -- CrowdSim step for small crowds (N <= 5 humans), register-resident ORCA solver, 1 .. n steps per launch.
+// step_flat.cuh -- CrowdSim step for small crowds (N <= 5 humans), register-resident ORCA solver, one step per launch.
 //
 // Same contract as step_kernel (crowd_sim/envs/crowd_sim.py:317-420 + orca.py:82-132 + explorer.py:41-72).
 // Mapping: one thread per (env, agent) solve, L = N + 1 lanes per env, floor(32 / L) whole envs per warp so an env
@@ -17,26 +17,15 @@
 // The queue is per BLOCK (WARPQ = false: one warp runs the pass for the whole block, the others wait at a barrier;
 // fewest instructions, best when the launch fills the chip) or per WARP (WARPQ = true: no block barrier, every warp runs
 // the pass for its own 1-2 solves; best for launches that leave the SMs mostly empty). cs::launch() picks by grid size
-// for the single-step kernel; the multi-step kernel always runs the block queue.
+// (the multi-step kernel, step_multi.cuh, runs the same block queue).
 // Two finer splits of the pass were tried, both bit-identical, both slower, neither kept: (a) projections on (i, j) lanes +
 // register-resident speculative sub-problems (orca_spec.cuh: lp3_project_pair / lp3_sub_spec, host-fuzzed); (b) four lane
 // levels with early-exit code (projections, lp1 candidates, lp2 scans, outer scan; 10 lanes per item). More lanes
 // per item means more warps with active lanes = more warp-instructions for the same work, and the all-pairs speculative
 // form executes more instructions than early-exit code; at 1-2 warps per scheduler a warp's time is its instruction count.
 //
-// MULTI = true: crowdsim_step_n. With an ORCA robot nothing leaves the device between steps (explorer.py:41-43 is a pure
-// loop), so a launch advances its envs n steps with the state in REGISTERS: one load of the state, n x (solve, collision,
-// ladder, bookkeeping, install of the prefetched next scene when an episode ends), one store. That removes the launch gap
-// and the load/store stage from every step but the first. Results are bit-identical to n x crowdsim_step.
-// Its workload is many such launches in flight at once (independent batches on parallel streams), which fills the chip, so
-// it is built for issue throughput: the block lp3 queue (one pass covers the 5-6 items of a block instead of one pass per
-// warp in ~3 of its 4 warps), a step loop that ends when no env of the BLOCK has anything left to do (__syncthreads_or:
-// the lp3 pass has block barriers), and the robot lane's own state (RobotRec) in shared memory rather than in registers
-// that every lane of the warp would pay for.
-//
-// The multi-step kernel writes its memory effects once, at the end of the launch, from the registers and the robot lanes'
-// shared-memory records; rare events (an
-// episode's result row, parking, slot hand-over) are written when they happen. The single-step kernel stores as it goes.
+// The single-step kernel stores as it goes. crowdsim_step_n (n steps per launch) has a kernel of its own, with the robots on
+// a warp of their own (step_multi.cuh); it shares this file's lp3 queue layout and the solver headers.
 #pragma once
 #include "crowdsim_common.cuh"
 #include "orca_spec.cuh"
@@ -48,14 +37,8 @@ namespace cs {
 // EPW = 32 / (N + 1) whole envs per warp (dense packing; sparser packings only multiply the instruction count, see
 // step_kernel.cu). STAGE is a profiling aid (scripts/latency_probe.cu instantiates cut-down variants to
 // attribute latency); the library only instantiates the full kernel (STAGE = 99).
-// Register budget of the single-step kernel: 6 resident blocks per SM (<= 80 registers), which pays off when a launch
-// fills the chip. Multi-step kernel: 5 blocks per SM (<= 96 registers; N = 5 compiles to 91 with no spills). Measured on an
-// H100 80GB (bench.py, 16 batches in flight, 700 W power limit, 1980 MHz): 5 blocks per SM ran 6 % faster than 4; 6 blocks
-// per SM (80 registers, 20 B of spills) another 5 % faster, but 17 % slower with one batch in flight, where a launch lasts
-// as long as one warp's dependent chains. Both budgets are -D knobs for A/B builds.
-// CS_FLAT_STRAIGHT_LINES = 1 (multi-step kernel): the M line constructions unconditionally and branch-free so that their
-// chains interleave. Off (default): the branchy form of the single-step kernel; it needs fewer registers (91 against 96
-// plus spills at this budget) and measured 3 % faster with 16 batches in flight (same H100 runs).
+// Register budget: 6 resident blocks per SM (<= 80 registers), which pays off when a launch fills the chip. A -D knob for
+// A/B builds.
 // ROT: the robot is a unicycle (CROWDSIM_ROBOT_EXTERNAL_ROT, agent.py:115-135). A template parameter so that the double
 // precision cos / sin / fmod code (12 % of the round-1 kernel's SASS) is only present in the kernels that execute it.
 #ifndef CS_FLAT_WPB
@@ -64,17 +47,11 @@ namespace cs {
 #ifndef CS_FLAT_MINBLOCKS
 #define CS_FLAT_MINBLOCKS 6
 #endif
-#ifndef CS_FLAT_STRAIGHT_LINES
-#define CS_FLAT_STRAIGHT_LINES 0
-#endif
-#ifndef CS_FLAT_MINBLOCKS_MULTI
-#define CS_FLAT_MINBLOCKS_MULTI 5
-#endif
 
-// What only an env's robot lane carries: the global time, the episode accumulators, the parked-and-waiting flag and, in the
+// What only an env's robot carries: the global time, the episode accumulators, the parked-and-waiting flag and, in the
 // multi-step kernel, the outputs of the env's last live step and what the launch changed. The single-step kernel keeps it
-// in registers; the multi-step kernel keeps one record per env of the block in shared memory, so that the other lanes of
-// the warp do not pay registers for it across the n steps.
+// in registers of the robot lane; the multi-step kernel (step_multi.cuh) keeps one record per env of the block in shared
+// memory, so that the human warps do not pay registers for it across the n steps.
 struct RobotRec {
     double gtime, ep_ret, ep_mds, o_reward, o_dmin;
     double2 o_act;
@@ -82,13 +59,10 @@ struct RobotRec {
     uint8_t want, o_done, any_live, dirty_ep, new_case;
 };
 
-template <int N, int STAGE = 99, bool ROT = false, bool MULTI = false, bool WARPQ = false>
-__global__ void __launch_bounds__(32 * CS_FLAT_WPB, (MULTI ? CS_FLAT_MINBLOCKS_MULTI : CS_FLAT_MINBLOCKS) * 4 / CS_FLAT_WPB)
+template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false>
+__global__ void __launch_bounds__(32 * CS_FLAT_WPB, CS_FLAT_MINBLOCKS * 4 / CS_FLAT_WPB)
 step_flat_kernel(const __grid_constant__ StepArgs A)
 {
-    static_assert(STAGE == 99 || !MULTI, "stage cut-offs exist for the single-step kernel only");
-    static_assert(!(ROT && MULTI), "a unicycle robot needs an external action every step");
-    static_assert(!(WARPQ && MULTI), "the multi-step kernel runs the block queue: its step loop exits block-uniformly");
     if constexpr (STAGE == 0) return;
     using namespace orca;
     constexpr int L = N + 1, M = N, EPW = 32 / L, WPB = CS_FLAT_WPB;
@@ -100,7 +74,6 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     __shared__ float s_r2[3][T];                            // per-thread sub-problem result (x, y, ok)
     __shared__ float s_res[2][T];
     __shared__ int s_qcount;
-    __shared__ RobotRec s_rr[MULTI ? WPB : 1][EPW + 1];    // multi-step: [warp][env] (le <= EPW on every lane)
 
     const KParams &k = A.k;
     const int tid = threadIdx.x, lane = tid & 31, wib = tid >> 5;
@@ -112,8 +85,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     const bool env_ok = (le < EPW) && (e < A.B);
     const size_t hi = (size_t)e * N + a;                    // my element of the [B][N][2] arrays (human lanes)
     if (!WARPQ && tid == 0) s_qcount = 0;
-    RobotRec reg_rr = {};
-    RobotRec &rr = MULTI ? s_rr[MULTI ? wib : 0][le] : reg_rr;     // read and written by the robot lane of a valid env only
+    RobotRec rr = {};                                       // read and written by the robot lane of a valid env only
 
     // ---- all global loads of the launch are issued up front, unconditionally for valid envs, so that they overlap into ONE
     // DRAM round trip ----
@@ -130,9 +102,9 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             RobotRec r0 = {}; r0.ep_c = -1;
             r0.gtime = A.st.g_time[e];
             if (ROT) theta = A.st.r_theta[e];
-            if (!MULTI && k.robot_policy != CROWDSIM_ROBOT_ORCA) ext = ld2(A.io.action, e);     // (multi-step: always ORCA)
+            if (k.robot_policy != CROWDSIM_ROBOT_ORCA) ext = ld2(A.io.action, e);
             if (A.has_ep) { r0.ep_t = A.ep.ep_steps[e]; r0.ep_ret = A.ep.ep_return[e]; r0.ep_tc = A.ep.ep_too_close[e]; r0.ep_mds = A.ep.ep_min_dist_sum[e]; r0.ep_c = A.ep.ep_case[e]; }
-            if (A.has_ar) { if (!MULTI) slot_state = ld_relaxed_u8(A.ar.n_state + e); r0.want = A.ar.want[e]; }
+            if (A.has_ar) { slot_state = ld_relaxed_u8(A.ar.n_state + e); r0.want = A.ar.want[e]; }
             rr = r0;
         }
     }
@@ -143,24 +115,13 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         return;
     }
 
-    // what this launch changed on this lane (decides the stores at the end; the robot lane's other flags are in rr)
-    bool dirty_kin = false, dirty_scene = false;
     const double dt = k.time_step;
-
-    const int n_steps = MULTI ? A.n_steps : 1;
-    #pragma unroll 1
-    for (int s = 0; s < n_steps; ++s) {
     const bool live = env_ok && (act_flag != 0);
-    if constexpr (MULTI) {
-        // nothing left to do for this block: every env is frozen and none is waiting for a scene. Block-uniform, because the
-        // step's linearProgram3 pass has block barriers that every thread must reach.
-        if (!__syncthreads_or(live || (is_robot && env_ok && A.has_ar && rr.want != 0))) break;
-    }
     // float32 view of myself for the other lanes of my env (rvo2 boundary casts, orca.py:100-110)
     const float fpx = (float)pos.x, fpy = (float)pos.y, fvx = (float)vel.x, fvy = (float)vel.y;
     const float frh = (float)(attr.x + 0.01 + k.human_safety_space);     // my radius as seen by a human observer
     const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
-    const bool solves = live && (MULTI || !is_robot || k.robot_policy == CROWDSIM_ROBOT_ORCA);
+    const bool solves = live && (!is_robot || k.robot_policy == CROWDSIM_ROBOT_ORCA);
 
     // ---- orca.py:113-115 preferred velocity (float64) ----
     const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
@@ -209,33 +170,6 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
 
     // ---- ORCA lines in rank order, in registers ----
     RegLines<M> R; bool valid[M];
-    if constexpr (CS_FLAT_STRAIGHT_LINES && MULTI) {
-        // for launches that leave 1-2 warps per scheduler (a launch lasts as long as one warp's dependent chains): all M constructions
-        // unconditionally and branch-free, so that their chains interleave; absent positions get a far-away dummy neighbour (no
-        // special values) and are zeroed afterwards, the rare overlapping lines (0.09 %) are repaired behind a warp vote.
-        V2 qp[M], qv[M]; float qr[M]; bool ov[M]; bool any_ov = false;
-        #pragma unroll
-        for (int kk = 0; kk < M; ++kk) {
-            const int sl = ebase + src[kk];
-            const float qx = __shfl_sync(CS_FULL, fpx, sl), qy = __shfl_sync(CS_FULL, fpy, sl);
-            const float wx = __shfl_sync(CS_FULL, fvx, sl), wy = __shfl_sync(CS_FULL, fvy, sl);
-            const float rh = __shfl_sync(CS_FULL, frh, sl), rr = __shfl_sync(CS_FULL, frr, sl);
-            valid[kk] = kk < nl;
-            qp[kk] = valid[kk] ? mk(qx, qy) : mk(fpx + 100.0f, fpy); qv[kk] = valid[kk] ? mk(wx, wy) : mk(0.f, 0.f);
-            qr[kk] = valid[kk] ? (is_robot ? rr : rh) : r;
-        }
-        #pragma unroll
-        for (int kk = 0; kk < M; ++kk) {
-            make_line_far(p, v, r, qp[kk], qv[kk], qr[kk], k.inv_time_horizon, R.p[kk], R.d[kk], ov[kk]);
-            ov[kk] = ov[kk] && valid[kk]; any_ov = any_ov || ov[kk];
-        }
-        if (__any_sync(CS_FULL, any_ov)) {
-            #pragma unroll
-            for (int kk = 0; kk < M; ++kk) if (ov[kk]) make_line_overlap(p, v, r, qp[kk], qv[kk], qr[kk], k.inv_time_step, R.p[kk], R.d[kk]);
-        }
-        #pragma unroll
-        for (int kk = 0; kk < M; ++kk) if (!valid[kk]) { R.p[kk] = mk(0.f, 0.f); R.d[kk] = mk(0.f, 0.f); }
-    } else {
     #pragma unroll
     for (int kk = 0; kk < M; ++kk) {
         const int sl = ebase + src[kk];
@@ -245,7 +179,6 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         valid[kk] = kk < nl;
         R.p[kk] = mk(0.f, 0.f); R.d[kk] = mk(0.f, 0.f);
         if (valid[kk]) make_line_sel(p, v, r, mk(qx, qy), mk(wx, wy), is_robot ? rr : rh, k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
-    }
     }
     if constexpr (STAGE == 2) {            // + preferred velocity, neighbour scan, ORCA lines
         float acc = pref.x + pref.y;
@@ -319,8 +252,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             __syncwarp();
         }
     } else {
-        // s_qcount = 0 visible (multi-step kernel: the barrier at the top of the step loop)
-        if constexpr (!MULTI) __syncthreads();
+        __syncthreads();                                     // s_qcount = 0 visible
         int slot = -1;
         if (need3) {
             slot = atomicAdd(&s_qcount, 1);
@@ -366,8 +298,6 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                 __syncthreads();
             }
             if (need3) nv = mk(s_res[0][slot], s_res[1][slot]);
-            // the queue is reused by the next step; every thread read cnt before the pass's first barrier
-            if (MULTI && tid == 0) s_qcount = 0;
         }
     }
 
@@ -378,7 +308,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     // ---- robot velocity of this step, broadcast inside the env ----
     double ax = 0, ay = 0, rvx = 0, rvy = 0;
     if (is_robot) {
-        if (MULTI || k.robot_policy == CROWDSIM_ROBOT_ORCA) { ax = (double)nv.x; ay = (double)nv.y; rvx = ax; rvy = ay; }
+        if (k.robot_policy == CROWDSIM_ROBOT_ORCA) { ax = (double)nv.x; ay = (double)nv.y; rvx = ax; rvy = ay; }
         else if (ROT) { ax = ext.x; ay = ext.y; rvx = ax * cos(ay + theta); rvy = ax * sin(ay + theta); }      // crowd_sim.py:340-341
         else { ax = ext.x; ay = ext.y; rvx = ax; rvy = ay; }
     }
@@ -426,20 +356,17 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             pos = make_double2(npx, npy); vel = make_double2(nvx, nvy);
             const double ntime = gtime + dt;
             rr.gtime = ntime;
-            if constexpr (MULTI) { rr.o_act = vel; rr.o_reward = reward; rr.o_dmin = dmin; rr.o_done = done ? 1 : 0; rr.o_info = info; rr.any_live = 1; dirty_kin = true; }
-            else {                                           // single step: nothing to carry, state and outputs leave at once
-                st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = ntime; if (ROT) A.st.r_theta[e] = theta;
-                if (A.io.action_out) st2(A.io.action_out, e, vel);
-                A.io.reward[e] = reward; A.io.dmin[e] = dmin; A.io.done[e] = done ? 1 : 0; A.io.info[e] = (uint8_t)info;
-            }
+            st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = ntime; if (ROT) A.st.r_theta[e] = theta;
+            if (A.io.action_out) st2(A.io.action_out, e, vel);
+            A.io.reward[e] = reward; A.io.dmin[e] = dmin; A.io.done[e] = done ? 1 : 0; A.io.info[e] = (uint8_t)info;
             if (A.has_ep) {
                 const crowdsim_episodes &ep = A.ep;
                 int ep_t = rr.ep_t, ep_tc = rr.ep_tc; double ep_ret = rr.ep_ret, ep_mds = rr.ep_mds;
                 const double disc = (ep_t < ep.discount_len) ? ep.discount[ep_t] : 0.0;
                 ep_ret = ep_ret + disc * reward; ep_t += 1;
-                if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; if constexpr (!MULTI) { ep.ep_too_close[e] = ep_tc; ep.ep_min_dist_sum[e] = ep_mds; } }
+                if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; ep.ep_too_close[e] = ep_tc; ep.ep_min_dist_sum[e] = ep_mds; }
                 rr.ep_t = ep_t; rr.ep_tc = ep_tc; rr.ep_ret = ep_ret; rr.ep_mds = ep_mds;
-                if constexpr (MULTI) rr.dirty_ep = 1; else { ep.ep_return[e] = ep_ret; ep.ep_steps[e] = ep_t; }
+                ep.ep_return[e] = ep_ret; ep.ep_steps[e] = ep_t;
                 if (done) {
                     const int ep_c = rr.ep_c;
                     if (ep_c >= 0) {
@@ -457,7 +384,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             // waiting, looks at its next-scene slot; a slot the generator publishes later is picked up by a later step
             const bool finished = live && done, parked = !live && rr.want != 0;
             if (finished || parked) {
-                const uint8_t sst = MULTI ? ld_relaxed_u8(A.ar.n_state + e) : slot_state;
+                const uint8_t sst = slot_state;
                 if (sst == CROWDSIM_SLOT_READY) install = 1;
                 else {
                     act_flag = 0; A.st.active[e] = 0;                             // park: nothing to install (yet)
@@ -469,68 +396,23 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     }
     if (A.has_ar) {                                          // warp-uniform
         install = __shfl_sync(CS_FULL, install, rl) && env_ok;
-        if constexpr (!MULTI) {
-            // single step: the scene goes straight from the slot to the live state (ar_install_*: acquire on the slot flag, copy)
-            if (install) {
-                if (is_robot) ar_install_robot(A, e);
-                else {
-                    ar_install_human(A, e, N, a);
-                    if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, hi); reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
-                }
+        // the scene goes straight from the slot to the live state (ar_install_*: acquire on the slot flag, copy)
+        if (install) {
+            if (is_robot) ar_install_robot(A, e);
+            else {
+                ar_install_human(A, e, N, a);
+                if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, hi); reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
             }
-        } else if (install) {
-            // acquire on the slot flag (every lane that reads slot data), then the scene (agent.py:47-58 set(px,py,gx,gy,0,0,..))
-            (void)ld_acquire_u8(A.ar.n_state + e);
-            if (!is_robot) {
-                pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); goal = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
-            } else {                                         // crowd_sim.py:262,274 + fresh episode accumulators
-                pos = make_double2(0.0, -A.ar.circle_radius); goal = make_double2(0.0, A.ar.circle_radius);
-                vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
-                theta = CS_PI / 2; rr.gtime = 0.0;
-                if (!ROT && A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
-                if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
-                act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
-            }
-            dirty_kin = true; dirty_scene = true;
         }
         __syncwarp();
         if (install && is_robot) st_release_u8(A.ar.n_state + e, CROWDSIM_SLOT_EMPTY);     // slot data consumed by all lanes of the env
-        if (MULTI) act_flag = (uint8_t)__shfl_sync(CS_FULL, (int)act_flag, rl);           // human lanes follow their robot lane's flag
-    } else if (MULTI) {
-        act_flag = (uint8_t)__shfl_sync(CS_FULL, (int)act_flag, rl);
     }
     if (live && !is_robot && !install) {
         // agent.py:122-135 holonomic step with the ORCA action (float32 values widened)
         const double hx = (double)nv.x, hy = (double)nv.y;
         pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
-        if constexpr (MULTI) dirty_kin = true;
-        else {
-            st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
-            if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, nv.x, nv.y);
-        }
-    }
-    }   // step loop
-
-    // ---- multi-step launches: one store of everything the launch changed ----
-    if constexpr (MULTI) if (env_ok) {
-        if (!is_robot) {
-            if (dirty_kin) {
-                st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
-                if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, (float)vel.x, (float)vel.y);
-            }
-            if (dirty_scene) { st2(A.st.h_goal, hi, goal); st2(A.st.h_attr, hi, attr); }
-        } else {
-            if (dirty_kin) { st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = rr.gtime; if (ROT) A.st.r_theta[e] = theta; }
-            if (dirty_scene) { st2(A.st.r_goal, e, goal); st2(A.st.r_attr, e, attr); }
-            if (rr.any_live) {                               // outputs of the env's last live step
-                if (A.io.action_out) st2(A.io.action_out, e, rr.o_act);
-                A.io.reward[e] = rr.o_reward; A.io.dmin[e] = rr.o_dmin; A.io.done[e] = rr.o_done; A.io.info[e] = (uint8_t)rr.o_info;
-            }
-            if (A.has_ep && rr.dirty_ep) {
-                A.ep.ep_steps[e] = rr.ep_t; A.ep.ep_return[e] = rr.ep_ret; A.ep.ep_too_close[e] = rr.ep_tc; A.ep.ep_min_dist_sum[e] = rr.ep_mds;
-                if (rr.new_case) A.ep.ep_case[e] = rr.ep_c;
-            }
-        }
+        st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
+        if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, nv.x, nv.y);
     }
 }
 

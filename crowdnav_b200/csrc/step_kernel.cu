@@ -74,6 +74,7 @@ __device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
 
 }  // namespace cs
 #include "step_flat.cuh"
+#include "step_multi.cuh"
 #include "step_mid.cuh"
 namespace cs {
 
@@ -350,28 +351,37 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         ++g_launches;
         return (int)cudaGetLastError();
     }
+    // n steps in one launch with the state in registers (step_multi.cuh): closed-loop only (the robot decides on device).
+    // Not for N = 1: ptxas (CUDA 12.9, sm_90a, -O1 and above) miscompiled that instantiation of the previous multi-step
+    // kernel -- its humans stored the position of the step before the last one -- so N = 1 runs n single-step launches.
+    if (n_steps > 1 && N >= 2 && N <= 5 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && !g_force_generic && !A.lookahead) {
+        const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
+        A.n_steps = n_steps;
+        #define CS_MULTI_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
+                                         else step_multi_kernel<NN, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
+        switch (N) {
+            case 2: CS_MULTI_LAUNCH(2); break;
+            case 3: CS_MULTI_LAUNCH(3); break;
+            case 4: CS_MULTI_LAUNCH(4); break;
+            default: CS_MULTI_LAUNCH(5); break;
+        }
+        #undef CS_MULTI_LAUNCH
+        ++g_launches;
+        return (int)cudaGetLastError();
+    }
     if (N >= 1 && N <= 5 && !g_force_generic && !A.lookahead) {
         // small crowds: register-resident solver, 32 / (N + 1) whole envs per warp (step_flat.cuh)
         const int epb = CS_FLAT_WPB * (32 / (N + 1));
         const int blocks = (B + epb - 1) / epb;
         const bool rot = A.k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT;
-        // n steps in one launch with the state in registers: closed-loop only (the robot decides on device). Not for N = 1:
-        // ptxas (CUDA 12.9, sm_90a, -O1 and above) miscompiles that instantiation -- its humans store the position of the
-        // step before the last one (correct at -Xptxas -O0; N = 2 .. 5 are bit-exact) -- so N = 1 runs n single-step launches.
-        const bool multi = n_steps > 1 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && N >= 2;
-        const int reps = multi ? 1 : n_steps;
-        if (multi) A.n_steps = n_steps;
         // linearProgram3 queue of the single-step kernel: per warp when the launch leaves SMs mostly empty (latency-bound: no
         // block barrier), per block when the chip is full (issue-bound: one warp runs the pass for the whole block).
-        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both. The multi-step kernel always
-        // uses the block queue: its launches are meant to run many at a time (independent batches on parallel streams), which
-        // fills the chip however small each grid is.
+        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        #define CS_FLAT_LAUNCH(NN) do { if (multi) step_flat_kernel<NN, 99, false, true, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                        else if (rot) step_flat_kernel<NN, 99, true, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                        else if (warpq) step_flat_kernel<NN, 99, false, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                        else step_flat_kernel<NN, 99, false, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
-        for (int rep = 0; rep < reps; ++rep) {
+        #define CS_FLAT_LAUNCH(NN) do { if (rot) step_flat_kernel<NN, 99, true, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
+                                        else if (warpq) step_flat_kernel<NN, 99, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
+                                        else step_flat_kernel<NN, 99, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
+        for (int rep = 0; rep < n_steps; ++rep) {
             switch (N) {
                 case 1: CS_FLAT_LAUNCH(1); break;
                 case 2: CS_FLAT_LAUNCH(2); break;

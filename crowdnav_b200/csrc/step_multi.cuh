@@ -1,0 +1,372 @@
+// step_multi.cuh -- crowdsim_step_n for small crowds (2 <= N <= 5 humans, ORCA robot): n env-steps per launch with the state
+// in registers, the robots on a warp of their own.
+//
+// Same contract as n x step_flat_kernel (crowd_sim/envs/crowd_sim.py:317-420 + orca.py:82-132 + explorer.py:41-72): with an
+// ORCA robot nothing leaves the device between steps (explorer.py:41-43 is a pure loop), so a launch loads its envs once,
+// runs n x (solve, collision, ladder, bookkeeping, install of the prefetched next scene when an episode ends) and stores
+// once; rare events (an episode's result row, parking, the slot hand-over) are written when they happen. Results are
+// bit-identical to n x crowdsim_step.
+//
+// Why a layout of its own: the instruction stream of the flat solver is almost independent of the data, so a warp runs the
+// union of what its lanes need. With humans and their robot side by side in a warp (step_flat.cuh), every warp builds and
+// solves N lines although a human with an invisible robot has N - 1, and every warp issues the robot's ladder and
+// bookkeeping with 5 of its 32 lanes active. Here a block holds E = 32 envs in N + 1 warps:
+//   * warps 0 .. N-1 are human warps: thread t handles (env t / N, human t % N), so the [B][N][2] arrays are read and
+//     written as contiguous 16-byte elements; an env's humans may straddle two warps. A human solves M = N - 1 lines when
+//     the robot is invisible (VIS = false), N when it is visible. The candidate slot of an invisible robot never passes the
+//     range test, so leaving it out changes no bit.
+//   * warp N is the robot warp, lane = env: the [B] and [B][2] robot arrays are read and written coalesced. It solves N
+//     lines, folds its humans' clearances in human order (first collision breaks), runs the ladder, the bookkeeping and the
+//     consumer side of the auto-reset protocol.
+// Intra-env exchange goes through shared memory. One step:
+//   1. every agent publishes its float32 view (position, velocity, the radius seen by a human and by the robot) and its
+//      float64 position, velocity and radius; the barrier that ends the step loop when no env of the block has work left
+//      (__syncthreads_or) makes them visible.
+//   2. every thread solves (flat solver of orca_spec.cuh, lines in registers); the solves that need linearProgram3 go to the
+//      block queue of step_flat.cuh (one item layout, sized for N lines), one pass over the whole block. The robot also
+//      publishes its lp2 result and its queue slot, so that after the pass the humans read its velocity without a barrier.
+//   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; a barrier.
+//   4. the robot folds the clearances, runs the env tail and publishes "install a scene" and "active"; a barrier; humans
+//      take over the flags and install their part of a new scene.
+// Measured and not kept (DESIGN §10): the robot computing the N clearances itself from the humans' float64 view, which
+// saves the barrier of step 3 but puts N float64 segment tests in a row on the robot warp.
+// The robot's per-env record (RobotRec: global time, episode accumulators, last step's outputs, flags) stays in shared
+// memory: in registers it would cost the human warps as much as the robot warp (one allocation for the whole kernel).
+#pragma once
+#include "step_flat.cuh"
+
+namespace cs {
+
+// Resident warps per SM the multi-step kernel is compiled for: blocks per SM = CS_MULTI_WARPS / (N + 1). N = 5: 4 blocks of
+// 6 warps (<= 80 registers; CUDA 12.9 spills 52 B). 3 blocks (18 warps, no spills) measured 16 % slower with 16 batches in
+// flight (DESIGN §10). A -D knob for A/B builds.
+#ifndef CS_MULTI_WARPS
+#define CS_MULTI_WARPS 24
+#endif
+
+// One solve of the multi-step kernel: agent a of the env whose float32 views start at slot ebase (robot: a = N). M lines
+// (candidates in the reference's order: the other humans, then the robot iff VIS; the robot sees all humans). Returns the
+// lp2 result; a solve that needs linearProgram3 is pushed to the block queue s_q (T columns, 4 * N + 5 rows) and gets its
+// slot, else slot = -1.
+template <int N, int M, bool ROBOT>
+__device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *s_view, const float *s_rview, int ebase, int a,
+                                                bool solves, double2 pos, double2 goal, double v_pref, orca::V2 p, orca::V2 v,
+                                                float r, float *s_q, int T, int *s_qcount, int &slot)
+{
+    using namespace orca;
+    // ---- orca.py:113-115 preferred velocity (float64) ----
+    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
+    const double speed = norm2(gvx, gvy);
+    const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+    const float max_speed = (float)v_pref;
+
+    // ---- neighbour scan and RVO2's stable order ----
+    float dsq[M]; bool inr[M]; int jj[M], src[M];
+    #pragma unroll
+    for (int c = 0; c < M; ++c) {
+        const int j = ROBOT ? c : ((c < N - 1) ? ((c < a) ? c : c + 1) : N);
+        jj[c] = j;
+        const float4 q = s_view[ebase + j];
+        dsq[c] = abssq(p - mk(q.x, q.y));
+        inr[c] = solves && (k.max_neighbors > 0) && dsq[c] < sqr(k.neighbor_dist);
+    }
+    int nl = neighbour_order<M>(dsq, inr, jj, src);
+    nl = nl < k.max_neighbors ? nl : k.max_neighbors;
+
+    // ---- ORCA lines in rank order, in registers ----
+    RegLines<M> R; bool valid[M];
+    #pragma unroll
+    for (int kk = 0; kk < M; ++kk) {
+        valid[kk] = kk < nl;
+        R.p[kk] = mk(0.f, 0.f); R.d[kk] = mk(0.f, 0.f);
+        if (valid[kk]) {
+            const int sl = ebase + src[kk];
+            const float4 q = s_view[sl];
+            make_line_sel(p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
+        }
+    }
+
+    // ---- speculative lp1 candidates, linearProgram2 as a scan ----
+    V2 cand[M]; bool feas[M];
+    lp1_all<M, M>(R, valid, max_speed, pref, false, cand, feas);
+    V2 nv = mk(0.f, 0.f);
+    const int fail = lp2_scan<M, M>(R, valid, nl, cand, feas, lp2_init(pref, max_speed), nv);
+
+    slot = -1;
+    if (solves && fail < nl) {
+        slot = atomicAdd(s_qcount, 1);
+        #pragma unroll
+        for (int kk = 0; kk < M; ++kk) {
+            s_q[(4 * kk + 0) * T + slot] = R.p[kk].x; s_q[(4 * kk + 1) * T + slot] = R.p[kk].y;
+            s_q[(4 * kk + 2) * T + slot] = R.d[kk].x; s_q[(4 * kk + 3) * T + slot] = R.d[kk].y;
+        }
+        s_q[(4 * N + 0) * T + slot] = __int_as_float(nl); s_q[(4 * N + 1) * T + slot] = __int_as_float(fail);
+        s_q[(4 * N + 2) * T + slot] = max_speed; s_q[(4 * N + 3) * T + slot] = nv.x; s_q[(4 * N + 4) * T + slot] = nv.y;
+    }
+    return nv;
+}
+
+template <int N, bool VIS>
+__global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
+step_multi_kernel(const __grid_constant__ StepArgs A)
+{
+    static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
+    using namespace orca;
+    constexpr int E = 32, L = N + 1, T = 32 * L;
+    constexpr int MH = VIS ? N : N - 1;                     // lines of a human solve
+    constexpr int SUB = N - 1;                              // lanes per queued lp3 item (sub-problems i = 1 .. N-1)
+    constexpr int QF = 4 * N + 5;                           // floats per queued lp3 work item
+    constexpr int PV = (4 * SUB > 6) ? 4 * SUB : 6;
+    __shared__ float s_q[QF][T];
+    // the float32 views (rows 0-3: position and velocity of slot le * L + a as a float4; rows 4, 5: radius as seen by a
+    // human / by the robot) are dead once the lines are built; the projected lines of the lp3 pass (4 * SUB rows) are only
+    // live inside the pass: one array serves both
+    __shared__ __align__(16) float s_pv[PV][T];
+    // per-thread sub-problem result (x, y, ok) inside the lp3 pass; after it, the humans' clearances (one double each)
+    __shared__ __align__(16) float s_r2[3][T];
+    // float64 position and velocity of every agent at the start of the step (threads 0 .. 32N-1 humans, then the robots):
+    // the humans' view for the robot's swept-segment test, and each thread's own copy, re-read after the solve, so that
+    // they hold no registers across it
+    __shared__ double2 s_pos[T], s_vel[T];
+    __shared__ double2 s_goal[T];                            // every agent's goal (changes only with the scene)
+    __shared__ double s_rad[T];                              // every agent's radius
+    __shared__ float2 s_rnv[E];                              // the robot's lp2 result and its lp3 queue slot (-1: none)
+    __shared__ int s_rslot[E];
+    __shared__ RobotRec s_rr[E];
+    __shared__ uint8_t s_flag[E];                            // robot -> humans: bit 0 active, bit 1 install the next scene
+    __shared__ int s_qcount;
+    float4 *const s_view = reinterpret_cast<float4 *>(&s_pv[0][0]);
+    float *const s_radh = s_pv[4], *const s_radr = s_pv[5];
+
+    const KParams &k = A.k;
+    const int tid = threadIdx.x;
+    const bool is_robot = tid >= 32 * N;
+    const int le = is_robot ? tid - 32 * N : tid / N;       // env within the block
+    const int a = is_robot ? N : tid - le * N;              // agent within the env
+    const int slot_me = le * L + a;                         // my float32 view
+    const int e = blockIdx.x * E + le;
+    const bool env_ok = e < A.B;
+    const size_t hi = (size_t)e * N + a;                    // my element of the [B][N][2] arrays (human threads)
+    if (tid == 0) s_qcount = 0;
+
+    // ---- all global loads of the launch up front (idle threads get a goal 5 m away: a zero goal vector would drag the warp
+    // through the f64 sqrt / division slow paths) ----
+    double2 pos = make_double2(0, 0), vel = pos, goal = make_double2(3, 4), attr = make_double2(0.3, 1.0);
+    uint8_t act_flag = 1;
+    if (env_ok) {
+        if (A.st.active) act_flag = A.st.active[e];
+        if (!is_robot) {
+            pos = ld2(A.st.h_pos, hi); vel = ld2(A.st.h_vel, hi); goal = ld2(A.st.h_goal, hi); attr = ld2(A.st.h_attr, hi);
+        } else {
+            pos = ld2(A.st.r_pos, e); vel = ld2(A.st.r_vel, e); goal = ld2(A.st.r_goal, e); attr = ld2(A.st.r_attr, e);
+            RobotRec r0 = {}; r0.ep_c = -1;
+            r0.gtime = A.st.g_time[e];
+            if (A.has_ep) { r0.ep_t = A.ep.ep_steps[e]; r0.ep_ret = A.ep.ep_return[e]; r0.ep_tc = A.ep.ep_too_close[e]; r0.ep_mds = A.ep.ep_min_dist_sum[e]; r0.ep_c = A.ep.ep_case[e]; }
+            if (A.has_ar) r0.want = A.ar.want[e];
+            s_rr[le] = r0;
+        }
+    }
+    s_goal[tid] = goal;
+    RobotRec &rr = s_rr[le];                                 // robot threads of valid envs only
+
+    // what this launch changed on this thread (decides the stores at the end)
+    bool dirty_kin = false, dirty_scene = false;
+    bool release = false;                                    // robot: hand the slot back once the humans have read it
+    const double dt = k.time_step;
+
+    #pragma unroll 1
+    for (int s = 0; ; ++s) {
+    const bool live = env_ok && (act_flag != 0);
+    // float32 view of myself for the other agents of my env (rvo2 boundary casts, orca.py:100-110), float64 view of the humans
+    const float fpx = (float)pos.x, fpy = (float)pos.y, fvx = (float)vel.x, fvy = (float)vel.y;
+    const float frh = (float)(attr.x + 0.01 + k.human_safety_space);     // my radius as seen by a human observer
+    const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
+    s_view[slot_me] = make_float4(fpx, fpy, fvx, fvy); s_radh[slot_me] = frh; s_radr[slot_me] = frr;
+    s_pos[tid] = pos; s_vel[tid] = vel; s_rad[tid] = attr.x;
+    // nothing left to do for this block: every env is frozen and none is waiting for a scene. Block-uniform, because the
+    // step's linearProgram3 pass has block barriers that every thread must reach. The views and the previous step's scene
+    // reads are complete here.
+    const bool work = live || (is_robot && env_ok && A.has_ar && rr.want != 0);
+    const int go = __syncthreads_or(s < A.n_steps && work);
+    if (release) { st_release_u8(A.ar.n_state + e, CROWDSIM_SLOT_EMPTY); release = false; }
+    if (!go) break;
+
+    // ---- ORCA solves ----
+    const V2 p = mk(fpx, fpy), v = mk(fvx, fvy);
+    int slot;
+    V2 nv = is_robot ? multi_solve<N, N, true>(k, s_view, s_radr, le * L, N, live, pos, s_goal[tid], attr.y, p, v, frr, &s_q[0][0], T, &s_qcount, slot)
+                     : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, &s_q[0][0], T, &s_qcount, slot);
+
+    if (is_robot) { s_rnv[le] = make_float2(nv.x, nv.y); s_rslot[le] = slot; }
+
+    // ---- linearProgram3 of the queued solves: the sub-problems of an item run on SUB threads in parallel (sequential
+    // shared-memory LP code of orca_device.cuh), the item's first thread finishes with the outer scan (step_flat.cuh) ----
+    if (__syncthreads_or(slot >= 0)) {
+        const int cnt = s_qcount;
+        constexpr int IPP = T / SUB;                         // items per pass
+        for (int base = 0; base < cnt; base += IPP) {
+            const int item = base + tid / SUB, i = tid % SUB + 1;
+            const bool mine = (tid < IPP * SUB) && item < cnt;
+            if (mine) {
+                const Lines Lq = { &s_q[0][item], T };
+                const int qn = __float_as_int(s_q[4 * N + 0][item]);
+                bool ok = false; V2 r2 = mk(0.f, 0.f);
+                if (i < qn) {
+                    const Lines Pq = { &s_pv[0][tid], T };
+                    ok = lp3_subproblem(Lq, i, s_q[4 * N + 2][item], Pq, r2);
+                }
+                s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
+            }
+            __syncthreads();
+            if (mine && i == 1) {
+                const Lines Lq = { &s_q[0][item], T };
+                const int qn = __float_as_int(s_q[4 * N + 0][item]), qf = __float_as_int(s_q[4 * N + 1][item]);
+                const float qr = s_q[4 * N + 2][item];
+                V2 res = mk(s_q[4 * N + 3][item], s_q[4 * N + 4][item]);
+                lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
+                    const int src_ = tid + (ii - 1);              // thread of sub-problem ii of this item
+                    r2 = mk(s_r2[0][src_], s_r2[1][src_]);
+                    return s_r2[2][src_] != 0.0f;
+                });
+                s_q[4 * N + 3][item] = res.x; s_q[4 * N + 4][item] = res.y;     // read back by the item's own thread only
+            }
+            __syncthreads();
+        }
+        if (slot >= 0) nv = mk(s_q[4 * N + 3][slot], s_q[4 * N + 4][slot]);
+        // the queue is reused by the next step; every thread read cnt before the pass's first barrier
+        if (tid == 0) s_qcount = 0;
+    }
+    pos = s_pos[tid]; vel = s_vel[tid];
+
+    double *const s_cl = reinterpret_cast<double *>(&s_r2[0][0]);     // [E * N]: the humans' clearances
+    if (!is_robot) {
+        if (live) {
+            // swept-segment clearance against the robot's velocity of this step (crowd_sim.py:333-345)
+            const int rt = 32 * N + le, rs = s_rslot[le];
+            const float2 rv = (rs >= 0) ? make_float2(s_q[4 * N + 3][rs], s_q[4 * N + 4][rs]) : s_rnv[le];
+            const double2 rp = s_pos[rt];
+            const double px = pos.x - rp.x, py = pos.y - rp.y;
+            const double vx = vel.x - (double)rv.x, vy = vel.y - (double)rv.y;    // the human's CURRENT velocity attribute (previous action)
+            const double ex = px + vx * dt, ey = py + vy * dt;
+            s_cl[tid] = point_to_segment_dist0(px, py, ex, ey) - attr.x - s_rad[rt];
+            // agent.py:122-135 holonomic step with the ORCA action (float32 values widened); a scene installed below replaces it
+            const double hx = (double)nv.x, hy = (double)nv.y;
+            pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
+            dirty_kin = true;
+        }
+    }
+    __syncthreads();
+    if (is_robot) {
+        int install = 0;
+        if (env_ok) {
+            bool done = false;
+            if (live) {
+                const double ax = (double)nv.x, ay = (double)nv.y;
+                // ordered fold of the humans' clearances (first collision breaks, crowd_sim.py:346-351)
+                double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
+                #pragma unroll
+                for (int i = 0; i < N; ++i) {
+                    const double ci = s_cl[le * N + i];
+                    if (!collision) { if (ci < 0) collision = true; else if (ci < dmin) dmin = ci; }
+                }
+                // ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72)
+                const double npx = pos.x + ax * dt, npy = pos.y + ay * dt;
+                const double2 goal = s_goal[tid];
+                const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
+                double reward; int info;
+                const double gtime = rr.gtime;
+                if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
+                else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
+                else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
+                else if (dmin < k.discomfort_dist) { reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt; done = false; info = CROWDSIM_INFO_DANGER; }
+                else { reward = 0; done = false; info = CROWDSIM_INFO_NOTHING; }
+                pos = make_double2(npx, npy); vel = make_double2(ax, ay);
+                const double ntime = gtime + dt;
+                rr.gtime = ntime;
+                rr.o_act = vel; rr.o_reward = reward; rr.o_dmin = dmin; rr.o_done = done ? 1 : 0; rr.o_info = info; rr.any_live = 1;
+                dirty_kin = true;
+                if (A.has_ep) {
+                    const crowdsim_episodes &ep = A.ep;
+                    int ep_t = rr.ep_t, ep_tc = rr.ep_tc; double ep_ret = rr.ep_ret, ep_mds = rr.ep_mds;
+                    const double disc = (ep_t < ep.discount_len) ? ep.discount[ep_t] : 0.0;
+                    ep_ret = ep_ret + disc * reward; ep_t += 1;
+                    if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; }
+                    rr.ep_t = ep_t; rr.ep_tc = ep_tc; rr.ep_ret = ep_ret; rr.ep_mds = ep_mds;
+                    rr.dirty_ep = 1;
+                    if (done) {
+                        const int ep_c = rr.ep_c;
+                        if (ep_c >= 0) {
+                            ep.res_info[ep_c] = (uint8_t)info; ep.res_steps[ep_c] = ep_t;
+                            ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
+                            ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
+                            if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
+                        }
+                        if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
+                    }
+                }
+            }
+            if (A.has_ar) {
+                // consumer side of the auto-reset protocol (include/crowdsim_b200.h): an env that just finished, or is parked
+                // waiting, looks at its next-scene slot; a slot the generator publishes later is picked up by a later step
+                const bool finished = live && done, parked = !live && rr.want != 0;
+                if (finished || parked) {
+                    const uint8_t sst = ld_relaxed_u8(A.ar.n_state + e);
+                    if (sst == CROWDSIM_SLOT_READY) install = 1;
+                    else {
+                        act_flag = 0; A.st.active[e] = 0;                             // park: nothing to install (yet)
+                        const uint8_t want = (sst == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1;
+                        rr.want = want; A.ar.want[e] = want;
+                    }
+                }
+                if (install) {
+                    // acquire on the slot flag (every thread that reads slot data), then crowd_sim.py:262,274 + fresh
+                    // episode accumulators
+                    (void)ld_acquire_u8(A.ar.n_state + e);
+                    pos = make_double2(0.0, -A.ar.circle_radius); s_goal[tid] = make_double2(0.0, A.ar.circle_radius);
+                    vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
+                    rr.gtime = 0.0;
+                    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
+                    if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
+                    act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
+                    dirty_kin = true; dirty_scene = true; release = true;
+                }
+            }
+        }
+        s_flag[le] = (uint8_t)((act_flag != 0) | (install << 1));
+    }
+    __syncthreads();
+    if (!is_robot) {                                         // humans follow their robot's flags
+        const unsigned f = s_flag[le];
+        act_flag = (uint8_t)(f & 1u);
+        if ((f & 2u) && env_ok) {                            // agent.py:47-58 set(px, py, gx, gy, 0, 0, ..)
+            (void)ld_acquire_u8(A.ar.n_state + e);
+            pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); s_goal[tid] = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
+            dirty_kin = true; dirty_scene = true;
+        }
+    }
+    }   // step loop
+
+    // ---- one store of everything the launch changed ----
+    if (env_ok) {
+        if (!is_robot) {
+            if (dirty_kin) {
+                st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
+                if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, (float)vel.x, (float)vel.y);
+            }
+            if (dirty_scene) { st2(A.st.h_goal, hi, s_goal[tid]); st2(A.st.h_attr, hi, attr); }
+        } else {
+            if (dirty_kin) { st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = rr.gtime; }
+            if (dirty_scene) { st2(A.st.r_goal, e, s_goal[tid]); st2(A.st.r_attr, e, attr); }
+            if (rr.any_live) {                               // outputs of the env's last live step
+                if (A.io.action_out) st2(A.io.action_out, e, rr.o_act);
+                A.io.reward[e] = rr.o_reward; A.io.dmin[e] = rr.o_dmin; A.io.done[e] = rr.o_done; A.io.info[e] = (uint8_t)rr.o_info;
+            }
+            if (A.has_ep && rr.dirty_ep) {
+                A.ep.ep_steps[e] = rr.ep_t; A.ep.ep_return[e] = rr.ep_ret; A.ep.ep_too_close[e] = rr.ep_tc; A.ep.ep_min_dist_sum[e] = rr.ep_mds;
+                if (rr.new_case) A.ep.ep_case[e] = rr.ep_c;
+            }
+        }
+    }
+}
+
+}  // namespace cs
