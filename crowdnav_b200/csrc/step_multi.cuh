@@ -22,9 +22,11 @@
 //   1. every agent publishes its float32 view (position, velocity, the radius seen by a human and by the robot) and its
 //      float64 position, velocity and radius; the barrier that ends the step loop when no env of the block has work left
 //      (__syncthreads_or) makes them visible.
-//   2. every thread solves (flat solver of orca_spec.cuh, lines in registers); the solves that need linearProgram3 go to the
-//      block queue of step_flat.cuh (one item layout, sized for N lines), one pass over the whole block. The robot also
-//      publishes its lp2 result and its queue slot, so that after the pass the humans read its velocity without a barrier.
+//   2. every human builds the robot's line against itself and arrives at named barrier 1; every thread solves (flat solver
+//      of orca_spec.cuh, lines in registers; the robot waits on barrier 1 and reads its lines instead of building them)
+//      and publishes its lp2 result; the solves that need linearProgram3 go to a block queue of T / (N - 1) items (one
+//      item layout, sized for N lines), one pass. The pass writes each result over its owner's lp2 result, so that after
+//      it the humans read their robot's velocity without a barrier.
 //   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; a barrier.
 //   4. the robot folds the clearances, runs the env tail and publishes "install a scene" and "active"; a barrier; humans
 //      take over the flags and install their part of a new scene.
@@ -37,21 +39,22 @@
 
 namespace cs {
 
-// Resident warps per SM the multi-step kernel is compiled for: blocks per SM = CS_MULTI_WARPS / (N + 1). N = 5: 4 blocks of
-// 6 warps (<= 80 registers; CUDA 12.9 spills 52 B). 3 blocks (18 warps, no spills) measured 16 % slower with 16 batches in
-// flight (DESIGN §10). A -D knob for A/B builds.
+// Resident warps per SM the multi-step kernel is compiled for: blocks per SM = CS_MULTI_WARPS / (N + 1). N = 5: 5 blocks of
+// 6 warps (64 registers; CUDA 12.9 spills 78 B, 34.6 KB of shared memory per block); 3 blocks (18 warps) measured 16 %
+// slower with 16 batches in flight (DESIGN §3.6, §10). A -D knob for A/B builds.
 #ifndef CS_MULTI_WARPS
-#define CS_MULTI_WARPS 24
+#define CS_MULTI_WARPS 30
 #endif
 
 // One solve of the multi-step kernel: agent a of the env whose float32 views start at slot ebase (robot: a = N). M lines
 // (candidates in the reference's order: the other humans, then the robot iff VIS; the robot sees all humans). Returns the
-// lp2 result; a solve that needs linearProgram3 is pushed to the block queue s_q (T columns, 4 * N + 5 rows) and gets its
-// slot, else slot = -1.
+// lp2 result, and what a linearProgram3 item needs (fail < nl): the lines in rank order (R, zero beyond M), nl, fail and
+// the maximum speed.
 template <int N, int M, bool ROBOT>
 __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *s_view, const float *s_rview, int ebase, int a,
                                                 bool solves, double2 pos, double2 goal, double v_pref, orca::V2 p, orca::V2 v,
-                                                float r, float *s_q, int T, int *s_qcount, int &slot)
+                                                float r, const float *s_rl, orca::RegLines<N> &Rq, int &nl_out, int &fail_out,
+                                                float &max_speed_out)
 {
     using namespace orca;
     // ---- orca.py:113-115 preferred velocity (float64) ----
@@ -73,16 +76,24 @@ __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *
     int nl = neighbour_order<M>(dsq, inr, jj, src);
     nl = nl < k.max_neighbors ? nl : k.max_neighbors;
 
-    // ---- ORCA lines in rank order, in registers ----
+    // ---- ORCA lines in rank order, in registers (the robot's were built by its humans: rows of s_rl, column = human
+    // thread; wait for them on named barrier 1, which the human warps arrive at) ----
+    constexpr int T = 32 * (N + 1);
+    if (ROBOT) asm volatile("barrier.sync 1, %0;" :: "r"(T) : "memory");
     RegLines<M> R; bool valid[M];
     #pragma unroll
     for (int kk = 0; kk < M; ++kk) {
         valid[kk] = kk < nl;
         R.p[kk] = mk(0.f, 0.f); R.d[kk] = mk(0.f, 0.f);
         if (valid[kk]) {
-            const int sl = ebase + src[kk];
-            const float4 q = s_view[sl];
-            make_line_sel(p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
+            if (ROBOT) {
+                const int c = (ebase / (N + 1)) * N + src[kk];
+                R.p[kk] = mk(s_rl[0 * T + c], s_rl[1 * T + c]); R.d[kk] = mk(s_rl[2 * T + c], s_rl[3 * T + c]);
+            } else {
+                const int sl = ebase + src[kk];
+                const float4 q = s_view[sl];
+                make_line_sel(p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
+            }
         }
     }
 
@@ -90,19 +101,10 @@ __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *
     V2 cand[M]; bool feas[M];
     lp1_all<M, M>(R, valid, max_speed, pref, false, cand, feas);
     V2 nv = mk(0.f, 0.f);
-    const int fail = lp2_scan<M, M>(R, valid, nl, cand, feas, lp2_init(pref, max_speed), nv);
-
-    slot = -1;
-    if (solves && fail < nl) {
-        slot = atomicAdd(s_qcount, 1);
-        #pragma unroll
-        for (int kk = 0; kk < M; ++kk) {
-            s_q[(4 * kk + 0) * T + slot] = R.p[kk].x; s_q[(4 * kk + 1) * T + slot] = R.p[kk].y;
-            s_q[(4 * kk + 2) * T + slot] = R.d[kk].x; s_q[(4 * kk + 3) * T + slot] = R.d[kk].y;
-        }
-        s_q[(4 * N + 0) * T + slot] = __int_as_float(nl); s_q[(4 * N + 1) * T + slot] = __int_as_float(fail);
-        s_q[(4 * N + 2) * T + slot] = max_speed; s_q[(4 * N + 3) * T + slot] = nv.x; s_q[(4 * N + 4) * T + slot] = nv.y;
-    }
+    fail_out = lp2_scan<M, M>(R, valid, nl, cand, feas, lp2_init(pref, max_speed), nv);
+    #pragma unroll
+    for (int kk = 0; kk < N; ++kk) { Rq.p[kk] = (kk < M) ? R.p[kk] : mk(0.f, 0.f); Rq.d[kk] = (kk < M) ? R.d[kk] : mk(0.f, 0.f); }
+    nl_out = nl; max_speed_out = max_speed;
     return nv;
 }
 
@@ -115,12 +117,14 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     constexpr int E = 32, L = N + 1, T = 32 * L;
     constexpr int MH = VIS ? N : N - 1;                     // lines of a human solve
     constexpr int SUB = N - 1;                              // lanes per queued lp3 item (sub-problems i = 1 .. N-1)
-    constexpr int QF = 4 * N + 5;                           // floats per queued lp3 work item
-    constexpr int PV = (4 * SUB > 6) ? 4 * SUB : 6;
-    __shared__ float s_q[QF][T];
+    constexpr int QC = T / SUB;                             // lp3 items queued per step = one pass (N = 5: 48 of 192 solves)
+    constexpr int QF = 4 * N + 4;                           // floats per queued lp3 item: lines, count, fail, radius, owner
+    constexpr int PV = (4 * SUB > 10) ? 4 * SUB : 10;
+    __shared__ float s_q[QF][QC];
     // the float32 views (rows 0-3: position and velocity of slot le * L + a as a float4; rows 4, 5: radius as seen by a
-    // human / by the robot) are dead once the lines are built; the projected lines of the lp3 pass (4 * SUB rows) are only
-    // live inside the pass: one array serves both
+    // human / by the robot) and the robot's lines (rows 6-9, column = the human thread that built it) are dead once the
+    // lines are built; the projected lines of the lp3 pass (4 * SUB rows) are only live inside the pass: one array serves
+    // all of them
     __shared__ __align__(16) float s_pv[PV][T];
     // per-thread sub-problem result (x, y, ok) inside the lp3 pass; after it, the humans' clearances (one double each)
     __shared__ __align__(16) float s_r2[3][T];
@@ -130,8 +134,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     __shared__ double2 s_pos[T], s_vel[T];
     __shared__ double2 s_goal[T];                            // every agent's goal (changes only with the scene)
     __shared__ double s_rad[T];                              // every agent's radius
-    __shared__ float2 s_rnv[E];                              // the robot's lp2 result and its lp3 queue slot (-1: none)
-    __shared__ int s_rslot[E];
+    __shared__ float2 s_nv[T];                               // every agent's velocity of the step: lp2 result, then lp3's
     __shared__ RobotRec s_rr[E];
     __shared__ uint8_t s_flag[E];                            // robot -> humans: bit 0 active, bit 1 install the next scene
     __shared__ int s_qcount;
@@ -193,48 +196,77 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
 
     // ---- ORCA solves ----
     const V2 p = mk(fpx, fpy), v = mk(fvx, fvy);
-    int slot;
-    V2 nv = is_robot ? multi_solve<N, N, true>(k, s_view, s_radr, le * L, N, live, pos, s_goal[tid], attr.y, p, v, frr, &s_q[0][0], T, &s_qcount, slot)
-                     : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, &s_q[0][0], T, &s_qcount, slot);
+    if (!is_robot) {
+        // the robot's half-plane against me, as the robot's solve would build it (the robot's view and radius as p, v, r;
+        // mine as seen by the robot as po, vo, ro): it shortens the robot warp, the critical path of every step. Every
+        // human thread arrives, inactive envs' included, so that the robot warp's barrier.sync completes.
+        const int rs = le * L + N;
+        const float4 q = s_view[rs];
+        V2 lp, ld;
+        make_line_sel(mk(q.x, q.y), mk(q.z, q.w), s_radr[rs], p, v, frr, k.inv_time_horizon, k.inv_time_step, lp, ld);
+        s_pv[6][tid] = lp.x; s_pv[7][tid] = lp.y; s_pv[8][tid] = ld.x; s_pv[9][tid] = ld.y;
+        asm volatile("barrier.arrive 1, %0;" :: "r"(T) : "memory");
+    }
+    RegLines<N> R; int nl, fail; float max_speed;
+    V2 nv = is_robot ? multi_solve<N, N, true>(k, s_view, s_radr, le * L, N, live, pos, s_goal[tid], attr.y, p, v, frr, s_pv[6], R, nl, fail, max_speed)
+                     : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, s_pv[6], R, nl, fail, max_speed);
 
-    if (is_robot) { s_rnv[le] = make_float2(nv.x, nv.y); s_rslot[le] = slot; }
-
-    // ---- linearProgram3 of the queued solves: the sub-problems of an item run on SUB threads in parallel (sequential
-    // shared-memory LP code of orca_device.cuh), the item's first thread finishes with the outer scan (step_flat.cuh) ----
-    if (__syncthreads_or(slot >= 0)) {
-        const int cnt = s_qcount;
-        constexpr int IPP = T / SUB;                         // items per pass
-        for (int base = 0; base < cnt; base += IPP) {
-            const int item = base + tid / SUB, i = tid % SUB + 1;
-            const bool mine = (tid < IPP * SUB) && item < cnt;
-            if (mine) {
-                const Lines Lq = { &s_q[0][item], T };
-                const int qn = __float_as_int(s_q[4 * N + 0][item]);
-                bool ok = false; V2 r2 = mk(0.f, 0.f);
-                if (i < qn) {
-                    const Lines Pq = { &s_pv[0][tid], T };
-                    ok = lp3_subproblem(Lq, i, s_q[4 * N + 2][item], Pq, r2);
-                }
-                s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
-            }
-            __syncthreads();
-            if (mine && i == 1) {
-                const Lines Lq = { &s_q[0][item], T };
-                const int qn = __float_as_int(s_q[4 * N + 0][item]), qf = __float_as_int(s_q[4 * N + 1][item]);
-                const float qr = s_q[4 * N + 2][item];
-                V2 res = mk(s_q[4 * N + 3][item], s_q[4 * N + 4][item]);
-                lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
-                    const int src_ = tid + (ii - 1);              // thread of sub-problem ii of this item
-                    r2 = mk(s_r2[0][src_], s_r2[1][src_]);
-                    return s_r2[2][src_] != 0.0f;
-                });
-                s_q[4 * N + 3][item] = res.x; s_q[4 * N + 4][item] = res.y;     // read back by the item's own thread only
-            }
-            __syncthreads();
+    // ---- linearProgram3 of the solves that need it: a block queue of QC items, one pass. The sub-problems of an item run
+    // on SUB threads in parallel (sequential shared-memory LP code of orca_device.cuh), the item's first thread finishes
+    // with the outer scan (step_flat.cuh) and writes the result over its owner's lp2 result in s_nv, where the humans also
+    // read their robot's. A solve that finds the queue full (more than QC in one block step: scenes where most agents
+    // overlap) runs RVO2's sequential linearProgram3 alone (out of line, on lines in local memory; tests/native/lp_fuzz.cu
+    // checks both forms against the oracle bit for bit) before the pass, so that no solve's lines stay live across it ----
+    const bool pending = live && fail < nl;
+    int slot = pending ? atomicAdd(&s_qcount, 1) : -1;
+    if (slot >= QC) {
+        float lq[4 * N], lp[4 * SUB];
+        #pragma unroll
+        for (int kk = 0; kk < N; ++kk) { lq[4 * kk + 0] = R.p[kk].x; lq[4 * kk + 1] = R.p[kk].y; lq[4 * kk + 2] = R.d[kk].x; lq[4 * kk + 3] = R.d[kk].y; }
+        const Lines Lq = { lq, 1 }, Pq = { lp, 1 };
+        lp3(Lq, nl, fail, max_speed, Pq, nv);
+        slot = -1;
+    } else if (slot >= 0) {
+        #pragma unroll
+        for (int kk = 0; kk < N; ++kk) {
+            s_q[4 * kk + 0][slot] = R.p[kk].x; s_q[4 * kk + 1][slot] = R.p[kk].y; s_q[4 * kk + 2][slot] = R.d[kk].x; s_q[4 * kk + 3][slot] = R.d[kk].y;
         }
-        if (slot >= 0) nv = mk(s_q[4 * N + 3][slot], s_q[4 * N + 4][slot]);
-        // the queue is reused by the next step; every thread read cnt before the pass's first barrier
-        if (tid == 0) s_qcount = 0;
+        s_q[4 * N + 0][slot] = __int_as_float(nl); s_q[4 * N + 1][slot] = __int_as_float(fail);
+        s_q[4 * N + 2][slot] = max_speed; s_q[4 * N + 3][slot] = __int_as_float(tid);
+    }
+    s_nv[tid] = make_float2(nv.x, nv.y);
+    const int cnt = __syncthreads_count(slot >= 0);
+    if (cnt > 0) {
+        if (tid == 0) s_qcount = 0;                          // every slot of the step is taken; the next step's come after more barriers
+        const int item = tid / SUB, i = tid % SUB + 1;
+        const bool mine = (tid < QC * SUB) && item < cnt;
+        if (mine) {
+            const Lines Lq = { &s_q[0][item], QC };
+            const int qn = __float_as_int(s_q[4 * N + 0][item]);
+            bool ok = false; V2 r2 = mk(0.f, 0.f);
+            if (i < qn) {
+                const Lines Pq = { &s_pv[0][tid], T };
+                ok = lp3_subproblem(Lq, i, s_q[4 * N + 2][item], Pq, r2);
+            }
+            s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
+        }
+        __syncthreads();
+        if (mine && i == 1) {
+            const Lines Lq = { &s_q[0][item], QC };
+            const int qn = __float_as_int(s_q[4 * N + 0][item]), qf = __float_as_int(s_q[4 * N + 1][item]);
+            const float qr = s_q[4 * N + 2][item];
+            const int owner = __float_as_int(s_q[4 * N + 3][item]);
+            const float2 r0 = s_nv[owner];
+            V2 res = mk(r0.x, r0.y);
+            lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
+                const int src_ = tid + (ii - 1);              // thread of sub-problem ii of this item
+                r2 = mk(s_r2[0][src_], s_r2[1][src_]);
+                return s_r2[2][src_] != 0.0f;
+            });
+            s_nv[owner] = make_float2(res.x, res.y);
+        }
+        __syncthreads();
+        if (slot >= 0) { const float2 q = s_nv[tid]; nv = mk(q.x, q.y); }
     }
     pos = s_pos[tid]; vel = s_vel[tid];
 
@@ -242,8 +274,8 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     if (!is_robot) {
         if (live) {
             // swept-segment clearance against the robot's velocity of this step (crowd_sim.py:333-345)
-            const int rt = 32 * N + le, rs = s_rslot[le];
-            const float2 rv = (rs >= 0) ? make_float2(s_q[4 * N + 3][rs], s_q[4 * N + 4][rs]) : s_rnv[le];
+            const int rt = 32 * N + le;
+            const float2 rv = s_nv[rt];
             const double2 rp = s_pos[rt];
             const double px = pos.x - rp.x, py = pos.y - rp.y;
             const double vx = vel.x - (double)rv.x, vy = vel.y - (double)rv.y;    // the human's CURRENT velocity attribute (previous action)
