@@ -226,7 +226,11 @@ __device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MT &rng
     const crowdsim_autoreset &ar = A.ar;
     const int N = A.N;
     uint32_t seed; int case_id;
-    if (!next_seed(A.a, e, A.assigned, seed, case_id)) { st_release_u8(ar.n_state + e, CROWDSIM_SLOT_EXHAUSTED); return; }
+    if (!next_seed(A.a, e, A.assigned, seed, case_id)) {
+        ar.n_case[e] = -1;                                   // no scene, no case (the queue entry drawn here is past the end)
+        st_release_u8(ar.n_state + e, CROWDSIM_SLOT_EXHAUSTED);
+        return;
+    }
     rng.seed(seed);
     generate_scene(rng, A.a, N, ar.n_h_pos + (size_t)e * N * 2, ar.n_h_goal + (size_t)e * N * 2, ar.n_h_attr + (size_t)e * N * 2);
     ar.n_case[e] = case_id;

@@ -166,7 +166,7 @@ typedef struct crowdsim_autoreset {
     double *n_h_pos;     /* [B][N][2] next scene: human start positions */
     double *n_h_goal;    /* [B][N][2] human goals */
     double *n_h_attr;    /* [B][N][2] human radius, v_pref */
-    int32_t *n_case;     /* [B] case index of the prefetched scene (-1 = untracked) */
+    int32_t *n_case;     /* [B] case index of the prefetched scene (-1 = untracked, and on an EXHAUSTED slot) */
     uint8_t *n_state;    /* [B] CROWDSIM_SLOT_* */
     uint8_t *want;       /* [B] 1 = env finished and is waiting for a scene */
     double circle_radius;  /* robot start/goal (0, -R) -> (0, R), crowd_sim.py:274 */

@@ -262,7 +262,7 @@ int oracle_crowdsim_prefetch_scenes(const crowdsim_reset_args *args, int B, int 
     for (int e = 0; e < B; ++e) {
         if (ar->n_state[e] != CROWDSIM_SLOT_EMPTY) continue;
         uint32_t seed; int case_id;
-        if (!next_seed(args, e, &seed, &case_id)) { ar->n_state[e] = CROWDSIM_SLOT_EXHAUSTED; continue; }
+        if (!next_seed(args, e, &seed, &case_id)) { ar->n_case[e] = -1; ar->n_state[e] = CROWDSIM_SLOT_EXHAUSTED; continue; }
         mt_state rng; mt_seed(&rng, seed);
         generate_scene(&rng, args, N, ar->n_h_pos + (size_t)e * N * 2, ar->n_h_goal + (size_t)e * N * 2, ar->n_h_attr + (size_t)e * N * 2);
         ar->n_case[e] = case_id;

@@ -80,6 +80,40 @@ def test_reset_scenes_match_reference(oracle):
             assert (st.h_attr[e] == h[:, 6:8]).all(), name
 
 
+def test_prefetch_random_attr_scenes_match_reference(oracle):
+    """The generator side of the auto-reset protocol with random human attributes: oracle.prefetch fills the next-scene
+    slots with the reference's own scenes of the same seeds (tests/golden/reset_scenes, *_random_attr rows), bit for bit,
+    unused `mixed` slots parked; the robot the install puts beside them is the reference's robot.set(0, -R, 0, R, 0, 0,
+    pi / 2) of the same rows."""
+    d = load_golden('reset_scenes')
+    names = ('circle5_random_attr', 'square5_random_attr', 'mixed5_random_attr')
+    for name in names:
+        kw, rows = d[name]['config'], d[name]['rows']
+        assert kw['randomize'], name
+        N, B = kw['human_num'], len(rows)
+        ar = oracle.HostAutoReset(B, N)
+        oracle.prefetch(ar, B, N, seeds=np.array([r['seed'] for r in rows], dtype=np.uint32), rule=kw['test_sim'],
+                        randomize_attributes=True)
+        assert (ar.n_state == 1).all() and (ar.n_case == -1).all(), name          # SLOT_READY, no case queue
+        for e, row in enumerate(rows):
+            r, h = scene_arrays(row['scene'], N)
+            for f, cols in (('n_h_pos', slice(0, 2)), ('n_h_goal', slice(4, 6)), ('n_h_attr', slice(6, 8))):
+                assert getattr(ar, f)[e].view(np.uint64).tolist() == h[:, cols].view(np.uint64).tolist(), (name, row['case'], f)
+            robot = [0.0, -ar.circle_radius, 0.0, 0.0, 0.0, ar.circle_radius, ar.robot_radius, ar.robot_v_pref, math.pi / 2]
+            assert np.array(robot).view(np.uint64).tolist() == r.view(np.uint64).tolist(), (name, row['case'])
+        assert len(np.unique(ar.n_h_attr[..., 0])) > B and len(np.unique(ar.n_h_attr[..., 1])) > B, name
+
+
+def test_prefetch_exhausted_slot_has_no_case(oracle):
+    """A slot the case queue cannot fill is EXHAUSTED with n_case = -1 (include/crowdsim_b200.h), not the case it held."""
+    ar = oracle.HostAutoReset(5, 2)
+    ar.n_case[:] = 7
+    counter = np.zeros(1, dtype=np.int32)
+    oracle.prefetch(ar, 5, 2, case_counter=counter, case_total=3, seed_base=1000)
+    assert sorted(ar.n_state.tolist()) == [1, 1, 1, 2, 2] and sorted(ar.n_case.tolist()) == [-1, -1, 0, 1, 2]
+    assert (ar.n_case[ar.n_state == 2] == -1).all()
+
+
 def test_trajectory_steps_match_reference(oracle):
     """Every recorded step of the golden trajectories: pre-state -> one oracle step == recorded post-state."""
     for name in ('circle5_invisible', 'square5_invisible', 'square20_invisible', 'circle5_visible', 'mixed5_invisible'):
