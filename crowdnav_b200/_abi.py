@@ -7,7 +7,7 @@ for its CPU library. No torch types cross the boundary.
 import ctypes as C
 import os
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_HUMANS = 63
 MAX_NEIGHBORS = 10
 
@@ -67,6 +67,17 @@ class AutoReset(C.Structure):
 SLOT_EMPTY, SLOT_READY, SLOT_EXHAUSTED, SLOT_CLAIMED = 0, 1, 2, 3
 
 
+class Record(C.Structure):
+    """crowdsim_record: one launch's imitation-learning staging, the per-slot trajectories and the memory ring."""
+    _fields_ = [('rows', C.c_void_p), ('reward', C.c_void_p), ('t', C.c_void_p), ('code', C.c_void_p), ('n_max', C.c_int32),
+                ('traj_rows', C.c_void_p), ('traj_reward', C.c_void_p), ('T', C.c_int32), ('g', C.c_void_p),
+                ('mem_states', C.c_void_p), ('mem_values', C.c_void_p), ('capacity', C.c_int64), ('position0', C.c_int64),
+                ('pushed', C.c_void_p), ('scan', C.c_void_p)]
+
+
+REC_NONE, REC_LIVE, REC_STORED, REC_DROPPED = 0, 1, 2, 3
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
     """Attach argtypes/restype for the compute entry points (shared by product and oracle libs)."""
     s = [C.c_void_p] if with_stream else []
@@ -76,6 +87,12 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
     if hasattr(lib, prefix + 'step_n'):
         f = getattr(lib, prefix + 'step_n')
         f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int] + s
+    if hasattr(lib, prefix + 'step_n_record'):
+        f = getattr(lib, prefix + 'step_n_record')
+        f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int,
+                                          P(Record)] + s
+        f = getattr(lib, prefix + 'record_flush')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), C.c_int] + s
     f = getattr(lib, prefix + 'prefetch_scenes')
     f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(AutoReset)] + s
     f = getattr(lib, prefix + 'orca_act')
@@ -91,7 +108,7 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
 
 
 EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_count', 'crowdsim_debug_force_generic', 'crowdsim_graph_launch',
-           'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n',
+           'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
            'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
            'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 

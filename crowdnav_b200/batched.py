@@ -314,11 +314,32 @@ class BatchedCrowdSim(object):
         _abi.check(rc, 'crowdsim_prefetch_scenes')
 
     # ---- step ----------------------------------------------------------------------------------------------------
-    def step(self, actions=None, n_steps=1):
+    def step(self, actions=None, n_steps=1, record=None):
         """One lockstep env-step. `actions` [B][2] float64 device tensor (vx,vy) / (v,r); None when the robot runs ORCA.
         n_steps > 1: crowdsim_step_n -- exactly n_steps single steps; with an ORCA robot and 2 <= N <= 5 they run inside ONE
         kernel launch with the state in registers (the closed episode loop of explorer.py:41-43). The returned reward /
-        done / info are those of each env's last live step."""
+        done / info are those of each env's last live step.
+        record: a memory.DeviceILRecorder -- the same steps through crowdsim_step_n_record (one launch for any n_steps),
+        then crowdsim_record_flush of their imitation-learning pairs into the recorder's memory. Needs an ORCA robot,
+        2 <= N <= 5, episode tracking and auto-reset (ValueError 'unsupported size' otherwise)."""
+        if record is not None:
+            if actions is not None:
+                raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
+            prm = self.params(); st = self.state.struct()
+            io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
+                             _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
+            ep = self.episodes.struct() if self.episodes is not None else None
+            ar = self.autoreset.struct() if self.autoreset is not None else None
+            rec = record.struct()
+            with torch.cuda.device(self.device):
+                rc = self.lib.crowdsim_step_n_record(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
+                                                     C.byref(ep) if ep is not None else None,
+                                                     C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
+                                                     self._stream())
+                _abi.check(rc, 'crowdsim_step_n_record')
+                rc = self.lib.crowdsim_record_flush(self.B, self.human_num, C.byref(rec), int(n_steps), self._stream())
+            _abi.check(rc, 'crowdsim_record_flush')
+            return self.observation(), self.reward, self.done, self.info
         if self.robot_policy != _abi.ROBOT_ORCA:
             if actions is None:
                 raise ValueError('robot policy is external: actions required')

@@ -1,0 +1,68 @@
+// step_args.cuh -- the argument block of the step kernels and the consumer side of the auto-reset protocol, shared by
+// step_kernel.cu (every step kernel) and record_kernel.cu (the recording instantiations of the multi-step kernel).
+#pragma once
+#include "crowdsim_common.cuh"
+
+namespace cs {
+
+struct StepArgs {
+    KParams k;
+    int B, N, L, EPB;
+    crowdsim_state st;
+    crowdsim_step_io io;
+    crowdsim_episodes ep;
+    crowdsim_autoreset ar;
+    int has_ep, has_ar;
+    int act_only;      // crowdsim_orca_act: robot lanes solve and write action_out, nothing is mutated
+    int n_steps;       // crowdsim_step_n: env-steps per launch (small-crowd kernel, ORCA robot)
+    // crowdsim_onestep_lookahead (generic / crowd kernel only): step(action, update=False) -- outputs are written, the state is
+    // not; the humans' next observable states go to la_pos / la_vel instead
+    int lookahead;
+    double *la_pos, *la_vel;
+    crowdsim_record rec;   // crowdsim_step_n_record: the staging the recording multi-step kernel writes (last, so that the
+                           // other fields keep their offsets)
+};
+
+// ---- auto-reset protocol, consumer side (include/crowdsim_b200.h: crowdsim_autoreset) ----
+// Robot lane: an env that just finished (or is parked waiting) looks at its next-scene slot. Returns 1 = install now.
+// `s` = the slot state read (volatile) earlier in this launch: a slot the generator publishes later is simply picked
+// up by the next step (the env parks for one step).
+__device__ __forceinline__ int ar_decide(const StepArgs &A, int e, uint8_t s, bool finished, bool parked)
+{
+    if (!(finished || parked)) return 0;
+    if (s == CROWDSIM_SLOT_READY) return 1;
+    A.st.active[e] = 0;                                        // park: nothing to install (yet)
+    A.ar.want[e] = (s == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1;
+    return 0;
+}
+// Human lane a of env e: copy the prefetched scene into the live state (agent.py:47-58 set(px,py,gx,gy,0,0,...)).
+// The generator published the slot with st.release; every lane that reads slot data acquires the flag first (and reads
+// with ld.global.cg: L2 is the coherence point).
+__device__ __forceinline__ void ar_install_human(const StepArgs &A, int e, int N, int a)
+{
+    const size_t i = (size_t)e * N + a;
+    (void)ld_acquire_u8(A.ar.n_state + e);
+    st2(A.st.h_pos, i, ld2_cg(A.ar.n_h_pos, i)); st2(A.st.h_vel, i, make_double2(0, 0));
+    st2(A.st.h_goal, i, ld2_cg(A.ar.n_h_goal, i)); st2(A.st.h_attr, i, ld2_cg(A.ar.n_h_attr, i));
+}
+// Robot lane of env e: crowd_sim.py:262,274 (global_time = 0, robot.set(0,-R,0,R,0,0,pi/2)) + fresh episode accumulators.
+__device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
+{
+    (void)ld_acquire_u8(A.ar.n_state + e);
+    st2(A.st.r_pos, e, make_double2(0.0, -A.ar.circle_radius)); st2(A.st.r_goal, e, make_double2(0.0, A.ar.circle_radius));
+    st2(A.st.r_vel, e, make_double2(0, 0)); st2(A.st.r_attr, e, make_double2(A.ar.robot_radius, A.ar.robot_v_pref));
+    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
+    A.st.g_time[e] = 0.0;
+    if (A.has_ep) {
+        A.ep.ep_steps[e] = 0; A.ep.ep_return[e] = 0.0; A.ep.ep_too_close[e] = 0; A.ep.ep_min_dist_sum[e] = 0.0;
+        A.ep.ep_case[e] = __ldcg(A.ar.n_case + e);
+    }
+    A.st.active[e] = 1; A.ar.want[e] = 0;
+}
+
+// record_kernel.cu: launch step_multi_kernel<N, VIS, true> (crowdsim_step_n_record) for 2 <= A.N <= 5. The recording
+// instantiations live in a unit of their own: their rows use CUDA's float32 atan2f / cosf / sinf (rotate.cuh), whose
+// library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code.
+int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream);
+
+}  // namespace cs

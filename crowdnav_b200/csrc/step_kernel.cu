@@ -19,60 +19,8 @@ namespace cs {
 unsigned long long g_launches = 0;
 int g_force_generic = 0;   // test hook: route every N through the generic one-thread-per-agent kernel
 
-struct StepArgs {
-    KParams k;
-    int B, N, L, EPB;
-    crowdsim_state st;
-    crowdsim_step_io io;
-    crowdsim_episodes ep;
-    crowdsim_autoreset ar;
-    int has_ep, has_ar;
-    int act_only;      // crowdsim_orca_act: robot lanes solve and write action_out, nothing is mutated
-    int n_steps;       // crowdsim_step_n: env-steps per launch (small-crowd kernel, ORCA robot)
-    // crowdsim_onestep_lookahead (generic / crowd kernel only): step(action, update=False) -- outputs are written, the state is
-    // not; the humans' next observable states go to la_pos / la_vel instead
-    int lookahead;
-    double *la_pos, *la_vel;
-};
-
-// ---- auto-reset protocol, consumer side (include/crowdsim_b200.h: crowdsim_autoreset) ----
-// Robot lane: an env that just finished (or is parked waiting) looks at its next-scene slot. Returns 1 = install now.
-// `s` = the slot state read (volatile) earlier in this launch: a slot the generator publishes later is simply picked
-// up by the next step (the env parks for one step).
-__device__ __forceinline__ int ar_decide(const StepArgs &A, int e, uint8_t s, bool finished, bool parked)
-{
-    if (!(finished || parked)) return 0;
-    if (s == CROWDSIM_SLOT_READY) return 1;
-    A.st.active[e] = 0;                                        // park: nothing to install (yet)
-    A.ar.want[e] = (s == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1;
-    return 0;
-}
-// Human lane a of env e: copy the prefetched scene into the live state (agent.py:47-58 set(px,py,gx,gy,0,0,...)).
-// The generator published the slot with st.release; every lane that reads slot data acquires the flag first (and reads
-// with ld.global.cg: L2 is the coherence point).
-__device__ __forceinline__ void ar_install_human(const StepArgs &A, int e, int N, int a)
-{
-    const size_t i = (size_t)e * N + a;
-    (void)ld_acquire_u8(A.ar.n_state + e);
-    st2(A.st.h_pos, i, ld2_cg(A.ar.n_h_pos, i)); st2(A.st.h_vel, i, make_double2(0, 0));
-    st2(A.st.h_goal, i, ld2_cg(A.ar.n_h_goal, i)); st2(A.st.h_attr, i, ld2_cg(A.ar.n_h_attr, i));
-}
-// Robot lane of env e: crowd_sim.py:262,274 (global_time = 0, robot.set(0,-R,0,R,0,0,pi/2)) + fresh episode accumulators.
-__device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
-{
-    (void)ld_acquire_u8(A.ar.n_state + e);
-    st2(A.st.r_pos, e, make_double2(0.0, -A.ar.circle_radius)); st2(A.st.r_goal, e, make_double2(0.0, A.ar.circle_radius));
-    st2(A.st.r_vel, e, make_double2(0, 0)); st2(A.st.r_attr, e, make_double2(A.ar.robot_radius, A.ar.robot_v_pref));
-    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
-    A.st.g_time[e] = 0.0;
-    if (A.has_ep) {
-        A.ep.ep_steps[e] = 0; A.ep.ep_return[e] = 0.0; A.ep.ep_too_close[e] = 0; A.ep.ep_min_dist_sum[e] = 0.0;
-        A.ep.ep_case[e] = __ldcg(A.ar.n_case + e);
-    }
-    A.st.active[e] = 1; A.ar.want[e] = 0;
-}
-
 }  // namespace cs
+#include "step_args.cuh"
 #include "step_flat.cuh"
 #include "step_multi.cuh"
 #include "step_mid.cuh"
@@ -311,9 +259,14 @@ static int sm_count()
 
 static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
                   const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int act_only, int n_steps, cudaStream_t stream,
-                  double *la_pos = nullptr, double *la_vel = nullptr)
+                  double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr)
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
+    if (rec) {
+        // the recording kernel is an instantiation of the multi-step kernel: nothing else records
+        if (N < 2 || N > 5 || prm->robot_policy != CROWDSIM_ROBOT_ORCA || g_force_generic) return CROWDSIM_EUNSUPPORTED;
+        if (!ep || !ar || !rec->rows || !rec->reward || !rec->t || !rec->code || n_steps > rec->n_max) return CROWDSIM_EINVAL;
+    }
     if (N > CROWDSIM_MAX_HUMANS || prm->max_neighbors > CROWDSIM_MAX_NEIGHBORS) return CROWDSIM_EUNSUPPORTED;
     if (N > 0 && (!st->h_pos || !st->h_vel || !st->h_goal || !st->h_attr)) return CROWDSIM_EINVAL;
     if (!st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr || !st->g_time) return CROWDSIM_EINVAL;
@@ -339,6 +292,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if (A.has_ep) A.ep = *ep; else memset(&A.ep, 0, sizeof(A.ep));
     A.has_ar = (ar != nullptr && !act_only);
     if (A.has_ar) A.ar = *ar; else memset(&A.ar, 0, sizeof(A.ar));
+    if (rec) A.rec = *rec; else memset(&A.rec, 0, sizeof(A.rec));
     if (act_only && N >= 1 && N <= 5 && !g_force_generic) {
         const int blocks = (B + 127) / 128;
         switch (N) {
@@ -354,11 +308,13 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     // n steps in one launch with the state in registers (step_multi.cuh): closed-loop only (the robot decides on device).
     // Not for N = 1: ptxas (CUDA 12.9, sm_90a, -O1 and above) miscompiled that instantiation of the previous multi-step
     // kernel -- its humans stored the position of the step before the last one -- so N = 1 runs n single-step launches.
-    if (n_steps > 1 && N >= 2 && N <= 5 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && !g_force_generic && !A.lookahead) {
+    // The recording instantiation runs for any n_steps (one step included).
+    if ((n_steps > 1 || rec) && N >= 2 && N <= 5 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && !g_force_generic && !A.lookahead) {
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
-        #define CS_MULTI_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
-                                         else step_multi_kernel<NN, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
+        if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream); }
+        #define CS_MULTI_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
+                                         else step_multi_kernel<NN, false, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
         switch (N) {
             case 2: CS_MULTI_LAUNCH(2); break;
             case 3: CS_MULTI_LAUNCH(3); break;
@@ -423,6 +379,14 @@ extern "C" int crowdsim_step_n(const crowdsim_params *prm, int B, int N, crowdsi
                                crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream)
 {
     return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream);
+}
+
+extern "C" int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                      crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                                      void *stream)
+{
+    if (!rec) return CROWDSIM_EINVAL;
+    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec);
 }
 
 extern "C" int crowdsim_onestep_lookahead(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, crowdsim_step_io *io,

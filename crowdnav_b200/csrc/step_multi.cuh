@@ -36,6 +36,7 @@
 // memory: in registers it would cost the human warps as much as the robot warp (one allocation for the whole kernel).
 #pragma once
 #include "step_flat.cuh"
+#include "rotate.cuh"
 
 namespace cs {
 
@@ -108,7 +109,34 @@ __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *
     return nv;
 }
 
-template <int N, bool VIS>
+// REC = true (crowdsim_step_n_record): the robot's v_pref as float32, published per env for its humans' recorded rows
+// (everything else a row needs is in the step's shared float64 view). Declared only by the recording instantiation.
+template <int E>
+__device__ __forceinline__ float *rec_vpref_smem()
+{
+    __shared__ float s_vp[E];
+    return s_vp;
+}
+
+// REC = true: human a of env e writes its row of step s, crowdsim_pack_joint(kinematics_unicycle = 0) of the pre-step state
+// (pack_kernel.cu: the same rotate code, the same float32 casts) to rows[s][e][a].
+__device__ __forceinline__ void rec_row(const crowdsim_record &rec, int B, int N, int s, int e, int a, double2 hp, double2 hv,
+                                        double hr, double2 rp, double2 rv, double2 rg, double rr, float rvp)
+{
+    float c, sn, rot, dg, rvx, rvy;
+    rotate_self((float)rp.x, (float)rp.y, (float)rv.x, (float)rv.y, (float)rg.x, (float)rg.y, c, sn, rot, dg, rvx, rvy);
+    float row[13];
+    rotate_row(row, (float)rp.x, (float)rp.y, (float)rr, rvp, 0.f, dg, rvx, rvy, c, sn, (float)hp.x, (float)hp.y, (float)hv.x,
+               (float)hv.y, (float)hr);
+    float *o = rec.rows + (((size_t)s * B + e) * N + a) * 13;
+    #pragma unroll
+    for (int i = 0; i < 13; ++i) o[i] = row[i];
+}
+
+// REC = false is crowdsim_step_n. REC = true also stages, per step and env, what an imitation-learning recorder needs
+// (include/crowdsim_b200.h: crowdsim_record): the humans write the rows of the envs live at the start of the step, the
+// robot the reward, the episode step and the CROWDSIM_REC_* code; steps a block does not run get CROWDSIM_REC_NONE.
+template <int N, bool VIS, bool REC>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
 step_multi_kernel(const __grid_constant__ StepArgs A)
 {
@@ -186,13 +214,23 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
     s_view[slot_me] = make_float4(fpx, fpy, fvx, fvy); s_radh[slot_me] = frh; s_radr[slot_me] = frr;
     s_pos[tid] = pos; s_vel[tid] = vel; s_rad[tid] = attr.x;
+    if constexpr (REC) { if (is_robot) rec_vpref_smem<E>()[le] = (float)attr.y; }
     // nothing left to do for this block: every env is frozen and none is waiting for a scene. Block-uniform, because the
     // step's linearProgram3 pass has block barriers that every thread must reach. The views and the previous step's scene
     // reads are complete here.
     const bool work = live || (is_robot && env_ok && A.has_ar && rr.want != 0);
     const int go = __syncthreads_or(s < A.n_steps && work);
     if (release) { st_release_u8(A.ar.n_state + e, CROWDSIM_SLOT_EMPTY); release = false; }
-    if (!go) break;
+    if (!go) {
+        if constexpr (REC) { if (is_robot && env_ok) for (int s2 = s; s2 < A.n_steps; ++s2) A.rec.code[(size_t)s2 * A.B + e] = CROWDSIM_REC_NONE; }
+        break;
+    }
+    if constexpr (REC) {
+        if (!is_robot && live) {
+            const int rt = 32 * N + le;
+            rec_row(A.rec, A.B, N, s, e, a, pos, vel, attr.x, s_pos[rt], s_vel[rt], s_goal[rt], s_rad[rt], rec_vpref_smem<E>()[le]);
+        }
+    }
 
     // ---- ORCA solves ----
     const V2 p = mk(fpx, fpy), v = mk(fvx, fvy);
@@ -307,6 +345,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
                 double reward; int info;
                 const double gtime = rr.gtime;
+                const int t_rec = rr.ep_t;                   // REC: the episode step the row was recorded at
                 if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
                 else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
                 else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
@@ -336,6 +375,13 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                         if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                     }
                 }
+                if constexpr (REC) {
+                    const size_t ri = (size_t)s * A.B + e;
+                    A.rec.reward[ri] = reward; A.rec.t[ri] = t_rec;
+                    A.rec.code[ri] = !done ? CROWDSIM_REC_LIVE : (info == CROWDSIM_INFO_TIMEOUT) ? CROWDSIM_REC_DROPPED : CROWDSIM_REC_STORED;
+                }
+            } else if constexpr (REC) {
+                A.rec.code[(size_t)s * A.B + e] = CROWDSIM_REC_NONE;
             }
             if (A.has_ar) {
                 // consumer side of the auto-reset protocol (include/crowdsim_b200.h): an env that just finished, or is parked

@@ -11,7 +11,10 @@ Robot policies:
   'orca'            the robot's ORCA solve is fused into the step kernel (test.py --policy orca)
   a policy object   anything with .act_batch(env) -> [B][2] float64 device tensor of ActionXY (policy.make_sarl() ...)
 With update_memory=True the rollout also fills a memory.DeviceReplayMemory like Explorer.update_memory does
-(explorer.py:92-125; imitation-learning returns or target-network bootstraps).
+(explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot,
+2 <= N <= 5 and no occupancy maps (train.py:116-132's IL phase) records inside the multi-step kernel and flushes on device
+(memory.DeviceILRecorder: a launch of steps_per_launch steps plus a flush); everything else records step by step
+(memory.TrajectoryRecorder). Both push the same pairs in the same order.
 
 Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous ranges per rank; there is no data-path
 collective; ONE gather of the per-case result rows (48 B per episode: 6 float64 columns; NCCL on GPU tensors, gloo in the CPU tests) brings
@@ -142,16 +145,23 @@ class BatchedExplorer(object):
         else:
             env.set_robot_policy('external_xy')
         env.reset_seeds(rule=rule, use_queue=True)
-        recorder = None
+        recorder = dev_rec = None
+        chunk = max(1, int(steps_per_launch))
         if update_memory:
-            from .memory import TrajectoryRecorder
+            from .memory import DeviceILRecorder, TrajectoryRecorder
             om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
-            recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om)
+            if self.robot_policy == 'orca' and imitation_learning and om is None and 2 <= env.human_num <= 5:
+                dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk)
+                dev_rec.begin()
+            else:
+                recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om)
         side = torch.cuda.Stream(device=env.device)
         main = torch.cuda.current_stream(env.device)
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per
-        # launch (crowdsim_step_n); a recorded rollout or a host-side policy needs every step
-        chunk = max(1, int(steps_per_launch)) if (self.robot_policy == 'orca' and recorder is None) else 1
+        # launch (crowdsim_step_n, or crowdsim_step_n_record when it also records); a step-by-step recorder or a host-side
+        # policy needs every step
+        if not (self.robot_policy == 'orca' and recorder is None):
+            chunk = 1
         if chunk > 1:
             prefetch_every, check_every = 1, max(1, check_every // chunk)
         from .batched import max_episode_steps
@@ -164,7 +174,9 @@ class BatchedExplorer(object):
                     env.prefetch()
             if recorder is not None:
                 recorder.before_step()
-            if self.robot_policy == 'orca':
+            if dev_rec is not None:
+                env.step(None, n_steps=chunk, record=dev_rec)
+            elif self.robot_policy == 'orca':
                 env.step(n_steps=chunk)
             else:
                 env.step(self.robot_policy.act_batch(env))
@@ -176,6 +188,8 @@ class BatchedExplorer(object):
             if it > guard:
                 raise RuntimeError('rollout did not terminate')
         main.wait_stream(side)
+        if dev_rec is not None:
+            dev_rec.finish()
         rows = gather_results(pack_results(ep, n_local), k, self.rank, self.world, self.group)
         env.case_counter[phase] = (first_case + k) % env.case_size[phase]
         env.autoreset = None

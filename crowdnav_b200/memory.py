@@ -6,6 +6,9 @@
                        (state_i, value_i) pairs are appended to the memory, with
                          imitation learning:  value_i = sum_{t >= i} pow(gamma, (t - i) * time_step * v_pref) * r_t
                          RL:                  value_i = r_i + gamma_bar * target_model(state_{i+1}),  r_i at the terminal step
+  DeviceILRecorder     the same for imitation learning with an ORCA robot and 2 <= N <= 5, recorded inside the multi-step
+                       kernel (crowdsim_step_n_record) and flushed to the memory on device (crowdsim_record_flush): same
+                       pairs, same order, same bits as TrajectoryRecorder, with no per-step launches or host syncs
 The IL return is accumulated forward in t (G_i += pow(...) * r_t as each reward arrives), i.e. in the same order and
 with the same pow() factors as the reference's sum(); it agrees to the last ulp of float64 (CPython >= 3.12 sums with
 Neumaier compensation) and is identical after the float32 cast the reference applies.
@@ -110,3 +113,64 @@ class TrajectoryRecorder(object):
         if bool(done.any()):
             self.returns[done] = 0.0
             self.rewards[done] = 0.0
+
+
+def il_discounts(gamma, time_step, v_pref, T):
+    """g[k] = pow(gamma, k * time_step * v_pref), k = 0..T-1: TrajectoryRecorder's W[t][i] at k = t - i, computed with the
+    same host expression (the exponent is (t - i) * (time_step * v_pref); EpisodeBuffers.discount rounds
+    t * time_step * v_pref, a different product)."""
+    expo = time_step * v_pref
+    return [pow(gamma, k * expo) for k in range(T)]
+
+
+class DeviceILRecorder(object):
+    """Imitation-learning demonstrations of an ORCA robot recorded on device (include/crowdsim_b200.h: crowdsim_record).
+
+    env.step(None, n_steps, record=self) runs n_steps closed-loop steps in one launch that also stages, per step and live
+    env, the rotated joint state, the reward, the episode step and how the step ended; a flush launch then appends them to
+    per-slot trajectories and writes the pairs of every episode that ends in ReachGoal or Collision to the memory ring, in
+    the order TrajectoryRecorder pushes them. The ring's write position and size live on the device during a run: call
+    begin() before the first step and finish() after the last (one host read).
+    Only for what the multi-step kernel runs: an ORCA robot, 2 <= N <= 5; RL targets, occupancy-map rows, other crowd
+    sizes and host-side policies use TrajectoryRecorder."""
+
+    def __init__(self, env, memory, gamma, n_max):
+        from .batched import max_episode_steps
+        B, N, dev = env.B, env.human_num, env.device
+        if tuple(memory.states.shape[1:]) != (N, 13):
+            raise ValueError('memory rows must be [N][13] joint states')
+        self.env, self.memory, self.n_max = env, memory, int(n_max)
+        self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
+        self.g = torch.tensor(il_discounts(gamma, env.time_step, env.robot_v_pref, self.T), dtype=torch.float64, device=dev)
+        n = self.n_max
+        self.rows = torch.empty((n, B, N, 13), dtype=torch.float32, device=dev)
+        self.reward = torch.empty((n, B), dtype=torch.float64, device=dev)
+        self.t = torch.empty((n, B), dtype=torch.int32, device=dev)
+        self.code = torch.zeros((n, B), dtype=torch.uint8, device=dev)
+        self.traj_rows = torch.zeros((B, self.T, N, 13), dtype=torch.float32, device=dev)
+        self.traj_reward = torch.zeros((B, self.T), dtype=torch.float64, device=dev)
+        self.pushed = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.scan = torch.empty(n * B + 2, dtype=torch.int64, device=dev)
+        self.position0 = memory.position
+
+    def begin(self):
+        """Start counting pushes at the memory's current write position."""
+        self.pushed.zero_()
+        self.position0 = self.memory.position
+
+    def finish(self):
+        """Move the memory's write position and size by what the flushes pushed since begin() (reads the counter)."""
+        n = int(self.pushed.item())
+        m = self.memory
+        m.position = (self.position0 + n) % m.capacity
+        m.size = min(m.capacity, m.size + n)
+        self.position0 = m.position
+        self.pushed.zero_()
+        return n
+
+    def struct(self):
+        m = self.memory
+        p = lambda t: t.data_ptr()  # noqa: E731
+        return _abi.Record(p(self.rows), p(self.reward), p(self.t), p(self.code), self.n_max, p(self.traj_rows),
+                           p(self.traj_reward), self.T, p(self.g), p(m.states), p(m.values), m.capacity, self.position0,
+                           p(self.pushed), p(self.scan))

@@ -15,6 +15,10 @@
  *                            per-step part of Explorer.run_k_episodes (explorer.py:41-72)
  *   crowdsim_step_n          the inner loop of Explorer.run_k_episodes for a robot that decides on device
  *                            (crowd_nav/utils/explorer.py:41-43: robot.act -> env.step, n times), closed on the GPU
+ *   crowdsim_step_n_record   crowdsim_step_n that also stages one launch's imitation-learning demonstrations
+ *   crowdsim_record_flush    ... and turns them into (state, value) pairs of the replay memory: Explorer.run_k_episodes
+ *                            (update_memory=True, imitation_learning=True) with an ORCA robot (explorer.py:41-43,66-69,
+ *                            92-105; crowd_nav/utils/memory.py:4-28)
  *   crowdsim_orca_act        crowd_sim/envs/utils/robot.py:9-14 with policy ORCA (orca.py:82-132), batched
  *   crowdsim_reset           crowd_sim/envs/crowd_sim.py:251-312 + generators :155-207 (np.random MT19937)
  *   crowdsim_prefetch_scenes the same generators, run ahead of time for the NEXT episode of each env slot
@@ -41,7 +45,7 @@
 extern "C" {
 #endif
 
-#define CROWDSIM_ABI_VERSION 4
+#define CROWDSIM_ABI_VERSION 5
 
 /* error codes */
 #define CROWDSIM_OK            0
@@ -247,6 +251,58 @@ int crowdsim_step(const crowdsim_params *prm, int B, int N, crowdsim_state *st, 
  */
 int crowdsim_step_n(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
                     crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream);
+
+/*
+ * Imitation-learning demonstrations recorded on device: Explorer.run_k_episodes(update_memory=True,
+ * imitation_learning=True) with an ORCA robot (crowd_nav/utils/explorer.py:41-43 the episode loop, :66-69 only ReachGoal
+ * and Collision episodes are stored, :92-105 update_memory with the IL value of every state).
+ *
+ * crowdsim_step_n_record = crowdsim_step_n that also stages, for every step s of the launch and every env e that is
+ * live (active) before it: rows[s][e] = crowdsim_pack_joint(kinematics_unicycle = 0) of the pre-step state (the same
+ * device code, so the same bits), reward[s][e] = the step's reward, t[s][e] = ep_steps before the step, and
+ * code[s][e] = CROWDSIM_REC_*. An env may end two episodes in one launch (one that started earlier, then a whole one
+ * after the install); the per-step codes keep them apart. Requires `ep` and `ar`. Returns CROWDSIM_EUNSUPPORTED wherever
+ * the one-launch multi-step kernel does not run: N < 2, N > 5, a robot that is not CROWDSIM_ROBOT_ORCA, or while
+ * crowdsim_debug_force_generic(1) is in effect. n_steps <= n_max.
+ *
+ * crowdsim_record_flush consumes the staging of one launch of n_steps in (s, e) order -- the order in which a per-step
+ * recorder pushes: each live step's row and reward go to the slot's trajectory at t (clamped at T - 1); when an episode
+ * ends with CROWDSIM_REC_STORED its L = t + 1 pairs (row_i, float32(G_i)), G_i = sum_{t=i}^{L-1} g[t-i] * r_t summed in
+ * ascending t from +0.0 with every product and sum rounded once, go to the memory ring at
+ * (position0 + *pushed + offset) % capacity, offset = the exclusive scan of stored lengths in (s, e) order; *pushed then
+ * grows by this flush's pairs (the caller reads it once at the end of a run and moves its ring's position and size).
+ * When one flush stores more than `capacity` pairs only the last `capacity` are written, which is what pushing them one
+ * by one would leave behind. A terminal code ends the slot's trajectory: the next episode starts again at t = 0.
+ * Two kernel launches (scan, copy); no host synchronisation.
+ */
+#define CROWDSIM_REC_NONE    0   /* env not live before the step: nothing recorded */
+#define CROWDSIM_REC_LIVE    1   /* live, the episode goes on */
+#define CROWDSIM_REC_STORED  2   /* live, the episode ended in ReachGoal or Collision: its pairs are stored */
+#define CROWDSIM_REC_DROPPED 3   /* live, the episode ended in Timeout: not stored (explorer.py:66-69) */
+typedef struct crowdsim_record {
+    /* staging of one launch, written by crowdsim_step_n_record */
+    float *rows;           /* [n_max][B][N][13] float32 */
+    double *reward;        /* [n_max][B] */
+    int32_t *t;            /* [n_max][B] */
+    uint8_t *code;         /* [n_max][B] CROWDSIM_REC_* */
+    int32_t n_max;
+    /* per-slot trajectories, kept across launches */
+    float *traj_rows;      /* [B][T][N][13] */
+    double *traj_reward;   /* [B][T] */
+    int32_t T;             /* >= the longest episode (max(128, max episode steps)) */
+    const double *g;       /* [T] g[k] = pow(gamma, k * time_step * v_pref), host-computed with C pow */
+    /* the replay memory ring (crowd_nav/utils/memory.py:4-28) */
+    float *mem_states;     /* [capacity][N][13] */
+    float *mem_values;     /* [capacity] */
+    int64_t capacity;
+    int64_t position0;     /* ring write position when *pushed was zeroed */
+    int64_t *pushed;       /* [1] pairs pushed since then (device counter) */
+    int64_t *scan;         /* [n_max * B + 2] flush scratch */
+} crowdsim_record;
+int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                           crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                           void *stream);
+int crowdsim_record_flush(int B, int N, const crowdsim_record *rec, int n_steps, void *stream);
 
 /* Robot ORCA action from the current state, no mutation: action_out[B][2]. */
 int crowdsim_orca_act(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, double *action_out,

@@ -3,7 +3,8 @@
    compute-sanitizer --tool racecheck python scripts/sanitize_run.py
 Covers: small-crowd step kernel (per-warp and per-block lp3 queue), multi-step kernel with auto-reset and a CONCURRENT scene
 prefetch on a side stream (the release / acquire slot hand-over), crowd kernel (N = 12), generic kernel, scene generation,
-lookahead pack / humans / onestep_lookahead, occupancy maps, human_times."""
+lookahead pack / humans / onestep_lookahead, occupancy maps, human_times, and the recording multi-step kernel with its flush
+(crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -39,6 +40,18 @@ for it in range(40):
     env.step_n(4)
 torch.cuda.synchronize()
 print('episodes finished', int((ep.res_steps > 0).sum()))
+
+# imitation-learning recording: crowdsim_step_n_record + crowdsim_record_flush, each launched once, into a ring that wraps
+from crowdnav_b200.memory import DeviceILRecorder, DeviceReplayMemory
+env = make(256, 5)
+ep = env.track_episodes(1000); env.set_case_queue(0, 1000, 'train'); env.enable_autoreset(); env.reset_seeds(use_queue=True); env.prefetch()
+for _ in range(30):
+    env.step_n(4)                           # episodes near their end, so that the recorded launch stores some
+mem = DeviceReplayMemory(500, 5, env.device)
+rec = DeviceILRecorder(env, mem, 0.9, 16)
+rec.begin()
+env.step(None, n_steps=16, record=rec)
+print('pairs recorded', rec.finish())
 
 # value-network support + lookahead + human times
 env = make(64, 5, policy='external_xy'); env.reset_seeds(torch.arange(64) + 1000)
