@@ -78,6 +78,12 @@ class Record(C.Structure):
 REC_NONE, REC_LIVE, REC_STORED, REC_DROPPED = 0, 1, 2, 3
 
 
+class RecordMaps(C.Structure):
+    """crowdsim_record_maps: occupancy-map rows of crowdsim_step_n_record_ex / crowdsim_record_flush_ex."""
+    _fields_ = [('h_pos', C.c_void_p), ('h_vel', C.c_void_p), ('maps', C.c_void_p), ('cell_num', C.c_int32),
+                ('channels', C.c_int32), ('cell_size', C.c_double)]
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
     """Attach argtypes/restype for the compute entry points (shared by product and oracle libs)."""
     s = [C.c_void_p] if with_stream else []
@@ -93,6 +99,12 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
                                           P(Record)] + s
         f = getattr(lib, prefix + 'record_flush')
         f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), C.c_int] + s
+    if hasattr(lib, prefix + 'step_n_record_ex'):
+        f = getattr(lib, prefix + 'step_n_record_ex')
+        f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int,
+                                          P(Record), P(RecordMaps)] + s
+        f = getattr(lib, prefix + 'record_flush_ex')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), C.c_int] + s
     f = getattr(lib, prefix + 'prefetch_scenes')
     f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(AutoReset)] + s
     f = getattr(lib, prefix + 'orca_act')
@@ -109,6 +121,7 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
 
 EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_count', 'crowdsim_debug_force_generic', 'crowdsim_graph_launch',
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
+           'crowdsim_step_n_record_ex', 'crowdsim_record_flush_ex',
            'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
            'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 

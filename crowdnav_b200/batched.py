@@ -319,9 +319,10 @@ class BatchedCrowdSim(object):
         n_steps > 1: crowdsim_step_n -- exactly n_steps single steps; with an ORCA robot and 2 <= N <= 5 they run inside ONE
         kernel launch with the state in registers (the closed episode loop of explorer.py:41-43). The returned reward /
         done / info are those of each env's last live step.
-        record: a memory.DeviceILRecorder -- the same steps through crowdsim_step_n_record (one launch for any n_steps),
-        then crowdsim_record_flush of their imitation-learning pairs into the recorder's memory. Needs an ORCA robot,
-        2 <= N <= 5, episode tracking and auto-reset (ValueError 'unsupported size' otherwise)."""
+        record: a memory.DeviceILRecorder -- the same steps through crowdsim_step_n_record_ex (one launch for any n_steps
+        at 2 <= N <= 5, the launch loop with its recording otherwise), then crowdsim_record_flush_ex of their
+        imitation-learning pairs (with occupancy maps when the recorder has them) into the recorder's memory. Needs an ORCA
+        robot, episode tracking and auto-reset (ValueError otherwise)."""
         if record is not None:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
@@ -330,15 +331,16 @@ class BatchedCrowdSim(object):
                              _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
             ep = self.episodes.struct() if self.episodes is not None else None
             ar = self.autoreset.struct() if self.autoreset is not None else None
-            rec = record.struct()
+            rec, maps = record.struct(), record.maps_struct()
+            mp = C.byref(maps) if maps is not None else None
             with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step_n_record(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                                     C.byref(ep) if ep is not None else None,
-                                                     C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
-                                                     self._stream())
-                _abi.check(rc, 'crowdsim_step_n_record')
-                rc = self.lib.crowdsim_record_flush(self.B, self.human_num, C.byref(rec), int(n_steps), self._stream())
-            _abi.check(rc, 'crowdsim_record_flush')
+                rc = self.lib.crowdsim_step_n_record_ex(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
+                                                        C.byref(ep) if ep is not None else None,
+                                                        C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
+                                                        mp, self._stream())
+                _abi.check(rc, 'crowdsim_step_n_record_ex')
+                rc = self.lib.crowdsim_record_flush_ex(self.B, self.human_num, C.byref(rec), mp, int(n_steps), self._stream())
+            _abi.check(rc, 'crowdsim_record_flush_ex')
             return self.observation(), self.reward, self.done, self.info
         if self.robot_policy != _abi.ROBOT_ORCA:
             if actions is None:

@@ -15,6 +15,7 @@
 // fully coalesced stores.
 #include "crowdsim_common.cuh"
 #include "rotate.cuh"
+#include "occupancy.cuh"
 
 namespace cs {
 
@@ -180,43 +181,12 @@ __global__ void __launch_bounds__(256) lookahead_humans_kernel(const __grid_cons
 // ---- MultiHumanRL.build_occupancy_maps (crowd_nav/policy/multi_human_rl.py:109-163): for every human i a cell_num x
 // cell_num grid (cell_size metres per cell) centred on i and aligned with i's velocity; channels = 1: occupancy,
 // 2: mean (vx, vy) of the occupants in i's frame, 3: (occupied, mean vx, mean vy). One thread per (env, human);
-// float64 like the reference's numpy code, output float32 like its torch tensor. ----
-#define CS_OM_MAX_CELLS 64
-struct OmArgs { int B, N, cell_num, channels; double cell_size; const double *pos, *vel; float *out; };
-
+// float64 like the reference's numpy code, output float32 like its torch tensor (occupancy.cuh). ----
 __global__ void __launch_bounds__(128) occupancy_kernel(const __grid_constant__ OmArgs G)
 {
-    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (size_t)G.B * G.N) return;
-    const int N = G.N, e = (int)(idx / N), i = (int)(idx - (size_t)e * N);
-    const int cells = G.cell_num * G.cell_num, C = G.channels;
-    double sx[CS_OM_MAX_CELLS], sy[CS_OM_MAX_CELLS]; int cnt[CS_OM_MAX_CELLS];
-    for (int c = 0; c < cells; ++c) { sx[c] = 0.0; sy[c] = 0.0; cnt[c] = 0; }
-    const double2 pi = ld2(G.pos, idx), vi = ld2(G.vel, idx);
-    const double angle = atan2(vi.y, vi.x);                                  // :124 new x-axis along the human's velocity
-    const double half = (double)G.cell_num / 2;
-    for (int j = 0; j < N; ++j) {
-        if (j == i) continue;
-        const double2 pj = ld2(G.pos, (size_t)e * N + j), vj = ld2(G.vel, (size_t)e * N + j);
-        const double ox = pj.x - pi.x, oy = pj.y - pi.y;
-        const double rot = atan2(oy, ox) - angle;
-        const double dist = sqrt(ox * ox + oy * oy);                         // :127 np.linalg.norm(axis=0)
-        const double rx = cos(rot) * dist, ry = sin(rot) * dist;
-        const double xi = floor(rx / G.cell_size + half), yi = floor(ry / G.cell_size + half);
-        if (!(xi >= 0 && xi < G.cell_num && yi >= 0 && yi < G.cell_num)) continue;     // :134-137 (-inf = outside)
-        const int cell = G.cell_num * (int)yi + (int)xi;
-        const double vrot = atan2(vj.y, vj.x) - angle;                      // :144-148
-        const double speed = sqrt(vj.x * vj.x + vj.y * vj.y);
-        sx[cell] += cos(vrot) * speed; sy[cell] += sin(vrot) * speed; cnt[cell] += 1;
-    }
-    float *o = G.out + idx * (size_t)(cells * C);
-    for (int c = 0; c < cells; ++c) {
-        const bool occ = cnt[c] > 0;
-        const double mx = occ ? sx[c] / cnt[c] : 0.0, my = occ ? sy[c] / cnt[c] : 0.0;
-        if (C == 1) o[c] = occ ? 1.f : 0.f;
-        else if (C == 2) { o[2 * c] = (float)mx; o[2 * c + 1] = (float)my; }
-        else { o[3 * c] = occ ? 1.f : 0.f; o[3 * c + 1] = (float)mx; o[3 * c + 2] = (float)my; }
-    }
+    #define CS_OM_KEEP_ROW(e) false
+    CS_OCCUPANCY_MAP_BODY(G, CS_OM_KEEP_ROW)
+    #undef CS_OM_KEEP_ROW
 }
 
 }  // namespace cs

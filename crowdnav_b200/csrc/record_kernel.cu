@@ -1,7 +1,11 @@
 // record_kernel.cu -- imitation-learning demonstrations recorded on device (sm_90a):
 //   launch_multi_record  the recording instantiations of the multi-step kernel (step_multi.cuh, REC = true), launched by
-//                        crowdsim_step_n_record (step_kernel.cu)
+//                        crowdsim_step_n_record and crowdsim_step_n_record_ex at 2 <= N <= 5 (step_kernel.cu)
+//   launch_record_between  the recording around each single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1,
+//                        N > 5, the forced generic kernel): the same staging, from the state between two launches
 //   crowdsim_record_flush  one launch's staging -> per-slot trajectories -> (state, value) pairs of the replay memory ring
+//   crowdsim_record_flush_ex  the same, optionally with occupancy-map rows: record_maps_kernel computes the map of every
+//                        staged (step, env) first (occupancy.cuh, the code of crowdsim_occupancy_maps)
 //
 // Replaces Explorer.update_memory with imitation_learning=True (crowd_nav/utils/explorer.py:92-105) for the episodes of
 // explorer.py:66-69 that are stored (ReachGoal, Collision), and ReplayMemory.push (crowd_nav/utils/memory.py:13-19). The
@@ -16,6 +20,7 @@
 // recorder's running sum, whose terms for t < i add +-0 and change no bit.
 #include "step_args.cuh"
 #include "step_multi.cuh"
+#include "occupancy.cuh"
 
 namespace cs {
 
@@ -34,7 +39,62 @@ int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream)
     return (int)cudaGetLastError();
 }
 
-struct FlushArgs { int B, N, n; crowdsim_record r; };
+// The launch loop's recording (crowdsim_step_n_record_ex at N = 1, N > 5 or with the forced generic kernel): between two
+// single-step launches, one thread per (env, human) of the state the step kernel left.
+//   post >= 0  TrajectoryRecorder.after_step of step `post` (memory.py): a step staged LIVE books io's reward; when io says
+//              the episode ended, its code becomes STORED (ReachGoal, Collision) or DROPPED (Timeout), as the recording
+//              multi-step kernel decides it. Human 0's thread.
+//   pre >= 0   TrajectoryRecorder.before_step of step `pre`: an env active now stages its rows (rec_row: the rotate code of
+//              crowdsim_pack_joint), its episode step and LIVE, and with occupancy maps its humans' float64 state; every
+//              other env stages NONE.
+// The two touch different steps' staging, so one launch serves post(s) and pre(s + 1).
+__global__ void __launch_bounds__(128) record_between_kernel(const __grid_constant__ StepArgs A, int post, int pre)
+{
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (size_t)A.B * A.N) return;
+    const int N = A.N, e = (int)(idx / N), a = (int)(idx - (size_t)e * N);
+    if (post >= 0 && a == 0) {
+        const size_t ri = (size_t)post * A.B + e;
+        if (A.rec.code[ri] == CROWDSIM_REC_LIVE) {
+            A.rec.reward[ri] = A.io.reward[e];
+            if (A.io.done[e]) A.rec.code[ri] = (A.io.info[e] == CROWDSIM_INFO_TIMEOUT) ? CROWDSIM_REC_DROPPED : CROWDSIM_REC_STORED;
+        }
+    }
+    if (pre >= 0) {
+        const size_t ri = (size_t)pre * A.B + e;
+        const bool live = A.st.active[e] != 0;
+        if (a == 0) {
+            A.rec.code[ri] = live ? CROWDSIM_REC_LIVE : CROWDSIM_REC_NONE;
+            if (live) A.rec.t[ri] = A.ep.ep_steps[e];
+        }
+        if (live) {
+            const double2 hp = ld2(A.st.h_pos, idx), hv = ld2(A.st.h_vel, idx), ha = ld2(A.st.h_attr, idx);
+            const double2 ra = ld2(A.st.r_attr, e);
+            rec_row(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e), ra.x,
+                    (float)ra.y);
+            if (A.recm.h_pos) rec_map_state(A.recm, A.B, N, pre, e, a, hp, hv);
+        }
+    }
+}
+
+void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream)
+{
+    const size_t n = (size_t)A.B * A.N;
+    record_between_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(A, post, pre);
+    ++g_launches;
+}
+
+struct FlushArgs { int B, N, n; crowdsim_record r; crowdsim_record_maps m; };
+
+// crowdsim_record_flush_ex with occupancy maps: the map of every human of every staged (step, env) (code != NONE) from the
+// staged float64 state, to maps.maps, with crowdsim_occupancy_maps' code (occupancy.cuh) over n_steps * B rows.
+
+__global__ void __launch_bounds__(128) record_maps_kernel(const __grid_constant__ OmArgs G, const uint8_t *code)
+{
+    #define CS_OM_NOT_STAGED(r) (code[r] == CROWDSIM_REC_NONE)     // rows r = s * B + e
+    CS_OCCUPANCY_MAP_BODY(G, CS_OM_NOT_STAGED)
+    #undef CS_OM_NOT_STAGED
+}
 
 __device__ __forceinline__ long long rec_len(const FlushArgs &F, size_t i)
 {
@@ -74,10 +134,13 @@ __global__ void __launch_bounds__(1024) record_scan_kernel(const __grid_constant
     }
 }
 
-__global__ void __launch_bounds__(128) record_copy_kernel(const __grid_constant__ FlushArgs F)
+// OM = false: rows of 13 floats. OM = true: rows of W = 13 + M floats, each human's staged row followed by its map.
+template <bool OM>
+__device__ __forceinline__ void record_copy(const FlushArgs &F)
 {
     const int e = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-    const int R = F.N * 13, T = F.r.T;
+    const int M = OM ? F.m.cell_num * F.m.cell_num * F.m.channels : 0, W = 13 + M;
+    const int R = OM ? F.N * W : F.N * 13, T = F.r.T;
     const long long items = (long long)F.n * F.B;
     const long long total = F.r.scan[items], base = F.r.scan[items + 1], cap = F.r.capacity;
     // pairs of this flush with a smaller index than `first` would be overwritten by later ones of the same flush
@@ -90,8 +153,16 @@ __global__ void __launch_bounds__(128) record_copy_kernel(const __grid_constant_
         const uint8_t code = F.r.code[i];                    // uniform over the block
         if (code == CROWDSIM_REC_NONE) continue;
         const int t = (F.r.t[i] < T - 1) ? F.r.t[i] : T - 1;
-        const float *row = F.r.rows + i * R;
-        for (int j = tid; j < R; j += nt) traj[(size_t)t * R + j] = row[j];
+        if constexpr (OM) {
+            const float *row = F.r.rows + i * (F.N * 13), *map = F.m.maps + i * ((size_t)F.N * M);
+            for (int j = tid; j < R; j += nt) {
+                const int h = j / W, c = j - h * W;
+                traj[(size_t)t * R + j] = (c < 13) ? row[h * 13 + c] : map[(size_t)h * M + (c - 13)];
+            }
+        } else {
+            const float *row = F.r.rows + i * R;
+            for (int j = tid; j < R; j += nt) traj[(size_t)t * R + j] = row[j];
+        }
         if (tid == 0) trew[t] = F.r.reward[i];
         __syncthreads();
         if (code == CROWDSIM_REC_STORED) {
@@ -113,18 +184,39 @@ __global__ void __launch_bounds__(128) record_copy_kernel(const __grid_constant_
     }
 }
 
+__global__ void __launch_bounds__(128) record_copy_kernel(const __grid_constant__ FlushArgs F) { record_copy<false>(F); }
+__global__ void __launch_bounds__(128) record_copy_om_kernel(const __grid_constant__ FlushArgs F) { record_copy<true>(F); }
+
 }  // namespace cs
 
-extern "C" int crowdsim_record_flush(int B, int N, const crowdsim_record *rec, int n_steps, void *stream)
+extern "C" int crowdsim_record_flush_ex(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
+                                        void *stream)
 {
     if (!rec || B < 0 || N < 1 || n_steps < 1 || n_steps > rec->n_max || rec->T < 1 || rec->capacity < 1) return CROWDSIM_EINVAL;
     if (!rec->rows || !rec->reward || !rec->t || !rec->code || !rec->traj_rows || !rec->traj_reward || !rec->g ||
         !rec->mem_states || !rec->mem_values || !rec->pushed || !rec->scan) return CROWDSIM_EINVAL;
     if (rec->position0 < 0 || rec->position0 >= rec->capacity) return CROWDSIM_EINVAL;
+    const int rc = cs::check_record_maps(N, maps);
+    if (rc != CROWDSIM_OK) return rc;
     if (B == 0) return CROWDSIM_OK;
     cs::FlushArgs F; F.B = B; F.N = N; F.n = n_steps; F.r = *rec;
+    if (maps) F.m = *maps; else memset(&F.m, 0, sizeof(F.m));
     cs::record_scan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(F);
-    cs::record_copy_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
-    cs::g_launches += 2;
+    if (maps) {
+        cs::OmArgs G; G.B = n_steps * B; G.N = N; G.cell_num = maps->cell_num; G.channels = maps->channels;
+        G.cell_size = maps->cell_size; G.pos = maps->h_pos; G.vel = maps->h_vel; G.out = maps->maps;
+        const size_t n = (size_t)n_steps * B * N;
+        cs::record_maps_kernel<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(G, rec->code);
+        cs::record_copy_om_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
+        cs::g_launches += 3;
+    } else {
+        cs::record_copy_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
+        cs::g_launches += 2;
+    }
     return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_record_flush(int B, int N, const crowdsim_record *rec, int n_steps, void *stream)
+{
+    return crowdsim_record_flush_ex(B, N, rec, nullptr, n_steps, stream);
 }

@@ -21,6 +21,8 @@ struct StepArgs {
     double *la_pos, *la_vel;
     crowdsim_record rec;   // crowdsim_step_n_record: the staging the recording multi-step kernel writes (last, so that the
                            // other fields keep their offsets)
+    crowdsim_record_maps recm;   // crowdsim_step_n_record_ex with occupancy-map rows (h_pos == NULL: none); after rec for
+                                 // the same reason
 };
 
 // ---- auto-reset protocol, consumer side (include/crowdsim_b200.h: crowdsim_autoreset) ----
@@ -60,9 +62,24 @@ __device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
     A.st.active[e] = 1; A.ar.want[e] = 0;
 }
 
+// crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the occupancy-map arguments, checked as crowdsim_occupancy_maps
+// checks its own (pack_kernel.cu). NULL = 13-float rows.
+static inline int check_record_maps(int N, const crowdsim_record_maps *m)
+{
+    if (!m) return CROWDSIM_OK;
+    if (!m->h_pos || !m->h_vel || !m->maps || N < 2 || m->cell_num < 1 || !(m->cell_size > 0) || m->channels < 1 ||
+        m->channels > 3) return CROWDSIM_EINVAL;
+    if (m->cell_num * m->cell_num > 64) return CROWDSIM_EUNSUPPORTED;
+    return CROWDSIM_OK;
+}
+
 // record_kernel.cu: launch step_multi_kernel<N, VIS, true> (crowdsim_step_n_record) for 2 <= A.N <= 5. The recording
 // instantiations live in a unit of their own: their rows use CUDA's float32 atan2f / cosf / sinf (rotate.cuh), whose
 // library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code.
 int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream);
+// record_kernel.cu: the recording around one single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1, N > 5, the
+// forced generic kernel). post >= 0: book step `post`'s reward and ending (TrajectoryRecorder.after_step); pre >= 0: stage
+// step `pre`'s rows of the envs live now (before_step). One launch.
+void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream);
 
 }  // namespace cs

@@ -259,13 +259,18 @@ static int sm_count()
 
 static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
                   const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int act_only, int n_steps, cudaStream_t stream,
-                  double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr)
+                  double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr,
+                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr)
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
     if (rec) {
-        // the recording kernel is an instantiation of the multi-step kernel: nothing else records
-        if (N < 2 || N > 5 || prm->robot_policy != CROWDSIM_ROBOT_ORCA || g_force_generic) return CROWDSIM_EUNSUPPORTED;
+        // crowdsim_step_n_record: only the recording instantiation of the multi-step kernel records. crowdsim_step_n_record_ex
+        // (rec_any_route): every N >= 1, through the launch loop where the multi-step kernel does not run
+        if (rec_any_route ? (N < 1 || N > CROWDSIM_MAX_HUMANS) : (N < 2 || N > 5 || g_force_generic)) return CROWDSIM_EUNSUPPORTED;
+        if (prm->robot_policy != CROWDSIM_ROBOT_ORCA) return CROWDSIM_EUNSUPPORTED;
         if (!ep || !ar || !rec->rows || !rec->reward || !rec->t || !rec->code || n_steps > rec->n_max) return CROWDSIM_EINVAL;
+        const int rc = check_record_maps(N, recm);
+        if (rc != CROWDSIM_OK) return rc;
     }
     if (N > CROWDSIM_MAX_HUMANS || prm->max_neighbors > CROWDSIM_MAX_NEIGHBORS) return CROWDSIM_EUNSUPPORTED;
     if (N > 0 && (!st->h_pos || !st->h_vel || !st->h_goal || !st->h_attr)) return CROWDSIM_EINVAL;
@@ -293,6 +298,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     A.has_ar = (ar != nullptr && !act_only);
     if (A.has_ar) A.ar = *ar; else memset(&A.ar, 0, sizeof(A.ar));
     if (rec) A.rec = *rec; else memset(&A.rec, 0, sizeof(A.rec));
+    if (recm) A.recm = *recm; else memset(&A.recm, 0, sizeof(A.recm));
     if (act_only && N >= 1 && N <= 5 && !g_force_generic) {
         const int blocks = (B + 127) / 128;
         switch (N) {
@@ -338,6 +344,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
                                         else if (warpq) step_flat_kernel<NN, 99, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
                                         else step_flat_kernel<NN, 99, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
         for (int rep = 0; rep < n_steps; ++rep) {
+            if (rec) launch_record_between(A, rep - 1, rep, stream);   // (crowdsim_step_n_record_ex at N = 1)
             switch (N) {
                 case 1: CS_FLAT_LAUNCH(1); break;
                 case 2: CS_FLAT_LAUNCH(2); break;
@@ -348,6 +355,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
             ++g_launches;
         }
         #undef CS_FLAT_LAUNCH
+        if (rec) launch_record_between(A, n_steps - 1, -1, stream);
         return (int)cudaGetLastError();
     }
     const int threads = A.EPB * A.L;
@@ -360,10 +368,12 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         if (err != cudaSuccess) return (int)err;
     }
     for (int rep = 0; rep < n_steps; ++rep) {
+        if (rec) launch_record_between(A, rep - 1, rep, stream);       // (crowdsim_step_n_record_ex)
         if (mid) step_kernel<true><<<blocks, threads, smem, stream>>>(A);
         else step_kernel<false><<<blocks, threads, smem, stream>>>(A);
         ++g_launches;
     }
+    if (rec) launch_record_between(A, n_steps - 1, -1, stream);
     return (int)cudaGetLastError();
 }
 
@@ -387,6 +397,14 @@ extern "C" int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, 
 {
     if (!rec) return CROWDSIM_EINVAL;
     return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec);
+}
+
+extern "C" int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                         crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                                         const crowdsim_record_maps *maps, void *stream)
+{
+    if (!rec) return CROWDSIM_EINVAL;
+    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec, true, maps);
 }
 
 extern "C" int crowdsim_onestep_lookahead(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, crowdsim_step_io *io,

@@ -133,6 +133,14 @@ __device__ __forceinline__ void rec_row(const crowdsim_record &rec, int B, int N
     for (int i = 0; i < 13; ++i) o[i] = row[i];
 }
 
+// crowdsim_step_n_record_ex with occupancy-map rows: human a of env e stages its pre-step float64 position and velocity of
+// step s, from which the flush computes the maps (occupancy.cuh).
+__device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int B, int N, int s, int e, int a, double2 hp, double2 hv)
+{
+    const size_t i = ((size_t)s * B + e) * N + a;
+    st2(m.h_pos, i, hp); st2(m.h_vel, i, hv);
+}
+
 // REC = false is crowdsim_step_n. REC = true also stages, per step and env, what an imitation-learning recorder needs
 // (include/crowdsim_b200.h: crowdsim_record): the humans write the rows of the envs live at the start of the step, the
 // robot the reward, the episode step and the CROWDSIM_REC_* code; steps a block does not run get CROWDSIM_REC_NONE.
@@ -229,6 +237,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
         if (!is_robot && live) {
             const int rt = 32 * N + le;
             rec_row(A.rec, A.B, N, s, e, a, pos, vel, attr.x, s_pos[rt], s_vel[rt], s_goal[rt], s_rad[rt], rec_vpref_smem<E>()[le]);
+            if (A.recm.h_pos) rec_map_state(A.recm, A.B, N, s, e, a, pos, vel);      // a runtime branch: one instantiation
         }
     }
 

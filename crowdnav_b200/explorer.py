@@ -11,10 +11,12 @@ Robot policies:
   'orca'            the robot's ORCA solve is fused into the step kernel (test.py --policy orca)
   a policy object   anything with .act_batch(env) -> [B][2] float64 device tensor of ActionXY (policy.make_sarl() ...)
 With update_memory=True the rollout also fills a memory.DeviceReplayMemory like Explorer.update_memory does
-(explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot,
-2 <= N <= 5 and no occupancy maps (train.py:116-132's IL phase) records inside the multi-step kernel and flushes on device
-(memory.DeviceILRecorder: a launch of steps_per_launch steps plus a flush); everything else records step by step
-(memory.TrajectoryRecorder). Both push the same pairs in the same order.
+(explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot
+(train.py:116-132's IL phase) records on device at every crowd size, with occupancy-map rows when the target policy has
+them (memory.DeviceILRecorder: steps_per_launch steps -- inside the multi-step kernel at 2 <= N <= 5 -- plus a flush);
+RL targets and host-side policies record step by step (memory.TrajectoryRecorder). Both push the same pairs in the same
+order. In imitation learning the rows are what target_policy.transform stores (explorer.py:102): its occupancy-map
+settings (with_om, cell_num, cell_size, om_channel_size) when target_policy is given.
 
 Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous ranges per rank; there is no data-path
 collective; ONE gather of the per-case result rows (48 B per episode: 6 float64 columns; NCCL on GPU tensors, gloo in the CPU tests) brings
@@ -110,6 +112,16 @@ def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure
     return stats
 
 
+def _om_settings(policy):
+    """(cell_num, cell_size, om_channel_size) of a policy whose rows carry occupancy maps (with_om, multi_human_rl.py:98-104),
+    else None: its `om` tuple (policy.make_sarl), or the reference MultiHumanRL's three attributes."""
+    if not getattr(policy, 'with_om', False):
+        return None
+    if getattr(policy, 'om', None) is not None:
+        return tuple(policy.om)
+    return (policy.cell_num, policy.cell_size, policy.om_channel_size)
+
+
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
                  rank=0, world=1, group=None):
@@ -149,16 +161,21 @@ class BatchedExplorer(object):
         chunk = max(1, int(steps_per_launch))
         if update_memory:
             from .memory import DeviceILRecorder, TrajectoryRecorder
-            om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
-            if self.robot_policy == 'orca' and imitation_learning and om is None and 2 <= env.human_num <= 5:
-                dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk)
+            # the rows are target_policy.transform(state) (explorer.py:102): in imitation learning the occupancy-map
+            # settings come from the target policy when there is one
+            if imitation_learning and self.target_policy is not None:
+                om = _om_settings(self.target_policy)
+            else:
+                om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
+            if self.robot_policy == 'orca' and imitation_learning:
+                dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om)
                 dev_rec.begin()
             else:
                 recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om)
         side = torch.cuda.Stream(device=env.device)
         main = torch.cuda.current_stream(env.device)
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per
-        # launch (crowdsim_step_n, or crowdsim_step_n_record when it also records); a step-by-step recorder or a host-side
+        # launch (crowdsim_step_n, or crowdsim_step_n_record_ex when it also records); a step-by-step recorder or a host-side
         # policy needs every step
         if not (self.robot_policy == 'orca' and recorder is None):
             chunk = 1

@@ -6,9 +6,10 @@
                        (state_i, value_i) pairs are appended to the memory, with
                          imitation learning:  value_i = sum_{t >= i} pow(gamma, (t - i) * time_step * v_pref) * r_t
                          RL:                  value_i = r_i + gamma_bar * target_model(state_{i+1}),  r_i at the terminal step
-  DeviceILRecorder     the same for imitation learning with an ORCA robot and 2 <= N <= 5, recorded inside the multi-step
-                       kernel (crowdsim_step_n_record) and flushed to the memory on device (crowdsim_record_flush): same
-                       pairs, same order, same bits as TrajectoryRecorder, with no per-step launches or host syncs
+  DeviceILRecorder     the same for imitation learning with an ORCA robot at any 1 <= N <= 63, with or without occupancy
+                       maps, recorded on device (crowdsim_step_n_record_ex: inside the multi-step kernel at 2 <= N <= 5, around
+                       each single-step launch otherwise) and flushed to the memory on device (crowdsim_record_flush_ex): same
+                       pairs, same order, same bits as TrajectoryRecorder, with no host syncs
 The IL return is accumulated forward in t (G_i += pow(...) * r_t as each reward arrives), i.e. in the same order and
 with the same pow() factors as the reference's sum(); it agrees to the last ulp of float64 (CPython >= 3.12 sums with
 Neumaier compensation) and is identical after the float32 cast the reference applies.
@@ -131,15 +132,21 @@ class DeviceILRecorder(object):
     per-slot trajectories and writes the pairs of every episode that ends in ReachGoal or Collision to the memory ring, in
     the order TrajectoryRecorder pushes them. The ring's write position and size live on the device during a run: call
     begin() before the first step and finish() after the last (one host read).
-    Only for what the multi-step kernel runs: an ORCA robot, 2 <= N <= 5; RL targets, occupancy-map rows, other crowd
-    sizes and host-side policies use TrajectoryRecorder."""
+    At 2 <= N <= 5 the steps run in the recording multi-step kernel (one launch); at N = 1 and N > 5 they run one launch
+    each, between launches that stage the rows and book the rewards (include/crowdsim_b200.h: crowdsim_step_n_record_ex).
+    om = (cell_num, cell_size, om_channel_size): every row is followed by the occupancy map of the pre-step human state, as
+    TrajectoryRecorder(om=...) records it (MultiHumanRL.transform with with_om); the memory holds [N][13 + cell_num^2 *
+    om_channel_size] rows. Only for an ORCA robot; RL targets and host-side policies use TrajectoryRecorder."""
 
-    def __init__(self, env, memory, gamma, n_max):
+    def __init__(self, env, memory, gamma, n_max, om=None):
         from .batched import max_episode_steps
         B, N, dev = env.B, env.human_num, env.device
-        if tuple(memory.states.shape[1:]) != (N, 13):
-            raise ValueError('memory rows must be [N][13] joint states')
-        self.env, self.memory, self.n_max = env, memory, int(n_max)
+        if om is not None and N < 2:
+            raise ValueError('need at least one array to concatenate')      # what env.occupancy_maps raises
+        F = 13 + (om[0] * om[0] * om[2] if om else 0)
+        if tuple(memory.states.shape[1:]) != (N, F):
+            raise ValueError('memory rows must be [N][%d] joint states%s' % (F, ' with occupancy maps' if om else ''))
+        self.env, self.memory, self.n_max, self.om = env, memory, int(n_max), om
         self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
         self.g = torch.tensor(il_discounts(gamma, env.time_step, env.robot_v_pref, self.T), dtype=torch.float64, device=dev)
         n = self.n_max
@@ -147,11 +154,15 @@ class DeviceILRecorder(object):
         self.reward = torch.empty((n, B), dtype=torch.float64, device=dev)
         self.t = torch.empty((n, B), dtype=torch.int32, device=dev)
         self.code = torch.zeros((n, B), dtype=torch.uint8, device=dev)
-        self.traj_rows = torch.zeros((B, self.T, N, 13), dtype=torch.float32, device=dev)
+        self.traj_rows = torch.zeros((B, self.T, N, F), dtype=torch.float32, device=dev)
         self.traj_reward = torch.zeros((B, self.T), dtype=torch.float64, device=dev)
         self.pushed = torch.zeros(1, dtype=torch.int64, device=dev)
         self.scan = torch.empty(n * B + 2, dtype=torch.int64, device=dev)
         self.position0 = memory.position
+        if om:
+            self.h_pos = torch.empty((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.h_vel = torch.empty((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.maps = torch.empty((n, B, N, F - 13), dtype=torch.float32, device=dev)
 
     def begin(self):
         """Start counting pushes at the memory's current write position."""
@@ -174,3 +185,11 @@ class DeviceILRecorder(object):
         return _abi.Record(p(self.rows), p(self.reward), p(self.t), p(self.code), self.n_max, p(self.traj_rows),
                            p(self.traj_reward), self.T, p(self.g), p(m.states), p(m.values), m.capacity, self.position0,
                            p(self.pushed), p(self.scan))
+
+    def maps_struct(self):
+        """The occupancy-map staging (include/crowdsim_b200.h: crowdsim_record_maps), or None without maps."""
+        if not self.om:
+            return None
+        cell_num, cell_size, channels = self.om
+        return _abi.RecordMaps(self.h_pos.data_ptr(), self.h_vel.data_ptr(), self.maps.data_ptr(), int(cell_num),
+                               int(channels), float(cell_size))

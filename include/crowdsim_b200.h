@@ -19,6 +19,8 @@
  *   crowdsim_record_flush    ... and turns them into (state, value) pairs of the replay memory: Explorer.run_k_episodes
  *                            (update_memory=True, imitation_learning=True) with an ORCA robot (explorer.py:41-43,66-69,
  *                            92-105; crowd_nav/utils/memory.py:4-28)
+ *   crowdsim_step_n_record_ex, crowdsim_record_flush_ex  the same at every crowd size, optionally with occupancy-map rows
+ *                            (multi_human_rl.py:98-104 with with_om)
  *   crowdsim_orca_act        crowd_sim/envs/utils/robot.py:9-14 with policy ORCA (orca.py:82-132), batched
  *   crowdsim_reset           crowd_sim/envs/crowd_sim.py:251-312 + generators :155-207 (np.random MT19937)
  *   crowdsim_prefetch_scenes the same generators, run ahead of time for the NEXT episode of each env slot
@@ -303,6 +305,36 @@ int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, crowdsim_st
                            crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
                            void *stream);
 int crowdsim_record_flush(int B, int N, const crowdsim_record *rec, int n_steps, void *stream);
+
+/*
+ * The same recording at every crowd size, and with occupancy-map rows (MultiHumanRL.transform with with_om,
+ * crowd_nav/policy/multi_human_rl.py:98-104, 109-163). crowdsim_step_n_record_ex / crowdsim_record_flush_ex take the
+ * arguments of crowdsim_step_n_record / crowdsim_record_flush plus `maps`:
+ *   maps == NULL  rows of 13 floats, as crowdsim_step_n_record / crowdsim_record_flush.
+ *   maps != NULL  rec->traj_rows and rec->mem_states are [..][N][F], F = 13 + cell_num^2 * channels: each human's 13-float
+ *                 row followed by its occupancy map (crowdsim_occupancy_maps' layout and device code) of the pre-step human
+ *                 state. rec->rows stays [n_max][B][N][13]. Requires N >= 2, 1 <= channels <= 3, cell_size > 0 and
+ *                 cell_num^2 <= 64 (CROWDSIM_EINVAL / CROWDSIM_EUNSUPPORTED as crowdsim_occupancy_maps returns them).
+ * Any 1 <= N <= CROWDSIM_MAX_HUMANS with an ORCA robot (N = 0 or another robot: CROWDSIM_EUNSUPPORTED). For 2 <= N <= 5
+ * the step is the one-launch recording multi-step kernel of crowdsim_step_n_record; for N = 1, N > 5 and while
+ * crowdsim_debug_force_generic(1) is in effect it is the launch loop of crowdsim_step_n, each single-step launch between a
+ * kernel that stages the rows of the envs live before it and one that books its reward and ending (2 n_steps + 1
+ * launches). The staging and the pairs are the same whichever route runs. The flush computes the maps of every staged
+ * (step, env) first (one more launch).
+ */
+typedef struct crowdsim_record_maps {
+    double *h_pos;     /* [n_max][B][N][2] staging: the pre-step human positions of every recorded (step, env) */
+    double *h_vel;     /* [n_max][B][N][2] ... and velocities */
+    float *maps;       /* [n_max][B][N][cell_num^2 * channels] flush scratch */
+    int32_t cell_num;  /* policy.config [om] cell_num */
+    int32_t channels;  /* om_channel_size */
+    double cell_size;  /* cell_size (metres) */
+} crowdsim_record_maps;
+int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                              crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                              const crowdsim_record_maps *maps, void *stream);
+int crowdsim_record_flush_ex(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
+                             void *stream);
 
 /* Robot ORCA action from the current state, no mutation: action_out[B][2]. */
 int crowdsim_orca_act(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, double *action_out,

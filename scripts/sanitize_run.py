@@ -3,8 +3,10 @@
    compute-sanitizer --tool racecheck python scripts/sanitize_run.py
 Covers: small-crowd step kernel (per-warp and per-block lp3 queue), multi-step kernel with auto-reset and a CONCURRENT scene
 prefetch on a side stream (the release / acquire slot hand-over), crowd kernel (N = 12), generic kernel, scene generation,
-lookahead pack / humans / onestep_lookahead, occupancy maps, human_times, and the recording multi-step kernel with its flush
-(crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps."""
+lookahead pack / humans / onestep_lookahead, occupancy maps, human_times, the recording multi-step kernel with its flush
+(crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps, and both routes of
+crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
+at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -52,6 +54,19 @@ rec = DeviceILRecorder(env, mem, 0.9, 16)
 rec.begin()
 env.step(None, n_steps=16, record=rec)
 print('pairs recorded', rec.finish())
+
+# crowdsim_step_n_record_ex: the launch loop's recording at N = 1 and N = 20, occupancy-map rows at N = 5
+for N, om in ((1, None), (20, None), (5, (4, 1.0, 3))):
+    env = make(128, N, rule='square_crossing' if N > 5 else 'circle_crossing')
+    env.track_episodes(600); env.set_case_queue(0, 600, 'train'); env.enable_autoreset(); env.reset_seeds(use_queue=True); env.prefetch()
+    for _ in range(6):
+        env.step_n(4)                       # episodes near their end, so that the recorded launch stores some
+    env.prefetch()
+    mem = DeviceReplayMemory(400, N, env.device, 13 + (om[0] * om[0] * om[2] if om else 0))
+    rec = DeviceILRecorder(env, mem, 0.9, 16, om=om)
+    rec.begin()
+    env.step(None, n_steps=16, record=rec)
+    print('N', N, 'maps', om, 'pairs recorded', rec.finish())
 
 # value-network support + lookahead + human times
 env = make(64, 5, policy='external_xy'); env.reset_seeds(torch.arange(64) + 1000)

@@ -9,13 +9,18 @@ alternated in one process, at each batch size. Reports episodes/s, pairs/s and t
 (untimed, with rings that hold every pair) that both paths store the same multiset of (state, value) pairs, and prints the
 card's name and power limit.
 
-  python scripts/time_il_rollout.py [--B 1024 4096] [--k 3000] [--reps 2] [--steps-per-launch 8]
+  python scripts/time_il_rollout.py [--B 1024 4096] [--k 3000] [--reps 2] [--steps-per-launch 8] [--N 5] [--om C S CH]
+
+--N sets the crowd size (the device path runs the multi-step kernel at 2 <= N <= 5, the launch loop with its recording
+otherwise; N = 1 is CADRL's single-human IL scene; above 5 the scenes are square crossing), --om CELL_NUM CELL_SIZE CHANNELS records OM-SARL's rows with occupancy
+maps (the per-step recorder with om=..., BatchedExplorer with an OM target policy).
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import types
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
@@ -25,12 +30,18 @@ from crowdnav_b200.batched import BatchedCrowdSim, default_config, max_episode_s
 from crowdnav_b200.explorer import BatchedExplorer  # noqa: E402
 from crowdnav_b200.memory import DeviceReplayMemory, TrajectoryRecorder  # noqa: E402
 
-GAMMA, CAPACITY, N = 0.9, 100000, 5
+GAMMA, CAPACITY = 0.9, 100000
+N, OM = 5, None                                              # set from --N / --om
+
+
+def feature_dim():
+    return 13 + (OM[0] * OM[0] * OM[2] if OM else 0)
 
 
 def make_env(B):
     env = BatchedCrowdSim(B)
-    env.configure(default_config(human_num=N))               # circle crossing, robot invisible
+    # circle crossing (square crossing, BASELINE config 4's rule, for crowds the circle cannot place), robot invisible
+    env.configure(default_config(human_num=N, train_val_sim='circle_crossing' if N <= 5 else 'square_crossing'))
     env.robot_safety_space = 0.15                            # train.py:121-127
     return env
 
@@ -42,7 +53,7 @@ def per_step(env, mem, k):
     env.enable_autoreset(env.train_val_sim)
     env.set_robot_policy('orca')
     env.reset_seeds(rule=env.train_val_sim, use_queue=True)
-    rec = TrajectoryRecorder(env, mem, GAMMA, True)
+    rec = TrajectoryRecorder(env, mem, GAMMA, True, om=OM)
     side = torch.cuda.Stream(device=env.device); main = torch.cuda.current_stream(env.device)
     it = 0
     while True:
@@ -59,7 +70,8 @@ def per_step(env, mem, k):
 
 
 def device(env, mem, k, steps_per_launch):
-    BatchedExplorer(env, 'orca', memory=mem, gamma=GAMMA).run_k_episodes(k, 'train', update_memory=True,
+    target = types.SimpleNamespace(with_om=True, om=OM) if OM else None        # OM-SARL's transform (explorer.py:102)
+    BatchedExplorer(env, 'orca', memory=mem, gamma=GAMMA, target_policy=target).run_k_episodes(k, 'train', update_memory=True,
                                                                          imitation_learning=True,
                                                                          steps_per_launch=steps_per_launch)
 
@@ -93,7 +105,13 @@ def main():
     ap.add_argument('--k', type=int, default=3000)
     ap.add_argument('--reps', type=int, default=2)
     ap.add_argument('--steps-per-launch', type=int, default=8)
+    ap.add_argument('--N', type=int, default=5)
+    ap.add_argument('--om', nargs=3, default=None, metavar=('CELL_NUM', 'CELL_SIZE', 'CHANNELS'))
     args = ap.parse_args()
+    global N, OM
+    N = args.N
+    OM = (int(args.om[0]), float(args.om[1]), int(args.om[2])) if args.om else None
+    workload = {} if (N, OM) == (5, None) else {'N': N, 'om': OM}   # (train.py's workload prints as it always did)
     assert torch.cuda.is_available(), 'needs a GPU'
     q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
     print(json.dumps({'device': torch.cuda.get_device_name(0), 'nvidia_smi_name_power_limit': q.stdout.strip().splitlines()[:1]}))
@@ -101,22 +119,22 @@ def main():
         paths = {'per_step': lambda env, mem, k: per_step(env, mem, k),
                  'device': lambda env, mem, k: device(env, mem, k, args.steps_per_launch)}
         for name, fn in paths.items():                      # warm-up: every kernel and allocation of the path
-            fn(make_env(B), DeviceReplayMemory(CAPACITY, N, 'cuda'), min(args.k, 2 * B))
+            fn(make_env(B), DeviceReplayMemory(CAPACITY, N, 'cuda', feature_dim()), min(args.k, 2 * B))
         mems = {}
         for rep in range(args.reps):
             for name, fn in paths.items():
-                env, mem = make_env(B), DeviceReplayMemory(CAPACITY, N, 'cuda')
+                env, mem = make_env(B), DeviceReplayMemory(CAPACITY, N, 'cuda', feature_dim())
                 t = timed(lambda: fn(env, mem, args.k))
                 mems[name] = mem
                 pairs = pairs_stored(env)
-                print(json.dumps({'B': B, 'path': name, 'rep': rep, 'k': args.k, 'pairs': pairs, 'ring_size': len(mem),
-                                  'wall_s': round(t, 4), 'episodes_per_s': round(args.k / t, 1),
-                                  'pairs_per_s': round(pairs / t, 1)}))
+                print(json.dumps(dict(workload, **{'B': B, 'path': name, 'rep': rep, 'k': args.k, 'pairs': pairs,
+                                                   'ring_size': len(mem), 'wall_s': round(t, 4),
+                                                   'episodes_per_s': round(args.k / t, 1), 'pairs_per_s': round(pairs / t, 1)})))
         # the timed rings wrap (k episodes store more pairs than the capacity), and which pairs a full ring keeps depends
         # on the order, which differs between the paths (refills on a side stream): compare untimed runs of the same
         # workload into rings that hold every pair
         big = args.k * (max_episode_steps(25, 0.25) + 1)
-        a, b = DeviceReplayMemory(big, N, 'cuda'), DeviceReplayMemory(big, N, 'cuda')
+        a, b = DeviceReplayMemory(big, N, 'cuda', feature_dim()), DeviceReplayMemory(big, N, 'cuda', feature_dim())
         per_step(make_env(B), a, args.k)
         device(make_env(B), b, args.k, args.steps_per_launch)
         same = len(a) == len(b) and np.array_equal(pair_multiset(a), pair_multiset(b))
