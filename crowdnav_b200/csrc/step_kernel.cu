@@ -463,6 +463,21 @@ extern "C" int crowdsim_abi_version(void) { return CROWDSIM_ABI_VERSION; }
 
 extern "C" unsigned long long crowdsim_launch_count(void) { return cs::g_launches; }
 
+#ifdef CS_PHASE_PROBE
+// Probe builds only (step_multi.cuh): copies crowdsim_step_n's phase totals, [human warps, robot warps][CS_PHASES cycles,
+// block steps], to out (2 * (CS_PHASES + 1) values) after the device has finished, then zeroes them if reset != 0.
+extern "C" int crowdsim_phase_probe(unsigned long long *out, int reset)
+{
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess && out) e = cudaMemcpyFromSymbol(out, cs::g_phase, sizeof(cs::g_phase));
+    if (e == cudaSuccess && reset) {
+        static const unsigned long long zero[2][CS_PHASES + 1] = {};
+        e = cudaMemcpyToSymbol(cs::g_phase, zero, sizeof(zero));
+    }
+    return (int)e;
+}
+#endif
+
 extern "C" int crowdsim_device_check(int *sm_count, int *cc_major, int *cc_minor)
 {
     int dev = 0; cudaDeviceProp p;

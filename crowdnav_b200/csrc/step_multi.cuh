@@ -27,9 +27,12 @@
 //      and publishes its lp2 result; the solves that need linearProgram3 go to a block queue of T / (N - 1) items (one
 //      item layout, sized for N lines), one pass. The pass writes each result over its owner's lp2 result, so that after
 //      it the humans read their robot's velocity without a barrier.
-//   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; a barrier.
-//   4. the robot folds the clearances, runs the env tail and publishes "install a scene" and "active"; a barrier; humans
-//      take over the flags and install their part of a new scene.
+//   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; meanwhile the robot
+//      publishes the rest of what the env's ending depends on (timeout, goal reached, its slot's state, read after its
+//      solve, and whether it is parked); a barrier.
+//   4. every human decides the ending from its env's clearances and those flags by the robot's rules and installs its part
+//      of a new scene at once; the robot folds the clearances and runs the env tail. No barrier: both go on to the next
+//      step's publish and meet at its loop-top barrier.
 // Measured and not kept (DESIGN §10): the robot computing the N clearances itself from the humans' float64 view, which
 // saves the barrier of step 3 but puts N float64 segment tests in a row on the robot warp.
 // The robot's per-env record (RobotRec: global time, episode accumulators, last step's outputs, flags) stays in shared
@@ -41,10 +44,29 @@
 namespace cs {
 
 // Resident warps per SM the multi-step kernel is compiled for: blocks per SM = CS_MULTI_WARPS / (N + 1). N = 5: 5 blocks of
-// 6 warps (64 registers; CUDA 12.9 spills 78 B, 34.6 KB of shared memory per block); 3 blocks (18 warps) measured 16 %
+// 6 warps (64 registers; CUDA 12.9 spills 86 B, 34.6 KB of shared memory per block); 3 blocks (18 warps) measured 16 %
 // slower with 16 batches in flight (DESIGN §3.6, §10). A -D knob for A/B builds.
 #ifndef CS_MULTI_WARPS
 #define CS_MULTI_WARPS 30
+#endif
+
+// Phase probe (-DCS_PHASE_PROBE, scripts/phase_probe.py): lane 0 of every warp sums the clock64() cycles of each phase of
+// a block step and adds them, with the number of steps its block ran, to g_phase[robot warp?][phase] when the launch ends
+// (read through crowdsim_phase_probe). Phases: 0 publish and loop-top barrier, 1 line build and solve, 2 queue barrier,
+// 3 lp3 pass, 4 clearance, 5 barrier after the clearances, 6 tail (robot) or install (humans), 7 flag barrier. Without the
+// define the hooks are empty and the kernel's SASS is what it is without them.
+#define CS_PHASES 8
+#ifdef CS_PHASE_PROBE
+static __device__ unsigned long long g_phase[2][CS_PHASES + 1];
+#define CS_PROBE_INIT unsigned ph_acc[CS_PHASES] = {}; long long ph_t = clock64();
+#define CS_PROBE(i) do { const long long t_ = clock64(); ph_acc[i] += (unsigned)(t_ - ph_t); ph_t = t_; } while (0)
+#define CS_PROBE_FLUSH(robot, steps) do { if ((threadIdx.x & 31) == 0) {                                                    \
+        for (int i_ = 0; i_ < CS_PHASES; ++i_) atomicAdd(&g_phase[(robot) ? 1 : 0][i_], (unsigned long long)ph_acc[i_]);    \
+        atomicAdd(&g_phase[(robot) ? 1 : 0][CS_PHASES], (unsigned long long)(steps)); } } while (0)
+#else
+#define CS_PROBE_INIT
+#define CS_PROBE(i) do { } while (0)
+#define CS_PROBE_FLUSH(robot, steps) do { } while (0)
 #endif
 
 // One solve of the multi-step kernel: agent a of the env whose float32 views start at slot ebase (robot: a = N). M lines
@@ -153,7 +175,8 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     constexpr int E = 32, L = N + 1, T = 32 * L;
     constexpr int MH = VIS ? N : N - 1;                     // lines of a human solve
     constexpr int SUB = N - 1;                              // lanes per queued lp3 item (sub-problems i = 1 .. N-1)
-    constexpr int QC = T / SUB;                             // lp3 items queued per step = one pass (N = 5: 48 of 192 solves)
+    constexpr int IPW = 32 / SUB;                           // lp3 items per warp: an item never straddles two warps
+    constexpr int QC = IPW * L;                             // lp3 items queued per step = one pass (N = 5: 48 of 192 solves)
     constexpr int QF = 4 * N + 4;                           // floats per queued lp3 item: lines, count, fail, radius, owner
     constexpr int PV = (4 * SUB > 10) ? 4 * SUB : 10;
     __shared__ float s_q[QF][QC];
@@ -172,8 +195,9 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     __shared__ double s_rad[T];                              // every agent's radius
     __shared__ float2 s_nv[T];                               // every agent's velocity of the step: lp2 result, then lp3's
     __shared__ RobotRec s_rr[E];
-    __shared__ uint8_t s_flag[E];                            // robot -> humans: bit 0 active, bit 1 install the next scene
+    __shared__ uint8_t s_pre[E];                             // robot -> humans: what the env's ending depends on besides the clearances (PRE_*)
     __shared__ int s_qcount;
+    constexpr unsigned PRE_TIMEOUT = 1, PRE_GOAL = 2, PRE_READY = 4, PRE_WANT = 8;   // timeout, goal reached, slot READY, parked
     float4 *const s_view = reinterpret_cast<float4 *>(&s_pv[0][0]);
     float *const s_radh = s_pv[4], *const s_radr = s_pv[5];
 
@@ -212,6 +236,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     bool dirty_kin = false, dirty_scene = false;
     bool release = false;                                    // robot: hand the slot back once the humans have read it
     const double dt = k.time_step;
+    CS_PROBE_INIT
 
     #pragma unroll 1
     for (int s = 0; ; ++s) {
@@ -231,8 +256,10 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     if (release) { st_release_u8(A.ar.n_state + e, CROWDSIM_SLOT_EMPTY); release = false; }
     if (!go) {
         if constexpr (REC) { if (is_robot && env_ok) for (int s2 = s; s2 < A.n_steps; ++s2) A.rec.code[(size_t)s2 * A.B + e] = CROWDSIM_REC_NONE; }
+        CS_PROBE_FLUSH(is_robot, s);
         break;
     }
+    CS_PROBE(0);
     if constexpr (REC) {
         if (!is_robot && live) {
             const int rt = 32 * N + le;
@@ -259,7 +286,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                      : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, s_pv[6], R, nl, fail, max_speed);
 
     // ---- linearProgram3 of the solves that need it: a block queue of QC items, one pass. The sub-problems of an item run
-    // on SUB threads in parallel (sequential shared-memory LP code of orca_device.cuh), the item's first thread finishes
+    // on SUB lanes of one warp in parallel (sequential shared-memory LP code of orca_device.cuh), the item's first lane finishes
     // with the outer scan (step_flat.cuh) and writes the result over its owner's lp2 result in s_nv, where the humans also
     // read their robot's. A solve that finds the queue full (more than QC in one block step: scenes where most agents
     // overlap) runs RVO2's sequential linearProgram3 alone (out of line, on lines in local memory; tests/native/lp_fuzz.cu
@@ -282,11 +309,27 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
         s_q[4 * N + 2][slot] = max_speed; s_q[4 * N + 3][slot] = __int_as_float(tid);
     }
     s_nv[tid] = make_float2(nv.x, nv.y);
+    // the state of the env's next-scene slot, for the ending of this step: read before the queue barrier, so that the L2
+    // round trip hides behind the lp3 pass and the clearances (issued before the solve it holds a register across it and
+    // spills more), and after this thread's release at the loop top, so that an env that ends again in this launch finds
+    // its slot EMPTY and parks. Reading it before the ending it decides is what the protocol allows anyway: a slot the
+    // generator publishes while the step runs is picked up by a later step; only this kernel moves a slot away from READY.
+    // The discount factor of this step's reward is loaded here too (ep_t changes only in the robot's tail), which takes an
+    // L2 round trip off the tail of every live step. (An acquire here, with n_case behind it, took the install's two round
+    // trips off the tail as well but measured slower at full chip: DESIGN §10.)
+    uint8_t sst = CROWDSIM_SLOT_EMPTY;
+    double disc = 0.0;
+    if (is_robot && env_ok) {
+        if (A.has_ar) sst = ld_relaxed_u8(A.ar.n_state + e);
+        if (A.has_ep && live) { const int t = rr.ep_t; disc = (t < A.ep.discount_len) ? A.ep.discount[t] : 0.0; }
+    }
+    CS_PROBE(1);
     const int cnt = __syncthreads_count(slot >= 0);
+    CS_PROBE(2);
     if (cnt > 0) {
         if (tid == 0) s_qcount = 0;                          // every slot of the step is taken; the next step's come after more barriers
-        const int item = tid / SUB, i = tid % SUB + 1;
-        const bool mine = (tid < QC * SUB) && item < cnt;
+        const int lane = tid & 31, item = (tid >> 5) * IPW + lane / SUB, i = lane % SUB + 1;
+        const bool mine = lane < IPW * SUB && item < cnt;
         if (mine) {
             const Lines Lq = { &s_q[0][item], QC };
             const int qn = __float_as_int(s_q[4 * N + 0][item]);
@@ -297,7 +340,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             }
             s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
         }
-        __syncthreads();
+        __syncwarp();                                        // an item's sub-problem results are read by its first lane, in the same warp
         if (mine && i == 1) {
             const Lines Lq = { &s_q[0][item], QC };
             const int qn = __float_as_int(s_q[4 * N + 0][item]), qf = __float_as_int(s_q[4 * N + 1][item]);
@@ -316,8 +359,12 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
         if (slot >= 0) { const float2 q = s_nv[tid]; nv = mk(q.x, q.y); }
     }
     pos = s_pos[tid]; vel = s_vel[tid];
+    CS_PROBE(3);
 
+    // s_cl lives in s_r2, whose next write is in the next step's lp3 pass, after its queue barrier: the humans and the robot
+    // read their env's clearances after the barrier below without another one
     double *const s_cl = reinterpret_cast<double *>(&s_r2[0][0]);     // [E * N]: the humans' clearances
+    bool timeout = false, reaching_goal = false;                       // robot lanes of live envs
     if (!is_robot) {
         if (live) {
             // swept-segment clearance against the robot's velocity of this step (crowd_sim.py:333-345)
@@ -333,10 +380,52 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
             dirty_kin = true;
         }
+    } else if (env_ok) {
+        // meanwhile the robot publishes everything else the env's ending depends on (PRE_*), so that after the barrier its
+        // humans decide the ending and start their install while the robot runs its tail
+        if (live) {
+            const double npx = pos.x + (double)nv.x * dt, npy = pos.y + (double)nv.y * dt;
+            const double2 goal = s_goal[tid];
+            reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
+            timeout = rr.gtime >= k.time_limit - 1;
+        }
+        s_pre[le] = (uint8_t)((timeout ? PRE_TIMEOUT : 0u) | (reaching_goal ? PRE_GOAL : 0u) |
+                              (sst == CROWDSIM_SLOT_READY ? PRE_READY : 0u) | (rr.want != 0 ? PRE_WANT : 0u));
     }
+    CS_PROBE(4);
     __syncthreads();
-    if (is_robot) {
-        int install = 0;
+    CS_PROBE(5);
+    // No block barrier follows until the next step's loop top, so the robot's tail overlaps its humans' install and their
+    // publish of the next step. What crosses between the roles is written before a barrier the reader passes after it:
+    //   * the robot's tail writes rr, and on an install its s_goal slot; its s_pos / s_vel / s_rad / view slots are written
+    //     at the next publish. The humans read those slots (clearance, REC's rec_row) after the next loop-top barrier.
+    //   * s_pre is read by the humans here and written by the robot after the next loop-top barrier.
+    //   * the humans' next publish writes their own slots, which the robot reads only after that barrier.
+    //   * the slot's release (loop top, after the barrier) still follows every human's reads of the slot data.
+    if (!is_robot) {
+        if (env_ok) {
+            // the robot's rules below, from the same values: collision is any clearance < 0 (the robot's fold breaks at
+            // the first one, which only decides dmin; a NaN clearance is no collision either way)
+            const unsigned pf = s_pre[le];
+            bool done = false;
+            if (live) {
+                bool collision = false;
+                #pragma unroll
+                for (int i = 0; i < N; ++i) collision |= s_cl[le * N + i] < 0;
+                done = (pf & PRE_TIMEOUT) || collision || (pf & PRE_GOAL);
+                if (done && A.has_ep && A.st.active && !A.has_ar) act_flag = 0;          // frozen
+            }
+            if (A.has_ar && ((live && done) || (!live && (pf & PRE_WANT)))) {
+                act_flag = (pf & PRE_READY) ? 1 : 0;                                      // install, or park
+                if (act_flag) {                              // agent.py:47-58 set(px, py, gx, gy, 0, 0, ..)
+                    (void)ld_acquire_u8(A.ar.n_state + e);
+                    pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); s_goal[tid] = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
+                    dirty_kin = true; dirty_scene = true;
+                }
+            }
+        }
+        CS_PROBE(6);
+    } else {
         if (env_ok) {
             bool done = false;
             if (live) {
@@ -350,12 +439,10 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 }
                 // ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72)
                 const double npx = pos.x + ax * dt, npy = pos.y + ay * dt;
-                const double2 goal = s_goal[tid];
-                const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
                 double reward; int info;
                 const double gtime = rr.gtime;
                 const int t_rec = rr.ep_t;                   // REC: the episode step the row was recorded at
-                if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
+                if (timeout) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
                 else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
                 else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
                 else if (dmin < k.discomfort_dist) { reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt; done = false; info = CROWDSIM_INFO_DANGER; }
@@ -368,7 +455,6 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 if (A.has_ep) {
                     const crowdsim_episodes &ep = A.ep;
                     int ep_t = rr.ep_t, ep_tc = rr.ep_tc; double ep_ret = rr.ep_ret, ep_mds = rr.ep_mds;
-                    const double disc = (ep_t < ep.discount_len) ? ep.discount[ep_t] : 0.0;
                     ep_ret = ep_ret + disc * reward; ep_t += 1;
                     if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; }
                     rr.ep_t = ep_t; rr.ep_tc = ep_tc; rr.ep_ret = ep_ret; rr.ep_mds = ep_mds;
@@ -394,42 +480,29 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             }
             if (A.has_ar) {
                 // consumer side of the auto-reset protocol (include/crowdsim_b200.h): an env that just finished, or is parked
-                // waiting, looks at its next-scene slot; a slot the generator publishes later is picked up by a later step
+                // waiting, looks at its next-scene slot (read at the top of the step)
                 const bool finished = live && done, parked = !live && rr.want != 0;
                 if (finished || parked) {
-                    const uint8_t sst = ld_relaxed_u8(A.ar.n_state + e);
-                    if (sst == CROWDSIM_SLOT_READY) install = 1;
-                    else {
+                    if (sst == CROWDSIM_SLOT_READY) {
+                        // acquire on the slot flag (every thread that reads slot data), then crowd_sim.py:262,274 + fresh
+                        // episode accumulators
+                        (void)ld_acquire_u8(A.ar.n_state + e);
+                        pos = make_double2(0.0, -A.ar.circle_radius); s_goal[tid] = make_double2(0.0, A.ar.circle_radius);
+                        vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
+                        rr.gtime = 0.0;
+                        if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
+                        if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
+                        act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
+                        dirty_kin = true; dirty_scene = true; release = true;
+                    } else {
                         act_flag = 0; A.st.active[e] = 0;                             // park: nothing to install (yet)
                         const uint8_t want = (sst == CROWDSIM_SLOT_EXHAUSTED) ? 0 : 1;
                         rr.want = want; A.ar.want[e] = want;
                     }
                 }
-                if (install) {
-                    // acquire on the slot flag (every thread that reads slot data), then crowd_sim.py:262,274 + fresh
-                    // episode accumulators
-                    (void)ld_acquire_u8(A.ar.n_state + e);
-                    pos = make_double2(0.0, -A.ar.circle_radius); s_goal[tid] = make_double2(0.0, A.ar.circle_radius);
-                    vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
-                    rr.gtime = 0.0;
-                    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
-                    if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
-                    act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
-                    dirty_kin = true; dirty_scene = true; release = true;
-                }
             }
         }
-        s_flag[le] = (uint8_t)((act_flag != 0) | (install << 1));
-    }
-    __syncthreads();
-    if (!is_robot) {                                         // humans follow their robot's flags
-        const unsigned f = s_flag[le];
-        act_flag = (uint8_t)(f & 1u);
-        if ((f & 2u) && env_ok) {                            // agent.py:47-58 set(px, py, gx, gy, 0, 0, ..)
-            (void)ld_acquire_u8(A.ar.n_state + e);
-            pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); s_goal[tid] = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
-            dirty_kin = true; dirty_scene = true;
-        }
+        CS_PROBE(6);
     }
     }   // step loop
 
