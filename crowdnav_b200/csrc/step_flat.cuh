@@ -351,6 +351,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             else { reward = 0; done = false; info = CROWDSIM_INFO_NOTHING; }
             if (ROT) {                                                                   // agent.py:133-135
                 double nth = fmod(theta + ay, 2 * CS_PI); if (nth < 0) nth += 2 * CS_PI;
+                else if (nth == 0) nth = 0.0;                                            // Python's % gives +0.0 for a zero remainder
                 theta = nth; nvx = ax * cos(nth); nvy = ax * sin(nth);
             }
             pos = make_double2(npx, npy); vel = make_double2(nvx, nvy);

@@ -131,6 +131,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
 
             if (k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT) {                        // agent.py:133-135
                 double nth = fmod(theta + ay, 2 * CS_PI); if (nth < 0) nth += 2 * CS_PI;
+                else if (nth == 0) nth = 0.0;                                           // Python's % gives +0.0 for a zero remainder
                 if (!A.lookahead) A.st.r_theta[e] = nth;
                 nvx = ax * cos(nth); nvy = ax * sin(nth);
             }

@@ -383,7 +383,8 @@ static void step_one(const crowdsim_params *p, int e, int N, crowdsim_state *st,
     /* crowd_sim.py:399-403 update (also on terminal steps); agent.py:122-135 */
     rp[0] = npx; rp[1] = npy;
     if (!rot) { rv[0] = nvx; rv[1] = nvy; }
-    else { ntheta = fmod(st->r_theta[e] + ay, 2 * PI_D); if (ntheta < 0) ntheta += 2 * PI_D;  /* Python float % */
+    else { ntheta = fmod(st->r_theta[e] + ay, 2 * PI_D); if (ntheta < 0) ntheta += 2 * PI_D;  /* Python float % ... */
+           else if (ntheta == 0) ntheta = 0.0;                                                  /* ... gives +0.0 for a zero remainder */
            st->r_theta[e] = ntheta; rv[0] = ax * cos(ntheta); rv[1] = ax * sin(ntheta); }
     for (int i = 0; i < N; ++i) { hp[2 * i] = hp[2 * i] + hax[i] * dt; hp[2 * i + 1] = hp[2 * i + 1] + hay[i] * dt; hv[2 * i] = hax[i]; hv[2 * i + 1] = hay[i]; }
     st->g_time[e] += dt;

@@ -275,6 +275,79 @@ def run_rotate(out_name='rotate_lookahead', profile=None, cases=(0, 3, 7), steps
     print('rotate/lookahead rows', len(rows))
 
 
+def R32(x):
+    """A float32 value as its shortest decimal string (np.float32(s) reads it back exactly)."""
+    return str(np.float32(x))
+
+
+def run_rotate_unicycle():
+    """run_rotate for a unicycle robot: policy.config with [action_space] kinematics = unicycle, i.e. CADRL.build_action_space's
+    81 ActionRot actions (5 speeds x 16 rotations in [-pi/4, pi/4], plus (0, 0)), reference code only. The robot drives
+    with the reference's own greedy ActionRot decision. Before every recorded step its heading is set from a seeded RNG:
+    uniform in [0, 2 pi), within 0.3 of 0 or within 0.3 of 2 pi, so that the heading update's % wraps in both directions.
+    Recorded at every `every`-th step: the scene with theta and global_time, rotate(current) (pack_joint), per action the
+    onestep_lookahead reward, the rotate rows of propagate + lookahead and the value, and env.step of the driving action
+    (reward, info, the robot's post-step px, py, vx, vy, theta). Rows as float32 shortest strings."""
+    rng = np.random.RandomState(11)
+    blocks = []
+    for tag, name, N, vis, cases, steps, every in (('sarl5_invisible', 'sarl', 5, False, (0, 3, 7), 12, 4),
+                                                  ('sarl10_visible', 'sarl', 10, True, (1, 4), 8, 4),
+                                                  ('cadrl1_invisible', 'cadrl', 1, False, (0, 2), 12, 2)):
+        pcfg = configparser.RawConfigParser()
+        pcfg.read(os.path.join(REF, 'crowd_nav', 'configs', 'policy.config'))
+        pcfg.set('action_space', 'kinematics', 'unicycle')
+        torch.manual_seed(0)
+        env, robot, _ = make_env(human_num=N, test_sim='circle_crossing', robot_visible=vis, policy_name=name, policy_config=pcfg)
+        policy = robot.policy
+        assert robot.kinematics == 'unicycle'
+        rows = []
+        for case in cases:
+            ob = env.reset('test', case)
+            for step in range(steps):
+                record = step % every == 0
+                if record:
+                    kind = len(rows) % 3
+                    robot.theta = float([rng.uniform(0, 2 * np.pi), rng.uniform(0, 0.3), 2 * np.pi - rng.uniform(0, 0.3)][kind])
+                state = JointState(robot.get_full_state(), ob)
+                if policy.action_space is None:
+                    policy.build_action_space(state.self_state.v_pref)
+                if record:
+                    per_action = []
+                    for action in policy.action_space:
+                        next_self_state = policy.propagate(state.self_state, action)
+                        next_human_states, reward, done, info = env.onestep_lookahead(action)
+                        batch = torch.cat([torch.Tensor([next_self_state + nhs]) for nhs in next_human_states], dim=0)
+                        rot = policy.rotate(batch)
+                        with torch.no_grad():
+                            value = (policy.model(rot.unsqueeze(0)).data.item() if name == 'sarl'
+                                     else torch.min(policy.model(rot), 0)[0].data.item())
+                        per_action.append({'reward': R(reward), 'value': R(value),
+                                           'rotated': [[R32(v) for v in row] for row in rot.tolist()]})
+                    cur = torch.cat([torch.Tensor([state.self_state + hs]) for hs in state.human_states], dim=0)
+                    row = {'case': case, 'step': step, 'scene': scene(env), 'global_time': R(env.global_time),
+                           'rotated_current': [[R32(v) for v in r] for r in policy.rotate(cur).tolist()],
+                           'lookahead': per_action}
+                np_state = np.random.get_state()
+                action = policy.predict(state)                  # the reference's own greedy ActionRot decision
+                np.random.set_state(np_state)
+                ob, reward, done, info = env.step(action)
+                if record:
+                    row['step_action'] = [R(action.v), R(action.r)]
+                    row['step_result'] = {'reward': R(reward), 'done': bool(done), 'info': INFO_CODE[type(info)],
+                                          'dmin': R(info.min_dist) if isinstance(info, Danger) else None,
+                                          'robot': [R(robot.px), R(robot.py), R(robot.vx), R(robot.vy), R(robot.theta)],
+                                          'global_time': R(env.global_time)}
+                    rows.append(row)
+                if done:
+                    break
+        space = [[R(a.v), R(a.r)] for a in policy.action_space]
+        blocks.append({'tag': tag, 'policy': name, 'N': N, 'robot_visible': int(vis), 'action_space': space, 'rows': rows})
+        wraps = sum(1 for r in rows if abs(float(r['step_result']['robot'][4]) - float(r['scene']['robot'][8])) > np.pi)
+        print(tag, 'rows', len(rows), 'heading wraps', wraps)
+    with gzip.open(os.path.join(OUT, 'rotate_lookahead_unicycle.json.gz'), 'wt') as f:
+        json.dump({'seed': 0, 'blocks': blocks}, f, separators=(',', ':'))
+
+
 def run_om():
     """MultiHumanRL.build_occupancy_maps (multi_human_rl.py:109-163), reference code only: (a) on the humans of real
     scenes a few steps into test episodes and on the next human states env.onestep_lookahead returns, (b) on random
@@ -593,6 +666,7 @@ ONLY = {
     'resets_envcfg': run_resets_envcfg,
     'human_times_envcfg': lambda: run_human_times('human_times_envcfg', HUMAN_TIMES_ENVCFG),
     'rotate_envcfg': lambda: run_rotate('rotate_lookahead_envcfg', 'env_config', cases=(0, 3, 11), steps=16, every=4),
+    'rotate_unicycle': run_rotate_unicycle,
 }
 
 

@@ -274,8 +274,21 @@ def family_e5(N, frame=HOLONOMIC):
 
 def ladder_scenes(N, unicycle=False):
     frame = UNICYCLE if unicycle else HOLONOMIC
-    return (family_e1(frame) + family_e2(frame=frame) + family_e3(unicycle) + family_e4(frame=frame)
-            + family_e5(N, frame))
+    out = (family_e1(frame) + family_e2(frame=frame) + family_e3(unicycle) + family_e4(frame=frame)
+           + family_e5(N, frame))
+    return out + negative_zero_twins(out) if unicycle else out
+
+
+def negative_zero_twins(scenes):
+    """Unicycle scenes again at theta = -0.0 with the action (v, -0.0). The heading update (theta + r) % 2 pi
+    (agent.py:133) then has a zero remainder, which Python's % returns as +0.0 where C's fmod keeps -0.0, and the new
+    velocity's y = v sin(theta) carries that sign. Everything else equals the theta = +0.0 scene's."""
+    out = []
+    for s in scenes:
+        robot = list(s.robot)
+        robot[8] = -0.0
+        out.append(Scene(s.label + ', theta -0.0', robot, s.humans, s.g_time, (s.action[0], -0.0), s.expect))
+    return out
 
 
 # ---- O: the ORCA neighbour scan and line construction (float32) --------------------------------------------------------
@@ -392,7 +405,8 @@ def batches(N, policy='orca', vis=0):
     """Every boundary batch a route with N humans runs. ORCA robot: the ladder scenes at max_neighbors = 0 (action = pref
     exactly); the ORCA families at the default constants (10 m, 10 neighbours), orca_tight (3 m, 2 neighbours) and
     orca_tight_mn1. External holonomic robot (action = the scene's action): everything at the default constants. External
-    unicycle robot: the ladder scenes at theta = 0 and r = 0 (its rotation leaves the ORCA families unchanged)."""
+    unicycle robot: the ladder scenes at theta = 0 and r = 0, and their twins at theta = -0.0 and r = -0.0 (its rotation
+    leaves the ORCA families unchanged)."""
     out = []
     if policy == 'orca':
         out.append(Batch('ladder_mn0', N, policy, vis, ladder_scenes(N), over=dict(max_neighbors=0)))

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from util import (SUITES, NON_DEFAULT, ORCA_TIGHT, PROFILE_SUITES, load_golden, scene_arrays, fill_host_state, pre_step_times,
-                  profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits)
+                  profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits, assert_unicycle_step_within_bounds)
 
 pytestmark = pytest.mark.gpu
 
@@ -25,6 +25,17 @@ def _assert_state_equal(env, host, fields=STATE_FIELDS, what=''):
 def _assert_io_equal(env, io, what=''):
     for f in ('done', 'info', 'reward', 'dmin', 'action_out'):
         assert_same_bits(getattr(env, f).cpu().numpy(), getattr(io, f), '%s %s' % (what, f))
+
+
+def _assert_unicycle_step(env, dev, pre, io, host, prm, what):
+    """External_rot step against the oracle's: heading, done and info exact, reward class exact, pose, r_vel,
+    action_out, reward and dmin within tests/util.py:assert_unicycle_step_within_bounds."""
+    got = dict(r_pos=dev['r_pos'], r_vel=dev['r_vel'], r_theta=dev['r_theta'], action_out=env.action_out.cpu().numpy(),
+               reward=env.reward.cpu().numpy(), dmin=env.dmin.cpu().numpy(), done=env.done.cpu().numpy(),
+               info=env.info.cpu().numpy())
+    want = dict(r_pos=host.r_pos, r_vel=host.r_vel, r_theta=host.r_theta, action_out=io.action_out, reward=io.reward,
+                dmin=io.dmin, done=io.done, info=io.info)
+    assert_unicycle_step_within_bounds(pre, io.action, prm, got, want, what)
 
 
 def _random_host_state(oracle, B, N, seed, spread=4.5):
@@ -100,16 +111,17 @@ def test_step_random_scenes_bit_exact(cuda_env, oracle, N, vis, policy, generic)
         else:
             io.action[...] = rng.uniform(-1, 1, (B, 2))
         act = torch.from_numpy(io.action).to(env.device)
+        pre = host.copy()
         env.step(None if policy == 'orca' else act)
         oracle.step(prm, host, io)
         torch.cuda.synchronize()
         if policy == 'external_rot':
-            # CUDA's double cos/sin are not glibc's: compare with a tolerance, then resynchronise the states
+            # CUDA's double cos/sin are not glibc's: pose, velocity, reward and dmin within their derived bounds, then
+            # resynchronise the states
             dev = env.state.to_host()
-            for f in ('h_pos', 'h_vel'):
+            for f in ('h_pos', 'h_vel', 'g_time'):
                 assert same_bits(dev[f], getattr(host, f))
-            assert np.allclose(dev['r_pos'], host.r_pos, rtol=0, atol=1e-12) and np.allclose(dev['r_theta'], host.r_theta, rtol=0, atol=1e-12)
-            assert same_bits(env.info.cpu().numpy(), io.info)
+            _assert_unicycle_step(env, dev, pre, io, host, prm, 'N=%d step %d' % (N, t))
             env.state.load_host(host)
         else:
             _assert_state_equal(env, host, what='N=%d step %d' % (N, t))
@@ -690,15 +702,15 @@ def _run_steps(cuda_env, oracle, prof, B, N, vis, policy, generic, steps, seed):
             io.action[:, 0] = rng.uniform(0, 1, B); io.action[:, 1] = rng.uniform(-0.8, 0.8, B)
         else:
             io.action[...] = rng.uniform(-1, 1, (B, 2))
+        pre = host.copy()
         env.step(None if policy == 'orca' else torch.from_numpy(io.action).to(env.device))
         oracle.step(prm, host, io)
         torch.cuda.synchronize()
-        if policy == 'external_rot':             # CUDA's double cos/sin: tolerance on the robot pose, then resynchronise
+        if policy == 'external_rot':             # CUDA's double cos/sin: derived bounds on the robot pose, then resynchronise
             dev = env.state.to_host()
             for f in ('h_pos', 'h_vel', 'g_time'):
                 assert same_bits(dev[f], getattr(host, f)), (what, t, f)
-            assert np.allclose(dev['r_pos'], host.r_pos, rtol=0, atol=1e-12) and np.allclose(dev['r_theta'], host.r_theta, rtol=0, atol=1e-12)
-            assert same_bits(env.info.cpu().numpy(), io.info), (what, t)
+            _assert_unicycle_step(env, dev, pre, io, host, prm, '%s step %d' % (what, t))
             env.state.load_host(host)
         else:
             _assert_state_equal(env, host, what='%s step %d' % (what, t))

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from util import (SUITES, PROFILE_SUITES, ORCA_TIGHT, load_golden, scene_arrays, fill_host_state, pre_step_times, profile,
-                  profile_params, reset_kw)
+                  profile_params, reset_kw, assert_same_bits, assert_rotate_within_model, pack_inputs, lookahead_inputs)
 
 # SURVEY.md Appendix B (independent throw-away restatement by the surveyor) -- the only external pin there is.
 APPENDIX_B = {
@@ -332,6 +332,53 @@ def test_occupancy_maps_match_reference(oracle):
         assert np.array_equal(got != 0, ref != 0), r['tag']
         assert np.abs(got - ref).max() <= 1e-6, r['tag']
     assert any(np.array(r['maps'], dtype=np.float64).any() for r in rows)
+
+
+def test_unicycle_pack_lookahead_and_step_match_reference(oracle):
+    """tests/golden/rotate_lookahead_unicycle (oracle/gen_golden.py --only rotate_unicycle): the reference's own unicycle
+    robot (81 ActionRot actions, headings set near 0, near 2 pi and anywhere) with SARL at N = 5 and 10 and CADRL at N = 1.
+    oracle.pack_joint(unicycle=True) and oracle.lookahead_pack(unicycle=True) against rotate(current) and the per-action
+    onestep_lookahead rewards and rotate rows: rewards bit for bit; rows within the float64-model bound of
+    tests/util.py:rotate_model, on the reference's rows (torch CPU) as on the oracle's (libm). Measured on this fixture:
+    the oracle's rows differ from the reference's by at most 9.5e-7 (|row| up to 8.3); the largest error / bound ratio is
+    0.86 for the oracle's rows and 0.74 for the reference's. The oracle's external_rot step of the recorded
+    driving action gives the reference's reward, done, info, dmin and post-step px, py, vx, vy, theta bit for bit."""
+    d = load_golden('rotate_lookahead_unicycle')
+    assert [b['N'] for b in d['blocks']] == [5, 10, 1]
+    wraps = 0
+    for b in d['blocks']:
+        N, rows = b['N'], b['rows']
+        actions = np.array([[float(x) for x in a] for a in b['action_space']])
+        assert actions.shape == (81, 2)
+        host = fill_host_state(oracle, [r['scene'] for r in rows], N)
+        host.g_time[:] = [float(r['global_time']) for r in rows]
+        prm = oracle.default_params(robot_visible=b['robot_visible'], robot_policy=2)
+        packed = oracle.pack_joint(host, unicycle=True)
+        states, reward = oracle.lookahead_pack(prm, host, actions, unicycle=True)
+        npos, nvel = oracle.lookahead_humans(prm, host)
+        s_cur, s_next = pack_inputs(host), lookahead_inputs(host, actions, npos, nvel, 0.25, True)
+        assert_rotate_within_model(packed, s_cur, True, what=b['tag'] + ' oracle pack_joint')
+        assert_rotate_within_model(states, s_next, True, what=b['tag'] + ' oracle lookahead_pack')
+        ref_cur = np.array([r['rotated_current'] for r in rows], dtype=np.float32)
+        ref_next = np.array([[la['rotated'] for la in r['lookahead']] for r in rows], dtype=np.float32)
+        assert_rotate_within_model(ref_cur, s_cur, True, what=b['tag'] + ' reference rotate(current)')
+        assert_rotate_within_model(ref_next, s_next, True, what=b['tag'] + ' reference rotate(lookahead)')
+        ref_reward = np.array([[float(la['reward']) for la in r['lookahead']] for r in rows])
+        assert_same_bits(reward, ref_reward, b['tag'] + ' lookahead rewards')
+        io = oracle.HostStepIO(len(rows))
+        io.action[...] = [[float(x) for x in r['step_action']] for r in rows]
+        oracle.step(prm, host, io)
+        for e, r in enumerate(rows):
+            res, what = r['step_result'], (b['tag'], r['case'], r['step'])
+            assert (int(io.done[e]), int(io.info[e])) == (int(res['done']), res['info']), what
+            assert_same_bits(np.float64(io.reward[e]), np.float64(float(res['reward'])), '%s reward' % (what,))
+            if res['dmin'] is not None:
+                assert_same_bits(np.float64(io.dmin[e]), np.float64(float(res['dmin'])), '%s dmin' % (what,))
+            pose = np.array([host.r_pos[e, 0], host.r_pos[e, 1], host.r_vel[e, 0], host.r_vel[e, 1], host.r_theta[e]])
+            assert_same_bits(pose, np.array([float(x) for x in res['robot']]), '%s pose' % (what,))
+            assert host.g_time[e] == float(res['global_time']), what
+            wraps += abs(host.r_theta[e] - float(r['scene']['robot'][8])) > math.pi
+    assert wraps >= 4                  # the heading update's % wrapped, past 2 pi and below 0
 
 
 def test_run_passes_equals_step_plus_reset(oracle):

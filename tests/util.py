@@ -168,6 +168,167 @@ def assert_same_bits(a, b, what=''):
             what, int(bad.sum()), tuple(int(x) for x in i), a[tuple(i)], b[tuple(i)]))
 
 
+U32, U64 = 2.0 ** -24, 2.0 ** -53       # unit roundoff of float32 / float64 (round to nearest)
+# Maximum errors in float32 ulps of the result: CUDA C Programming Guide, single-precision mathematical functions (atan2f 3,
+# cosf 2, sinf 2). glibc's libm and torch CPU's vectorised functions are within 1 ulp, so these bound every side.
+ULP_ATAN2F, ULP_COSF, ULP_SINF = 3, 2, 2
+# CUDA's double cos / sin are within 2 ulps (same guide), glibc's within 1: two sides differ by at most 3 ulps.
+ULP_COS_SIN_SIDES = 3
+
+
+def ulp32(x):
+    """Spacing of float32 values at |x| (normal range; subnormal spacing below)."""
+    e = np.floor(np.log2(np.maximum(np.abs(np.asarray(x, dtype=np.float64)), 2.0 ** -126)))
+    return 2.0 ** (e - 23)
+
+
+def ulp64(x):
+    return np.spacing(np.abs(np.asarray(x, dtype=np.float64)))
+
+
+def rotate_model(s, unicycle, robot_ulps=0):
+    """CADRL.rotate (cadrl.py:187-222) evaluated in float64 on float32 14-tuples s [..., 14], and a bound on how far any
+    float32 implementation of it can be from that value: (model [..., 13], bound [..., 13]).
+
+    Derivation, u = 2^-24: dx = gx - px is rounded once (|err| <= u |dx|). atan2 moves by at most (|dx| e_y + |dy| e_x) / r^2
+    for input errors e_x, e_y, and atan2f adds ULP_ATAN2F ulps of its result: drot. cos(rot + drot) is within |sin| drot
+    of cos(rot), and cosf adds ULP_COSF ulps: dc (ds likewise). A product a * c rounds once, a sum of two products once more,
+    a coordinate difference once more (px1: 3 roundings of |dx c| + |dy s|). A norm sqrtf(x*x + y*y) carries 3u
+    relative (2u from the squares' and the sum's rounding, halved by the square root, plus sqrtf's own rounding).
+    robot_ulps: the robot's px, py, vx, vy (and theta) may differ by that many float32 ulps between two implementations
+    (they come from double cos / sin, rounded to float32 once: 1 when one rounding may go either way); their effect is
+    propagated through the same terms. The bound is widened by 1 % for the second-order terms (products of two errors,
+    relatively O(u))."""
+    s = np.asarray(s, dtype=np.float32).astype(np.float64)
+    px, py, vx, vy, rad, gx, gy, vpref, th, hx, hy, hvx, hvy, hr = (s[..., i] for i in range(14))
+    dx, dy, ax, ay = gx - px, gy - py, hx - px, hy - py          # exact in float64
+    rot = np.arctan2(dy, dx)
+    c, sn = np.cos(rot), np.sin(rot)
+    r2 = dx * dx + dy * dy
+    dg, da = np.sqrt(r2), np.sqrt(ax * ax + ay * ay)
+    zero = np.zeros_like(dg)
+    model = np.stack([dg, vpref, (th - rot) if unicycle else zero, rad, vx * c + vy * sn, vy * c - vx * sn,
+                      ax * c + ay * sn, ay * c - ax * sn, hvx * c + hvy * sn, hvy * c - hvx * sn, hr, da, rad + hr], -1)
+    dp = robot_ulps * np.maximum(ulp32(px), ulp32(py))
+    dv = robot_ulps * np.maximum(ulp32(vx), ulp32(vy))
+    dth = robot_ulps * ulp32(th)
+    ex, ey = U32 * np.abs(dx) + dp, U32 * np.abs(dy) + dp
+    with np.errstate(divide='ignore', invalid='ignore'):
+        drot_in = np.where(r2 > 0, (np.abs(dx) * ey + np.abs(dy) * ex) / r2, np.pi)
+    drot = drot_in + ULP_ATAN2F * ulp32(rot)
+    dc = np.abs(sn) * drot + ULP_COSF * ulp32(c)
+    ds = np.abs(c) * drot + ULP_SINF * ulp32(sn)
+    acs = np.abs(c) + np.abs(sn)
+
+    def turn(a, b, k, d_in):
+        """a c + b s (and b c - a s): k roundings of the products' magnitudes, cos / sin errors, input errors."""
+        return np.abs(a) * dc + np.abs(b) * ds + k * U32 * (np.abs(a * c) + np.abs(b * sn)) + d_in * acs
+
+    bound = np.stack([3 * U32 * dg + 1.5 * dp, zero, (drot + dth + U32 * np.abs(th - rot)) if unicycle else zero, zero,
+                      turn(vx, vy, 2, dv), turn(vy, vx, 2, dv), turn(ax, ay, 3, dp), turn(ay, ax, 3, dp),
+                      turn(hvx, hvy, 2, 0), turn(hvy, hvx, 2, 0), zero, 3 * U32 * da + 1.5 * dp, U32 * np.abs(rad + hr)], -1)
+    return model, 1.01 * bound
+
+
+def assert_rotate_within_model(rows, s, unicycle, robot_ulps=0, what=''):
+    """Every float32 row element within rotate_model's bound of the float64 value; returns the largest |error| / bound."""
+    model, bound = rotate_model(s, unicycle, robot_ulps)
+    err = np.abs(np.asarray(rows, dtype=np.float64) - model)
+    bad = err > bound
+    if bad.any():
+        i = tuple(int(x) for x in np.argwhere(bad)[0])
+        raise AssertionError('%s: %d row elements outside the float64-model bound, first at %s: %r vs model %r (bound %r)' % (
+            what, int(bad.sum()), i, float(np.asarray(rows)[i]), float(model[i]), float(bound[i])))
+    with np.errstate(divide='ignore', invalid='ignore'):
+        return float(np.nanmax(np.where(bound > 0, err / bound, 0.0)))
+
+
+def _tuples(rp, rv, ra, rg, th, hp, hv, hr):
+    """state.py:17-18,36-37 14-tuples, cast to float32 (multi_human_rl.py transform); robot arrays broadcast over humans."""
+    cols = [rp[..., 0], rp[..., 1], rv[..., 0], rv[..., 1], ra[..., 0], rg[..., 0], rg[..., 1], ra[..., 1], th,
+            hp[..., 0], hp[..., 1], hv[..., 0], hv[..., 1], hr]
+    return np.stack(np.broadcast_arrays(*cols), -1).astype(np.float32)
+
+
+def pack_inputs(st):
+    """The [B][N][14] float32 tuples crowdsim_pack_joint rotates (the current state of a HostState-like object)."""
+    e = lambda a: np.asarray(a)[:, None]          # noqa: E731  robot [B] -> [B][1]
+    return _tuples(e(st.r_pos), e(st.r_vel), e(st.r_attr), e(st.r_goal), e(st.r_theta), st.h_pos, st.h_vel, st.h_attr[..., 0])
+
+
+def lookahead_inputs(st, actions, next_pos, next_vel, dt, unicycle):
+    """The [B][A][N][14] float32 tuples crowdsim_lookahead_pack rotates: the robot after CADRL.propagate (cadrl.py:104-125;
+    unicycle: theta + r, v cos / v sin with numpy's cos / sin, i.e. glibc's), the humans' next observable states
+    (next_pos / next_vel [B][N][2], lookahead_humans)."""
+    a = np.asarray(actions, dtype=np.float64)[None, :, None, :]                      # [1][A][1][2]
+    r = lambda x: np.asarray(x, dtype=np.float64)[:, None, None]                   # noqa: E731  [B] (or [B][2]) -> [B][1][1]
+    rp, th = r(st.r_pos), r(st.r_theta)
+    if unicycle:
+        nth = th + a[..., 1]
+        nv = np.stack([a[..., 0] * np.cos(nth), a[..., 0] * np.sin(nth)], -1)
+    else:
+        nth = th + 0 * a[..., 1]
+        nv = a
+    npos = rp + nv * dt
+    h = lambda x: np.asarray(x, dtype=np.float64)[:, None]                         # noqa: E731  [B][N].. -> [B][1][N]..
+    return _tuples(npos, nv, r(st.r_attr), r(st.r_goal), nth, h(next_pos), h(next_vel), h(st.h_attr[..., 0]))
+
+
+def clearance_bound(st, speed, dt):
+    """How far the swept-segment clearance (crowd_sim.py:331-345, hence dmin) of two implementations can be apart when
+    their robot velocity v (cos phi, sin phi) comes from different double cos / sin ([B] or [B][A] speeds |v|).
+    Each component differs by at most ULP_COS_SIN_SIDES ulps of cos (<= 2 U64 |cos| each) times |v| plus one rounding of the
+    product: 8 U64 |v|, so |dV| <= 12 U64 |v|. The clearance is 1-Lipschitz in the segment's end, which moves by dt |dV|.
+    The ~12 float64 operations of point_to_segment_dist on either side are within 16 U64 S of their exact value, S bounding
+    every intermediate magnitude (relative position, its sweep over dt, radii)."""
+    speed = np.asarray(speed, dtype=np.float64)
+    sp = speed if speed.ndim == 2 else speed[:, None]                                   # [B][A]
+    rel = np.abs(st.h_pos - st.r_pos[:, None]).sum(-1) + np.abs(st.h_vel).sum(-1) * dt + st.h_attr[..., 0]
+    S = rel.max(-1) + st.r_attr[:, 0] + 2 * dt * sp.max(-1)                            # [B]
+    bound = dt * 12 * U64 * sp + 2 * 16 * U64 * S[:, None]
+    return bound if speed.ndim == 2 else bound[:, 0]
+
+
+def reward_bound(reward, closest_bound, discomfort_penalty_factor, dt):
+    """A discomfort reward (dmin - d) f dt moves by f dt times dmin's bound, plus its two roundings on either side."""
+    return discomfort_penalty_factor * dt * closest_bound * (1 + 4 * U64) + 4 * U64 * np.abs(reward)
+
+
+def reward_class(reward, prm):
+    """0 nothing / timeout, 1 collision, 2 success, 3 discomfort (crowd_sim.py:368-389)."""
+    r = np.asarray(reward)
+    return np.where(r == 0, 0, np.where(r == prm.collision_penalty, 1, np.where(r == prm.success_reward, 2, 3)))
+
+
+def assert_unicycle_step_within_bounds(pre, actions, prm, got, want, what=''):
+    """One external_rot step of two implementations from the same pre-step state `pre`: `got` / `want` dicts of r_pos,
+    r_vel, r_theta, action_out, reward, dmin, done, info. The heading (fmod of a sum) and every flag are exact; the pose and
+    velocity come from double cos / sin, ULP_COS_SIN_SIDES ulps apart: px + cos(th) v dt differs by at most 3 ulps of
+    cos(th) times v dt (<= 6 ulps of cos(th) v dt), plus one rounding each of cos * v and * dt (3 ulps) and of the sum (1 ulp
+    of the result); v cos(theta') by 6 + 1 ulps of v cos(theta'). dmin and reward within clearance_bound / reward_bound."""
+    v, r = actions[:, 0], actions[:, 1]
+    dt = prm.time_step
+    th = pre.r_theta + r
+    step = np.stack([np.cos(th) * v * dt, np.sin(th) * v * dt], -1)
+    pos_bound = 9 * ulp64(step) + ulp64(pre.r_pos + step)
+    nth = np.asarray(want['r_theta'])
+    vel_bound = 7 * ulp64(np.stack([v * np.cos(nth), v * np.sin(nth)], -1))
+    cb = clearance_bound(pre, np.abs(v), dt)
+    for f in ('r_theta', 'done', 'info'):
+        assert_same_bits(got[f], want[f], '%s: %s' % (what, f))
+    assert (reward_class(got['reward'], prm) == reward_class(want['reward'], prm)).all(), what + ': reward class'
+    checks = (('r_pos', pos_bound), ('r_vel', vel_bound), ('action_out', vel_bound),
+              ('reward', reward_bound(want['reward'], cb, prm.discomfort_penalty_factor, dt)), ('dmin', cb))
+    for f, bound in checks:
+        a, b = np.asarray(got[f], dtype=np.float64), np.asarray(want[f], dtype=np.float64)
+        with np.errstate(invalid='ignore'):
+            err = np.where(np.isinf(a) & (a == b), 0.0, np.abs(a - b))
+        bad = ~(err <= bound)
+        if bad.any():
+            i = tuple(int(x) for x in np.argwhere(bad)[0])
+            raise AssertionError('%s: %s outside its bound at %s: %r vs %r (bound %r)' % (what, f, i, a[i], b[i], bound[i]))
+
+
 def ulp_diff(a, b):
     """Elementwise distance in float64 ulps (for values of equal sign / finite)."""
     a = np.ascontiguousarray(a, dtype=np.float64); b = np.ascontiguousarray(b, dtype=np.float64)
