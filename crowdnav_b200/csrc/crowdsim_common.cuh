@@ -27,6 +27,54 @@ __device__ __forceinline__ double point_to_segment_dist0(double x1, double y1, d
     return norm2(x, y);
 }
 
+// The reference's per-step rules, one copy each for every kernel; operations in the reference's order.
+
+// orca.py:113-115 preferred velocity: goal - position, normalised if longer than 1 (numpy float64), then the float32 cast
+// of the rvo2 boundary
+__device__ __forceinline__ orca::V2 pref_velocity(double2 pos, double2 goal)
+{
+    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
+    const double speed = norm2(gvx, gvy);
+    return orca::mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+}
+
+// orca.py:100-104 radius of an agent in an ORCA simulation: the radius plus 0.01 plus the safety space in float64, then the
+// float32 cast
+__device__ __forceinline__ float orca_radius(double radius, double safety_space) { return (float)(radius + 0.01 + safety_space); }
+
+// crowd_sim.py:333-345 clearance between a human and the robot over one step: the human's segment relative to the robot
+// (the human's CURRENT velocity attribute, i.e. its previous action, against the robot's velocity of this step) to the
+// origin, minus the human's radius, then minus the robot's
+__device__ __forceinline__ double swept_clearance(double2 h_pos, double2 h_vel, double2 r_pos, double2 r_vel, double h_radius,
+                                                  double r_radius, double dt)
+{
+    const double px = h_pos.x - r_pos.x, py = h_pos.y - r_pos.y;
+    const double vx = h_vel.x - r_vel.x, vy = h_vel.y - r_vel.y;
+    const double ex = px + vx * dt, ey = py + vy * dt;
+    return point_to_segment_dist0(px, py, ex, ey) - h_radius - r_radius;
+}
+
+// agent.py:115-120 compute_position: the robot's position after one step of action (ax, ay) = (vx, vy) (holonomic) or
+// (v, r) (unicycle, heading theta)
+__device__ __forceinline__ double2 robot_position(bool unicycle, double2 pos, double theta, double ax, double ay, double dt)
+{
+    if (!unicycle) return make_double2(pos.x + ax * dt, pos.y + ay * dt);
+    const double th = theta + ay;
+    return make_double2(pos.x + cos(th) * ax * dt, pos.y + sin(th) * ax * dt);
+}
+
+// agent.py:128-135 the robot's velocity after that step; a unicycle also turns: theta = (theta + r) % (2 pi) by Python's
+// rules (the result takes the sign of 2 pi, and a zero remainder is +0.0)
+__device__ __forceinline__ double2 robot_velocity(bool unicycle, double &theta, double ax, double ay)
+{
+    if (!unicycle) return make_double2(ax, ay);
+    double nth = fmod(theta + ay, 2 * CS_PI);
+    if (nth < 0) nth += 2 * CS_PI;
+    else if (nth == 0) nth = 0.0;
+    theta = nth;
+    return make_double2(ax * cos(nth), ax * sin(nth));
+}
+
 __device__ __forceinline__ double2 ld2(const double *p, size_t i) { return reinterpret_cast<const double2 *>(p)[i]; }
 __device__ __forceinline__ void st2(double *p, size_t i, double2 v) { reinterpret_cast<double2 *>(p)[i] = v; }
 __device__ __forceinline__ double2 ld2_cg(const double *p, size_t i) { return __ldcg(reinterpret_cast<const double2 *>(p) + i); }
@@ -67,12 +115,35 @@ inline KParams make_kparams(const crowdsim_params *p, int N)
     return k;
 }
 
+// crowd_sim.py:368-389 reward and terminal ladder of one step; returns info (CROWDSIM_INFO_*), done = ends_episode(info).
+// Danger / Nothing are selects, not a branch: the robot lanes of a warp take different rungs, and in the multi-step kernel
+// the robot's tail is the critical path of every step.
+__device__ __forceinline__ int reward_ladder(bool timeout, bool collision, bool reaching_goal, double dmin, const KParams &k, double dt,
+                                             double &reward)
+{
+    int info;
+    if (timeout) { reward = 0; info = CROWDSIM_INFO_TIMEOUT; }
+    else if (collision) { reward = k.collision_penalty; info = CROWDSIM_INFO_COLLISION; }
+    else if (reaching_goal) { reward = k.success_reward; info = CROWDSIM_INFO_REACHGOAL; }
+    else {
+        const bool danger = dmin < k.discomfort_dist;
+        reward = danger ? (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt : 0;
+        info = danger ? CROWDSIM_INFO_DANGER : CROWDSIM_INFO_NOTHING;
+    }
+    return info;
+}
+
+// Timeout, Collision and ReachGoal end the episode; Danger and Nothing do not
+static_assert(CROWDSIM_INFO_NOTHING < CROWDSIM_INFO_REACHGOAL && CROWDSIM_INFO_DANGER < CROWDSIM_INFO_REACHGOAL &&
+              CROWDSIM_INFO_REACHGOAL < CROWDSIM_INFO_COLLISION && CROWDSIM_INFO_COLLISION < CROWDSIM_INFO_TIMEOUT, "ending infos last");
+__device__ __forceinline__ bool ends_episode(int info) { return info >= CROWDSIM_INFO_REACHGOAL; }
+
 // Shared-memory staging of one block's environments: L = N + 1 agents per env (humans 0..N-1, robot N).
 struct Stage {
     double2 *pos64, *vel64;      // [EPB * L]
     double *rad64;               // [EPB * L]
     float2 *pos32, *vel32;       // [EPB * L]  float32 casts consumed by the ORCA solver
-    float *radh, *radr;          // [EPB * L]  (float)(radius + 0.01 + safety) as seen by humans / by the robot
+    float *radh, *radr;          // [EPB * L]  orca_radius() as seen by humans / by the robot
     double2 *act;                // [EPB]      robot velocity applied this step
     double *closest;             // [EPB * L]  per-human clearance of the swept segment test
     float *lines, *proj;         // [4 * maxnb * T] each: per-thread columns (orca::Lines)
@@ -123,8 +194,8 @@ __device__ __forceinline__ void stage_agent(const Stage &s, const KParams &k, in
     s.pos64[slot] = pos; s.vel64[slot] = vel; s.rad64[slot] = radius;
     s.pos32[slot] = make_float2((float)pos.x, (float)pos.y);
     s.vel32[slot] = make_float2((float)vel.x, (float)vel.y);
-    s.radh[slot] = (float)(radius + 0.01 + k.human_safety_space);    // orca.py:100-104
-    s.radr[slot] = (float)(radius + 0.01 + k.robot_safety_space);
+    s.radh[slot] = orca_radius(radius, k.human_safety_space);
+    s.radr[slot] = orca_radius(radius, k.robot_safety_space);
 }
 
 // ORCA.predict for agent `a` of local env `le` (a == N: the robot). crowd_sim/envs/policy/orca.py:82-132.
@@ -138,11 +209,7 @@ __device__ __forceinline__ orca::V2 orca_predict(const Stage &s, const KParams &
     using namespace orca;
     const bool is_robot = (a == N);
     const int base = le * L;
-    // orca.py:113-115 preferred velocity in float64 (numpy), then the float32 cast of the rvo2 boundary
-    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-    const double speed = norm2(gvx, gvy);
-    const double pvx = (speed > 1) ? gvx / speed : gvx, pvy = (speed > 1) ? gvy / speed : gvy;
-    const V2 pref = mk((float)pvx, (float)pvy);
+    const V2 pref = pref_velocity(pos, goal);
     const float2 p2 = s.pos32[base + a], v2 = s.vel32[base + a];
     const V2 p = mk(p2.x, p2.y), v = mk(v2.x, v2.y);
     const float *rad_view = is_robot ? s.radr : s.radh;

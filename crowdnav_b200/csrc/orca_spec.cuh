@@ -17,7 +17,9 @@
 // one common instruction stream with M(M-1)/2 independent divisions in flight instead of the union of 32 divergent
 // control paths.
 // linearProgram3 has a similar structure one level up (its per-line sub-problems do not depend on the running result);
-// step_flat.cuh exploits that by running the sub-problems of a queued solve on parallel lanes.
+// step_flat.cuh exploits that by running the sub-problems of a queued solve on parallel lanes, each with the sequential
+// code of orca_device.cuh. A finer split, the (i, j) projections on lanes of their own and every sub-problem speculative
+// in registers (lp1_all + lp2_scan over the projected lines), was bit-identical and slower, and was not kept.
 #pragma once
 #include "orca_device.cuh"
 
@@ -25,9 +27,8 @@ namespace orca {
 
 template <int M> struct RegLines { V2 p[M], d[M]; };
 
-// Neighbour order of the small-crowd kernel (step_flat.cuh carries the same statements inline; this host-compilable copy
-// is what tests/native/lp_fuzz.cu checks against RVO2's insertion sort -- folding the kernel onto it changes the
-// generated code, so that waits for a GPU parity run). candidates c = 0..M-1 in RVO2's scan order with squared distance dsq[c],
+// Neighbour order of the small-crowd kernels (step_flat.cuh, step_multi.cuh, orca_act_kernel; tests/native/lp_fuzz.cu
+// checks it against RVO2's insertion sort). candidates c = 0..M-1 in RVO2's scan order with squared distance dsq[c],
 // inr[c] = "within neighbour range" and agent index id[c] (< 8). Rank of an in-range candidate = the position RVO2's
 // insertAgentNeighbor (strict <, so ties keep scan order) would give it: for cc < c, cc precedes c iff dsq[cc] <= dsq[c]
 // -- one comparison per unordered pair. The agent index of the kk-th nearest is then read from a packed word (3 bits per
@@ -61,7 +62,9 @@ ORCA_HD __forceinline__ int neighbour_order(const float (&dsq)[M], const bool (&
 // already-overlapping case (0.09 % of lines) stays a real branch. Operation order inside each variant is RVO2's
 // (make_line in orca_device.cuh). A fully branch-free form (overlap folded in, no per-line valid branch) was slower in
 // the single-step kernel (scripts/latency_probe.cu): the extra arithmetic costs more than the removed divergence.
-// Keeping it out of line (__noinline__, to shrink the 5 k-instruction kernel) was slower too.
+// Keeping it out of line (__noinline__, to shrink the 5 k-instruction kernel) was slower too. An earlier multi-step kernel
+// built its lines straight-line instead: the non-overlapping variants without a branch for every line, the overlapping
+// ones repaired afterwards; it was removed with that kernel's layout (DESIGN §10).
 ORCA_HD __forceinline__ void make_line_sel(V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_th, float inv_dt,
                                               V2 &point, V2 &dir)
 {
@@ -99,53 +102,6 @@ ORCA_HD __forceinline__ void make_line_sel(V2 p, V2 v, float r, V2 po, V2 vo, fl
         dir = mk(unit_w.y, -unit_w.x);
         u = (comb_r * inv_dt - w_len) * unit_w;
     }
-    point = v + 0.5f * u;
-}
-
-// The same half-plane split for straight-line issue: make_line_far is make_line_sel's non-overlapping branch on its own (both
-// variants evaluated, selected; NO branch), make_line_overlap the already-overlapping branch. A caller evaluates make_line_far
-// for all its lines unconditionally -- the constructions are independent, so their dependent chains (2 sqrt + 2 div each)
-// interleave -- and repairs the rare overlapping lines (0.09 % of all) afterwards. For an overlapping pair make_line_far
-// computes sqrtf of a negative number (NaN); the result is discarded. Same operations per line => same bits.
-ORCA_HD __forceinline__ void make_line_far(V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_th, V2 &point, V2 &dir, bool &overlap)
-{
-    const V2 rel_pos = po - p;
-    const V2 rel_vel = v - vo;
-    const float dist_sq = abssq(rel_pos);
-    const float comb_r = r + ro;
-    const float comb_r_sq = sqr(comb_r);
-    overlap = !(dist_sq > comb_r_sq);
-    const V2 w = rel_vel - inv_th * rel_pos;
-    const float w_len_sq = abssq(w);
-    const float dot1 = dot(w, rel_pos);
-    const float w_len = sqrtf(w_len_sq);
-    const V2 unit_w = vdiv(w, w_len);
-    const V2 dir_c = mk(unit_w.y, -unit_w.x);
-    const V2 u_c = (comb_r * inv_th - w_len) * unit_w;
-    const float leg = sqrtf(dist_sq - comb_r_sq);
-    const bool left = det(rel_pos, w) > 0.0f;
-    const V2 num_l = mk(rel_pos.x * leg - rel_pos.y * comb_r, rel_pos.x * comb_r + rel_pos.y * leg);
-    const V2 num_r = mk(rel_pos.x * leg + rel_pos.y * comb_r, -rel_pos.x * comb_r + rel_pos.y * leg);
-    const V2 q = vdiv(left ? num_l : num_r, dist_sq);
-    const V2 dir_l = left ? q : -q;
-    const float dot2 = dot(rel_vel, dir_l);
-    const V2 u_l = dot2 * dir_l - rel_vel;
-    const bool cutoff = dot1 < 0.0f && sqr(dot1) > comb_r_sq * w_len_sq;
-    dir = cutoff ? dir_c : dir_l;
-    const V2 u = cutoff ? u_c : u_l;
-    point = v + 0.5f * u;
-}
-
-ORCA_HD __forceinline__ void make_line_overlap(V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_dt, V2 &point, V2 &dir)
-{
-    const V2 rel_pos = po - p;
-    const V2 rel_vel = v - vo;
-    const float comb_r = r + ro;
-    const V2 w = rel_vel - inv_dt * rel_pos;
-    const float w_len = sqrtf(abssq(w));
-    const V2 unit_w = vdiv(w, w_len);
-    dir = mk(unit_w.y, -unit_w.x);
-    const V2 u = (comb_r * inv_dt - w_len) * unit_w;
     point = v + 0.5f * u;
 }
 
@@ -229,48 +185,6 @@ ORCA_HD __forceinline__ void insert_sorted(float dd, int j, float (&td)[M], int 
         td[kk] = ltp ? td[km] : (lt ? dd : td[kk]);
         tj[kk] = ltp ? tj[km] : (lt ? j : tj[kk]);
     }
-}
-
-// ---- linearProgram3 spread over lanes (step_flat.cuh, step_mid.cuh) ----------------------------------------------------
-// RVO2's linearProgram3 visits the lines i = begin .. n-1; for a line that is violated by more than the running `distance`
-// it builds the lines j < i projected onto i and solves linearProgram2 over them in direction-optimisation mode, STARTING
-// FROM optVelocity * radius -- so the sub-problem of line i depends only on the lines, never on the running result.
-// That gives three levels of independent work per solve: the (i, j) projections (one division + one normalisation each),
-// the per-i sub-problems (speculative lp1_all + lp2_scan over <= M-1 projected lines, all pair intersections in flight at
-// once), and a short outer scan. The kernels put each level on its own set of lanes; these are the per-lane functions
-// (host-compilable: tests/native/lp_fuzz.cu part F checks the composition against the oracle's sequential lp3).
-
-// pair index q = i (i - 1) / 2 + j  <->  (i, j), 0 <= j < i <= 9
-ORCA_HD __forceinline__ void lp3_pair_of(int q, int &i, int &j)
-{
-    i = 1 + (q >= 1) + (q >= 3) + (q >= 6) + (q >= 10) + (q >= 15) + (q >= 21) + (q >= 28) + (q >= 36);
-    j = q - i * (i - 1) / 2;
-}
-
-// Line j projected onto line i (the loop body of linearProgram3, same operations as lp3_project). Returns false for the
-// pairs RVO2 skips (parallel, same direction). Parallel lanes divide 1 by 1 (the quotient is unused there): a zero
-// denominator would send the whole warp through the IEEE-division slow path.
-ORCA_HD __forceinline__ bool lp3_project_pair(V2 pi, V2 di, V2 pj, V2 dj, V2 &pp, V2 &pd)
-{
-    const float d = det(di, dj);
-    const bool par = fabsf(d) <= kEps;
-    if (par && dot(di, dj) > 0.0f) { pp = mk(0.f, 0.f); pd = mk(0.f, 0.f); return false; }
-    const float t = (par ? 1.0f : det(dj, pi - pj)) / (par ? 1.0f : d);
-    pp = par ? 0.5f * (pi + pj) : pi + t * di;
-    pd = normalize(dj - di);
-    return true;
-}
-
-// Sub-problem of line i: linearProgram2 (direction optimisation, opt = perpendicular of dir_i) over its K projected-line
-// positions (absent / skipped positions: valid = false, zero lines). Returns false when it fails (RVO2 keeps the running
-// result then); r2 = the point it returns.
-template <int K>
-ORCA_HD __forceinline__ bool lp3_sub_spec(const RegLines<K> &P, const bool (&valid)[K], float radius, V2 di, V2 &r2)
-{
-    const V2 opt = mk(-di.y, di.x);
-    V2 cand[K]; bool feas[K];
-    lp1_all<K, K>(P, valid, radius, opt, true, cand, feas);
-    return lp2_scan<K, K>(P, valid, K, cand, feas, mk(opt.x * radius, opt.y * radius), r2) == K;
 }
 
 }  // namespace orca

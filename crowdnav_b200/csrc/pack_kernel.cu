@@ -102,11 +102,7 @@ __global__ void __launch_bounds__(256) lookahead_kernel(const __grid_constant__ 
             if (G.unicycle) { avx = act.x * cos(act.y + tt.x); avy = act.x * sin(act.y + tt.x); }
             double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
             for (int i = 0; i < N; ++i) {
-                const double2 hp = s.pos64[base + i], hv = s.vel64[base + i];
-                const double px = hp.x - rp.x, py = hp.y - rp.y;
-                const double vx = hv.x - avx, vy = hv.y - avy;
-                const double ex = px + vx * dt, ey = py + vy * dt;
-                const double c = point_to_segment_dist0(px, py, ex, ey) - s.rad64[base + i] - ra.x;
+                const double c = swept_clearance(s.pos64[base + i], s.vel64[base + i], rp, make_double2(avx, avy), s.rad64[base + i], ra.x, dt);
                 if (c < 0) { collision = true; break; } else if (c < dmin) dmin = c;
             }
             // cadrl.py:104-129 propagate(self_state, action); agent.py:110-120 compute_position for the goal test
@@ -119,11 +115,7 @@ __global__ void __launch_bounds__(256) lookahead_kernel(const __grid_constant__ 
             }
             const bool reaching_goal = norm2(gpx - rg.x, gpy - rg.y) < ra.x;
             double reward;
-            if (tt.y >= k.time_limit - 1) reward = 0;
-            else if (collision) reward = k.collision_penalty;
-            else if (reaching_goal) reward = k.success_reward;
-            else if (dmin < k.discomfort_dist) reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt;
-            else reward = 0;
+            reward_ladder(tt.y >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
             G.out_reward[(size_t)e2 * A + kk] = reward;
 
             float c, sn, rot, dg, rvx, rvy;

@@ -18,8 +18,8 @@
 // fewest instructions, best when the launch fills the chip) or per WARP (WARPQ = true: no block barrier, every warp runs
 // the pass for its own 1-2 solves; best for launches that leave the SMs mostly empty). cs::launch() picks by grid size
 // (the multi-step kernel, step_multi.cuh, runs the same block queue).
-// Two finer splits of the pass were tried, both bit-identical, both slower, neither kept: (a) projections on (i, j) lanes +
-// register-resident speculative sub-problems (orca_spec.cuh: lp3_project_pair / lp3_sub_spec, host-fuzzed); (b) four lane
+// Two finer splits of the pass were tried, both bit-identical, both slower, neither kept: (a) the (i, j) projections on
+// lanes of their own + register-resident speculative sub-problems (lp1_all + lp2_scan over the projected lines); (b) four lane
 // levels with early-exit code (projections, lp1 candidates, lp2 scans, outer scan; 10 lanes per item). More lanes
 // per item means more warps with active lanes = more warp-instructions for the same work, and the all-pairs speculative
 // form executes more instructions than early-exit code; at 1-2 warps per scheduler a warp's time is its instruction count.
@@ -119,20 +119,17 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     const bool live = env_ok && (act_flag != 0);
     // float32 view of myself for the other lanes of my env (rvo2 boundary casts, orca.py:100-110)
     const float fpx = (float)pos.x, fpy = (float)pos.y, fvx = (float)vel.x, fvy = (float)vel.y;
-    const float frh = (float)(attr.x + 0.01 + k.human_safety_space);     // my radius as seen by a human observer
-    const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
+    const float frh = orca_radius(attr.x, k.human_safety_space);         // my radius as seen by a human observer
+    const float frr = orca_radius(attr.x, k.robot_safety_space);         // ... by the robot
     const bool solves = live && (!is_robot || k.robot_policy == CROWDSIM_ROBOT_ORCA);
 
-    // ---- orca.py:113-115 preferred velocity (float64) ----
-    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-    const double speed = norm2(gvx, gvy);
-    const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+    const V2 pref = pref_velocity(pos, goal);
     const V2 p = mk(fpx, fpy), v = mk(fvx, fvy);
     const float r = is_robot ? frr : frh;
     const float max_speed = (float)attr.y;
 
     // ---- neighbour scan: candidate slot c -> agent j (reference order: other humans, then the robot iff visible) ----
-    float dsq[M]; bool inr[M]; int jj[M];
+    float dsq[M]; bool inr[M]; int jj[M], src[M];
     #pragma unroll
     for (int c = 0; c < M; ++c) {
         int j; bool cv;
@@ -144,28 +141,8 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         dsq[c] = abssq(p - mk(qx, qy));
         inr[c] = solves && cv && (k.max_neighbors > 0) && dsq[c] < sqr(k.neighbor_dist);
     }
-    // rank of each candidate = position RVO2's insertion sort (strict <, ties in scan order) would give it: for cc < c,
-    // cc precedes c iff dsq[cc] <= dsq[c] -- one comparison per unordered pair. The agent index of the kk-th nearest is
-    // then read from a packed word (3 bits per position, N <= 5) instead of an M x M select cascade (orca_spec.cuh:
-    // neighbour_order is the host-checked copy of these statements).
-    int rank[M];
-    #pragma unroll
-    for (int c = 0; c < M; ++c) rank[c] = 0;
-    #pragma unroll
-    for (int c = 1; c < M; ++c) {
-        #pragma unroll
-        for (int cc = 0; cc < c; ++cc) {
-            const bool le_ = dsq[cc] <= dsq[c];
-            rank[c] += (inr[cc] && le_) ? 1 : 0;
-            rank[cc] += (inr[c] && !le_) ? 1 : 0;
-        }
-    }
-    int nl = 0; unsigned packed = 0u;
-    #pragma unroll
-    for (int c = 0; c < M; ++c) if (inr[c]) { packed |= (unsigned)jj[c] << (3 * rank[c]); ++nl; }
-    int src[M];                             // src[kk] = agent index of the kk-th nearest (0 beyond nl)
-    #pragma unroll
-    for (int kk = 0; kk < M; ++kk) src[kk] = (int)((packed >> (3 * kk)) & 7u);
+    // src[kk] = agent index of the kk-th nearest (0 beyond nl), in RVO2's stable insertion order
+    int nl = neighbour_order<M>(dsq, inr, jj, src);
     nl = nl < k.max_neighbors ? nl : k.max_neighbors;
 
     // ---- ORCA lines in rank order, in registers ----
@@ -316,14 +293,9 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     const double Rpx = __shfl_sync(CS_FULL, pos.x, rl), Rpy = __shfl_sync(CS_FULL, pos.y, rl);
     const double Rrad = __shfl_sync(CS_FULL, attr.x, rl);
 
-    // ---- human lanes: swept-segment clearance (crowd_sim.py:333-345) ----
+    // ---- human lanes: swept-segment clearance ----
     double closest = 0.0;
-    if (live && !is_robot) {
-        const double px = pos.x - Rpx, py = pos.y - Rpy;
-        const double vx = vel.x - Rvx, vy = vel.y - Rvy;    // the human's CURRENT velocity attribute (previous action)
-        const double ex = px + vx * dt, ey = py + vy * dt;
-        closest = point_to_segment_dist0(px, py, ex, ey) - attr.x - Rrad;
-    }
+    if (live && !is_robot) closest = swept_clearance(pos, vel, make_double2(Rpx, Rpy), make_double2(Rvx, Rvy), attr.x, Rrad, dt);
     // ordered fold over the env's humans (first collision breaks, crowd_sim.py:346-351); consumed by the robot lane
     double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
     #pragma unroll
@@ -338,23 +310,14 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     if (is_robot && env_ok) {
         bool done = false;
         if (live) {
-            double npx, npy, nvx, nvy;
-            if (!ROT) { npx = pos.x + ax * dt; npy = pos.y + ay * dt; nvx = ax; nvy = ay; }
-            else { const double th = theta + ay; npx = pos.x + cos(th) * ax * dt; npy = pos.y + sin(th) * ax * dt; nvx = nvy = 0; }
-            const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;
-            double reward; int info;
+            const double2 npos = robot_position(ROT, pos, theta, ax, ay, dt);
+            const bool reaching_goal = norm2(npos.x - goal.x, npos.y - goal.y) < attr.x;
             const double gtime = rr.gtime;
-            if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
-            else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
-            else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
-            else if (dmin < k.discomfort_dist) { reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt; done = false; info = CROWDSIM_INFO_DANGER; }
-            else { reward = 0; done = false; info = CROWDSIM_INFO_NOTHING; }
-            if (ROT) {                                                                   // agent.py:133-135
-                double nth = fmod(theta + ay, 2 * CS_PI); if (nth < 0) nth += 2 * CS_PI;
-                else if (nth == 0) nth = 0.0;                                            // Python's % gives +0.0 for a zero remainder
-                theta = nth; nvx = ax * cos(nth); nvy = ax * sin(nth);
-            }
-            pos = make_double2(npx, npy); vel = make_double2(nvx, nvy);
+            double reward;
+            const int info = reward_ladder(gtime >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
+            done = ends_episode(info);
+            vel = robot_velocity(ROT, theta, ax, ay);
+            pos = npos;
             const double ntime = gtime + dt;
             rr.gtime = ntime;
             st2(A.st.r_pos, e, pos); st2(A.st.r_vel, e, vel); A.st.g_time[e] = ntime; if (ROT) A.st.r_theta[e] = theta;

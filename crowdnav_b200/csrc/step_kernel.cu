@@ -94,15 +94,9 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
     }
     __syncthreads();
 
-    // ---- human lanes: swept-segment clearance against the robot (crowd_sim.py:333-345) ----
+    // ---- human lanes: swept-segment clearance against the robot ----
     const double dt = k.time_step;
-    if (live && !is_robot) {
-        const double2 rp = s.pos64[le * L + N], ra = s.act[le];
-        const double px = pos.x - rp.x, py = pos.y - rp.y;
-        const double vx = vel.x - ra.x, vy = vel.y - ra.y;     // human's CURRENT velocity attribute (previous action)
-        const double ex = px + vx * dt, ey = py + vy * dt;
-        s.closest[tid] = point_to_segment_dist0(px, py, ex, ey) - attr.x - s.rad64[le * L + N];
-    }
+    if (live && !is_robot) s.closest[tid] = swept_clearance(pos, vel, s.pos64[le * L + N], s.act[le], attr.x, s.rad64[le * L + N], dt);
     __syncthreads();
 
     // ---- robot lane: reduce clearances, ladder, update, bookkeeping; decides about auto-reset ----
@@ -117,31 +111,22 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
                 if (c < 0) { collision = true; break; }
                 else if (c < dmin) dmin = c;
             }
-            double npx, npy, nvx, nvy;
-            if (k.robot_policy != CROWDSIM_ROBOT_EXTERNAL_ROT) { npx = pos.x + ax * dt; npy = pos.y + ay * dt; nvx = ax; nvy = ay; }
-            else { const double th = theta + ay; npx = pos.x + cos(th) * ax * dt; npy = pos.y + sin(th) * ax * dt; nvx = nvy = 0; }  // agent.py:115-118
-            const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < attr.x;      // crowd_sim.py:365-366
-
-            double reward; int info;                                                   // crowd_sim.py:368-389
-            if (gtime >= k.time_limit - 1) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
-            else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
-            else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
-            else if (dmin < k.discomfort_dist) { reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt; done = false; info = CROWDSIM_INFO_DANGER; }
-            else { reward = 0; done = false; info = CROWDSIM_INFO_NOTHING; }
-
-            if (k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT) {                        // agent.py:133-135
-                double nth = fmod(theta + ay, 2 * CS_PI); if (nth < 0) nth += 2 * CS_PI;
-                else if (nth == 0) nth = 0.0;                                           // Python's % gives +0.0 for a zero remainder
-                if (!A.lookahead) A.st.r_theta[e] = nth;
-                nvx = ax * cos(nth); nvy = ax * sin(nth);
-            }
+            const bool rot = k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT;
+            const double2 npos = robot_position(rot, pos, theta, ax, ay, dt);
+            const bool reaching_goal = norm2(npos.x - goal.x, npos.y - goal.y) < attr.x;    // crowd_sim.py:365-366
+            double reward;
+            const int info = reward_ladder(gtime >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
+            done = ends_episode(info);
+            double nth = theta;
+            const double2 nvel = robot_velocity(rot, nth, ax, ay);
+            if (rot && !A.lookahead) A.st.r_theta[e] = nth;
             const double ntime = gtime + dt;
             if (!A.lookahead) {
-                st2(A.st.r_pos, e, make_double2(npx, npy));
-                st2(A.st.r_vel, e, make_double2(nvx, nvy));
+                st2(A.st.r_pos, e, npos);
+                st2(A.st.r_vel, e, nvel);
                 A.st.g_time[e] = ntime;
             }
-            if (A.io.action_out) st2(A.io.action_out, e, make_double2(nvx, nvy));
+            if (A.io.action_out) st2(A.io.action_out, e, nvel);
             A.io.reward[e] = reward; A.io.dmin[e] = dmin; A.io.done[e] = done ? 1 : 0; A.io.info[e] = (uint8_t)info;
 
             if (A.has_ep) {                                                            // explorer.py:41-72
@@ -158,7 +143,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
                         ep.res_info[c] = (uint8_t)info; ep.res_steps[c] = t + 1;
                         ep.res_time[c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[c] = ret; ep.res_too_close[c] = tc; ep.res_min_dist_sum[c] = mds;
-                        if (ep.res_final_rpos) st2(ep.res_final_rpos, c, make_double2(npx, npy));
+                        if (ep.res_final_rpos) st2(ep.res_final_rpos, c, npos);
                     }
                     if (A.st.active && !A.has_ar) A.st.active[e] = 0;
                 }
@@ -211,17 +196,15 @@ __global__ void __launch_bounds__(128) orca_act_kernel(const __grid_constant__ S
     if (A.st.active && !A.st.active[e]) return;
     const KParams &k = A.k;
     const double2 pos = ld2(A.st.r_pos, e), vel = ld2(A.st.r_vel, e), goal = ld2(A.st.r_goal, e), attr = ld2(A.st.r_attr, e);
-    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-    const double speed = norm2(gvx, gvy);
-    const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+    const V2 pref = pref_velocity(pos, goal);
     const V2 p = mk((float)pos.x, (float)pos.y), v = mk((float)vel.x, (float)vel.y);
-    const float r = (float)(attr.x + 0.01 + k.robot_safety_space), max_speed = (float)attr.y;
+    const float r = orca_radius(attr.x, k.robot_safety_space), max_speed = (float)attr.y;
     V2 hp[M], hv[M]; float hr[M]; float dsq[M]; bool inr[M]; int id[M], src[M];
     #pragma unroll
     for (int c = 0; c < M; ++c) {
         const size_t i = (size_t)e * N + c;
         const double2 q = ld2(A.st.h_pos, i), w = ld2(A.st.h_vel, i), at = ld2(A.st.h_attr, i);
-        hp[c] = mk((float)q.x, (float)q.y); hv[c] = mk((float)w.x, (float)w.y); hr[c] = (float)(at.x + 0.01 + k.robot_safety_space);
+        hp[c] = mk((float)q.x, (float)q.y); hv[c] = mk((float)w.x, (float)w.y); hr[c] = orca_radius(at.x, k.robot_safety_space);
         dsq[c] = abssq(p - hp[c]); inr[c] = (k.max_neighbors > 0) && dsq[c] < sqr(k.neighbor_dist); id[c] = c;
     }
     int nl = neighbour_order<M>(dsq, inr, id, src);

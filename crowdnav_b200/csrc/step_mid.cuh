@@ -49,10 +49,7 @@ __device__ __forceinline__ orca::V2 mid_solve(const Stage &s, const KParams &k, 
     if (solve) {
         const bool is_robot = (a == N);
         const int base = le * L;
-        // orca.py:113-115 preferred velocity in float64 (numpy), then the float32 cast of the rvo2 boundary
-        const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-        const double speed = norm2(gvx, gvy);
-        const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+        const V2 pref = pref_velocity(pos, goal);
         const float2 p2 = s.pos32[base + a], v2 = s.vel32[base + a];
         const V2 p = mk(p2.x, p2.y), v = mk(v2.x, v2.y);
         const float *rad_view = is_robot ? s.radr : s.radh;

@@ -80,10 +80,7 @@ __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *
                                                 float &max_speed_out)
 {
     using namespace orca;
-    // ---- orca.py:113-115 preferred velocity (float64) ----
-    const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-    const double speed = norm2(gvx, gvy);
-    const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+    const V2 pref = pref_velocity(pos, goal);
     const float max_speed = (float)v_pref;
 
     // ---- neighbour scan and RVO2's stable order ----
@@ -243,8 +240,8 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     const bool live = env_ok && (act_flag != 0);
     // float32 view of myself for the other agents of my env (rvo2 boundary casts, orca.py:100-110), float64 view of the humans
     const float fpx = (float)pos.x, fpy = (float)pos.y, fvx = (float)vel.x, fvy = (float)vel.y;
-    const float frh = (float)(attr.x + 0.01 + k.human_safety_space);     // my radius as seen by a human observer
-    const float frr = (float)(attr.x + 0.01 + k.robot_safety_space);     // ... by the robot
+    const float frh = orca_radius(attr.x, k.human_safety_space);         // my radius as seen by a human observer
+    const float frr = orca_radius(attr.x, k.robot_safety_space);         // ... by the robot
     s_view[slot_me] = make_float4(fpx, fpy, fvx, fvy); s_radh[slot_me] = frh; s_radr[slot_me] = frr;
     s_pos[tid] = pos; s_vel[tid] = vel; s_rad[tid] = attr.x;
     if constexpr (REC) { if (is_robot) rec_vpref_smem<E>()[le] = (float)attr.y; }
@@ -367,14 +364,10 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     bool timeout = false, reaching_goal = false;                       // robot lanes of live envs
     if (!is_robot) {
         if (live) {
-            // swept-segment clearance against the robot's velocity of this step (crowd_sim.py:333-345)
+            // swept-segment clearance against the robot's velocity of this step
             const int rt = 32 * N + le;
             const float2 rv = s_nv[rt];
-            const double2 rp = s_pos[rt];
-            const double px = pos.x - rp.x, py = pos.y - rp.y;
-            const double vx = vel.x - (double)rv.x, vy = vel.y - (double)rv.y;    // the human's CURRENT velocity attribute (previous action)
-            const double ex = px + vx * dt, ey = py + vy * dt;
-            s_cl[tid] = point_to_segment_dist0(px, py, ex, ey) - attr.x - s_rad[rt];
+            s_cl[tid] = swept_clearance(pos, vel, s_pos[rt], make_double2((double)rv.x, (double)rv.y), attr.x, s_rad[rt], dt);
             // agent.py:122-135 holonomic step with the ORCA action (float32 values widened); a scene installed below replaces it
             const double hx = (double)nv.x, hy = (double)nv.y;
             pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
@@ -439,14 +432,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 }
                 // ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72)
                 const double npx = pos.x + ax * dt, npy = pos.y + ay * dt;
-                double reward; int info;
                 const double gtime = rr.gtime;
                 const int t_rec = rr.ep_t;                   // REC: the episode step the row was recorded at
-                if (timeout) { reward = 0; done = true; info = CROWDSIM_INFO_TIMEOUT; }
-                else if (collision) { reward = k.collision_penalty; done = true; info = CROWDSIM_INFO_COLLISION; }
-                else if (reaching_goal) { reward = k.success_reward; done = true; info = CROWDSIM_INFO_REACHGOAL; }
-                else if (dmin < k.discomfort_dist) { reward = (dmin - k.discomfort_dist) * k.discomfort_penalty_factor * dt; done = false; info = CROWDSIM_INFO_DANGER; }
-                else { reward = 0; done = false; info = CROWDSIM_INFO_NOTHING; }
+                double reward;
+                const int info = reward_ladder(timeout, collision, reaching_goal, dmin, k, dt, reward);
+                done = ends_episode(info);
                 pos = make_double2(npx, npy); vel = make_double2(ax, ay);
                 const double ntime = gtime + dt;
                 rr.gtime = ntime;

@@ -58,10 +58,7 @@ __global__ void __launch_bounds__(64) human_times_kernel(const __grid_constant__
         if (a > 0 && ht == 0.0) atomicOr(&s_pending, 1);             // crowd_sim.py:231 while not all(self.human_times)
         __syncthreads();
         if (!s_pending) break;
-        // preferred velocity (crowd_sim.py:229-233)
-        const double gvx = goal.x - pos.x, gvy = goal.y - pos.y;
-        const double speed = norm2(gvx, gvy);
-        const V2 pref = mk((float)((speed > 1) ? gvx / speed : gvx), (float)((speed > 1) ? gvy / speed : gvy));
+        const V2 pref = pref_velocity(pos, goal);                    // crowd_sim.py:229-233
         // neighbours: all other agents in index order, the <= 10 nearest within range
         float td[M]; int tj[M];
         #pragma unroll

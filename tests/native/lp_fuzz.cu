@@ -5,8 +5,6 @@
 //   B  sequential lp2 + lp3 (shared-memory-column code path of the generic kernel, n <= 10)   vs  orc_lp2 / orc_lp3
 //   C  speculative lp1_all + lp2_scan (register path of the small-crowd kernel, n <= 5)        vs  orc_lp2
 //   D  lp3 as independent per-line sub-problems + lp3_outer_scan (the lane-parallel pass)      vs  orc_lp3
-//   F  lp3 on lanes: (i, j) pair projections + speculative per-line sub-problems (lp3_project_pair, lp3_sub_spec<4> and <9>)
-//      + lp3_outer_scan                                                                        vs  orc_lp3
 //   H  insert_sorted<10> (sorted register list of the crowd kernel, 20-60 candidates incl. ties) vs  orc_insert_neighbor
 //   E  neighbour_order (pair-wise ranks + packed indices of the small-crowd kernel)            vs  orc_insert_neighbor
 // Build (tests/test_native_cpu.py): nvcc -O2 --fmad=false -Xcompiler -ffp-contract=off -std=c++17 lp_fuzz.cu
@@ -15,7 +13,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <cstdint>
-#include <type_traits>
 #include "../../crowdnav_b200/csrc/orca_device.cuh"
 #include "../../crowdnav_b200/csrc/orca_spec.cuh"
 extern "C" {
@@ -50,27 +47,6 @@ static bool check_case(int n, const orc_line *ol, float radius, orc_v2 opt, long
         V2 rd = r;
         lp3_outer_scan(L, n, f, radius, rd, [&](int ii, V2 &r2) { r2 = sub_r[ii]; return sub_ok[ii]; });
         if (!same(rd.x, ores3.x) || !same(rd.y, ores3.y)) { printf("D lp3 sub-problem mismatch n=%d fail=%d\n", n, f); return false; }
-    }
-    // ---- F: the lane-parallel pass of the kernels: every (i, j) projection on its own, every sub-problem speculative ----
-    if (f < n) {
-        V2 sub_r[16]; bool sub_ok[16];
-        auto run = [&](auto kc) {
-            constexpr int K = decltype(kc)::value;
-            for (int i = 1; i < n; ++i) {
-                RegLines<K> Pr; bool pv[K];
-                for (int j = 0; j < K; ++j) {
-                    Pr.p[j] = mk(0.f, 0.f); Pr.d[j] = mk(0.f, 0.f); pv[j] = false;
-                    if (j < i) pv[j] = lp3_project_pair(L.point(i), L.dir(i), L.point(j), L.dir(j), Pr.p[j], Pr.d[j]);
-                }
-                sub_ok[i] = lp3_sub_spec<K>(Pr, pv, radius, L.dir(i), sub_r[i]);
-            }
-            V2 rd = r;
-            lp3_outer_scan(L, n, f, radius, rd, [&](int ii, V2 &r2) { r2 = sub_r[ii]; return sub_ok[ii]; });
-            return same(rd.x, ores3.x) && same(rd.y, ores3.y);
-        };
-        if (n <= 5 && !run(std::integral_constant<int, 4>())) { printf("F lane-parallel lp3 (K=4) mismatch n=%d fail=%d\n", n, f); return false; }
-        if (!run(std::integral_constant<int, 9>())) { printf("F lane-parallel lp3 (K=9) mismatch n=%d fail=%d\n", n, f); return false; }
-        cov[6]++;
     }
     // ---- C: speculative register path (n <= M) ----
     if (n <= M) {
@@ -133,7 +109,7 @@ static bool check_sorted_insert(long *cov)
     int nl = in_range < max_nb ? in_range : max_nb;
     if (nl != cnt) { printf("H count mismatch %d vs %d\n", nl, cnt); return false; }
     for (int k = 0; k < nl; ++k) if (tj[k] != ni[k] || !same(td[k], nd[k])) { printf("H order mismatch at %d (n=%d max_nb=%d)\n", k, n, max_nb); return false; }
-    cov[7] += 1;
+    cov[6] += 1;
     return true;
 }
 
@@ -141,9 +117,8 @@ int main(int argc, char **argv)
 {
     const long cases = argc > 1 ? atol(argv[1]) : 200000;
     rng_state = argc > 2 ? strtoull(argv[2], nullptr, 10) * 2654435761ull + 88172645463325252ull : 88172645463325252ull;
-    long cov[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    long cov[7] = {0, 0, 0, 0, 0, 0, 0};
     using namespace orca;
-    for (int i = 1, q = 0; i <= 9; ++i) for (int j = 0; j < i; ++j, ++q) { int a, b; lp3_pair_of(q, a, b); if (a != i || b != j) { printf("lp3_pair_of(%d)\n", q); return 1; } }
     for (long c = 0; c < cases; ++c) {
         const int kind = rnd() % 4;
         const int n = 1 + rnd() % ((kind == 3) ? 10 : 5);
@@ -162,12 +137,6 @@ int main(int argc, char **argv)
                 V2 lp, ld, sp, sd;
                 make_line(mk(p.x, p.y), mk(v.x, v.y), r, mk(po.x, po.y), mk(vo.x, vo.y), ro, 1.0f / 5.0f, 1.0f / 0.25f, lp, ld);
                 make_line_sel(mk(p.x, p.y), mk(v.x, v.y), r, mk(po.x, po.y), mk(vo.x, vo.y), ro, 1.0f / 5.0f, 1.0f / 0.25f, sp, sd);
-                {   // straight-line form + overlap repair (multi-step kernel)
-                    V2 fp, fd; bool ov;
-                    make_line_far(mk(p.x, p.y), mk(v.x, v.y), r, mk(po.x, po.y), mk(vo.x, vo.y), ro, 1.0f / 5.0f, fp, fd, ov);
-                    if (ov) make_line_overlap(mk(p.x, p.y), mk(v.x, v.y), r, mk(po.x, po.y), mk(vo.x, vo.y), ro, 1.0f / 0.25f, fp, fd);
-                    if (!same(fp.x, lp.x) || !same(fp.y, lp.y) || !same(fd.x, ld.x) || !same(fd.y, ld.y)) { printf("A far/overlap line mismatch\n"); return 1; }
-                }
                 if (!same(lp.x, ol[k].point.x) || !same(lp.y, ol[k].point.y) || !same(ld.x, ol[k].dir.x) || !same(ld.y, ol[k].dir.y) ||
                     !same(sp.x, lp.x) || !same(sp.y, lp.y) || !same(sd.x, ld.x) || !same(sd.y, ld.y)) { printf("A line mismatch\n"); return 1; }
                 const float dsq = po.x * po.x + po.y * po.y; cov[2] += (dsq <= (r + ro) * (r + ro));
@@ -184,10 +153,10 @@ int main(int argc, char **argv)
             }
         }
         if (!check_case<5>(n, ol, radius, opt, cov)) { printf("case %ld kind %d\n", c, kind); return 1; }
-        if (n > 5) { long dummy[8] = {0}; if (!check_case<10>(n, ol, radius, opt, dummy)) { printf("case %ld kind %d (M = 10)\n", c, kind); return 1; } cov[1] += dummy[1]; }
+        if (n > 5) { long dummy[7] = {0}; if (!check_case<10>(n, ol, radius, opt, dummy)) { printf("case %ld kind %d (M = 10)\n", c, kind); return 1; } cov[1] += dummy[1]; }
         if (!check_sorted_insert(cov)) { printf("case %ld\n", c); return 1; }
         if (!(check_order<5>(cov) && check_order<4>(cov) && check_order<2>(cov) && check_order<1>(cov))) { printf("case %ld\n", c); return 1; }
     }
-    printf("ok cases=%ld lp3_needed=%ld speculative_checked=%ld overlapping_pairs=%ld forced_parallel_lines=%ld neighbour_orders=%ld neighbour_ties=%ld lane_lp3_checked=%ld sorted_lists=%ld\n", cases, cov[0], cov[1], cov[2], cov[3], cov[4], cov[5], cov[6], cov[7]);
+    printf("ok cases=%ld lp3_needed=%ld speculative_checked=%ld overlapping_pairs=%ld forced_parallel_lines=%ld neighbour_orders=%ld neighbour_ties=%ld sorted_lists=%ld\n", cases, cov[0], cov[1], cov[2], cov[3], cov[4], cov[5], cov[6]);
     return 0;
 }
