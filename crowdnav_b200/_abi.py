@@ -116,6 +116,10 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
     f = getattr(lib, prefix + 'lookahead_pack')
     f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), C.c_void_p, C.c_int, C.c_int,
                                       C.c_void_p, C.c_void_p] + s
+    if hasattr(lib, prefix + 'propagate_pack'):
+        f = getattr(lib, prefix + 'propagate_pack')
+        f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p] + s
     return lib
 
 
@@ -123,7 +127,7 @@ EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_cou
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
            'crowdsim_step_n_record_ex', 'crowdsim_record_flush_ex',
            'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
-           'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
+           'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 
 # CROWDSIM_B200_LIB selects another build of the SAME library (A/B runs of kernel variants built into build_probe/);
 # it is never a fallback: the named file must exist.

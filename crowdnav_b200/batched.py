@@ -407,6 +407,27 @@ class BatchedCrowdSim(object):
         _abi.check(rc, 'crowdsim_lookahead_pack')
         return out_states, out_reward
 
+    def propagate_pack(self, actions, unicycle=False, order_by_distance=False, out_states=None, out_reward=None, out_pos=None,
+                       out_vel=None, out_order=None):
+        """The lookahead of a value-network policy with query_env = false (crowdsim_propagate_pack): actions [A][2] float64
+        device tensor -> (states [B][A][N][13] f32, reward [B][A] f64 of the policy's compute_reward, next human positions /
+        velocities [B][N][2] f64 and order [B][N] int32, all in row order: row i of env e is human order[e][i]).
+        order_by_distance: LSTM-RL's rows, by decreasing distance to the robot; otherwise env order. Nothing is mutated."""
+        B, N, A = self.B, self.human_num, actions.shape[0]
+        f = lambda t, shape, dtype: torch.empty(shape, dtype=dtype, device=self.device) if t is None else t  # noqa: E731
+        out_states = f(out_states, (B, A, N, 13), torch.float32)
+        out_reward = f(out_reward, (B, A), torch.float64)
+        out_pos = f(out_pos, (B, N, 2), torch.float64)
+        out_vel = f(out_vel, (B, N, 2), torch.float64)
+        out_order = f(out_order, (B, N), torch.int32)
+        prm = self.params(); st = self.state.struct()
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_propagate_pack(C.byref(prm), B, N, C.byref(st), _ptr(actions), A, int(unicycle),
+                                                  int(order_by_distance), _ptr(out_states), _ptr(out_reward), _ptr(out_pos),
+                                                  _ptr(out_vel), _ptr(out_order), self._stream())
+        _abi.check(rc, 'crowdsim_propagate_pack')
+        return out_states, out_reward, out_pos, out_vel, out_order
+
 
     def human_counts(self):
         """Humans present per env [B] (int64). Differs from human_num only for scenes of rule `mixed` (crowd_sim.py:103-151),

@@ -75,6 +75,20 @@ __device__ __forceinline__ double2 robot_velocity(bool unicycle, double &theta, 
     return make_double2(ax * cos(nth), ax * sin(nth));
 }
 
+// cadrl.py:104-129 CADRL.propagate(self_state, action): the robot's next position, velocity and heading as the policy
+// predicts them. A unicycle turns by r with NO % 2 pi (unlike robot_velocity) and moves by its new velocity times dt (unlike
+// robot_position's cos(th) * v * dt); a holonomic robot keeps theta.
+__device__ __forceinline__ void propagate_robot(bool unicycle, double2 pos, double theta, double ax, double ay, double dt,
+                                                double &npx, double &npy, double &nvx, double &nvy, double &nth)
+{
+    nth = theta;
+    if (!unicycle) { npx = pos.x + ax * dt; npy = pos.y + ay * dt; nvx = ax; nvy = ay; }
+    else {
+        nth = theta + ay; nvx = ax * cos(nth); nvy = ax * sin(nth);
+        npx = pos.x + nvx * dt; npy = pos.y + nvy * dt;
+    }
+}
+
 __device__ __forceinline__ double2 ld2(const double *p, size_t i) { return reinterpret_cast<const double2 *>(p)[i]; }
 __device__ __forceinline__ void st2(double *p, size_t i, double2 v) { reinterpret_cast<double2 *>(p)[i] = v; }
 __device__ __forceinline__ double2 ld2_cg(const double *p, size_t i) { return __ldcg(reinterpret_cast<const double2 *>(p) + i); }
@@ -131,6 +145,26 @@ __device__ __forceinline__ int reward_ladder(bool timeout, bool collision, bool 
         info = danger ? CROWDSIM_INFO_DANGER : CROWDSIM_INFO_NOTHING;
     }
     return info;
+}
+
+// multi_human_rl.py:65-88 MultiHumanRL.compute_reward(nav, humans), the reward of query_env = false: literal constants (not
+// env.config [reward]), no timeout rung, and the collision test is a point distance at the next positions, not the swept
+// segment. (npx, npy): the propagated robot; h_pos / h_rad: the N propagated humans. dist_i = norm((nav - h_i)) - nav.radius -
+// h_i.radius left to right; the fold stops at the first dist < 0, else dmin is the running minimum.
+__device__ __forceinline__ double policy_reward(double npx, double npy, double radius, double2 goal, const double2 *h_pos,
+                                                const double *h_rad, int N, double dt)
+{
+    double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
+    for (int i = 0; i < N; ++i) {
+        const double2 h = h_pos[i];
+        const double dist = norm2(npx - h.x, npy - h.y) - radius - h_rad[i];
+        if (dist < 0) { collision = true; break; }
+        if (dist < dmin) dmin = dist;
+    }
+    const bool reaching_goal = norm2(npx - goal.x, npy - goal.y) < radius;
+    if (collision) return -0.25;
+    if (reaching_goal) return 1.0;
+    return dmin < 0.2 ? (dmin - 0.2) * 0.5 * dt : 0.0;
 }
 
 // Timeout, Collision and ReachGoal end the episode; Danger and Nothing do not

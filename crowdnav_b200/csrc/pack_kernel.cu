@@ -8,6 +8,8 @@
 //                          agent.py:63-74), CADRL.propagate (cadrl.py:104-129) and rotate. The reference re-solves the N human
 //                          ORCA problems for every action although they do not depend on it; here they are solved once
 //                          per env (same lane mapping and staging as the step kernel) and shared by the A actions.
+// crowdsim_propagate_pack  the same loop with query_env=false: the humans are extrapolated at their own velocities and
+//                          the reward is the policy's compute_reward (multi_human_rl.py:35-45,65-88); no ORCA solve.
 //
 // Output rows are float32 like the reference's torch tensors; atan2f/cosf/sinf are CUDA's single-precision
 // functions (the reference's are torch CPU's), so parity on these rows is a 1e-5 tolerance, not bit-exact.
@@ -106,14 +108,10 @@ __global__ void __launch_bounds__(256) lookahead_kernel(const __grid_constant__ 
                 if (c < 0) { collision = true; break; } else if (c < dmin) dmin = c;
             }
             // cadrl.py:104-129 propagate(self_state, action); agent.py:110-120 compute_position for the goal test
-            double npx, npy, nvx, nvy, nth = tt.x, gpx, gpy;
-            if (!G.unicycle) { npx = rp.x + act.x * dt; npy = rp.y + act.y * dt; nvx = act.x; nvy = act.y; gpx = npx; gpy = npy; }
-            else {
-                nth = tt.x + act.y; nvx = act.x * cos(nth); nvy = act.x * sin(nth);
-                npx = rp.x + nvx * dt; npy = rp.y + nvy * dt;
-                gpx = rp.x + cos(nth) * act.x * dt; gpy = rp.y + sin(nth) * act.x * dt;
-            }
-            const bool reaching_goal = norm2(gpx - rg.x, gpy - rg.y) < ra.x;
+            double npx, npy, nvx, nvy, nth;
+            propagate_robot(G.unicycle, rp, tt.x, act.x, act.y, dt, npx, npy, nvx, nvy, nth);
+            const double2 gp = robot_position(G.unicycle, rp, tt.x, act.x, act.y, dt);
+            const bool reaching_goal = norm2(gp.x - rg.x, gp.y - rg.y) < ra.x;
             double reward;
             reward_ladder(tt.y >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
             G.out_reward[(size_t)e2 * A + kk] = reward;
@@ -138,6 +136,102 @@ __global__ void __launch_bounds__(256) lookahead_kernel(const __grid_constant__ 
     }
 }
 
+
+// ---- MultiHumanRL.predict with query_env = false (multi_human_rl.py:35-45): per action, CADRL.propagate of the robot, every
+// human propagated at its own velocity (cadrl.py:104-112), compute_reward (multi_human_rl.py:65-88) and rotate. One block per
+// env: the humans are read once and propagated once; LSTM-RL's row order is a rank by comparison (ties: lower index first,
+// = sorted(..., reverse=True)'s stability). The robot's propagate, rotate_self and the reward are computed once per (env,
+// action) for a tile of PP_TILE_ACTIONS actions; the tile's rows are assembled in a fixed-size shared-memory tile of whole
+// rows and written back with coalesced stores, so every N <= CROWDSIM_MAX_HUMANS and any A run. ----
+constexpr int PP_THREADS = 128;
+constexpr int PP_TILE_ACTIONS = PP_THREADS;
+constexpr int PP_TILE_ROWS = 472;                  // 472 x 13 floats = 24.5 KB
+
+struct PropArgs {
+    int B, N, A, unicycle, sort;
+    double dt;
+    crowdsim_state st;
+    const double *actions;
+    float *out_states;
+    double *out_reward, *next_pos, *next_vel;
+    int32_t *order;
+};
+
+// The robot's part of a rotated row for one action: position, heading column, and rotate_self's outputs.
+struct RobotRow { float px, py, th_out, dg, rvx, rvy, c, s; };
+
+__global__ void __launch_bounds__(PP_THREADS) propagate_pack_kernel(const __grid_constant__ PropArgs G)
+{
+    __shared__ double2 s_hpos[CROWDSIM_MAX_HUMANS];        // propagated humans, row order, float64 (reward)
+    __shared__ double s_hrad[CROWDSIM_MAX_HUMANS];
+    __shared__ double s_key[CROWDSIM_MAX_HUMANS];          // distance to the robot at the current positions
+    __shared__ float4 s_hrow[CROWDSIM_MAX_HUMANS];         // float32 casts of the propagated humans: px, py, vx, vy
+    __shared__ RobotRow s_rob[PP_TILE_ACTIONS];
+    __shared__ float tile[PP_TILE_ROWS * 13];
+
+    const int e = blockIdx.x, tid = threadIdx.x, N = G.N, A = G.A;
+    const double dt = G.dt;
+    const double2 rp = ld2(G.st.r_pos, e);
+    const bool human = tid < N;
+    double2 hp = make_double2(0, 0), hv = hp, ha = hp;
+    if (human) {
+        const size_t i = (size_t)e * N + tid;
+        hp = ld2(G.st.h_pos, i); hv = ld2(G.st.h_vel, i); ha = ld2(G.st.h_attr, i);
+        if (G.sort) s_key[tid] = norm2(hp.x - rp.x, hp.y - rp.y);    // lstm_rl.py:99-101
+    }
+    __syncthreads();
+    if (human) {
+        int row = tid;
+        if (G.sort) {
+            const double k = s_key[tid]; row = 0;
+            for (int j = 0; j < N; ++j) { const double kj = s_key[j]; row += (kj > k) || (kj == k && j < tid); }
+        }
+        const double2 np = make_double2(hp.x + hv.x * dt, hp.y + hv.y * dt);
+        s_hpos[row] = np; s_hrad[row] = ha.x;
+        s_hrow[row] = make_float4((float)np.x, (float)np.y, (float)hv.x, (float)hv.y);
+        const size_t o = (size_t)e * N + row;
+        if (G.next_pos) st2(G.next_pos, o, np);
+        if (G.next_vel) st2(G.next_vel, o, hv);
+        if (G.order) G.order[o] = tid;
+    }
+    __syncthreads();
+
+    const double2 rg = ld2(G.st.r_goal, e), ra = ld2(G.st.r_attr, e);
+    const double th = G.unicycle ? G.st.r_theta[e] : 0.0;
+    const float fra = (float)ra.x, fvp = (float)ra.y;
+    const int row_floats = N * 13;
+    for (int a0 = 0; a0 < A; a0 += PP_TILE_ACTIONS) {
+        const int na = min(PP_TILE_ACTIONS, A - a0);
+        if (tid < na) {
+            const double2 act = ld2(G.actions, a0 + tid);
+            double npx, npy, nvx, nvy, nth;
+            propagate_robot(G.unicycle, rp, th, act.x, act.y, dt, npx, npy, nvx, nvy, nth);
+            G.out_reward[(size_t)e * A + a0 + tid] = policy_reward(npx, npy, ra.x, rg, s_hpos, s_hrad, N, dt);
+            RobotRow r;
+            float rot;
+            r.px = (float)npx; r.py = (float)npy;
+            rotate_self(r.px, r.py, (float)nvx, (float)nvy, (float)rg.x, (float)rg.y, r.c, r.s, rot, r.dg, r.rvx, r.rvy);
+            r.th_out = G.unicycle ? ((float)nth - rot) : 0.f;
+            s_rob[tid] = r;
+        }
+        __syncthreads();
+        const int pairs = na * N;
+        float *dst0 = G.out_states + ((size_t)e * A + a0) * row_floats;
+        for (int p0 = 0; p0 < pairs; p0 += PP_TILE_ROWS) {
+            const int np = min(PP_TILE_ROWS, pairs - p0);
+            for (int q = tid; q < np; q += PP_THREADS) {
+                const int p = p0 + q, kk = p / N, i = p - kk * N;
+                const RobotRow r = s_rob[kk]; const float4 h = s_hrow[i];
+                rotate_row(tile + q * 13, r.px, r.py, fra, fvp, r.th_out, r.dg, r.rvx, r.rvy, r.c, r.s, h.x, h.y, h.z, h.w,
+                           (float)s_hrad[i]);
+            }
+            __syncthreads();
+            float *dst = dst0 + (size_t)p0 * 13;
+            for (int j = tid; j < np * 13; j += PP_THREADS) dst[j] = tile[j];
+            __syncthreads();
+        }
+    }
+}
 
 // ---- onestep_lookahead's observation (crowd_sim.py:414-416, agent.py:63-74): the humans' next observable states for the
 // CURRENT state, nothing mutated. Same staging and solver as the lookahead kernel. ----
@@ -218,6 +312,25 @@ extern "C" int crowdsim_lookahead_pack(const crowdsim_params *prm, int B, int N,
         if (err != cudaSuccess) return (int)err;
     }
     cs::lookahead_kernel<<<blocks, threads, smem, (cudaStream_t)stream>>>(G);
+    ++cs::g_launches;
+    return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_propagate_pack(const crowdsim_params *prm, int B, int N, const crowdsim_state *st,
+                                       const double *actions, int A, int kinematics_unicycle, int order_by_distance,
+                                       float *out_states, double *out_reward, double *next_h_pos, double *next_h_vel,
+                                       int32_t *order, void *stream)
+{
+    if (!prm || !st || !actions || !out_states || !out_reward || B < 0 || N < 1 || A < 1) return CROWDSIM_EINVAL;
+    if (N > CROWDSIM_MAX_HUMANS) return CROWDSIM_EUNSUPPORTED;
+    if (!st->h_pos || !st->h_vel || !st->h_attr || !st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr) return CROWDSIM_EINVAL;
+    if (kinematics_unicycle && !st->r_theta) return CROWDSIM_EINVAL;
+    if (B == 0) return CROWDSIM_OK;
+    cs::PropArgs G;
+    G.B = B; G.N = N; G.A = A; G.unicycle = kinematics_unicycle ? 1 : 0; G.sort = order_by_distance ? 1 : 0;
+    G.dt = prm->time_step; G.st = *st; G.actions = actions; G.out_states = out_states; G.out_reward = out_reward;
+    G.next_pos = next_h_pos; G.next_vel = next_h_vel; G.order = order;
+    cs::propagate_pack_kernel<<<B, cs::PP_THREADS, 0, (cudaStream_t)stream>>>(G);
     ++cs::g_launches;
     return (int)cudaGetLastError();
 }

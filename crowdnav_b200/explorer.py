@@ -9,7 +9,8 @@ reference does (explorer.py:74-90).
 
 Robot policies:
   'orca'            the robot's ORCA solve is fused into the step kernel (test.py --policy orca)
-  a policy object   anything with .act_batch(env) -> [B][2] float64 device tensor of ActionXY (policy.make_sarl() ...)
+  a policy object   anything with .act_batch(env) -> [B][2] float64 device tensor of ActionXY (policy.make_sarl() ...), or
+                    of ActionRot (v, r) when its .kinematics is 'unicycle' (the env then steps external_rot)
 With update_memory=True the rollout also fills a memory.DeviceReplayMemory like Explorer.update_memory does
 (explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot
 (train.py:116-132's IL phase) records on device at every crowd size, with occupancy-map rows when the target policy has
@@ -152,10 +153,11 @@ class BatchedExplorer(object):
         rule = env.test_sim if phase == 'test' else env.train_val_sim
         env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
         env.enable_autoreset(rule)
+        unicycle = self.robot_policy != 'orca' and getattr(self.robot_policy, 'kinematics', 'holonomic') == 'unicycle'
         if self.robot_policy == 'orca':
             env.set_robot_policy('orca')
         else:
-            env.set_robot_policy('external_xy')
+            env.set_robot_policy('external_rot' if unicycle else 'external_xy')
         env.reset_seeds(rule=rule, use_queue=True)
         recorder = dev_rec = None
         chunk = max(1, int(steps_per_launch))
@@ -171,7 +173,8 @@ class BatchedExplorer(object):
                 dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om)
                 dev_rec.begin()
             else:
-                recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om)
+                recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om,
+                                              unicycle=unicycle)
         side = torch.cuda.Stream(device=env.device)
         main = torch.cuda.current_stream(env.device)
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per

@@ -56,10 +56,12 @@ class DeviceReplayMemory(object):
 
 
 class TrajectoryRecorder(object):
-    def __init__(self, env, memory, gamma, imitation_learning=True, target_model=None, max_steps=None, om=None):
+    def __init__(self, env, memory, gamma, imitation_learning=True, target_model=None, max_steps=None, om=None, unicycle=False):
         """om = None or (cell_num, cell_size, om_channel_size): append the occupancy maps of the current human states to
-        every recorded row, as MultiHumanRL.transform does with with_om (multi_human_rl.py:98-104)."""
+        every recorded row, as MultiHumanRL.transform does with with_om (multi_human_rl.py:98-104). unicycle: the rows of a
+        unicycle robot (pack_joint's theta column, cadrl.py:205-209)."""
         self.env, self.memory = env, memory
+        self.unicycle = bool(unicycle)
         self.om = om
         F = 13 + (om[0] * om[0] * om[2] if om else 0)
         self.il, self.target_model = imitation_learning, target_model
@@ -82,7 +84,7 @@ class TrajectoryRecorder(object):
         env = self.env
         self._t = env.episodes.ep_steps.long().clamp_(max=self.T - 1)
         self._live = env.state.active.bool()
-        packed = env.pack_joint()
+        packed = env.pack_joint(unicycle=self.unicycle)
         if self.om:
             packed = torch.cat([packed, env.occupancy_maps(None, None, *self.om)], dim=2)
         rows = torch.arange(env.B, device=env.device)

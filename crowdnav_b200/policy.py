@@ -127,16 +127,27 @@ class BatchedValuePolicy(object):
         argmax_a  reward(s, a) + gamma ** (time_step * v_pref) * V(rotate(next_state(s, a)))       multi_human_rl.py:52
     or the zero action when the robot already is within its radius of the goal (policy.py:41-48).
     `joint` selects how humans enter the network: True = one [N][13] set per action (SARL, LSTM-RL, multi_human_rl.py:45),
-    False = CADRL's min over per-human values (cadrl.py:163-166)."""
+    False = CADRL's min over per-human values (cadrl.py:163-166).
+    query_env (policy.config [action_space]): True asks the simulator (env.onestep_lookahead: lookahead_pack, the humans' ORCA
+    decisions and the env's reward); False extrapolates every human at its own velocity and uses the policy's compute_reward
+    (multi_human_rl.py:38-42: propagate_pack). CADRL always queries the env (cadrl.py:156-170), so joint=False with
+    query_env=False is refused. order_by_distance: with query_env=False the rows follow LSTM-RL's sort by decreasing
+    distance to the robot (lstm_rl.py:99-103). kinematics 'holonomic' or 'unicycle': the action space of
+    build_action_space and the robot's propagate; the env's robot must step the same kinematics (external_xy / external_rot)."""
 
     name = 'BatchedValuePolicy'
-    kinematics = 'holonomic'
     trainable = True
     multiagent_training = True
 
     def __init__(self, model, gamma=0.9, v_pref=1.0, time_step=0.25, joint=True, speed_samples=5, rotation_samples=16,
-                 with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3):
+                 with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3, query_env=True, kinematics='holonomic',
+                 order_by_distance=False):
+        if kinematics not in ('holonomic', 'unicycle'):
+            raise ValueError('kinematics must be holonomic or unicycle, not %r' % (kinematics,))
+        if not joint and not query_env:
+            raise ValueError('CADRL always queries the env (cadrl.py:156-170): query_env=False needs a joint policy')
         self.model = model
+        self.query_env, self.kinematics, self.order_by_distance = bool(query_env), kinematics, bool(order_by_distance)
         # policy.config [om] + with_om: occupancy maps of the NEXT human states are appended to every row
         # (multi_human_rl.py:46-49; they do not depend on the action, so they are built once per env and broadcast)
         self.with_om = with_om
@@ -144,7 +155,7 @@ class BatchedValuePolicy(object):
         self.gamma = gamma
         self.v_pref, self.time_step = v_pref, time_step
         self.joint = joint
-        self.action_space_np = build_action_space(v_pref, speed_samples, rotation_samples)
+        self.action_space_np = build_action_space(v_pref, speed_samples, rotation_samples, kinematics)
         self.actions = None
         self.device = None
         self.phase = 'test'
@@ -152,7 +163,7 @@ class BatchedValuePolicy(object):
         self._gen = None; self._seed = 0
         self.action_values = None
         self.explored = None                 # [B] bool: which envs took a random action in the last act_batch (train phase)
-        self._buf_states = None; self._buf_reward = None
+        self._buf_states = None; self._buf_reward = None; self._buf_next = None
 
     def set_device(self, device):
         self.device = torch.device(device)
@@ -182,13 +193,24 @@ class BatchedValuePolicy(object):
         if self._buf_states is None or self._buf_states.shape[0] != B:
             self._buf_states = torch.empty((B, A, N, 13), dtype=torch.float32, device=self.device)
             self._buf_reward = torch.empty((B, A), dtype=torch.float64, device=self.device)
-        states, reward = env.lookahead_pack(self.actions, out_states=self._buf_states, out_reward=self._buf_reward)
+        unicycle = self.kinematics == 'unicycle'
+        if self.query_env:
+            uni = {'unicycle': True} if unicycle else {}              # holonomic: lookahead_pack's default, the call as before
+            states, reward = env.lookahead_pack(self.actions, out_states=self._buf_states, out_reward=self._buf_reward, **uni)
+        else:
+            if self._buf_next is None or self._buf_next[0].shape[0] != B:
+                self._buf_next = (torch.empty((B, N, 2), dtype=torch.float64, device=self.device),
+                                  torch.empty((B, N, 2), dtype=torch.float64, device=self.device),
+                                  torch.empty((B, N), dtype=torch.int32, device=self.device))
+            states, reward, npos, nvel, _ = env.propagate_pack(self.actions, unicycle, self.order_by_distance, self._buf_states,
+                                                               self._buf_reward, *self._buf_next)
         # multi_human_rl.py:52: pow(gamma, time_step * state.self_state.v_pref) -- the robot's v_pref of THIS env
         discount = torch.pow(torch.full((B,), float(self.gamma), dtype=torch.float64, device=self.device),
                              self.time_step * env.state.r_attr[:, 1]).unsqueeze(1)
         F = 13
         if self.with_om:
-            npos, nvel = env.lookahead_humans()
+            if self.query_env:
+                npos, nvel = env.lookahead_humans()
             om = env.occupancy_maps(npos, nvel, *self.om)                # [B][N][cells * channels]
             states = torch.cat([states, om.unsqueeze(1).expand(B, A, N, om.shape[2])], dim=3)
             F = states.shape[3]
@@ -215,7 +237,7 @@ class BatchedValuePolicy(object):
 
 
 def make_sarl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_om=False, cell_num=4, cell_size=1.0,
-              om_channel_size=3, **net_kw):
+              om_channel_size=3, query_env=True, kinematics='holonomic', **net_kw):
     """SARL with the reference's default architecture (crowd_nav/configs/policy.config:43-50); random-init weights when
     no checkpoint is loaded (there are no checkpoints in the reference repo). with_om=True gives OM-SARL: input_dim grows
     by cell_num^2 * om_channel_size (multi_human_rl.py:106-107)."""
@@ -224,26 +246,31 @@ def make_sarl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_om=False, c
     if with_om:
         net_kw.setdefault('input_dim', 13 + cell_num * cell_num * om_channel_size)
     p = BatchedValuePolicy(SARLValueNetwork(**net_kw), gamma, v_pref, time_step, joint=True, with_om=with_om,
-                           cell_num=cell_num, cell_size=cell_size, om_channel_size=om_channel_size)
+                           cell_num=cell_num, cell_size=cell_size, om_channel_size=om_channel_size, query_env=query_env,
+                           kinematics=kinematics)
     p.name = 'OM-SARL' if with_om else 'SARL'
     return p
 
 
-def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None):
+def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='holonomic'):
+    """CADRL queries the env whatever policy.config's query_env says (cadrl.py:156-170), so there is no query_env here."""
     if seed is not None:
         torch.manual_seed(seed)
-    p = BatchedValuePolicy(CADRLValueNetwork(), gamma, v_pref, time_step, joint=False)
+    p = BatchedValuePolicy(CADRLValueNetwork(), gamma, v_pref, time_step, joint=False, kinematics=kinematics)
     p.name = 'CADRL'
     p.multiagent_training = False
     return p
 
 
-def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interaction_module=False):
-    """LSTM-RL with the reference's default sizes (crowd_nav/configs/policy.config:24-31)."""
+def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interaction_module=False, query_env=True,
+                 kinematics='holonomic'):
+    """LSTM-RL with the reference's default sizes (crowd_nav/configs/policy.config:24-31). With query_env=False its rows
+    follow the reference's sort of the humans by decreasing distance to the robot (lstm_rl.py:99-103)."""
     if seed is not None:
         torch.manual_seed(seed)
     net = LSTMRLValueNetwork(mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
                              mlp1_dims=(150, 100, 100, 50) if with_interaction_module else None)
-    p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True)
+    p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True, query_env=query_env, kinematics=kinematics,
+                           order_by_distance=not query_env)
     p.name = 'LSTM-RL'
     return p

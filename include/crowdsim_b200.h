@@ -28,6 +28,8 @@
  *   crowdsim_lookahead_pack  crowd_nav/policy/multi_human_rl.py:35-45 = 81 x env.onestep_lookahead
  *                            (crowd_sim.py:314-315,414-416) + CADRL.propagate (cadrl.py:104-129) +
  *                            CADRL.rotate (cadrl.py:187-222), fused
+ *   crowdsim_propagate_pack  the same loop with query_env=false: CADRL.propagate of the robot and of every human at its
+ *                            own velocity, MultiHumanRL.compute_reward (multi_human_rl.py:65-88), rotate, fused
  *   crowdsim_pack_joint      crowd_sim/envs/utils/state.py:17-18,36-37 (14-tuple) + cadrl.py:187-222 (rotate)
  *   crowdsim_lookahead_humans  the observation of env.onestep_lookahead (crowd_sim.py:314-315,414-416; agent.py:63-74)
  *   crowdsim_occupancy_maps  crowd_nav/policy/multi_human_rl.py:109-163 (MultiHumanRL.build_occupancy_maps)
@@ -374,6 +376,24 @@ int crowdsim_lookahead_pack(const crowdsim_params *prm, int B, int N, const crow
  */
 int crowdsim_lookahead_humans(const crowdsim_params *prm, int B, int N, const crowdsim_state *st,
                               double *next_h_pos, double *next_h_vel, void *stream);
+
+/*
+ * One-step lookahead without asking the simulator (multi_human_rl.py:35-45 with query_env=false): for each of A robot
+ * actions, CADRL.propagate of the robot (cadrl.py:104-129; unicycle: theta + r with no % 2 pi), every human extrapolated
+ * at its current velocity (no ORCA solve), the policy's own compute_reward (multi_human_rl.py:65-88: literal constants
+ * -0.25 / 1 / (dmin - 0.2) * 0.5 * dt, point distances at the next positions, no timeout; only prm->time_step is read).
+ *   out_states [B][A][N][13] float32  rotate(next_self_state + next_human_state), rows in row order
+ *   out_reward [B][A]        float64
+ *   next_h_pos, next_h_vel [B][N][2] float64 the extrapolated humans in row order (NULL: not written)
+ *   order      [B][N] int32  row i of env e is human order[e][i] (NULL: not written)
+ * order_by_distance: rows in LSTM-RL's order (lstm_rl.py:99-103), decreasing distance to the robot at the current
+ * positions, stable among equal distances; otherwise env order. Reads h_pos, h_vel, h_attr, r_pos, r_vel, r_goal, r_attr
+ * and r_theta (unicycle only). Nothing is mutated. Any 1 <= N <= CROWDSIM_MAX_HUMANS and A >= 1.
+ */
+int crowdsim_propagate_pack(const crowdsim_params *prm, int B, int N, const crowdsim_state *st,
+                            const double *actions, int A, int kinematics_unicycle, int order_by_distance,
+                            float *out_states, double *out_reward, double *next_h_pos, double *next_h_vel,
+                            int32_t *order, void *stream);
 
 /*
  * Occupancy maps of MultiHumanRL.build_occupancy_maps (multi_human_rl.py:109-163; policy.config [om] cell_num,

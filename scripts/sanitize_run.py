@@ -3,7 +3,8 @@
    compute-sanitizer --tool racecheck python scripts/sanitize_run.py
 Covers: small-crowd step kernel (per-warp and per-block lp3 queue), multi-step kernel with auto-reset and a CONCURRENT scene
 prefetch on a side stream (the release / acquire slot hand-over), crowd kernel (N = 12), generic kernel, scene generation,
-lookahead pack / humans / onestep_lookahead, occupancy maps, human_times, the recording multi-step kernel with its flush
+lookahead pack / humans / onestep_lookahead, propagate pack (query_env = false; N = 63 and 200 actions: several action and
+row tiles), occupancy maps, human_times, the recording multi-step kernel with its flush
 (crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps, and both routes of
 crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
 at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush)."""
@@ -72,9 +73,12 @@ for N, om in ((1, None), (20, None), (5, (4, 1.0, 3))):
 env = make(64, 5, policy='external_xy'); env.reset_seeds(torch.arange(64) + 1000)
 acts = torch.tensor([[0.0, 0.0], [1.0, 0.0], [0.0, 1.0]], dtype=torch.float64, device=env.device)
 env.lookahead_pack(acts); env.lookahead_humans(); env.pack_joint(); env.occupancy_maps()
+env.propagate_pack(acts, unicycle=True, order_by_distance=True)
 env.onestep_lookahead(torch.zeros((64, 2), dtype=torch.float64, device=env.device))
 env.human_times(max_steps=60)
 env = make(16, 20, policy='external_xy', rule='square_crossing'); env.reset_seeds(torch.arange(16) + 1000, rule='square_crossing')
 env.lookahead_pack(acts); env.human_times(max_steps=20)
+env = make(3, 63, policy='external_xy', rule='square_crossing'); env.reset_seeds(torch.arange(3) + 1000, rule='square_crossing')
+env.propagate_pack(torch.rand((200, 2), dtype=torch.float64, device=env.device), order_by_distance=True)   # several tiles
 torch.cuda.synchronize()
 print('sanitize run done, launches:', lib.crowdsim_launch_count())
