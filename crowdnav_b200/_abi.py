@@ -84,6 +84,11 @@ class RecordMaps(C.Structure):
                 ('channels', C.c_int32), ('cell_size', C.c_double)]
 
 
+class RecordRL(C.Structure):
+    """crowdsim_record_rl: the target network's values of the staged rows for crowdsim_record_flush_rl."""
+    _fields_ = [('boot', C.c_void_p), ('traj_boot', C.c_void_p), ('gamma_bar', C.c_double)]
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
     """Attach argtypes/restype for the compute entry points (shared by product and oracle libs)."""
     s = [C.c_void_p] if with_stream else []
@@ -105,6 +110,14 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
                                           P(Record), P(RecordMaps)] + s
         f = getattr(lib, prefix + 'record_flush_ex')
         f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), C.c_int] + s
+    if hasattr(lib, prefix + 'record_flush_rl'):
+        f = getattr(lib, prefix + 'record_book')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(Record), P(RecordMaps),
+                                          C.c_int, C.c_int] + s
+        f = getattr(lib, prefix + 'record_flush_maps')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), C.c_int] + s
+        f = getattr(lib, prefix + 'record_flush_rl')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), P(RecordRL), C.c_int] + s
     f = getattr(lib, prefix + 'prefetch_scenes')
     f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(AutoReset)] + s
     f = getattr(lib, prefix + 'orca_act')
@@ -125,8 +138,8 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
 
 EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_count', 'crowdsim_debug_force_generic', 'crowdsim_graph_launch',
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
-           'crowdsim_step_n_record_ex', 'crowdsim_record_flush_ex',
-           'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
+           'crowdsim_step_n_record_ex', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
+           'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
            'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 
 # CROWDSIM_B200_LIB selects another build of the SAME library (A/B runs of kernel variants built into build_probe/);

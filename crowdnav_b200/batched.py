@@ -322,7 +322,12 @@ class BatchedCrowdSim(object):
         record: a memory.DeviceILRecorder -- the same steps through crowdsim_step_n_record_ex (one launch for any n_steps
         at 2 <= N <= 5, the launch loop with its recording otherwise), then crowdsim_record_flush_ex of their
         imitation-learning pairs (with occupancy maps when the recorder has them) into the recorder's memory. Needs an ORCA
-        robot, episode tracking and auto-reset (ValueError otherwise)."""
+        robot, episode tracking and auto-reset (ValueError otherwise).
+        record: a memory.DeviceRLRecorder -- with an ORCA robot the same n_steps steps through crowdsim_step_n_record_ex
+        (no actions); with an external robot one step with `actions` (n_steps = 1), booked around it by crowdsim_record_book
+        and its rows staged by pack_joint. The recorder flushes its reinforcement-learning pairs when its staging is full."""
+        if record is not None and getattr(record, 'rl', False):
+            return self._step_record_rl(actions, int(n_steps), record)
         if record is not None:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
@@ -364,6 +369,50 @@ class BatchedCrowdSim(object):
                                               C.byref(ep) if ep is not None else None, C.byref(ar) if ar is not None else None,
                                               int(n_steps), self._stream())
         _abi.check(rc, 'crowdsim_step')
+        return self.observation(), self.reward, self.done, self.info
+
+    def _step_record_rl(self, actions, n_steps, record):
+        """step(actions, n_steps, record=DeviceRLRecorder): stage the steps at the recorder's next free staging slots."""
+        ep = self.episodes.struct() if self.episodes is not None else None
+        if ep is None or self.autoreset is None:
+            raise ValueError('a recorded rollout needs episode tracking and auto-reset')
+        io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
+                         _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
+        if self.robot_policy == _abi.ROBOT_ORCA:
+            if actions is not None:
+                raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
+            if not 1 <= n_steps <= record.n_max:
+                raise ValueError('n_steps must be between 1 and the recorder\'s n_max')
+            if record.s + n_steps > record.n_max:
+                record.flush()
+            rec, maps = record.struct(record.s), record.maps_struct(record.s)
+            prm = self.params(); st = self.state.struct(); ar = self.autoreset.struct()
+            with torch.cuda.device(self.device):
+                rc = self.lib.crowdsim_step_n_record_ex(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
+                                                        C.byref(ep), C.byref(ar), n_steps, C.byref(rec),
+                                                        C.byref(maps) if maps is not None else None, self._stream())
+            _abi.check(rc, 'crowdsim_step_n_record_ex')
+            record.staged(n_steps)
+            return self.observation(), self.reward, self.done, self.info
+        if actions is None:
+            raise ValueError('robot policy is external: actions required')
+        if n_steps != 1:
+            raise ValueError('an external robot records one step per call')
+        s = record.s
+        rec, maps = record.struct(), record.maps_struct()
+        mp = C.byref(maps) if maps is not None else None
+        st = self.state.struct()
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
+                                               -1, s, self._stream())
+        _abi.check(rc, 'crowdsim_record_book')
+        self.pack_joint(unicycle=record.unicycle, out=record.rows[s])       # TrajectoryRecorder.before_step's rows
+        self.step(actions)
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
+                                               s, -1, self._stream())
+        _abi.check(rc, 'crowdsim_record_book')
+        record.staged(1)
         return self.observation(), self.reward, self.done, self.info
 
     def step_n(self, n_steps):

@@ -6,6 +6,11 @@
 //   crowdsim_record_flush  one launch's staging -> per-slot trajectories -> (state, value) pairs of the replay memory ring
 //   crowdsim_record_flush_ex  the same, optionally with occupancy-map rows: record_maps_kernel computes the map of every
 //                        staged (step, env) first (occupancy.cuh, the code of crowdsim_occupancy_maps)
+//   crowdsim_record_book  the launch loop's booking without its rows (record_book_kernel), for robots stepped with external
+//                        actions, whose rows the caller stages with crowdsim_pack_joint
+//   crowdsim_record_flush_maps, crowdsim_record_flush_rl  the flush with reinforcement-learning values (explorer.py:107-113): the
+//                        maps on their own first, so that the caller's target network and the ring see the same map; then
+//                        the scan and record_copy_rl_kernel / record_copy_om_rl_kernel with the caller's boot values
 //
 // Replaces Explorer.update_memory with imitation_learning=True (crowd_nav/utils/explorer.py:92-105) for the episodes of
 // explorer.py:66-69 that are stored (ReachGoal, Collision), and ReplayMemory.push (crowd_nav/utils/memory.py:13-19). The
@@ -48,7 +53,10 @@ int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream)
 //              crowdsim_pack_joint), its episode step and LIVE, and with occupancy maps its humans' float64 state; every
 //              other env stages NONE.
 // The two touch different steps' staging, so one launch serves post(s) and pre(s + 1).
-__global__ void __launch_bounds__(128) record_between_kernel(const __grid_constant__ StepArgs A, int post, int pre)
+// ROWS = false (crowdsim_record_book, robots stepped with external actions): the same booking without rec_row, whose rows
+// carry only the holonomic theta column; the caller stages the rows with crowdsim_pack_joint.
+template <bool ROWS>
+__device__ __forceinline__ void record_between(const StepArgs &A, int post, int pre)
 {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (size_t)A.B * A.N) return;
@@ -68,13 +76,26 @@ __global__ void __launch_bounds__(128) record_between_kernel(const __grid_consta
             if (live) A.rec.t[ri] = A.ep.ep_steps[e];
         }
         if (live) {
-            const double2 hp = ld2(A.st.h_pos, idx), hv = ld2(A.st.h_vel, idx), ha = ld2(A.st.h_attr, idx);
-            const double2 ra = ld2(A.st.r_attr, e);
-            rec_row(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e), ra.x,
-                    (float)ra.y);
+            const double2 hp = ld2(A.st.h_pos, idx), hv = ld2(A.st.h_vel, idx);
+            if constexpr (ROWS) {
+                const double2 ha = ld2(A.st.h_attr, idx);
+                const double2 ra = ld2(A.st.r_attr, e);
+                rec_row(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e), ra.x,
+                        (float)ra.y);
+            }
             if (A.recm.h_pos) rec_map_state(A.recm, A.B, N, pre, e, a, hp, hv);
         }
     }
+}
+
+__global__ void __launch_bounds__(128) record_between_kernel(const __grid_constant__ StepArgs A, int post, int pre)
+{
+    record_between<true>(A, post, pre);
+}
+
+__global__ void __launch_bounds__(128) record_book_kernel(const __grid_constant__ StepArgs A, int post, int pre)
+{
+    record_between<false>(A, post, pre);
 }
 
 void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream)
@@ -134,9 +155,15 @@ __global__ void __launch_bounds__(1024) record_scan_kernel(const __grid_constant
     }
 }
 
+// crowdsim_record_flush_rl: the target network's value of every staged (step, env) and the per-slot copies of it.
+struct FlushRLArgs { FlushArgs f; crowdsim_record_rl rl; };
+
 // OM = false: rows of 13 floats. OM = true: rows of W = 13 + M floats, each human's staged row followed by its map.
-template <bool OM>
-__device__ __forceinline__ void record_copy(const FlushArgs &F)
+// RL = false: IL values from rec.g. RL = true (crowdsim_record_flush_rl): each live step also keeps its boot at t, and a
+// stored episode's pair i gets r_i + gamma_bar * boot_{i+1}, or r_{L-1} + 0.0 at its last step, as TrajectoryRecorder's
+// float64 torch ops round them (one rounding per product and sum), then cast to float32.
+template <bool OM, bool RL = false>
+__device__ __forceinline__ void record_copy(const FlushArgs &F, const crowdsim_record_rl *rl = nullptr)
 {
     const int e = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int M = OM ? F.m.cell_num * F.m.cell_num * F.m.channels : 0, W = 13 + M;
@@ -163,16 +190,24 @@ __device__ __forceinline__ void record_copy(const FlushArgs &F)
             const float *row = F.r.rows + i * R;
             for (int j = tid; j < R; j += nt) traj[(size_t)t * R + j] = row[j];
         }
-        if (tid == 0) trew[t] = F.r.reward[i];
+        if (tid == 0) {
+            trew[t] = F.r.reward[i];
+            if constexpr (RL) rl->traj_boot[(size_t)e * T + t] = rl->boot[i];
+        }
         __syncthreads();
         if (code == CROWDSIM_REC_STORED) {
             const int L = t + 1;
             const long long off = F.r.scan[i];
             for (int q = tid; q < L; q += nt) {
                 if (off + q < first) continue;
-                double G = 0.0;
-                for (int u = q; u < L; ++u) G = __dadd_rn(G, __dmul_rn(F.r.g[u - q], trew[u]));
-                F.r.mem_values[(pos0 + off + q) % cap] = (float)G;
+                if constexpr (RL) {
+                    const double b = (q < L - 1) ? __dmul_rn(rl->gamma_bar, (double)rl->traj_boot[(size_t)e * T + q + 1]) : 0.0;
+                    F.r.mem_values[(pos0 + off + q) % cap] = (float)__dadd_rn(trew[q], b);
+                } else {
+                    double G = 0.0;
+                    for (int u = q; u < L; ++u) G = __dadd_rn(G, __dmul_rn(F.r.g[u - q], trew[u]));
+                    F.r.mem_values[(pos0 + off + q) % cap] = (float)G;
+                }
             }
             for (int j = tid; j < L * R; j += nt) {
                 const int q = j / R;
@@ -186,33 +221,96 @@ __device__ __forceinline__ void record_copy(const FlushArgs &F)
 
 __global__ void __launch_bounds__(128) record_copy_kernel(const __grid_constant__ FlushArgs F) { record_copy<false>(F); }
 __global__ void __launch_bounds__(128) record_copy_om_kernel(const __grid_constant__ FlushArgs F) { record_copy<true>(F); }
+__global__ void __launch_bounds__(128) record_copy_rl_kernel(const __grid_constant__ FlushRLArgs F) { record_copy<false, true>(F.f, &F.rl); }
+__global__ void __launch_bounds__(128) record_copy_om_rl_kernel(const __grid_constant__ FlushRLArgs F) { record_copy<true, true>(F.f, &F.rl); }
+
+// The argument rules of the flushes (include/crowdsim_b200.h), all decided before any CUDA call. rec->g only for IL values.
+static int check_flush(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps, bool need_g)
+{
+    if (!rec || B < 0 || N < 1 || n_steps < 1 || n_steps > rec->n_max || rec->T < 1 || rec->capacity < 1) return CROWDSIM_EINVAL;
+    if (!rec->rows || !rec->reward || !rec->t || !rec->code || !rec->traj_rows || !rec->traj_reward || (need_g && !rec->g) ||
+        !rec->mem_states || !rec->mem_values || !rec->pushed || !rec->scan) return CROWDSIM_EINVAL;
+    if (rec->position0 < 0 || rec->position0 >= rec->capacity) return CROWDSIM_EINVAL;
+    return check_record_maps(N, maps);
+}
+
+// The map of every staged (step, env) of n_steps from the staged float64 human state (the first launch of a flush with maps).
+static void launch_record_maps(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
+                               cudaStream_t stream)
+{
+    OmArgs G; G.B = n_steps * B; G.N = N; G.cell_num = maps->cell_num; G.channels = maps->channels;
+    G.cell_size = maps->cell_size; G.pos = maps->h_pos; G.vel = maps->h_vel; G.out = maps->maps;
+    const size_t n = (size_t)n_steps * B * N;
+    record_maps_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(G, rec->code);
+    ++g_launches;
+}
 
 }  // namespace cs
 
 extern "C" int crowdsim_record_flush_ex(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
                                         void *stream)
 {
-    if (!rec || B < 0 || N < 1 || n_steps < 1 || n_steps > rec->n_max || rec->T < 1 || rec->capacity < 1) return CROWDSIM_EINVAL;
-    if (!rec->rows || !rec->reward || !rec->t || !rec->code || !rec->traj_rows || !rec->traj_reward || !rec->g ||
-        !rec->mem_states || !rec->mem_values || !rec->pushed || !rec->scan) return CROWDSIM_EINVAL;
-    if (rec->position0 < 0 || rec->position0 >= rec->capacity) return CROWDSIM_EINVAL;
-    const int rc = cs::check_record_maps(N, maps);
+    const int rc = cs::check_flush(B, N, rec, maps, n_steps, true);
     if (rc != CROWDSIM_OK) return rc;
     if (B == 0) return CROWDSIM_OK;
     cs::FlushArgs F; F.B = B; F.N = N; F.n = n_steps; F.r = *rec;
     if (maps) F.m = *maps; else memset(&F.m, 0, sizeof(F.m));
     cs::record_scan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(F);
     if (maps) {
-        cs::OmArgs G; G.B = n_steps * B; G.N = N; G.cell_num = maps->cell_num; G.channels = maps->channels;
-        G.cell_size = maps->cell_size; G.pos = maps->h_pos; G.vel = maps->h_vel; G.out = maps->maps;
-        const size_t n = (size_t)n_steps * B * N;
-        cs::record_maps_kernel<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(G, rec->code);
+        cs::launch_record_maps(B, N, rec, maps, n_steps, (cudaStream_t)stream);
         cs::record_copy_om_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
-        cs::g_launches += 3;
+        cs::g_launches += 2;
     } else {
         cs::record_copy_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
         cs::g_launches += 2;
     }
+    return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_record_flush_maps(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
+                                    void *stream)
+{
+    if (!maps) return CROWDSIM_EINVAL;
+    const int rc = cs::check_flush(B, N, rec, maps, n_steps, false);
+    if (rc != CROWDSIM_OK) return rc;
+    if (B == 0) return CROWDSIM_OK;
+    cs::launch_record_maps(B, N, rec, maps, n_steps, (cudaStream_t)stream);
+    return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_record_flush_rl(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps,
+                                        const crowdsim_record_rl *rl, int n_steps, void *stream)
+{
+    const int rc = cs::check_flush(B, N, rec, maps, n_steps, false);
+    if (rc != CROWDSIM_OK) return rc;
+    if (!rl || !rl->boot || !rl->traj_boot) return CROWDSIM_EINVAL;
+    if (B == 0) return CROWDSIM_OK;
+    cs::FlushRLArgs F; F.f.B = B; F.f.N = N; F.f.n = n_steps; F.f.r = *rec; F.rl = *rl;
+    if (maps) F.f.m = *maps; else memset(&F.f.m, 0, sizeof(F.f.m));
+    cs::record_scan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(F.f);
+    if (maps) cs::record_copy_om_rl_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
+    else cs::record_copy_rl_kernel<<<B, 128, 0, (cudaStream_t)stream>>>(F);
+    cs::g_launches += 2;
+    return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_record_book(int B, int N, const crowdsim_state *st, const crowdsim_step_io *io, const crowdsim_episodes *ep,
+                                    const crowdsim_record *rec, const crowdsim_record_maps *maps, int post, int pre, void *stream)
+{
+    if (!st || !io || !ep || !rec || B < 0) return CROWDSIM_EINVAL;
+    if (N < 1 || N > CROWDSIM_MAX_HUMANS) return CROWDSIM_EUNSUPPORTED;
+    if (post < -1 || pre < -1 || post >= rec->n_max || pre >= rec->n_max) return CROWDSIM_EINVAL;
+    if (!rec->reward || !rec->t || !rec->code || !io->reward || !io->done || !io->info || !st->active || !st->h_pos ||
+        !st->h_vel || !ep->ep_steps) return CROWDSIM_EINVAL;
+    const int rc = cs::check_record_maps(N, maps);
+    if (rc != CROWDSIM_OK) return rc;
+    if (B == 0 || (post < 0 && pre < 0)) return CROWDSIM_OK;
+    cs::StepArgs A; memset(&A, 0, sizeof(A));
+    A.B = B; A.N = N; A.st = *st; A.io = *io; A.ep = *ep; A.rec = *rec;
+    if (maps) A.recm = *maps;
+    const size_t n = (size_t)B * N;
+    cs::record_book_kernel<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(A, post, pre);
+    ++cs::g_launches;
     return (int)cudaGetLastError();
 }
 

@@ -14,9 +14,11 @@ Robot policies:
 With update_memory=True the rollout also fills a memory.DeviceReplayMemory like Explorer.update_memory does
 (explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot
 (train.py:116-132's IL phase) records on device at every crowd size, with occupancy-map rows when the target policy has
-them (memory.DeviceILRecorder: steps_per_launch steps -- inside the multi-step kernel at 2 <= N <= 5 -- plus a flush);
-RL targets and host-side policies record step by step (memory.TrajectoryRecorder). Both push the same pairs in the same
-order. In imitation learning the rows are what target_policy.transform stores (explorer.py:102): its occupancy-map
+them (memory.DeviceILRecorder: steps_per_launch steps -- inside the multi-step kernel at 2 <= N <= 5 -- plus a flush).
+Reinforcement learning with a target model records on device too, for the ORCA robot (steps_per_launch steps per launch)
+and for act_batch policies (one step per call), flushing every steps_per_launch steps with one target-network forward
+(memory.DeviceRLRecorder); without a target model, or with any other policy, the rollout records step by step
+(memory.TrajectoryRecorder). All of them push the same pairs in the same order. In imitation learning the rows are what target_policy.transform stores (explorer.py:102): its occupancy-map
 settings (with_om, cell_num, cell_size, om_channel_size) when target_policy is given.
 
 Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous ranges per rank; there is no data-path
@@ -162,7 +164,7 @@ class BatchedExplorer(object):
         recorder = dev_rec = None
         chunk = max(1, int(steps_per_launch))
         if update_memory:
-            from .memory import DeviceILRecorder, TrajectoryRecorder
+            from .memory import DeviceILRecorder, DeviceRLRecorder, TrajectoryRecorder
             # the rows are target_policy.transform(state) (explorer.py:102): in imitation learning the occupancy-map
             # settings come from the target policy when there is one
             if imitation_learning and self.target_policy is not None:
@@ -171,6 +173,11 @@ class BatchedExplorer(object):
                 om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
             if self.robot_policy == 'orca' and imitation_learning:
                 dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om)
+                dev_rec.begin()
+            elif not imitation_learning and self.target_model is not None and (
+                    self.robot_policy == 'orca' or hasattr(self.robot_policy, 'act_batch')):
+                # RL targets: staged on device, the target network runs once per flush of `chunk` steps
+                dev_rec = DeviceRLRecorder(env, self.memory, self.gamma, self.target_model, chunk, om=om, unicycle=unicycle)
                 dev_rec.begin()
             else:
                 recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om,
@@ -194,8 +201,10 @@ class BatchedExplorer(object):
                     env.prefetch()
             if recorder is not None:
                 recorder.before_step()
-            if dev_rec is not None:
+            if dev_rec is not None and self.robot_policy == 'orca':
                 env.step(None, n_steps=chunk, record=dev_rec)
+            elif dev_rec is not None:
+                env.step(self.robot_policy.act_batch(env), record=dev_rec)
             elif self.robot_policy == 'orca':
                 env.step(n_steps=chunk)
             else:

@@ -10,6 +10,9 @@
                        maps, recorded on device (crowdsim_step_n_record_ex: inside the multi-step kernel at 2 <= N <= 5, around
                        each single-step launch otherwise) and flushed to the memory on device (crowdsim_record_flush_ex): same
                        pairs, same order, same bits as TrajectoryRecorder, with no host syncs
+  DeviceRLRecorder     the same for reinforcement learning (target-network values), for the ORCA robot and for robots
+                       stepped with external actions (holonomic or unicycle): same pairs, same order and same rows as
+                       TrajectoryRecorder; the values differ only by how the batch a target network sees rounds
 The IL return is accumulated forward in t (G_i += pow(...) * r_t as each reward arrives), i.e. in the same order and
 with the same pow() factors as the reference's sum(); it agrees to the last ulp of float64 (CPython >= 3.12 sums with
 Neumaier compensation) and is identical after the float32 cast the reference applies.
@@ -138,7 +141,7 @@ class DeviceILRecorder(object):
     each, between launches that stage the rows and book the rewards (include/crowdsim_b200.h: crowdsim_step_n_record_ex).
     om = (cell_num, cell_size, om_channel_size): every row is followed by the occupancy map of the pre-step human state, as
     TrajectoryRecorder(om=...) records it (MultiHumanRL.transform with with_om); the memory holds [N][13 + cell_num^2 *
-    om_channel_size] rows. Only for an ORCA robot; RL targets and host-side policies use TrajectoryRecorder."""
+    om_channel_size] rows. Only for an ORCA robot; RL targets use DeviceRLRecorder."""
 
     def __init__(self, env, memory, gamma, n_max, om=None):
         from .batched import max_episode_steps
@@ -195,3 +198,119 @@ class DeviceILRecorder(object):
         cell_num, cell_size, channels = self.om
         return _abi.RecordMaps(self.h_pos.data_ptr(), self.h_vel.data_ptr(), self.maps.data_ptr(), int(cell_num),
                                int(channels), float(cell_size))
+
+
+class DeviceRLRecorder(object):
+    """Reinforcement-learning transitions recorded on device: TrajectoryRecorder(imitation_learning=False) with the same
+    pairs in the same order and no host synchronisation between steps (include/crowdsim_b200.h: crowdsim_record_flush_rl).
+
+    The recorder stages up to n_max steps, then flushes them: the target network runs once over all n_max * B staged rows
+    (with their occupancy maps when om is given) and writes each row's value to `boot`; the flush appends rows, rewards and
+    values to per-slot trajectories and writes the pairs of every episode that ends in ReachGoal or Collision to the memory,
+      value_i = float32(r_i + gamma_bar * boot_{i+1}),  float32(r_{L-1} + 0.0) at an episode's last step,
+    the float64 operations TrajectoryRecorder runs in torch. How the steps are staged depends on the robot (env.step(...,
+    record=self)):
+      ORCA robot       n_steps per call through crowdsim_step_n_record_ex, as DeviceILRecorder stages them (inside the
+                       multi-step kernel at 2 <= N <= 5, around each single-step launch otherwise)
+      external robot   one step per call with the caller's actions: crowdsim_record_book books the step, env.pack_joint stages
+                       its rows (unicycle: the rows of a unicycle robot, as TrajectoryRecorder(unicycle=True) packs them)
+    It flushes when its staging is full and at finish(). The ring's write position and size live on the device during a run:
+    call begin() before the first step and finish() after the last (one host read)."""
+
+    rl = True
+
+    def __init__(self, env, memory, gamma, target_model, n_max, om=None, unicycle=False):
+        from .batched import max_episode_steps
+        B, N, dev = env.B, env.human_num, env.device
+        if om is not None and N < 2:
+            raise ValueError('need at least one array to concatenate')      # what env.occupancy_maps raises
+        F = 13 + (om[0] * om[0] * om[2] if om else 0)
+        if tuple(memory.states.shape[1:]) != (N, F):
+            raise ValueError('memory rows must be [N][%d] joint states%s' % (F, ' with occupancy maps' if om else ''))
+        if int(n_max) < 1:
+            raise ValueError('n_max must be at least 1')
+        self.env, self.memory, self.target_model, self.n_max = env, memory, target_model, int(n_max)
+        self.om, self.unicycle = om, bool(unicycle)
+        self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
+        self.gamma_bar = pow(gamma, env.time_step * env.robot_v_pref)              # TrajectoryRecorder.gamma_bar
+        n = self.n_max
+        self.rows = torch.zeros((n, B, N, 13), dtype=torch.float32, device=dev)
+        self.reward = torch.zeros((n, B), dtype=torch.float64, device=dev)
+        self.t = torch.zeros((n, B), dtype=torch.int32, device=dev)
+        self.code = torch.zeros((n, B), dtype=torch.uint8, device=dev)
+        self.boot = torch.zeros((n, B), dtype=torch.float32, device=dev)
+        self.traj_rows = torch.zeros((B, self.T, N, F), dtype=torch.float32, device=dev)
+        self.traj_reward = torch.zeros((B, self.T), dtype=torch.float64, device=dev)
+        self.traj_boot = torch.zeros((B, self.T), dtype=torch.float32, device=dev)
+        self.pushed = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.scan = torch.empty(n * B + 2, dtype=torch.int64, device=dev)
+        self.position0 = memory.position
+        if om:
+            self.h_pos = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.h_vel = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.maps = torch.zeros((n, B, N, F - 13), dtype=torch.float32, device=dev)
+        self.s = 0                                  # steps staged since the last flush
+
+    def begin(self):
+        """Start counting pushes at the memory's current write position."""
+        self.pushed.zero_()
+        self.position0 = self.memory.position
+
+    def finish(self):
+        """Flush what is staged, then move the memory's write position and size by what the flushes pushed since begin()
+        (reads the counter)."""
+        self.flush()
+        n = int(self.pushed.item())
+        m = self.memory
+        m.position = (self.position0 + n) % m.capacity
+        m.size = min(m.capacity, m.size + n)
+        self.position0 = m.position
+        self.pushed.zero_()
+        return n
+
+    def struct(self, s=0):
+        """crowdsim_record with its staging starting at step s of the window."""
+        m = self.memory
+        p = lambda t: t.data_ptr()  # noqa: E731
+        return _abi.Record(p(self.rows[s]), p(self.reward[s]), p(self.t[s]), p(self.code[s]), self.n_max - s,
+                           p(self.traj_rows), p(self.traj_reward), self.T, None, p(m.states), p(m.values), m.capacity,
+                           self.position0, p(self.pushed), p(self.scan))
+
+    def maps_struct(self, s=0):
+        """crowdsim_record_maps with its staging starting at step s, or None without maps."""
+        if not self.om:
+            return None
+        cell_num, cell_size, channels = self.om
+        return _abi.RecordMaps(self.h_pos[s].data_ptr(), self.h_vel[s].data_ptr(), self.maps[s].data_ptr(), int(cell_num),
+                               int(channels), float(cell_size))
+
+    def rl_struct(self):
+        return _abi.RecordRL(self.boot.data_ptr(), self.traj_boot.data_ptr(), float(self.gamma_bar))
+
+    def staged(self, n):
+        """env.step staged n more steps; a full staging is flushed."""
+        self.s += int(n)
+        if self.s >= self.n_max:
+            self.flush()
+
+    def flush(self):
+        """Evaluate the target network on every staged row and write the stored episodes' pairs to the memory."""
+        n, self.s = self.s, 0
+        env = self.env
+        B, N = env.B, env.human_num
+        if n == 0 or B == 0:
+            return
+        import ctypes as C
+        rec, maps, rl = self.struct(), self.maps_struct(), self.rl_struct()
+        mp = C.byref(maps) if maps is not None else None
+        with torch.cuda.device(env.device):
+            if maps is not None:
+                _abi.check(env.lib.crowdsim_record_flush_maps(B, N, C.byref(rec), mp, n, env._stream()),
+                           'crowdsim_record_flush_maps')
+            x = self.rows[:n].view(n * B, N, 13)
+            if maps is not None:
+                x = torch.cat([x, self.maps[:n].view(n * B, N, -1)], dim=2)
+            with torch.no_grad():
+                self.boot[:n].copy_(self.target_model(x).view(n, B))
+            _abi.check(env.lib.crowdsim_record_flush_rl(B, N, C.byref(rec), mp, C.byref(rl), n, env._stream()),
+                       'crowdsim_record_flush_rl')

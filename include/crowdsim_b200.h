@@ -21,6 +21,9 @@
  *                            92-105; crowd_nav/utils/memory.py:4-28)
  *   crowdsim_step_n_record_ex, crowdsim_record_flush_ex  the same at every crowd size, optionally with occupancy-map rows
  *                            (multi_human_rl.py:98-104 with with_om)
+ *   crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl  the same with reinforcement-learning values
+ *                            (explorer.py:107-113: reward + gamma_bar * target_model(next state)), for an ORCA robot and
+ *                            for robots stepped with external actions
  *   crowdsim_orca_act        crowd_sim/envs/utils/robot.py:9-14 with policy ORCA (orca.py:82-132), batched
  *   crowdsim_reset           crowd_sim/envs/crowd_sim.py:251-312 + generators :155-207 (np.random MT19937)
  *   crowdsim_prefetch_scenes the same generators, run ahead of time for the NEXT episode of each env slot
@@ -337,6 +340,45 @@ int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int N, crowdsim
                               const crowdsim_record_maps *maps, void *stream);
 int crowdsim_record_flush_ex(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
                              void *stream);
+
+/*
+ * Reinforcement-learning transitions recorded on device: Explorer.run_k_episodes(update_memory=True,
+ * imitation_learning=False) (crowd_nav/utils/explorer.py:66-69, 107-113). A stored episode of length L gives the pairs
+ * (row_i, float32(r_i + gamma_bar * (double)boot_{i+1})) for i < L - 1 and (row_{L-1}, float32(r_{L-1} + 0.0)), every
+ * product and sum rounded once, where boot_j = target_model(row_j) is the float32 value the caller's target network gave the
+ * staged row of step j (with its occupancy maps when there are maps). The network runs outside this library, once per flush
+ * over all n_steps * B staged rows, so how many pairs a flush stores never has to reach the host.
+ *
+ * Staging:
+ *   ORCA robot       crowdsim_step_n_record_ex, unchanged.
+ *   external robot   per step s of the window (the caller picks s < n_max): crowdsim_record_book(pre = s) books t[s], code[s]
+ *                    (and, with maps, the float64 human state of the rows); crowdsim_pack_joint(kinematics_unicycle,
+ *                    out = rec->rows + s * B * N * 13) stages the rows; crowdsim_step (or crowdsim_step_n) with the actions;
+ *                    crowdsim_record_book(post = s) books the step's reward and ending. Any 1 <= N <= CROWDSIM_MAX_HUMANS.
+ * crowdsim_record_book is the launch loop's booking of crowdsim_step_n_record_ex without its rows: post >= 0 books step post's
+ * reward and ending from io (reward, done, info), pre >= 0 stages step pre from st (active) and ep (ep_steps); -1 skips
+ * either half. One launch.
+ *
+ * Flush (crowdsim_record_flush_rl, the arguments of crowdsim_record_flush_ex plus `rl`):
+ *   maps == NULL  rl->boot[s][e] must hold target_model(rec->rows[s][e]).
+ *   maps != NULL  first crowdsim_record_flush_maps computes the occupancy map of every staged (step, env) to maps->maps (the first
+ *                 launch of crowdsim_record_flush_ex); the caller evaluates its network on rows ++ maps; crowdsim_record_flush_rl
+ *                 then writes the same maps to the ring without computing them again.
+ * The rows, their order in the ring, the ring wrap and *pushed are those of crowdsim_record_flush_ex; rec->g is not read (may
+ * be NULL). rl->traj_boot keeps each slot's boot per episode step across flushes, beside rec->traj_rows and
+ * rec->traj_reward, because boot_{i+1} can come from an earlier flush than the episode's end. Two launches (scan, copy).
+ */
+typedef struct crowdsim_record_rl {
+    const float *boot;     /* [n_max][B] target_model(row) of every staged (step, env), written by the caller */
+    float *traj_boot;      /* [B][T] per-slot boot, kept across flushes */
+    double gamma_bar;      /* pow(gamma, time_step * v_pref), host-computed */
+} crowdsim_record_rl;
+int crowdsim_record_book(int B, int N, const crowdsim_state *st, const crowdsim_step_io *io, const crowdsim_episodes *ep,
+                         const crowdsim_record *rec, const crowdsim_record_maps *maps, int post, int pre, void *stream);
+int crowdsim_record_flush_maps(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
+                         void *stream);
+int crowdsim_record_flush_rl(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps,
+                             const crowdsim_record_rl *rl, int n_steps, void *stream);
 
 /* Robot ORCA action from the current state, no mutation: action_out[B][2]. */
 int crowdsim_orca_act(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, double *action_out,

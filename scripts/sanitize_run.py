@@ -7,7 +7,8 @@ lookahead pack / humans / onestep_lookahead, propagate pack (query_env = false; 
 row tiles), occupancy maps, human_times, the recording multi-step kernel with its flush
 (crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps, and both routes of
 crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
-at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush)."""
+at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush), and the reinforcement-learning recording
+(crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl) for the ORCA robot and external robots."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -68,6 +69,27 @@ for N, om in ((1, None), (20, None), (5, (4, 1.0, 3))):
     rec.begin()
     env.step(None, n_steps=16, record=rec)
     print('N', N, 'maps', om, 'pairs recorded', rec.finish())
+
+# reinforcement-learning recording (crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl): the ORCA
+# robot through the multi-step kernel (N = 5, with maps) and the launch loop (N = 20), a holonomic and a unicycle robot
+# stepped with external actions (N = 5, with maps)
+from crowdnav_b200.memory import DeviceRLRecorder
+for N, robot, om in ((5, 'orca', (4, 1.0, 3)), (20, 'orca', None), (5, 'external_xy', (4, 1.0, 3)), (5, 'external_rot', None)):
+    env = make(128, N, rule='square_crossing' if N > 5 else 'circle_crossing')
+    env.track_episodes(600); env.set_case_queue(0, 600, 'train'); env.enable_autoreset(); env.reset_seeds(use_queue=True); env.prefetch()
+    for _ in range(6):
+        env.step_n(4)                       # episodes near their end, so that the recorded steps store some
+    env.prefetch(); env.set_robot_policy(robot)
+    F = 13 + (om[0] * om[0] * om[2] if om else 0)
+    mem = DeviceReplayMemory(400, N, env.device, F)
+    rec = DeviceRLRecorder(env, mem, 0.9, lambda x: x[:, 0, :1] * 0.5 + x[:, -1, 4:5], 8, om=om, unicycle=robot == 'external_rot')
+    rec.begin()
+    if robot == 'orca':
+        env.step(None, n_steps=8, record=rec); env.step(None, n_steps=4, record=rec)
+    else:
+        for _ in range(12):
+            env.step(torch.full((128, 2), 0.5, dtype=torch.float64, device=env.device), record=rec)
+    print('RL', robot, 'N', N, 'maps', om, 'pairs recorded', rec.finish())
 
 # value-network support + lookahead + human times
 env = make(64, 5, policy='external_xy'); env.reset_seeds(torch.arange(64) + 1000)
