@@ -110,6 +110,10 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
                                           P(Record), P(RecordMaps)] + s
         f = getattr(lib, prefix + 'record_flush_ex')
         f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), C.c_int] + s
+    if hasattr(lib, prefix + 'step_n_record_rot'):
+        f = getattr(lib, prefix + 'step_n_record_rot')
+        f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int,
+                                          P(Record), P(RecordMaps)] + s
     if hasattr(lib, prefix + 'record_flush_rl'):
         f = getattr(lib, prefix + 'record_book')
         f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(Record), P(RecordMaps),
@@ -138,7 +142,7 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
 
 EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_count', 'crowdsim_debug_force_generic', 'crowdsim_graph_launch',
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
-           'crowdsim_step_n_record_ex', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
+           'crowdsim_step_n_record_ex', 'crowdsim_step_n_record_rot', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
            'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
            'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 

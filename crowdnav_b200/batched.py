@@ -321,8 +321,9 @@ class BatchedCrowdSim(object):
         done / info are those of each env's last live step.
         record: a memory.DeviceILRecorder -- the same steps through crowdsim_step_n_record_ex (one launch for any n_steps
         at 2 <= N <= 5, the launch loop with its recording otherwise), then crowdsim_record_flush_ex of their
-        imitation-learning pairs (with occupancy maps when the recorder has them) into the recorder's memory. Needs an ORCA
-        robot, episode tracking and auto-reset (ValueError otherwise).
+        imitation-learning pairs (with occupancy maps when the recorder has them) into the recorder's memory; a recorder
+        with unicycle=True stages through crowdsim_step_n_record_rot (a unicycle target's rows). Needs an ORCA robot, episode
+        tracking and auto-reset (ValueError otherwise).
         record: a memory.DeviceRLRecorder -- with an ORCA robot the same n_steps steps through crowdsim_step_n_record_ex
         (no actions); with an external robot one step with `actions` (n_steps = 1), booked around it by crowdsim_record_book
         and its rows staged by pack_joint. The recorder flushes its reinforcement-learning pairs when its staging is full."""
@@ -338,12 +339,13 @@ class BatchedCrowdSim(object):
             ar = self.autoreset.struct() if self.autoreset is not None else None
             rec, maps = record.struct(), record.maps_struct()
             mp = C.byref(maps) if maps is not None else None
+            name = 'crowdsim_step_n_record_rot' if getattr(record, 'unicycle', False) else 'crowdsim_step_n_record_ex'
             with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step_n_record_ex(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                                        C.byref(ep) if ep is not None else None,
-                                                        C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
-                                                        mp, self._stream())
-                _abi.check(rc, 'crowdsim_step_n_record_ex')
+                rc = getattr(self.lib, name)(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
+                                             C.byref(ep) if ep is not None else None,
+                                             C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
+                                             mp, self._stream())
+                _abi.check(rc, name)
                 rc = self.lib.crowdsim_record_flush_ex(self.B, self.human_num, C.byref(rec), mp, int(n_steps), self._stream())
             _abi.check(rc, 'crowdsim_record_flush_ex')
             return self.observation(), self.reward, self.done, self.info

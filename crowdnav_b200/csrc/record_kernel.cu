@@ -3,6 +3,8 @@
 //                        crowdsim_step_n_record and crowdsim_step_n_record_ex at 2 <= N <= 5 (step_kernel.cu)
 //   launch_record_between  the recording around each single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1,
 //                        N > 5, the forced generic kernel): the same staging, from the state between two launches
+//   (both with rot: crowdsim_step_n_record_rot, the rows of a unicycle robot -- step_multi_kernel<N, VIS, true, true> and
+//                        record_between_rot_kernel, the theta column (float)r_theta - rot)
 //   crowdsim_record_flush  one launch's staging -> per-slot trajectories -> (state, value) pairs of the replay memory ring
 //   crowdsim_record_flush_ex  the same, optionally with occupancy-map rows: record_maps_kernel computes the map of every
 //                        staged (step, env) first (occupancy.cuh, the code of crowdsim_occupancy_maps)
@@ -29,10 +31,13 @@
 
 namespace cs {
 
-int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream)
+int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot)
 {
-    #define CS_MULTI_REC_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
-                                         else step_multi_kernel<NN, false, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
+    #define CS_MULTI_REC_LAUNCH(NN) do {                                                                                    \
+        if (rot) { if (A.k.robot_visible) step_multi_kernel<NN, true, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
+                   else step_multi_kernel<NN, false, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); }                \
+        else if (A.k.robot_visible) step_multi_kernel<NN, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A);             \
+        else step_multi_kernel<NN, false, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
     switch (A.N) {
         case 2: CS_MULTI_REC_LAUNCH(2); break;
         case 3: CS_MULTI_REC_LAUNCH(3); break;
@@ -55,7 +60,8 @@ int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream)
 // The two touch different steps' staging, so one launch serves post(s) and pre(s + 1).
 // ROWS = false (crowdsim_record_book, robots stepped with external actions): the same booking without rec_row, whose rows
 // carry only the holonomic theta column; the caller stages the rows with crowdsim_pack_joint.
-template <bool ROWS>
+// ROT = true (crowdsim_step_n_record_rot): rec_row with a unicycle robot's theta column, from the state's r_theta.
+template <bool ROWS, bool ROT = false>
 __device__ __forceinline__ void record_between(const StepArgs &A, int post, int pre)
 {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -80,8 +86,12 @@ __device__ __forceinline__ void record_between(const StepArgs &A, int post, int 
             if constexpr (ROWS) {
                 const double2 ha = ld2(A.st.h_attr, idx);
                 const double2 ra = ld2(A.st.r_attr, e);
-                rec_row(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e), ra.x,
-                        (float)ra.y);
+                if constexpr (ROT)
+                    rec_row<true>(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e),
+                                  ra.x, (float)ra.y, (float)A.st.r_theta[e]);
+                else
+                    rec_row(A.rec, A.B, N, pre, e, a, hp, hv, ha.x, ld2(A.st.r_pos, e), ld2(A.st.r_vel, e), ld2(A.st.r_goal, e), ra.x,
+                            (float)ra.y);
             }
             if (A.recm.h_pos) rec_map_state(A.recm, A.B, N, pre, e, a, hp, hv);
         }
@@ -98,10 +108,16 @@ __global__ void __launch_bounds__(128) record_book_kernel(const __grid_constant_
     record_between<false>(A, post, pre);
 }
 
-void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream)
+__global__ void __launch_bounds__(128) record_between_rot_kernel(const __grid_constant__ StepArgs A, int post, int pre)
+{
+    record_between<true, true>(A, post, pre);
+}
+
+void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream, bool rot)
 {
     const size_t n = (size_t)A.B * A.N;
-    record_between_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(A, post, pre);
+    if (rot) record_between_rot_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(A, post, pre);
+    else record_between_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(A, post, pre);
     ++g_launches;
 }
 

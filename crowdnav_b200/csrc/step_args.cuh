@@ -75,11 +75,12 @@ static inline int check_record_maps(int N, const crowdsim_record_maps *m)
 
 // record_kernel.cu: launch step_multi_kernel<N, VIS, true> (crowdsim_step_n_record) for 2 <= A.N <= 5. The recording
 // instantiations live in a unit of their own: their rows use CUDA's float32 atan2f / cosf / sinf (rotate.cuh), whose
-// library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code.
-int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream);
+// library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code. rot: the unicycle-row
+// instantiation step_multi_kernel<N, VIS, true, true> (crowdsim_step_n_record_rot).
+int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot = false);
 // record_kernel.cu: the recording around one single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1, N > 5, the
 // forced generic kernel). post >= 0: book step `post`'s reward and ending (TrajectoryRecorder.after_step); pre >= 0: stage
-// step `pre`'s rows of the envs live now (before_step). One launch.
-void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream);
+// step `pre`'s rows of the envs live now (before_step). One launch. rot: the rows of a unicycle robot.
+void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream, bool rot = false);
 
 }  // namespace cs

@@ -244,7 +244,7 @@ static int sm_count()
 static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
                   const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int act_only, int n_steps, cudaStream_t stream,
                   double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr,
-                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr)
+                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr, bool rec_rot = false)
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
     if (rec) {
@@ -253,6 +253,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         if (rec_any_route ? (N < 1 || N > CROWDSIM_MAX_HUMANS) : (N < 2 || N > 5 || g_force_generic)) return CROWDSIM_EUNSUPPORTED;
         if (prm->robot_policy != CROWDSIM_ROBOT_ORCA) return CROWDSIM_EUNSUPPORTED;
         if (!ep || !ar || !rec->rows || !rec->reward || !rec->t || !rec->code || n_steps > rec->n_max) return CROWDSIM_EINVAL;
+        if (rec_rot && !st->r_theta) return CROWDSIM_EINVAL;   // crowdsim_step_n_record_rot: the rows' heading
         const int rc = check_record_maps(N, recm);
         if (rc != CROWDSIM_OK) return rc;
     }
@@ -302,7 +303,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if ((n_steps > 1 || rec) && N >= 2 && N <= 5 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && !g_force_generic && !A.lookahead) {
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
-        if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream); }
+        if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream, rec_rot); }
         #define CS_MULTI_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
                                          else step_multi_kernel<NN, false, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
         switch (N) {
@@ -328,7 +329,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
                                         else if (warpq) step_flat_kernel<NN, 99, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
                                         else step_flat_kernel<NN, 99, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
         for (int rep = 0; rep < n_steps; ++rep) {
-            if (rec) launch_record_between(A, rep - 1, rep, stream);   // (crowdsim_step_n_record_ex at N = 1)
+            if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);   // (crowdsim_step_n_record_ex at N = 1)
             switch (N) {
                 case 1: CS_FLAT_LAUNCH(1); break;
                 case 2: CS_FLAT_LAUNCH(2); break;
@@ -339,7 +340,7 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
             ++g_launches;
         }
         #undef CS_FLAT_LAUNCH
-        if (rec) launch_record_between(A, n_steps - 1, -1, stream);
+        if (rec) launch_record_between(A, n_steps - 1, -1, stream, rec_rot);
         return (int)cudaGetLastError();
     }
     const int threads = A.EPB * A.L;
@@ -352,12 +353,12 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         if (err != cudaSuccess) return (int)err;
     }
     for (int rep = 0; rep < n_steps; ++rep) {
-        if (rec) launch_record_between(A, rep - 1, rep, stream);       // (crowdsim_step_n_record_ex)
+        if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);       // (crowdsim_step_n_record_ex)
         if (mid) step_kernel<true><<<blocks, threads, smem, stream>>>(A);
         else step_kernel<false><<<blocks, threads, smem, stream>>>(A);
         ++g_launches;
     }
-    if (rec) launch_record_between(A, n_steps - 1, -1, stream);
+    if (rec) launch_record_between(A, n_steps - 1, -1, stream, rec_rot);
     return (int)cudaGetLastError();
 }
 
@@ -389,6 +390,14 @@ extern "C" int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int 
 {
     if (!rec) return CROWDSIM_EINVAL;
     return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec, true, maps);
+}
+
+extern "C" int crowdsim_step_n_record_rot(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                          crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                                          const crowdsim_record_maps *maps, void *stream)
+{
+    if (!rec) return CROWDSIM_EINVAL;
+    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec, true, maps, true);
 }
 
 extern "C" int crowdsim_onestep_lookahead(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, crowdsim_step_io *io,

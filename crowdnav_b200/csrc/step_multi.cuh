@@ -137,16 +137,27 @@ __device__ __forceinline__ float *rec_vpref_smem()
     return s_vp;
 }
 
-// REC = true: human a of env e writes its row of step s, crowdsim_pack_joint(kinematics_unicycle = 0) of the pre-step state
-// (pack_kernel.cu: the same rotate code, the same float32 casts) to rows[s][e][a].
+// ROT = true (crowdsim_step_n_record_rot): the robot's heading as float32, (float)r_theta, published per env like v_pref.
+// Declared only by the unicycle-row instantiation.
+template <int E>
+__device__ __forceinline__ float *rec_theta_smem()
+{
+    __shared__ float s_th[E];
+    return s_th;
+}
+
+// REC = true: human a of env e writes its row of step s, crowdsim_pack_joint(kinematics_unicycle = ROT) of the pre-step
+// state (pack_kernel.cu: the same rotate code, the same float32 casts) to rows[s][e][a]. rth: the robot's (float)r_theta,
+// read only when ROT (the theta column th - rot, cadrl.py:205-209); the holonomic rows carry 0.
+template <bool ROT = false>
 __device__ __forceinline__ void rec_row(const crowdsim_record &rec, int B, int N, int s, int e, int a, double2 hp, double2 hv,
-                                        double hr, double2 rp, double2 rv, double2 rg, double rr, float rvp)
+                                        double hr, double2 rp, double2 rv, double2 rg, double rr, float rvp, float rth = 0.f)
 {
     float c, sn, rot, dg, rvx, rvy;
     rotate_self((float)rp.x, (float)rp.y, (float)rv.x, (float)rv.y, (float)rg.x, (float)rg.y, c, sn, rot, dg, rvx, rvy);
     float row[13];
-    rotate_row(row, (float)rp.x, (float)rp.y, (float)rr, rvp, 0.f, dg, rvx, rvy, c, sn, (float)hp.x, (float)hp.y, (float)hv.x,
-               (float)hv.y, (float)hr);
+    rotate_row(row, (float)rp.x, (float)rp.y, (float)rr, rvp, ROT ? (rth - rot) : 0.f, dg, rvx, rvy, c, sn, (float)hp.x,
+               (float)hp.y, (float)hv.x, (float)hv.y, (float)hr);
     float *o = rec.rows + (((size_t)s * B + e) * N + a) * 13;
     #pragma unroll
     for (int i = 0; i < 13; ++i) o[i] = row[i];
@@ -163,10 +174,14 @@ __device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int
 // REC = false is crowdsim_step_n. REC = true also stages, per step and env, what an imitation-learning recorder needs
 // (include/crowdsim_b200.h: crowdsim_record): the humans write the rows of the envs live at the start of the step, the
 // robot the reward, the episode step and the CROWDSIM_REC_* code; steps a block does not run get CROWDSIM_REC_NONE.
-template <int N, bool VIS, bool REC>
+// ROT = true (REC only, crowdsim_step_n_record_rot): the rows of a unicycle robot, crowdsim_pack_joint(kinematics_unicycle = 1).
+// The robot's heading comes from st.r_theta at the launch's start; its ORCA step leaves it as it is, and an auto-reset
+// install carries on with the value the install writes to r_theta. ROT = false compiles to the SASS it had before ROT.
+template <int N, bool VIS, bool REC, bool ROT = false>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
 step_multi_kernel(const __grid_constant__ StepArgs A)
 {
+    static_assert(REC || !ROT, "unicycle rows are a recording variant");
     static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
     using namespace orca;
     constexpr int E = 32, L = N + 1, T = 32 * L;
@@ -224,6 +239,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             if (A.has_ep) { r0.ep_t = A.ep.ep_steps[e]; r0.ep_ret = A.ep.ep_return[e]; r0.ep_tc = A.ep.ep_too_close[e]; r0.ep_mds = A.ep.ep_min_dist_sum[e]; r0.ep_c = A.ep.ep_case[e]; }
             if (A.has_ar) r0.want = A.ar.want[e];
             s_rr[le] = r0;
+            if constexpr (ROT) rec_theta_smem<E>()[le] = (float)A.st.r_theta[e];
         }
     }
     s_goal[tid] = goal;
@@ -260,7 +276,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     if constexpr (REC) {
         if (!is_robot && live) {
             const int rt = 32 * N + le;
-            rec_row(A.rec, A.B, N, s, e, a, pos, vel, attr.x, s_pos[rt], s_vel[rt], s_goal[rt], s_rad[rt], rec_vpref_smem<E>()[le]);
+            if constexpr (ROT)
+                rec_row<true>(A.rec, A.B, N, s, e, a, pos, vel, attr.x, s_pos[rt], s_vel[rt], s_goal[rt], s_rad[rt],
+                              rec_vpref_smem<E>()[le], rec_theta_smem<E>()[le]);
+            else
+                rec_row(A.rec, A.B, N, s, e, a, pos, vel, attr.x, s_pos[rt], s_vel[rt], s_goal[rt], s_rad[rt], rec_vpref_smem<E>()[le]);
             if (A.recm.h_pos) rec_map_state(A.recm, A.B, N, s, e, a, pos, vel);      // a runtime branch: one instantiation
         }
     }
@@ -481,6 +501,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                         vel = make_double2(0, 0); attr = make_double2(A.ar.robot_radius, A.ar.robot_v_pref);
                         rr.gtime = 0.0;
                         if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
+                        if constexpr (ROT) rec_theta_smem<E>()[le] = (float)A.st.r_theta[e];     // the heading installed
                         if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
                         act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
                         dirty_kin = true; dirty_scene = true; release = true;

@@ -14,7 +14,8 @@ Robot policies:
 With update_memory=True the rollout also fills a memory.DeviceReplayMemory like Explorer.update_memory does
 (explorer.py:92-125; imitation-learning returns or target-network bootstraps). Imitation learning with the ORCA robot
 (train.py:116-132's IL phase) records on device at every crowd size, with occupancy-map rows when the target policy has
-them (memory.DeviceILRecorder: steps_per_launch steps -- inside the multi-step kernel at 2 <= N <= 5 -- plus a flush).
+them and a unicycle robot's rows when its kinematics is 'unicycle' (memory.DeviceILRecorder: steps_per_launch steps --
+inside the multi-step kernel at 2 <= N <= 5 -- plus a flush).
 Reinforcement learning with a target model records on device too, for the ORCA robot (steps_per_launch steps per launch)
 and for act_batch policies (one step per call), flushing every steps_per_launch steps with one target-network forward
 (memory.DeviceRLRecorder); without a target model, or with any other policy, the rollout records step by step
@@ -125,6 +126,12 @@ def _om_settings(policy):
     return (policy.cell_num, policy.cell_size, policy.om_channel_size)
 
 
+def _unicycle_rows(policy):
+    """True when a policy's transform() rotates its rows with a unicycle robot's theta column (cadrl.py:205-209):
+    policy.config [action_space] kinematics = unicycle."""
+    return getattr(policy, 'kinematics', 'holonomic') == 'unicycle'
+
+
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
                  rank=0, world=1, group=None):
@@ -166,13 +173,16 @@ class BatchedExplorer(object):
         if update_memory:
             from .memory import DeviceILRecorder, DeviceRLRecorder, TrajectoryRecorder
             # the rows are target_policy.transform(state) (explorer.py:102): in imitation learning the occupancy-map
-            # settings come from the target policy when there is one
+            # settings and the row kinematics (a unicycle target's theta column, cadrl.py:205-209) come from the target
+            # policy when there is one, while the robot keeps running ORCA
             if imitation_learning and self.target_policy is not None:
                 om = _om_settings(self.target_policy)
+                rows_unicycle = _unicycle_rows(self.target_policy)
             else:
                 om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
+                rows_unicycle = unicycle
             if self.robot_policy == 'orca' and imitation_learning:
-                dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om)
+                dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om, unicycle=rows_unicycle)
                 dev_rec.begin()
             elif not imitation_learning and self.target_model is not None and (
                     self.robot_policy == 'orca' or hasattr(self.robot_policy, 'act_batch')):
@@ -181,7 +191,7 @@ class BatchedExplorer(object):
                 dev_rec.begin()
             else:
                 recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om,
-                                              unicycle=unicycle)
+                                              unicycle=rows_unicycle)
         side = torch.cuda.Stream(device=env.device)
         main = torch.cuda.current_stream(env.device)
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per

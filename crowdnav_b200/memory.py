@@ -7,9 +7,10 @@
                          imitation learning:  value_i = sum_{t >= i} pow(gamma, (t - i) * time_step * v_pref) * r_t
                          RL:                  value_i = r_i + gamma_bar * target_model(state_{i+1}),  r_i at the terminal step
   DeviceILRecorder     the same for imitation learning with an ORCA robot at any 1 <= N <= 63, with or without occupancy
-                       maps, recorded on device (crowdsim_step_n_record_ex: inside the multi-step kernel at 2 <= N <= 5, around
-                       each single-step launch otherwise) and flushed to the memory on device (crowdsim_record_flush_ex): same
-                       pairs, same order, same bits as TrajectoryRecorder, with no host syncs
+                       maps, with a holonomic or a unicycle target's rows, recorded on device (crowdsim_step_n_record_ex /
+                       crowdsim_step_n_record_rot: inside the multi-step kernel at 2 <= N <= 5, around each single-step launch
+                       otherwise) and flushed to the memory on device (crowdsim_record_flush_ex): same pairs, same order, same
+                       bits as TrajectoryRecorder, with no host syncs
   DeviceRLRecorder     the same for reinforcement learning (target-network values), for the ORCA robot and for robots
                        stepped with external actions (holonomic or unicycle): same pairs, same order and same rows as
                        TrajectoryRecorder; the values differ only by how the batch a target network sees rounds
@@ -141,9 +142,11 @@ class DeviceILRecorder(object):
     each, between launches that stage the rows and book the rewards (include/crowdsim_b200.h: crowdsim_step_n_record_ex).
     om = (cell_num, cell_size, om_channel_size): every row is followed by the occupancy map of the pre-step human state, as
     TrajectoryRecorder(om=...) records it (MultiHumanRL.transform with with_om); the memory holds [N][13 + cell_num^2 *
-    om_channel_size] rows. Only for an ORCA robot; RL targets use DeviceRLRecorder."""
+    om_channel_size] rows. unicycle: the rows of a unicycle target policy (crowdsim_step_n_record_rot: the theta column
+    r_theta - rot, cadrl.py:205-209), as TrajectoryRecorder(unicycle=True) packs them; the robot still runs ORCA and keeps
+    the heading its reset gave it. Only for an ORCA robot; RL targets use DeviceRLRecorder."""
 
-    def __init__(self, env, memory, gamma, n_max, om=None):
+    def __init__(self, env, memory, gamma, n_max, om=None, unicycle=False):
         from .batched import max_episode_steps
         B, N, dev = env.B, env.human_num, env.device
         if om is not None and N < 2:
@@ -152,6 +155,7 @@ class DeviceILRecorder(object):
         if tuple(memory.states.shape[1:]) != (N, F):
             raise ValueError('memory rows must be [N][%d] joint states%s' % (F, ' with occupancy maps' if om else ''))
         self.env, self.memory, self.n_max, self.om = env, memory, int(n_max), om
+        self.unicycle = bool(unicycle)
         self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
         self.g = torch.tensor(il_discounts(gamma, env.time_step, env.robot_v_pref, self.T), dtype=torch.float64, device=dev)
         n = self.n_max

@@ -21,6 +21,9 @@
  *                            92-105; crowd_nav/utils/memory.py:4-28)
  *   crowdsim_step_n_record_ex, crowdsim_record_flush_ex  the same at every crowd size, optionally with occupancy-map rows
  *                            (multi_human_rl.py:98-104 with with_om)
+ *   crowdsim_step_n_record_rot  crowdsim_step_n_record_ex with the rows of a unicycle target policy: Explorer.update_memory
+ *                            stores target_policy.transform(state) (explorer.py:102), whose theta column is
+ *                            theta - rot (crowd_nav/policy/cadrl.py:205-209) while ORCA drives the robot (train.py:116-132)
  *   crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl  the same with reinforcement-learning values
  *                            (explorer.py:107-113: reward + gamma_bar * target_model(next state)), for an ORCA robot and
  *                            for robots stepped with external actions
@@ -340,6 +343,18 @@ int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int N, crowdsim
                               const crowdsim_record_maps *maps, void *stream);
 int crowdsim_record_flush_ex(int B, int N, const crowdsim_record *rec, const crowdsim_record_maps *maps, int n_steps,
                              void *stream);
+
+/*
+ * Imitation learning for a target policy with [action_space] kinematics = unicycle: crowdsim_step_n_record_ex with the
+ * arguments, routes, argument rules and staging of crowdsim_step_n_record_ex, except that each staged row is
+ * crowdsim_pack_joint(kinematics_unicycle = 1) of the pre-step state: column 2 is (float)st->r_theta[e] - rot instead of 0
+ * (CADRL.rotate, cadrl.py:205-209). The robot still runs ORCA, which leaves r_theta as it is; an auto-reset install sets it
+ * to pi / 2 as Robot.set does in CrowdSim.reset (crowd_sim.py:274). st->r_theta is required (CROWDSIM_EINVAL). Flush with
+ * crowdsim_record_flush_ex, unchanged: occupancy maps do not depend on the robot's heading.
+ */
+int crowdsim_step_n_record_rot(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                               crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_record *rec,
+                               const crowdsim_record_maps *maps, void *stream);
 
 /*
  * Reinforcement-learning transitions recorded on device: Explorer.run_k_episodes(update_memory=True,

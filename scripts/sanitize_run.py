@@ -7,7 +7,8 @@ lookahead pack / humans / onestep_lookahead, propagate pack (query_env = false; 
 row tiles), occupancy maps, human_times, the recording multi-step kernel with its flush
 (crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps, and both routes of
 crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
-at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush), and the reinforcement-learning recording
+at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush), both routes of crowdsim_step_n_record_rot
+(a unicycle target's rows), and the reinforcement-learning recording
 (crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl) for the ORCA robot and external robots."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -57,18 +58,19 @@ rec.begin()
 env.step(None, n_steps=16, record=rec)
 print('pairs recorded', rec.finish())
 
-# crowdsim_step_n_record_ex: the launch loop's recording at N = 1 and N = 20, occupancy-map rows at N = 5
-for N, om in ((1, None), (20, None), (5, (4, 1.0, 3))):
+# crowdsim_step_n_record_ex: the launch loop's recording at N = 1 and N = 20, occupancy-map rows at N = 5; then
+# crowdsim_step_n_record_rot (a unicycle target's rows) through both routes, N = 5 with maps and N = 20
+for N, om, unicycle in ((1, None, False), (20, None, False), (5, (4, 1.0, 3), False), (5, (4, 1.0, 3), True), (20, None, True)):
     env = make(128, N, rule='square_crossing' if N > 5 else 'circle_crossing')
     env.track_episodes(600); env.set_case_queue(0, 600, 'train'); env.enable_autoreset(); env.reset_seeds(use_queue=True); env.prefetch()
     for _ in range(6):
         env.step_n(4)                       # episodes near their end, so that the recorded launch stores some
     env.prefetch()
     mem = DeviceReplayMemory(400, N, env.device, 13 + (om[0] * om[0] * om[2] if om else 0))
-    rec = DeviceILRecorder(env, mem, 0.9, 16, om=om)
+    rec = DeviceILRecorder(env, mem, 0.9, 16, om=om, unicycle=unicycle)
     rec.begin()
     env.step(None, n_steps=16, record=rec)
-    print('N', N, 'maps', om, 'pairs recorded', rec.finish())
+    print('N', N, 'maps', om, 'unicycle rows', unicycle, 'pairs recorded', rec.finish())
 
 # reinforcement-learning recording (crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl): the ORCA
 # robot through the multi-step kernel (N = 5, with maps) and the launch loop (N = 20), a holonomic and a unicycle robot

@@ -10,10 +10,14 @@ alternated in one process, at each batch size. Reports episodes/s, pairs/s and t
 card's name and power limit.
 
   python scripts/time_il_rollout.py [--B 1024 4096] [--k 3000] [--reps 2] [--steps-per-launch 8] [--N 5] [--om C S CH]
+                                    [--unicycle]
 
 --N sets the crowd size (the device path runs the multi-step kernel at 2 <= N <= 5, the launch loop with its recording
 otherwise; N = 1 is CADRL's single-human IL scene; above 5 the scenes are square crossing), --om CELL_NUM CELL_SIZE CHANNELS records OM-SARL's rows with occupancy
-maps (the per-step recorder with om=..., BatchedExplorer with an OM target policy).
+maps (the per-step recorder with om=..., BatchedExplorer with an OM target policy). --unicycle records a unicycle target's
+rows (the theta column r_theta - rot, cadrl.py:205-209: TrajectoryRecorder(unicycle=True), BatchedExplorer with a target whose
+kinematics is 'unicycle', i.e. crowdsim_step_n_record_rot) and adds a third path, device_holonomic, the same device run with
+the holonomic rows, alternated with the other two so that the two row formats are timed side by side.
 """
 import argparse
 import json
@@ -31,7 +35,7 @@ from crowdnav_b200.explorer import BatchedExplorer  # noqa: E402
 from crowdnav_b200.memory import DeviceReplayMemory, TrajectoryRecorder  # noqa: E402
 
 GAMMA, CAPACITY = 0.9, 100000
-N, OM = 5, None                                              # set from --N / --om
+N, OM, UNICYCLE = 5, None, False                             # set from --N / --om / --unicycle
 
 
 def feature_dim():
@@ -53,7 +57,7 @@ def per_step(env, mem, k):
     env.enable_autoreset(env.train_val_sim)
     env.set_robot_policy('orca')
     env.reset_seeds(rule=env.train_val_sim, use_queue=True)
-    rec = TrajectoryRecorder(env, mem, GAMMA, True, om=OM)
+    rec = TrajectoryRecorder(env, mem, GAMMA, True, om=OM, unicycle=UNICYCLE)
     side = torch.cuda.Stream(device=env.device); main = torch.cuda.current_stream(env.device)
     it = 0
     while True:
@@ -69,8 +73,13 @@ def per_step(env, mem, k):
     env.autoreset = None
 
 
-def device(env, mem, k, steps_per_launch):
+def device(env, mem, k, steps_per_launch, unicycle=None):
+    """unicycle: the target's row kinematics (default: --unicycle)."""
+    unicycle = UNICYCLE if unicycle is None else unicycle
     target = types.SimpleNamespace(with_om=True, om=OM) if OM else None        # OM-SARL's transform (explorer.py:102)
+    if unicycle:
+        target = target or types.SimpleNamespace(with_om=False)
+        target.kinematics = 'unicycle'
     BatchedExplorer(env, 'orca', memory=mem, gamma=GAMMA, target_policy=target).run_k_episodes(k, 'train', update_memory=True,
                                                                          imitation_learning=True,
                                                                          steps_per_launch=steps_per_launch)
@@ -107,17 +116,22 @@ def main():
     ap.add_argument('--steps-per-launch', type=int, default=8)
     ap.add_argument('--N', type=int, default=5)
     ap.add_argument('--om', nargs=3, default=None, metavar=('CELL_NUM', 'CELL_SIZE', 'CHANNELS'))
+    ap.add_argument('--unicycle', action='store_true')
     args = ap.parse_args()
-    global N, OM
-    N = args.N
+    global N, OM, UNICYCLE
+    N, UNICYCLE = args.N, args.unicycle
     OM = (int(args.om[0]), float(args.om[1]), int(args.om[2])) if args.om else None
     workload = {} if (N, OM) == (5, None) else {'N': N, 'om': OM}   # (train.py's workload prints as it always did)
+    if UNICYCLE:
+        workload['unicycle'] = True
     assert torch.cuda.is_available(), 'needs a GPU'
     q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
     print(json.dumps({'device': torch.cuda.get_device_name(0), 'nvidia_smi_name_power_limit': q.stdout.strip().splitlines()[:1]}))
     for B in args.B:
         paths = {'per_step': lambda env, mem, k: per_step(env, mem, k),
                  'device': lambda env, mem, k: device(env, mem, k, args.steps_per_launch)}
+        if UNICYCLE:
+            paths['device_holonomic'] = lambda env, mem, k: device(env, mem, k, args.steps_per_launch, unicycle=False)
         for name, fn in paths.items():                      # warm-up: every kernel and allocation of the path
             fn(make_env(B), DeviceReplayMemory(CAPACITY, N, 'cuda', feature_dim()), min(args.k, 2 * B))
         mems = {}
@@ -138,6 +152,8 @@ def main():
         per_step(make_env(B), a, args.k)
         device(make_env(B), b, args.k, args.steps_per_launch)
         same = len(a) == len(b) and np.array_equal(pair_multiset(a), pair_multiset(b))
+        if UNICYCLE:
+            assert bool((b.states[:len(b), :, 2] != 0).any()), 'the device rows must carry the unicycle theta column'
         print(json.dumps({'B': B, 'pairs': len(a), 'timed_ring_size': [len(m) for m in mems.values()],
                           'same_pair_multiset': bool(same)}))
         assert same, 'the two recorders stored different pairs'
