@@ -67,6 +67,17 @@ class AutoReset(C.Structure):
 SLOT_EMPTY, SLOT_READY, SLOT_EXHAUSTED, SLOT_CLAIMED = 0, 1, 2, 3
 
 
+class MTStream(C.Structure):
+    """crowdsim_mt_stream: per-env MT19937 state of the policy's exploration draws ([624][B] words, [B] positions)."""
+    _fields_ = [('mt', C.c_void_p), ('pos', C.c_void_p)]
+
+
+class PolicyDraw(C.Structure):
+    """crowdsim_policy_draw: one decision's epsilon-greedy draws per env."""
+    _fields_ = [('epsilon', C.c_double), ('A', C.c_int32), ('train', C.c_int32), ('u', C.c_void_p), ('explored', C.c_void_p),
+                ('index', C.c_void_p), ('reached', C.c_void_p)]
+
+
 class Record(C.Structure):
     """crowdsim_record: one launch's imitation-learning staging, the per-slot trajectories and the memory ring."""
     _fields_ = [('rows', C.c_void_p), ('reward', C.c_void_p), ('t', C.c_void_p), ('code', C.c_void_p), ('n_max', C.c_int32),
@@ -124,6 +135,11 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
         f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(Record), P(RecordMaps), P(RecordRL), C.c_int] + s
     f = getattr(lib, prefix + 'prefetch_scenes')
     f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(AutoReset)] + s
+    if hasattr(lib, prefix + 'policy_draws'):
+        f = getattr(lib, prefix + 'policy_draws')
+        f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(State), P(Episodes), P(MTStream), P(PolicyDraw)] + s
+        f = getattr(lib, prefix + 'mt_streams')
+        f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(MTStream)] + s
     f = getattr(lib, prefix + 'orca_act')
     f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), C.c_void_p] + s
     f = getattr(lib, prefix + 'reset')
@@ -143,7 +159,8 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
 EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_count', 'crowdsim_debug_force_generic', 'crowdsim_graph_launch',
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
            'crowdsim_step_n_record_ex', 'crowdsim_step_n_record_rot', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
-           'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
+           'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes',
+           'crowdsim_policy_draws', 'crowdsim_mt_streams', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
            'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 
 # CROWDSIM_B200_LIB selects another build of the SAME library (A/B runs of kernel variants built into build_probe/);

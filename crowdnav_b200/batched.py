@@ -177,6 +177,8 @@ class BatchedCrowdSim(object):
         self.state = None; self.episodes = None; self.autoreset = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
+        self._scene_src = None                      # (rule, from the case queue?) of the scenes the envs now hold
+        self._draw_bufs = None
 
     # ---- configuration -------------------------------------------------------------------------------------------
     def configure(self, config):
@@ -220,6 +222,9 @@ class BatchedCrowdSim(object):
         self.obs32 = self.out_slab['obs32']
         self.write_obs32 = False                 # step() also writes the float32 observation (HostStepper(obs='f32'))
         self._seed32 = torch.zeros(B, dtype=torch.int32, device=self.device)
+        # the per-slot seed each env's current scene was generated from (reset_seeds without the case queue): a masked reset
+        # or a seed_stride rewrites _seed32 for slots whose scene it leaves alone, so policy_draws reads this copy
+        self._scene_seed32 = torch.zeros(B, dtype=torch.int32, device=self.device)
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -277,6 +282,14 @@ class BatchedCrowdSim(object):
         if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
             mask = torch.as_tensor(mask).to(device=self.device, dtype=torch.uint8)
         a = self._reset_args(mask, rule, seed_stride, use_queue)
+        q = use_queue and self._case_counter is not None
+        self._scene_src = (rule, q)
+        if not q:
+            # the seeds this call generates from, before a seed_stride advances them
+            if mask is None:
+                self._scene_seed32.copy_(self._seed32)
+            else:
+                self._scene_seed32.copy_(torch.where(mask != 0, self._seed32, self._scene_seed32))
         st = self.state.struct()
         ep = self.episodes.struct() if self.episodes is not None else None
         with torch.cuda.device(self.device):
@@ -304,6 +317,8 @@ class BatchedCrowdSim(object):
         self.autoreset = AutoResetBuffers(self.B, self.human_num, self.device, self.circle_radius, self.robot_radius,
                                           self.robot_v_pref)
         self._ar_rule, self._ar_seed_stride = rule, seed_stride
+        # installed scenes come from the case queue; per-slot prefetch seeds are not tracked (policy_draws refuses them)
+        self._scene_src = (rule, True) if self._case_counter is not None else (rule, None)
         return self.autoreset
 
     def prefetch(self):
@@ -312,6 +327,66 @@ class BatchedCrowdSim(object):
         with torch.cuda.device(self.device):
             rc = self.lib.crowdsim_prefetch_scenes(C.byref(a), self.B, self.human_num, C.byref(ar), self._stream())
         _abi.check(rc, 'crowdsim_prefetch_scenes')
+
+    # ---- exploration draws from numpy's stream ---------------------------------------------------------------------
+    def _stream_bufs(self):
+        """The live exploration streams of policy_draws and its outputs (one set per env batch)."""
+        if self._draw_bufs is None or self._draw_bufs['pos'].shape[0] != self.B:
+            z = lambda shape, dtype: torch.zeros(shape, dtype=dtype, device=self.device)  # noqa: E731
+            self._draw_bufs = {'mt': z((624, self.B), torch.int32), 'pos': z((self.B,), torch.int32),
+                               'u': z((self.B,), torch.float64), 'explored': z((self.B,), torch.uint8),
+                               'index': z((self.B,), torch.int32), 'reached': z((self.B,), torch.uint8)}
+        return self._draw_bufs
+
+    def policy_draws(self, epsilon, A, train):
+        """One decision's epsilon-greedy draws of MultiHumanRL.predict / CADRL.predict (multi_human_rl.py:22-30,
+        cadrl.py:144-151) per live env, from numpy's global stream as the reference's CrowdSim.reset leaves it
+        (crowdsim_policy_draws): an env whose robot has reached its goal draws nothing; the others draw
+        u = np.random.random() and, when `train` and u < epsilon, index = np.random.choice(A). Call it once per env-step.
+        The stream of an env is re-derived at its episode's first decision from the seed and the rule of its scene: the
+        case queue with its episode tracking, or the per-slot seed reset() / reset_seeds() last generated the slot's scene
+        from (masked resets and seed_stride included). Auto-reset from per-slot seeds is not followed (ValueError).
+        Returns device tensors (u [B] float64, -1 where nothing was drawn; explored [B] bool; index [B] int64;
+        reached [B] bool)."""
+        if self.episodes is None:
+            raise ValueError('policy_draws needs episode tracking (track_episodes)')
+        if self._scene_src is None:
+            raise ValueError('policy_draws needs the envs reset first')
+        rule, use_queue = self._scene_src
+        if use_queue is None:
+            raise ValueError('policy_draws follows scenes of the case queue or of reset_seeds, not per-slot auto-reset')
+        b = self._stream_bufs()
+        a = self._reset_args(None, rule, 0, use_queue)
+        if not use_queue:
+            a.seed = _ptr(self._scene_seed32)
+        st, ep = self.state.struct(), self.episodes.struct()
+        ms = _abi.MTStream(_ptr(b['mt']), _ptr(b['pos']))
+        d = _abi.PolicyDraw(float(epsilon), int(A), int(bool(train)), _ptr(b['u']), _ptr(b['explored']), _ptr(b['index']),
+                            _ptr(b['reached']))
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_policy_draws(C.byref(a), self.B, self.human_num, C.byref(st), C.byref(ep), C.byref(ms),
+                                                C.byref(d), self._stream())
+        _abi.check(rc, 'crowdsim_policy_draws')
+        return b['u'], b['explored'].bool(), b['index'].long(), b['reached'].bool()
+
+    def mt_streams(self, seeds=None, rule='circle_crossing'):
+        """numpy's generator state after the reset of per-slot seeds (crowdsim_mt_streams): (words [624][B] int32 holding
+        uint32 bit patterns, pos [B] int32) in new tensors, lazily twisted as include/crowdsim_b200.h describes; see
+        numpy_state() for numpy's own representation. seeds: [B] integers (default: the seeds of the scenes reset_seeds
+        last generated). Touches neither the per-slot seeds nor policy_draws' streams."""
+        seed32 = self._scene_seed32
+        if seeds is not None:
+            seeds = torch.as_tensor(seeds, dtype=torch.int64).to(self.device)
+            seed32 = ((seeds + 2 ** 31) % 2 ** 32 - 2 ** 31).to(torch.int32)
+        words = torch.empty((624, self.B), dtype=torch.int32, device=self.device)
+        pos = torch.empty((self.B,), dtype=torch.int32, device=self.device)
+        a = self._reset_args(None, rule, 0, False)
+        a.seed = _ptr(seed32)
+        ms = _abi.MTStream(_ptr(words), _ptr(pos))
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_mt_streams(C.byref(a), self.B, self.human_num, C.byref(ms), self._stream())
+        _abi.check(rc, 'crowdsim_mt_streams')
+        return words, pos
 
     # ---- step ----------------------------------------------------------------------------------------------------
     def step(self, actions=None, n_steps=1, record=None):
@@ -694,6 +769,21 @@ class HostStepperGroup(object):
 
     def wait(self):
         return [s.wait() for s in self.steppers]
+
+
+def numpy_state(words, pos):
+    """numpy's RandomState.get_state() tuple for one env's device stream (words: 624 uint32 bit patterns, pos: 0..623).
+    The device twists lazily: words [pos, 624) are still the previous block's. pos == 0 is numpy's pos 624 with the words
+    as they are -- both "just seeded" and "a whole block consumed" continue with a full twist; otherwise the twist of the
+    current block is completed on a copy and numpy's pos is the device's."""
+    key = np.asarray(words).astype(np.uint32).copy()
+    pos = int(pos)
+    if pos == 0:
+        return ('MT19937', key, 624, 0, 0.0)
+    for i in range(pos, 624):                          # the in-place twist, in the device's order (scene.cuh MT::next)
+        y = (int(key[i]) & 0x80000000) | (int(key[(i + 1) % 624]) & 0x7fffffff)
+        key[i] = int(key[(i + 397) % 624]) ^ (y >> 1) ^ (0x9908b0df if y & 1 else 0)
+    return ('MT19937', key, pos, 0, 0.0)
 
 
 def default_config(human_num=5, test_sim='circle_crossing', train_val_sim='circle_crossing', robot_visible=False,

@@ -34,8 +34,12 @@ def _module(name, **attrs):
     return m
 
 
-def install(force_gym_shim=False):
+def install(force_gym_shim=False, numpy_stream=False):
+    """numpy_stream=True: CrowdSim.reset leaves np.random in the state the reference's reset leaves it in (the case's seed
+    advanced by the scene generator's draws), so the reference's own policies explore from the reference's stream. The
+    hand-placed debug scene (test case -1) is not seeded by the reference either: numpy's state is left alone there."""
     t = state_types
+    crowd_sim_env.NUMPY_STREAM = bool(numpy_stream)
     _module('crowd_sim')
     _module('crowd_sim.envs', CrowdSim=CrowdSim)
     _module('crowd_sim.envs.crowd_sim', CrowdSim=CrowdSim)

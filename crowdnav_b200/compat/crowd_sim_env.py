@@ -14,9 +14,14 @@ import logging
 import numpy as np
 import torch
 
-from ..batched import BatchedCrowdSim
+from ..batched import BatchedCrowdSim, numpy_state
 from .agents import Human
 from .statetypes import ActionRot, ObservableState, info_from_code
+
+# compat.install(numpy_stream=True): reset() leaves numpy's global generator where the reference's reset leaves it (seeded
+# with the case's seed, then advanced by the scene generator's draws), so that a policy drawing from np.random -- the
+# reference's own MultiHumanRL / CADRL explore that way -- continues the reference's stream
+NUMPY_STREAM = False
 
 
 class CrowdSim(object):
@@ -112,6 +117,9 @@ class CrowdSim(object):
             if eng.human_num != n_slots:
                 eng.human_num = n_slots; eng._alloc()
             eng.reset(phase, cases=[case], rule=rule)
+            if NUMPY_STREAM:
+                words, pos = eng.mt_streams(rule=rule)        # the seed reset() just used
+                np.random.set_state(numpy_state(words[:, 0].cpu().numpy(), int(pos[0])))
             self.case_counter[phase] = (case + 1) % self.case_size[phase]
             n = n_slots
             if rule == 'mixed':

@@ -119,9 +119,11 @@ class BatchedValuePolicy(object):
     """One-step-lookahead policy over a value network (MultiHumanRL.predict / CADRL.predict): greedy in the test / val
     phases, epsilon-greedy in the train phase (multi_human_rl.py:27-31, cadrl.py:148-152: with probability epsilon a
     uniformly drawn action of the 81-action space). The reference draws from numpy's GLOBAL generator (re-seeded by every
-    env.reset, shared with scenario generation); here every env has its own uniform draw from a torch.Generator on the
-    policy's device (set_seed): same distribution, a different random stream -- RL-phase rollouts are statistically, not
-    bitwise, reproductions of the reference's.
+    env.reset, shared with scenario generation). exploration='torch' (default): every env has its own uniform draw from a
+    torch.Generator on the policy's device (set_seed): same distribution, a different random stream -- RL-phase rollouts
+    are statistically, not bitwise, reproductions of the reference's. exploration='numpy': the draws come from each env's
+    copy of numpy's stream as the reference's reset leaves it (env.policy_draws, once per act_batch), so the exploring
+    decisions are the reference's own; the env needs episode tracking.
 
     act_batch(env) -> [B][2] float64 device tensor with, per env,
         argmax_a  reward(s, a) + gamma ** (time_step * v_pref) * V(rotate(next_state(s, a)))       multi_human_rl.py:52
@@ -141,9 +143,12 @@ class BatchedValuePolicy(object):
 
     def __init__(self, model, gamma=0.9, v_pref=1.0, time_step=0.25, joint=True, speed_samples=5, rotation_samples=16,
                  with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3, query_env=True, kinematics='holonomic',
-                 order_by_distance=False):
+                 order_by_distance=False, exploration='torch'):
         if kinematics not in ('holonomic', 'unicycle'):
             raise ValueError('kinematics must be holonomic or unicycle, not %r' % (kinematics,))
+        if exploration not in ('torch', 'numpy'):
+            raise ValueError('exploration must be torch or numpy, not %r' % (exploration,))
+        self.exploration = exploration
         if not joint and not query_env:
             raise ValueError('CADRL always queries the env (cadrl.py:156-170): query_env=False needs a joint policy')
         self.model = model
@@ -220,8 +225,16 @@ class BatchedValuePolicy(object):
             v = self.model(states.view(B * A * N, 13)).view(B, A, N).min(dim=2).values
         values = reward + discount * v.double()                        # python-float arithmetic in the reference
         self.action_values = values
-        best = values.argmax(dim=1)
+        best = values.argmax(dim=1)                                    # the first maximum, like predict's strict >
         self.explored = None
+        if self.exploration == 'numpy':                                # every phase draws (multi_human_rl.py:26)
+            _, explored, index, reached = env.policy_draws(self.epsilon, A, self.phase == 'train')
+            if self.phase == 'train':
+                self.explored = explored
+                best = torch.where(explored, index, best)
+            # the kernel's reach_destination decided which envs drew: the zero action follows the same decision
+            act = self.actions[best]
+            return torch.where(reached.unsqueeze(1), torch.zeros_like(act), act)
         if self.phase == 'train' and self.epsilon > 0.0:                # epsilon-greedy (multi_human_rl.py:27-31)
             if self._gen is None:
                 self._gen = torch.Generator(device=self.device); self._gen.manual_seed(self._seed)
@@ -237,7 +250,7 @@ class BatchedValuePolicy(object):
 
 
 def make_sarl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_om=False, cell_num=4, cell_size=1.0,
-              om_channel_size=3, query_env=True, kinematics='holonomic', **net_kw):
+              om_channel_size=3, query_env=True, kinematics='holonomic', exploration='torch', **net_kw):
     """SARL with the reference's default architecture (crowd_nav/configs/policy.config:43-50); random-init weights when
     no checkpoint is loaded (there are no checkpoints in the reference repo). with_om=True gives OM-SARL: input_dim grows
     by cell_num^2 * om_channel_size (multi_human_rl.py:106-107)."""
@@ -247,23 +260,24 @@ def make_sarl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_om=False, c
         net_kw.setdefault('input_dim', 13 + cell_num * cell_num * om_channel_size)
     p = BatchedValuePolicy(SARLValueNetwork(**net_kw), gamma, v_pref, time_step, joint=True, with_om=with_om,
                            cell_num=cell_num, cell_size=cell_size, om_channel_size=om_channel_size, query_env=query_env,
-                           kinematics=kinematics)
+                           kinematics=kinematics, exploration=exploration)
     p.name = 'OM-SARL' if with_om else 'SARL'
     return p
 
 
-def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='holonomic'):
+def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='holonomic', exploration='torch'):
     """CADRL queries the env whatever policy.config's query_env says (cadrl.py:156-170), so there is no query_env here."""
     if seed is not None:
         torch.manual_seed(seed)
-    p = BatchedValuePolicy(CADRLValueNetwork(), gamma, v_pref, time_step, joint=False, kinematics=kinematics)
+    p = BatchedValuePolicy(CADRLValueNetwork(), gamma, v_pref, time_step, joint=False, kinematics=kinematics,
+                           exploration=exploration)
     p.name = 'CADRL'
     p.multiagent_training = False
     return p
 
 
 def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interaction_module=False, query_env=True,
-                 kinematics='holonomic'):
+                 kinematics='holonomic', exploration='torch'):
     """LSTM-RL with the reference's default sizes (crowd_nav/configs/policy.config:24-31). With query_env=False its rows
     follow the reference's sort of the humans by decreasing distance to the robot (lstm_rl.py:99-103)."""
     if seed is not None:
@@ -271,6 +285,6 @@ def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interact
     net = LSTMRLValueNetwork(mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
                              mlp1_dims=(150, 100, 100, 50) if with_interaction_module else None)
     p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True, query_env=query_env, kinematics=kinematics,
-                           order_by_distance=not query_env)
+                           order_by_distance=not query_env, exploration=exploration)
     p.name = 'LSTM-RL'
     return p

@@ -31,6 +31,9 @@
  *   crowdsim_reset           crowd_sim/envs/crowd_sim.py:251-312 + generators :155-207 (np.random MT19937)
  *   crowdsim_prefetch_scenes the same generators, run ahead of time for the NEXT episode of each env slot
  *                            (explorer.py:35-36: reset() of the following episode)
+ *   crowdsim_policy_draws    the epsilon-greedy draws of MultiHumanRL.predict / CADRL.predict (multi_human_rl.py:22-30,
+ *                            cadrl.py:144-151) from numpy's global generator as CrowdSim.reset leaves it
+ *   crowdsim_mt_streams      ... that generator's state after the reset of given seeds
  *   crowdsim_lookahead_pack  crowd_nav/policy/multi_human_rl.py:35-45 = 81 x env.onestep_lookahead
  *                            (crowd_sim.py:314-315,414-416) + CADRL.propagate (cadrl.py:104-129) +
  *                            CADRL.rotate (cadrl.py:187-222), fused
@@ -406,6 +409,51 @@ int crowdsim_reset(const crowdsim_reset_args *args, int B, int N, crowdsim_state
 
 /* Fill the EMPTY next-scene slots of `ar` (generator side of the auto-reset protocol above). `args->mask` is ignored. */
 int crowdsim_prefetch_scenes(const crowdsim_reset_args *args, int B, int N, const crowdsim_autoreset *ar, void *stream);
+
+/*
+ * Exploration draws of a value-network robot policy from numpy's global MT19937 stream, as the reference makes them:
+ * CrowdSim.reset seeds the generator (crowd_sim.py:276) and the scene generator draws from it; until the next reset only
+ * MultiHumanRL.predict / CADRL.predict draw (multi_human_rl.py:22-30, cadrl.py:144-151).
+ *
+ * crowdsim_mt_stream: one generator per env, between two decisions. Word i of env e is mt[i * B + e]. The twist is lazy:
+ * words [0, pos) belong to the current block and words [pos, 624) are still the previous block's; pos == 0 is numpy's
+ * pos 624 with key = the words as they are ("just seeded" or "a whole block consumed", which continue the same way). For
+ * pos > 0, numpy's key is the block completed by the in-place twist of words pos..623, with numpy's pos = pos.
+ */
+typedef struct crowdsim_mt_stream {
+    uint32_t *mt;            /* [624][B] */
+    int32_t *pos;            /* [B] next word, 0..623 */
+} crowdsim_mt_stream;
+
+/* One decision's draws per env. Outputs are written for every env; an env that draws nothing gets u = -1, explored = 0,
+ * index = 0. */
+typedef struct crowdsim_policy_draw {
+    double epsilon;          /* policy.set_epsilon */
+    int32_t A;               /* len(action_space), >= 1 */
+    int32_t train;           /* 1 = train phase: draw the random action when u < epsilon */
+    double *u;               /* [B] np.random.random() */
+    uint8_t *explored;       /* [B] train && u < epsilon */
+    int32_t *index;          /* [B] np.random.choice(A) where explored: masked rejection with the smallest 2^k - 1 >= A - 1 */
+    uint8_t *reached;        /* [B] reach_destination (policy.py:41-48): sqrt(dy * dy + dx * dx) < radius, no draw */
+} crowdsim_policy_draw;
+
+/*
+ * One policy decision of every live env (st->active[e] != 0): if its robot has reached its goal it draws nothing;
+ * otherwise u = genrand_res53 and, when train && u < epsilon, index = the choice of one of A actions. Call it once per
+ * env-step, as the reference calls predict once per step. At the first decision of an episode (ep->ep_steps[e] == 0) the
+ * env's stream is first re-derived: seeded with the seed of its current scene and run through the generator of `args`
+ * (the same rule and parameters that generated the scene), which leaves it where the reference's reset leaves numpy's.
+ * The scene's seed: with args->case_counter, queue entry ep->ep_case[e] (crowdsim_reset_args' derivation; ep_case
+ * required); otherwise args->seed[e], with seed_stride == 0 (CROWDSIM_EUNSUPPORTED otherwise). Reads active, r_pos,
+ * r_goal, r_attr and ep_steps (CROWDSIM_EINVAL without them, without `ep` or without the stream's buffers).
+ */
+int crowdsim_policy_draws(const crowdsim_reset_args *args, int B, int N, const crowdsim_state *st,
+                          const crowdsim_episodes *ep, const crowdsim_mt_stream *ms, const crowdsim_policy_draw *d,
+                          void *stream);
+
+/* The stream each env is left with after crowdsim_reset from its per-slot seed args->seed[e] (envs selected by
+ * args->mask, NULL = all). Needs args->seed; the case queue and seed_stride != 0 return CROWDSIM_EUNSUPPORTED. */
+int crowdsim_mt_streams(const crowdsim_reset_args *args, int B, int N, const crowdsim_mt_stream *ms, void *stream);
 
 /*
  * Rotated joint state of the CURRENT state for value-net policies: out[B][N][13] float32

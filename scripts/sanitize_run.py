@@ -9,7 +9,8 @@ row tiles), occupancy maps, human_times, the recording multi-step kernel with it
 crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
 at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush), both routes of crowdsim_step_n_record_rot
 (a unicycle target's rows), and the reinforcement-learning recording
-(crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl) for the ORCA robot and external robots."""
+(crowdsim_record_book, crowdsim_record_flush_maps, crowdsim_record_flush_rl) for the ORCA robot and external robots, and the
+exploration draws from numpy's stream (crowdsim_mt_streams, crowdsim_policy_draws at N = 63 with starting and running envs)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -104,5 +105,10 @@ env = make(16, 20, policy='external_xy', rule='square_crossing'); env.reset_seed
 env.lookahead_pack(acts); env.human_times(max_steps=20)
 env = make(3, 63, policy='external_xy', rule='square_crossing'); env.reset_seeds(torch.arange(3) + 1000, rule='square_crossing')
 env.propagate_pack(torch.rand((200, 2), dtype=torch.float64, device=env.device), order_by_distance=True)   # several tiles
+# exploration draws from numpy's stream: the post-generation streams, then decisions with episodes starting and running
+env = make(200, 63, policy='external_xy', rule='square_crossing'); env.track_episodes(200)
+env.reset_seeds(torch.arange(200) + 2000, rule='square_crossing'); env.mt_streams(rule='square_crossing')
+for dec in range(3):
+    env.policy_draws(0.5, 81, True); env.episodes.ep_steps[::3] = dec + 1
 torch.cuda.synchronize()
 print('sanitize run done, launches:', lib.crowdsim_launch_count())
