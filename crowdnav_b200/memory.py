@@ -15,8 +15,10 @@
                        stepped with external actions (holonomic or unicycle): same pairs, same order and same rows as
                        TrajectoryRecorder; the values differ only by how the batch a target network sees rounds
 The IL return is accumulated forward in t (G_i += pow(...) * r_t as each reward arrives), i.e. in the same order and
-with the same pow() factors as the reference's sum(); it agrees to the last ulp of float64 (CPython >= 3.12 sums with
-Neumaier compensation) and is identical after the float32 cast the reference applies.
+with the same pow() factors as the reference's sum(). That is the project's summation rule for every discounted return: a
+plain left fold from +0.0, one rounding per product and per sum, which is sum() before CPython 3.12. CPython 3.12's
+compensated sum() can differ in the last float64 bits; after the float32 cast the reference applies to this value the
+two agree on every recorded episode (tests/test_returns_cpu.py).
 """
 import torch
 

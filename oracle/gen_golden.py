@@ -64,6 +64,17 @@ def R(x):
     return repr(float(x))
 
 
+def discounted_return(gamma, time_step, v_pref, rewards):
+    """explorer.py:71-72, sum([pow(gamma, t * time_step * v_pref) * r ...]), as a plain left fold from +0.0: each product
+    and each sum rounded once, in ascending t. That is sum() before CPython 3.12, the interpreter the reference was
+    written for, and what the step kernels and the CPU oracle accumulate. CPython 3.12's sum() of floats is compensated
+    (Neumaier) and can differ in the last bits, so the fixtures never call sum() on a return."""
+    ret = 0.0
+    for t, r in enumerate(rewards):
+        ret = ret + pow(gamma, t * time_step * v_pref) * float(r)
+    return ret
+
+
 def make_env(human_num=5, test_sim='circle_crossing', robot_visible=False, randomize=False, policy_name='orca',
              policy_config=None, profile=None, safety_space=0):
     """profile: a tests/util.py PROFILES entry whose env.config values are written into the config the reference reads;
@@ -157,7 +168,7 @@ def run_suite(name, cases, phase='test', gamma=0.9, record_traj=(), fresh_robot_
                               'done': bool(done), 'info': INFO_CODE[type(info)],
                               'dmin': R(info.min_dist) if isinstance(info, Danger) else None,
                               'post': scene(env), 'global_time': R(env.global_time)})
-        ret = sum([pow(gamma, t * robot.time_step * robot.v_pref) * r for t, r in enumerate(rewards)])
+        ret = discounted_return(gamma, robot.time_step, robot.v_pref, rewards)
         total_steps += len(rewards)
         per_case.append({'case': case, 'info': INFO_CODE[type(info)], 'steps': len(rewards),
                          'global_time': R(env.global_time), 'return': R(ret), 'too_close': too_close,

@@ -30,7 +30,7 @@ import os
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle'))
-from gen_golden import R, REF, OUT, INFO_CODE, make_env, configparser  # noqa: E402
+from gen_golden import R, REF, OUT, INFO_CODE, make_env, configparser, discounted_return  # noqa: E402
 from gen_golden import np, torch, Explorer  # noqa: E402
 
 GAMMA = 0.9
@@ -143,8 +143,8 @@ def run_block(tag, policy, N, rule, k, epsilon, randomize=False, profile=None, r
     assert len(resets) == k
     if steps:
         ts, vp = env.time_step, robot.v_pref
-        for ep in episodes:          # explorer.py:71-72
-            ep['result']['return'] = R(sum(pow(GAMMA, t * ts * vp) * float(s['reward']) for t, s in enumerate(ep['steps'])))
+        for ep in episodes:          # explorer.py:71-72, as a plain fold whatever the interpreter's sum() does
+            ep['result']['return'] = R(discounted_return(GAMMA, ts, vp, [s['reward'] for s in ep['steps']]))
     kept = None
     if steps:
         kept = [i for i, ep in enumerate(episodes) if all(s.get('margin', 1.0) > 1e-4 for s in ep['steps'])]

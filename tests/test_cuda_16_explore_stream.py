@@ -112,25 +112,57 @@ def _block_env(block, B):
 
 
 def _reward_tol(block):
-    """Bit for bit, except: a unicycle robot's pose comes from CUDA's cos / sin (poses and rewards within 1e-12); in the
-    one-human CADRL scenes one Danger reward of the env's own step differs from the reference's in its last bits (DESIGN
-    section 8: the env step, not the draws; every draw and action there is exact)."""
-    if block['kinematics'] == 'unicycle':
-        return 1e-12
-    return 1e-15 if block['tag'] == 'cadrl1' else 0.0
+    """Bit for bit, except: a unicycle robot's pose comes from CUDA's cos / sin (poses and rewards within 1e-12)."""
+    return 1e-12 if block['kinematics'] == 'unicycle' else 0.0
+
+
+def _reference_scenes(block, oracle):
+    """The block's train scenes as the reference generated them: the CPU oracle's reset of seeds 2000 + case (glibc's cos /
+    sin, which reproduce every recorded reset)."""
+    p = util.profile(block['profile'])
+    k, N = block['k'], eo.block_humans(block)
+    host = oracle.HostState(k, N)
+    oracle.reset(host, np.arange(2000, 2000 + k, dtype=np.uint32), block['rule'] if block['multiagent_training'] else 'circle_crossing',
+                 randomize_attributes=bool(block['randomize']), **util.reset_kw(block['profile']))
+    assert host.r_attr[0, 1] == p['robot_v_pref']
+    return host
+
+
+def _device_scenes_match(env, host):
+    """Per env: the device-generated scene equals the reference's bit for bit. Circle scenes place humans with CUDA's
+    double cos / sin, so a coordinate can be one ulp from the reference's (DESIGN section 4: within 2e-15)."""
+    dev = env.state.to_host()
+    same = np.ones(host.B, dtype=bool)
+    for f in ('h_pos', 'h_goal', 'h_attr', 'r_pos', 'r_goal', 'r_attr'):
+        a, b = dev[f], getattr(host, f)
+        assert np.abs(a - b).max() <= 2e-15, f
+        same &= (a.reshape(host.B, -1).view(np.uint64) == b.reshape(host.B, -1).view(np.uint64)).all(1)
+    return same
 
 
 STEP_BLOCKS = [b['tag'] for b in eo.golden() if b['episodes'] is not None]
 
 
 @pytest.mark.parametrize('tag', STEP_BLOCKS)
-def test_lockstep_reproduces_reference_decisions(tag):
-    """One env per recorded episode, stepped in lockstep: every draw, action, reward and info as the reference's."""
+def test_lockstep_reproduces_reference_decisions(tag, oracle):
+    """One env per recorded episode, stepped in lockstep from the reference's own scenes: every draw, action, reward and
+    info as the reference's. A holonomic robot's steps are also replayed through the CPU oracle with the same actions, and
+    every step's reward, dmin and info and the whole state after it must be the oracle's bit for bit."""
+    from crowdnav_b200 import _abi
     block = next(b for b in eo.golden() if b['tag'] == tag)
     k = block['k']
     env, rule = _block_env(block, k)
     env.track_episodes(k, block['gamma'])
     env.reset('train', cases=list(range(k)), rule=rule)
+    host = _reference_scenes(block, oracle)
+    _device_scenes_match(env, host)
+    env.state.load_host(host)                         # the draws still follow each slot's scene seed
+    replay = block['kinematics'] == 'holonomic'
+    prm = util.profile_params(oracle, block['profile'], robot_policy=_abi.ROBOT_EXTERNAL_XY)
+    io = oracle.HostStepIO(k)
+    p = util.profile(block['profile'])
+    host_ep = oracle.HostEpisodes(k, k, block['gamma'], p['time_step'], p['robot_v_pref'], float(p['time_limit']))
+    host_ep.ep_case[:] = np.arange(k)                 # (the episode bookkeeping ends an episode, as on the device)
     pol = _policy(block, env.device)
     space = torch.from_numpy(pol.action_space_np)
     done = np.zeros(k, dtype=bool)
@@ -144,6 +176,15 @@ def test_lockstep_reproduces_reference_decisions(tag):
         env.step(act.to(env.device))
         reward, info = env.reward.cpu().numpy(), env.info.cpu().numpy()
         r_pos, r_theta = env.state.r_pos.cpu().numpy(), env.state.r_theta.cpu().numpy()
+        if replay:
+            live = host.active.astype(bool)
+            io.action[...] = act.numpy()
+            oracle.step(prm, host, io, host_ep)
+            for f, got in (('reward', reward), ('dmin', env.dmin.cpu().numpy()), ('info', info)):
+                util.assert_same_bits(got[live], getattr(io, f)[live], '%s step %d: %s against the oracle' % (tag, t, f))
+            dev = env.state.to_host()
+            for f in ('h_pos', 'h_vel', 'r_pos', 'r_vel', 'g_time', 'active'):
+                util.assert_same_bits(dev[f], getattr(host, f), '%s step %d: %s against the oracle' % (tag, t, f))
         for e in range(k):
             if done[e]:
                 continue
@@ -165,30 +206,84 @@ def test_lockstep_reproduces_reference_decisions(tag):
                 assert info[e] in (2, 3, 4), where
                 done[e] = True
         t += 1
+    if replay:                                        # each slot's discounted return: the oracle's and the reference's
+        kept = [e for e in range(k) if block['kept'] is None or e in block['kept']]
+        got = env.episodes.ep_return.cpu().numpy()[kept]
+        util.assert_same_bits(got, host_ep.ep_return[kept], tag + ': returns against the oracle')
+        for j, e in enumerate(kept):
+            assert got[j] == float(block['episodes'][e]['result']['return']), (tag, e)
 
 
-# DESIGN section 8: in these auto-reset runs a discounted return differs from the reference's in its last bit although the
-# same episodes stepped without auto-reset reproduce every reward bit for bit; the env step's, not the draws'
-RETURN_TOL = {'sarl_const_eps05': 1e-15, 'sarl_a33': 1e-15, 'cadrl1': 1e-15}
+def _replayed_returns(block, oracle, host):
+    """The return of every episode of the block when the fixture's actions are replayed through the CPU oracle from the
+    scenes in `host`, accumulated by the oracle's episode bookkeeping (the plain fold of tests/test_returns_cpu.py)."""
+    from crowdnav_b200 import _abi
+    p = util.profile(block['profile'])
+    k = block['k']
+    prm = util.profile_params(oracle, block['profile'], robot_policy=_abi.ROBOT_EXTERNAL_XY)
+    ep = oracle.HostEpisodes(k, k, block['gamma'], p['time_step'], p['robot_v_pref'], float(p['time_limit']))
+    ep.ep_case[:] = np.arange(k)
+    io = oracle.HostStepIO(k)
+    from crowdnav_b200.policy import build_action_space
+    space = build_action_space(p['robot_v_pref'], block['speed_samples'], block['rotation_samples'])
+    for t in range(max(len(e['steps']) for e in block['episodes'])):
+        for e, episode in enumerate(block['episodes']):
+            s = episode['steps'][t] if t < len(episode['steps']) else None
+            io.action[e] = space[s['index']] if s is not None and s['u'] is not None else 0.0
+        oracle.step(prm, host, io, ep)
+    assert not host.active.any()
+    return ep.res_return
 
 
-@pytest.mark.parametrize('tag', ['sarl_const_eps05', 'cadrl1', 'sarl_a33', 'sarl_const_eps1'])
-def test_explorer_with_auto_reset_reproduces_episode_rows(tag):
-    """B < k: slots take the next case when their episode ends and re-derive their stream from the new scene's seed."""
+AUTO_RESET_BLOCKS = ['sarl_const_eps1', 'sarl_seeded', 'sarl_unicycle', 'sarl_const_eps05', 'sarl_const_eps01', 'cadrl1',
+                     'square_random', 'circle_envcfg', 'sarl_a33']
+
+
+def test_auto_reset_blocks_cover_every_block_with_episodes():
+    assert sorted(AUTO_RESET_BLOCKS) == sorted(STEP_BLOCKS)
+
+
+@pytest.mark.parametrize('tag', AUTO_RESET_BLOCKS)
+def test_explorer_with_auto_reset_reproduces_episode_rows(tag, oracle):
+    """B < k: slots take the next case when their episode ends and re-derive their stream from the new scene's seed.
+    Every row equals the reference's. A holonomic return equals, bit for bit, the fixture's actions replayed through the
+    CPU oracle from the scenes the device generates, and the fixture's own return wherever that scene is the reference's
+    bit for bit (circle scenes come from CUDA's cos / sin, one ulp from the reference's in some coordinates, DESIGN
+    section 8). A unicycle robot's return is within 1e-12 of the fixture's: its rewards come from poses that CUDA's cos /
+    sin place within 1e-12."""
     from crowdnav_b200.explorer import BatchedExplorer
     block = next(b for b in eo.golden() if b['tag'] == tag)
+    k = block['k']
     env, _ = _block_env(block, 2)
     pol = _policy(block, env.device)
     ex = BatchedExplorer(env, pol, gamma=block['gamma'])
-    ex.run_k_episodes(block['k'], 'train')
+    ex.run_k_episodes(k, 'train')
     rows = ex.last_rows.cpu().numpy()
     time_limit = float(util.profile(block['profile'])['time_limit'])
+    unicycle = block['kinematics'] == 'unicycle'
+    if not unicycle:
+        gen, rule = _block_env(block, k)              # the device's scenes of cases 0 .. k-1, as the auto-reset installs them
+        gen.reset('train', cases=list(range(k)), rule=rule)
+        ref = _reference_scenes(block, oracle)
+        same = _device_scenes_match(gen, ref)
+        dev = oracle.HostState(k, eo.block_humans(block))
+        dev_state = gen.state.to_host()
+        for f in oracle.HostState.FIELDS:
+            getattr(dev, f)[...] = dev_state[f]
+        want = _replayed_returns(block, oracle, dev)
     for i, ep in enumerate(block['episodes']):
+        if block['kept'] is not None and i not in block['kept']:
+            continue                                  # seeded weights: a near-tie can reorder the other episodes' argmax
         r = ep['result']
         assert rows[i, 0] == r['info'] and rows[i, 1] == r['steps'], (tag, i)
         # a timeout's time is time_limit (explorer.py:62), the fixture holds env.global_time
         assert rows[i, 2] == (time_limit if r['info'] == 4 else float(r['time'])), (tag, i)
-        assert abs(rows[i, 3] - float(r['return'])) <= RETURN_TOL.get(tag, 0.0), (tag, i)
+        if unicycle:
+            assert abs(rows[i, 3] - float(r['return'])) <= 1e-12, (tag, i)
+            continue
+        util.assert_same_bits(rows[i, 3:4], want[i:i + 1], '%s episode %d: return against the oracle replay' % (tag, i))
+        if same[i]:
+            assert rows[i, 3] == float(r['return']), (tag, i)
 
 
 def test_compat_numpy_stream():
