@@ -55,7 +55,8 @@ class ResetArgs(C.Structure):
                 ('human_v_pref', C.c_double), ('robot_radius', C.c_double), ('robot_v_pref', C.c_double),
                 ('discomfort_dist', C.c_double), ('randomize_attributes', C.c_int32),
                 ('case_counter', C.c_void_p), ('case_total', C.c_int32),
-                ('seed_base', C.c_uint32), ('case_first', C.c_int32), ('case_wrap', C.c_int32)]
+                ('seed_base', C.c_uint32), ('case_first', C.c_int32), ('case_wrap', C.c_int32),
+                ('scene_mt', C.c_void_p)]
 
 
 class AutoReset(C.Structure):

@@ -225,6 +225,9 @@ class BatchedCrowdSim(object):
         # the per-slot seed each env's current scene was generated from (reset_seeds without the case queue): a masked reset
         # or a seed_stride rewrites _seed32 for slots whose scene it leaves alone, so policy_draws reads this copy
         self._scene_seed32 = torch.zeros(B, dtype=torch.int32, device=self.device)
+        # MT19937 state of the scene being generated for each slot (crowdsim_reset_args.scene_mt): reset and prefetch
+        # run on this batch's streams one after the other, so they share it
+        self._scene_mt = torch.empty((624, B), dtype=torch.int32, device=self.device)
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -271,7 +274,7 @@ class BatchedCrowdSim(object):
                               self.square_width, self.human_radius, self.human_v_pref, self.robot_radius, self.robot_v_pref,
                               self.discomfort_dist, int(bool(self.randomize_attributes)),
                               _ptr(self._case_counter) if q else None, self._case_total if q else 0, self._seed_base if q else 0,
-                              self._case_first if q else 0, self._case_wrap if q else 0)
+                              self._case_first if q else 0, self._case_wrap if q else 0, _ptr(self._scene_mt))
 
     def reset_seeds(self, seeds=None, mask=None, rule='circle_crossing', seed_stride=0, use_queue=False):
         """crowdsim_reset for the envs selected by `mask` (uint8 device tensor, None = all) from the per-slot seeds.

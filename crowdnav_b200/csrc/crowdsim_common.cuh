@@ -101,6 +101,61 @@ __device__ __forceinline__ double2 ld2_cg(const double *p, size_t i) { return __
 __device__ __forceinline__ uint8_t ld_relaxed_u8(const uint8_t *p) { unsigned v; asm volatile("ld.relaxed.gpu.global.u8 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return (uint8_t)v; }
 __device__ __forceinline__ uint8_t ld_acquire_u8(const uint8_t *p) { unsigned v; asm volatile("ld.acquire.gpu.global.u8 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return (uint8_t)v; }
 __device__ __forceinline__ void st_release_u8(uint8_t *p, uint8_t v) { asm volatile("st.release.gpu.global.u8 [%0], %1;" :: "l"(p), "r"((unsigned)v) : "memory"); }
+// After a batch of ld_relaxed_u8: every flag read before the fence acts as an ld.acquire (PTX acquire pattern), without
+// the acquire loads' one-at-a-time round trips.
+__device__ __forceinline__ void fence_acquire_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+
+// Residency probe (-DCS_RESIDENCY_PROBE, scripts/residency_probe.py): thread 0 of every multi-step block (crowdsim_step_n)
+// and every refill block appends its %smid, the %globaltimer at its start and at its end, and its kind to this translation
+// unit's g_res, read and cleared through crowdsim_residency_probe_step / _refill. Without the define the hooks are empty
+// and the kernels' SASS is what it is without them.
+#define CS_RES_STEP 0
+#define CS_RES_ASSIGN 1
+#define CS_RES_SCENE 2
+#ifdef CS_RESIDENCY_PROBE
+struct ResRec { unsigned long long t0, t1; unsigned smid, kind; };
+constexpr unsigned kResCap = 1u << 18;
+static __device__ ResRec g_res[kResCap];
+static __device__ unsigned g_res_n;
+__device__ __forceinline__ unsigned long long res_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+#define CS_RES_BEGIN const unsigned long long res_t0_ = res_now();
+#define CS_RES_END(kind) do { if (threadIdx.x == 0) {                                                                       \
+        unsigned smid_; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid_));                                              \
+        const unsigned i_ = atomicAdd(&g_res_n, 1u);                                                                     \
+        if (i_ < kResCap) g_res[i_] = ResRec{res_t0_, res_now(), smid_, (unsigned)(kind)}; } } while (0)
+// Copies up to cap records to out after the device has finished, stores how many the launches appended in *n (more than
+// cap: the rest were dropped), then clears the buffer.
+static inline int res_read(ResRec *out, unsigned cap, unsigned *n)
+{
+    unsigned cnt = 0;
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(&cnt, g_res_n, sizeof(cnt));
+    const unsigned m = cnt < cap ? cnt : cap, k = m < kResCap ? m : kResCap;
+    if (e == cudaSuccess && out && k) e = cudaMemcpyFromSymbol(out, g_res, (size_t)k * sizeof(ResRec));
+    if (n) *n = cnt;
+    const unsigned zero = 0;
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_res_n, &zero, sizeof(zero));
+    return (int)e;
+}
+#else
+#define CS_RES_BEGIN
+#define CS_RES_END(kind) do { } while (0)
+#endif
+
+// One shared-memory carve-out for the multi-step kernel and the scene refill kernels, which share SMs whenever a refill
+// runs beside another batch's steps: the largest shared-memory configuration, where five multi-step blocks fit. The
+// attribute is per device and per kernel; set_carveout sets it once for each (device, kernel) pair.
+template <auto Kernel>
+inline cudaError_t set_carveout()
+{
+    static bool done[64];
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess || dev < 0 || dev >= 64 || done[dev]) return err;
+    err = cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    if (err == cudaSuccess) done[dev] = true;
+    return err;
+}
 
 // Device-side copy of the scalar parameters (passed by value as a kernel argument).
 struct KParams {

@@ -33,11 +33,13 @@ namespace cs {
 
 int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot)
 {
+    #define CS_MULTI_REC_RUN(...) do { if (cudaError_t err_ = set_carveout<step_multi_kernel<__VA_ARGS__>>()) return (int)err_; \
+                                       step_multi_kernel<__VA_ARGS__><<<blocks, 32 * (A.N + 1), 0, stream>>>(A); } while (0)
     #define CS_MULTI_REC_LAUNCH(NN) do {                                                                                    \
-        if (rot) { if (A.k.robot_visible) step_multi_kernel<NN, true, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
-                   else step_multi_kernel<NN, false, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); }                \
-        else if (A.k.robot_visible) step_multi_kernel<NN, true, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A);             \
-        else step_multi_kernel<NN, false, true><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
+        if (rot) { if (A.k.robot_visible) CS_MULTI_REC_RUN(NN, true, true, true);                                           \
+                   else CS_MULTI_REC_RUN(NN, false, true, true); }                                                          \
+        else if (A.k.robot_visible) CS_MULTI_REC_RUN(NN, true, true);                                                       \
+        else CS_MULTI_REC_RUN(NN, false, true); } while (0)
     switch (A.N) {
         case 2: CS_MULTI_REC_LAUNCH(2); break;
         case 3: CS_MULTI_REC_LAUNCH(3); break;
@@ -46,6 +48,7 @@ int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool
         default: return CROWDSIM_EUNSUPPORTED;
     }
     #undef CS_MULTI_REC_LAUNCH
+    #undef CS_MULTI_REC_RUN
     return (int)cudaGetLastError();
 }
 

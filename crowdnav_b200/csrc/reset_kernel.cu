@@ -3,11 +3,12 @@
 // Replaces crowd_sim/envs/crowd_sim.py:251-312 (CrowdSim.reset); the generator and the MT19937 it draws from are
 // scene.cuh's (np.random.seed(seed) == init_genrand(seed), np.random.random() == genrand_res53).
 //
-// Only a few env slots need a scene at any time (~3 % of the envs finish per step), so each 128-slot block first
-// compacts the slots that do into a shared-memory list; the first kGen threads of the block then generate scenes, each
-// with its 624-word MT19937 state in its own SHARED-MEMORY column ([624][kGen] words, conflict-free across lanes). The
-// earlier version kept the state in a global [624][B] scratch: every draw then paid three dependent L2 round trips; in
-// shared memory a scene is bounded by the 624-step seeding recurrence, which is inherently sequential.
+// The refill kernels run beside other batches' multi-step kernels (bench: 16 streams, each a batch's steps and then its
+// refill), so they are sized to fit in what five multi-step blocks leave of an SM (DESIGN §3.3): one-warp scene blocks
+// without shared memory, a two-warp case assigner, and the multi-step kernel's shared-memory carve-out. The generator
+// (MTScene, scene.cuh) keeps the seeded MT19937 words it needs in registers and writes only the twisted words, to the slot's
+// column of a global [624][B] scratch (crowdsim_reset_args.scene_mt), so a scene reads no memory for its draws.
+#include <limits.h>
 #include "scene.cuh"
 
 namespace cs {
@@ -39,7 +40,7 @@ struct ResetKArgs {
 };
 
 // Live-state reset of env e from its generated scene (crowd_sim.py:251-312).
-__device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MT &rng)
+__device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MTScene &rng)
 {
     const crowdsim_reset_args &a = A.a;
     const int N = A.N;
@@ -67,7 +68,7 @@ __device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MT &rng)
 
 // Generator side of the auto-reset protocol (include/crowdsim_b200.h): fill an EMPTY (case queue: CLAIMED) next-scene slot,
 // mark it READY.
-__device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MT &rng)
+__device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MTScene &rng)
 {
     const crowdsim_autoreset &ar = A.ar;
     const int N = A.N;
@@ -83,27 +84,44 @@ __device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MT &rng
     st_release_u8(ar.n_state + e, CROWDSIM_SLOT_READY);    // scene visible before the flag (release at gpu scope)
 }
 
+// One warp per block, kSceneSlots slots per block: the lanes ballot which of the block's slots need a scene, and the k-th
+// of those (in slot order) goes to lane k % 32, so every lane generates scenes while any are left. The block holds 32
+// threads x <= 64 registers and no shared memory, so two fit in what five multi-step blocks leave of an SM and a refill
+// never waits for step blocks to drain. A lane's twisted MT19937 words go to column base + lane of the caller's [624][B]
+// scratch (base + lane < B whenever the lane has a scene), so the stores of lanes drawing in step are one 128-byte line.
+// 32 slots per block: at most one scene per lane, so a block lives one scene. 128 slots per block (two to three scenes in
+// a row per lane, four times fewer blocks) measured 1.34e9 against 1.48-1.50e9 env-steps/s at full chip (DESIGN §3.6).
+constexpr int kSceneSlots = 32;
 template <bool PREFETCH>
-__global__ void __launch_bounds__(kSlotsPerBlock) scene_kernel(const __grid_constant__ ResetKArgs A)
+__global__ void __launch_bounds__(32, 32) scene_kernel(const __grid_constant__ ResetKArgs A)
 {
-    extern __shared__ uint32_t s_mt[];                     // [624][kGen]
-    __shared__ int s_list[kSlotsPerBlock];
-    __shared__ int s_count;
-    const int e = blockIdx.x * kSlotsPerBlock + threadIdx.x;
-    bool need = e < A.B;
-    if (need) {
-        // acquire: the consumer's reads of the previous scene happen-before the writes of the next one (the generating
-        // thread is ordered behind this one by the block barrier of compact_block)
-        if (PREFETCH) need = ld_acquire_u8(A.ar.n_state + e) == (A.assigned ? CROWDSIM_SLOT_CLAIMED : CROWDSIM_SLOT_EMPTY);
-        else need = !(A.a.mask && !A.a.mask[e]);
+    CS_RES_BEGIN
+    const int lane = threadIdx.x, base = blockIdx.x * kSceneSlots;
+    unsigned bal[kSceneSlots / 32];
+    int count = 0;
+    #pragma unroll
+    for (int j = 0; j < kSceneSlots / 32; ++j) {
+        const int e = base + 32 * j + lane;
+        // acquire: the consumer's reads of the previous scene happen-before the writes of the next one
+        const bool need = e < A.B && (PREFETCH ? ld_acquire_u8(A.ar.n_state + e) == (A.assigned ? CROWDSIM_SLOT_CLAIMED : CROWDSIM_SLOT_EMPTY)
+                                               : !(A.a.mask && !A.a.mask[e]));
+        bal[j] = __ballot_sync(0xffffffffu, need);
+        count += __popc(bal[j]);
     }
-    const int count = compact_block(need, e, s_list, &s_count);
-    if (threadIdx.x >= kGen) return;                       // the generating warp; no barriers below
-    MT rng; rng.mt = s_mt + threadIdx.x; rng.stride = kGen;
-    for (int base = 0; base + (int)threadIdx.x < count; base += kGen) {
-        const int ee = s_list[base + threadIdx.x];
-        if (PREFETCH) prefetch_env(A, ee, rng); else reset_env(A, ee, rng);
+    MTScene rng; rng.mt = A.a.scene_mt + base + lane; rng.stride = A.B;
+    for (int k = lane; k < count; k += 32) {
+        int j = 0, r = k;                                    // the k-th slot that needs a scene: bit r of ballot j
+        unsigned bj = bal[0];
+        #pragma unroll
+        for (int jj = 1; jj < kSceneSlots / 32; ++jj)
+            if (j == jj - 1 && r >= __popc(bj)) { r -= __popc(bj); j = jj; bj = bal[jj]; }
+        const int e = base + 32 * j + (int)__fns(bj, 0, r + 1);
+        if (PREFETCH) prefetch_env(A, e, rng); else reset_env(A, e, rng);
     }
+#ifdef CS_RESIDENCY_PROBE
+    __syncwarp();                                            // the block ends with its last lane
+#endif
+    CS_RES_END(CS_RES_SCENE);
 }
 
 // Case queue in slot order: ONE block walks the slots in ascending order and hands the next queue entries to the slots that
@@ -111,69 +129,83 @@ __global__ void __launch_bounds__(kSlotsPerBlock) scene_kernel(const __grid_cons
 // the order in which blocks or threads run -- the CPU oracle's serial loop gives the same assignment. PREFETCH marks the
 // slots it claimed CLAIMED: the generator launch that follows on the same stream fills exactly those, even if a step on
 // another stream empties more slots in between.
-constexpr int kAssignThreads = 1024;
+// Two warps, each thread owning kAssignRun consecutive slots of a chunk: a thread issues its run's flag loads together
+// (relaxed, then one acquire fence) instead of one acquire round trip after the other, and the block fits, like the scene
+// blocks, beside five multi-step blocks.
+constexpr int kAssignThreads = 64;
+constexpr int kAssignRun = 32;                              // slots per thread per chunk (bits of one mask word)
 template <bool PREFETCH>
-__global__ void __launch_bounds__(kAssignThreads) assign_cases_kernel(const __grid_constant__ ResetKArgs A)
+__global__ void __launch_bounds__(kAssignThreads, 16) assign_cases_kernel(const __grid_constant__ ResetKArgs A)
 {
+    CS_RES_BEGIN
     __shared__ int s_warp[kAssignThreads / 32];
-    __shared__ int s_total;
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     int base = *A.a.case_counter;
-    for (int start = 0; start < A.B; start += kAssignThreads) {
-        const int e = start + tid;
-        bool need = false;
-        if (e < A.B) {
-            // acquire: the consumer's reads of the previous scene happen-before the generator's writes of the next one
-            if (PREFETCH) need = ld_acquire_u8(A.ar.n_state + e) == CROWDSIM_SLOT_EMPTY;
-            else need = !(A.a.mask && !A.a.mask[e]);
+    for (int start = 0; start < A.B; start += kAssignThreads * kAssignRun) {
+        const int e0 = start + tid * kAssignRun;
+        uint8_t flag[kAssignRun];
+        #pragma unroll
+        for (int j = 0; j < kAssignRun; ++j) {
+            const int e = e0 + j;
+            flag[j] = 0;
+            if (e < A.B) {
+                if (PREFETCH) flag[j] = ld_relaxed_u8(A.ar.n_state + e) == CROWDSIM_SLOT_EMPTY;
+                else flag[j] = !(A.a.mask && !A.a.mask[e]);
+            }
         }
-        const unsigned bal = __ballot_sync(0xffffffffu, need);
-        if (lane == 0) s_warp[w] = __popc(bal);
+        // acquire: the consumer's reads of the previous scene happen-before the generator's writes of the next one
+        if (PREFETCH) fence_acquire_gpu();
+        unsigned need = 0;
+        #pragma unroll
+        for (int j = 0; j < kAssignRun; ++j) need |= (unsigned)flag[j] << j;
+        const int cnt = __popc(need);
+        int incl = cnt;                                      // inclusive scan of the counts over the warp
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
+        if (lane == 31) s_warp[w] = incl;
         __syncthreads();
-        if (w == 0) {                                        // exclusive scan of the per-warp counts
-            const int v = s_warp[lane];
-            int incl = v;
-            #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
-            s_warp[lane] = incl - v;
-            if (lane == 31) s_total = incl;
+        int next = base + incl - cnt;
+        #pragma unroll
+        for (int v = 0; v < kAssignThreads / 32; ++v) if (v < w) next += s_warp[v];
+        int total = 0;
+        #pragma unroll
+        for (int v = 0; v < kAssignThreads / 32; ++v) total += s_warp[v];
+        while (need) {
+            const int j = __ffs(need) - 1;
+            need &= need - 1u;
+            A.assigned[e0 + j] = next++;
+            if (PREFETCH) A.ar.n_state[e0 + j] = CROWDSIM_SLOT_CLAIMED;
         }
-        __syncthreads();
-        if (need) {
-            A.assigned[e] = base + s_warp[w] + __popc(bal & ((1u << lane) - 1u));
-            if (PREFETCH) A.ar.n_state[e] = CROWDSIM_SLOT_CLAIMED;
-        }
-        base += s_total;
-        __syncthreads();                                     // s_warp / s_total are rewritten by the next chunk
+        base += total;
+        __syncthreads();                                     // s_warp is rewritten by the next chunk
     }
     if (tid == 0) *A.a.case_counter = base;
+    CS_RES_END(CS_RES_ASSIGN);
 }
 
 template <bool PREFETCH>
 static int launch_scene_kernel(ResetKArgs A, int B, cudaStream_t stream)
 {
+    cudaError_t err = set_carveout<scene_kernel<PREFETCH>>();
+    if (err == cudaSuccess) err = set_carveout<assign_cases_kernel<PREFETCH>>();
+    if (err != cudaSuccess) return (int)err;
     A.assigned = nullptr;
     if (A.a.case_counter && (PREFETCH || A.has_ep)) {
         A.assigned = PREFETCH ? A.ar.n_case : A.ep.ep_case;
         assign_cases_kernel<PREFETCH><<<1, kAssignThreads, 0, stream>>>(A);
         ++g_launches;
     }
-    const size_t smem = (size_t)624 * kGen * sizeof(uint32_t);
-    static bool attr_set_dev[2][64];                       // the attribute is per DEVICE: cache keyed by the current device
-    int dev = 0; cudaGetDevice(&dev);
-    bool dummy = false; bool &attr_done = (dev >= 0 && dev < 64) ? attr_set_dev[PREFETCH][dev] : dummy;
-    if (!attr_done) {
-        cudaError_t err = cudaFuncSetAttribute(scene_kernel<PREFETCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (err != cudaSuccess) return (int)err;
-        attr_done = true;
-    }
-    const int blocks = (B + kSlotsPerBlock - 1) / kSlotsPerBlock;
-    scene_kernel<PREFETCH><<<blocks, kSlotsPerBlock, smem, stream>>>(A);
+    scene_kernel<PREFETCH><<<(B + kSceneSlots - 1) / kSceneSlots, 32, 0, stream>>>(A);
     ++g_launches;
     return (int)cudaGetLastError();
 }
 
 }  // namespace cs
+
+#ifdef CS_RESIDENCY_PROBE
+// Probe builds only: the refill blocks' records (crowdsim_common.cuh, CS_RESIDENCY_PROBE).
+extern "C" int crowdsim_residency_probe_refill(cs::ResRec *out, unsigned cap, unsigned *n) { return cs::res_read(out, cap, n); }
+#endif
 
 static int check_reset_args(const crowdsim_reset_args *args, int B, int N)
 {
@@ -182,6 +214,8 @@ static int check_reset_args(const crowdsim_reset_args *args, int B, int N)
     if (N > CROWDSIM_MAX_HUMANS) return CROWDSIM_EUNSUPPORTED;
     if (args->rule != CROWDSIM_RULE_CIRCLE && args->rule != CROWDSIM_RULE_SQUARE && args->rule != CROWDSIM_RULE_MIXED) return CROWDSIM_EUNSUPPORTED;
     if (args->rule == CROWDSIM_RULE_MIXED && N < 5) return CROWDSIM_EUNSUPPORTED;      // the rule draws up to 5 humans whatever N is
+    if (!args->scene_mt) return CROWDSIM_EINVAL;
+    if (B > INT_MAX / 624) return CROWDSIM_EUNSUPPORTED;                                // [624][B] scratch, int indexing
     return CROWDSIM_OK;
 }
 

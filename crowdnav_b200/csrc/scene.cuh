@@ -11,8 +11,9 @@
 
 namespace cs {
 
-// One generator's 624-word state, addressed through a pointer and a stride: a thread's column of a shared-memory
-// [624][columns] array while a scene is generated, an env's column of a global [624][B] array between policy decisions.
+// One generator's 624-word state, addressed through a pointer and a stride: an env's column of a global [624][B] array
+// between policy decisions, a thread's column of a shared-memory [624][columns] array while the draws kernel regenerates a
+// stream (scene_kernel's generator is MTScene below).
 // The twist is done lazily, in place and in order (word i of the next block needs old words i, i+1 and word i+397 mod 624,
 // which is old for i < 227 and already-new afterwards -- exactly the dependency order of the classic in-place loop), so a
 // scene only pays for the words it actually draws. Words [0, pos) therefore belong to the current block and words
@@ -54,12 +55,58 @@ struct MT {
     }
 };
 
+// The same stream as MT for a generator that starts from a seed (scene_kernel), without storing the seeded state.
+// In the first block after seeding, word i is twisted from seeded words s[i], s[i + 1] and, for i < 227, s[i + 397];
+// those are never rewritten before they are read, so two cursors of the seeding recurrence in registers produce them as
+// the draws need them (seeding = 397 recurrence steps to place the second cursor, no stores). Only the twisted words go to
+// the column: word i >= 227 of the first block reads twisted word i - 227, word 623 reads twisted word 0, and from the
+// second block on the column holds a whole block of twisted words and the generator is MT's lazy twist. A scene (tens of
+// words) therefore reads no memory at all; each draw writes its word, a store nobody waits for.
+struct MTScene {
+    uint32_t *mt;      // this generator's column of the state array (twisted words)
+    int stride;        // columns of the state array
+    int pos;           // next word to produce, 0..623 (wraps)
+    bool first;        // still in the first block after seeding
+    uint32_t a, a1, m; // first block: seeded words s[pos], s[pos + 1], s[pos + 397]
+    __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
+    static __device__ __forceinline__ uint32_t init_step(uint32_t s, int k) { return 1812433253u * (s ^ (s >> 30)) + (uint32_t)k; }
+    __device__ void seed(uint32_t s) {
+        a = s; a1 = init_step(s, 1);
+        m = a1;
+        for (int k = 2; k <= 397; ++k) m = init_step(m, k);
+        pos = 0; first = true;
+    }
+    __device__ __forceinline__ uint32_t next() {
+        const int i = pos;
+        const int i1 = (i == 623) ? 0 : i + 1;
+        const int im = (i < 227) ? i + 397 : i - 227;
+        uint32_t wi, wi1, wm;
+        if (first) { wi = a; wi1 = (i == 623) ? w(0) : a1; wm = (i < 227) ? m : w(im); }
+        else { wi = w(i); wi1 = w(i1); wm = w(im); }
+        const uint32_t y0 = (wi & 0x80000000u) | (wi1 & 0x7fffffffu);
+        uint32_t y = wm ^ (y0 >> 1) ^ ((y0 & 1u) ? 0x9908b0dfu : 0u);
+        w(i) = y;
+        if (first) {                                          // cursors to s[i + 1], s[i + 2], s[i + 398]
+            a = a1; a1 = init_step(a1, i + 2); m = init_step(m, i + 398);
+            first = i != 623;
+        }
+        pos = i1;
+        y ^= (y >> 11); y ^= (y << 7) & 0x9d2c5680u; y ^= (y << 15) & 0xefc60000u; y ^= (y >> 18);
+        return y;
+    }
+    __device__ __forceinline__ double next_double() {          // genrand_res53, as MT::next_double
+        const uint32_t a_ = next() >> 5, b_ = next() >> 6;
+        return (a_ * 67108864.0 + b_) / 9007199254740992.0;
+    }
+};
+
 // Scene of one env: N humans by rejection sampling (crowd_sim.py:84-207), written to hp/hg/ha ([N][2] each).
 // The robot is fixed at (0, -R) -> (0, R) (crowd_sim.py:274) and takes part in the separation tests.
 // Rule `mixed` (crowd_sim.py:103-151) draws the number of humans per scene (0..5, capped at N); the remaining slots of
 // the fixed-N layout are PARKED: position = goal = (CROWDSIM_PARKED_X + 100 i, CROWDSIM_PARKED_X), i.e. outside every
 // neighbour range and far from the robot, so they take no part in any solve, collision test or minimum distance.
-__device__ __forceinline__ void generate_scene(MT &rng, const crowdsim_reset_args &a, int N, double *hp, double *hg, double *ha)
+template <class RNG>
+__device__ __forceinline__ void generate_scene(RNG &rng, const crowdsim_reset_args &a, int N, double *hp, double *hg, double *ha)
 {
     const double rpx = 0.0, rpy = -a.circle_radius, rgx = 0.0, rgy = a.circle_radius;
     auto put = [&](int i, double px, double py, double gx, double gy, double radius, double v_pref) {
@@ -169,8 +216,8 @@ __device__ __forceinline__ uint32_t queue_seed(const crowdsim_reset_args &a, int
     return a.seed_base + (a.case_wrap > 0 ? (uint32_t)(((long long)a.case_first + c) % a.case_wrap) : (uint32_t)c);
 }
 
-constexpr int kSlotsPerBlock = 128;   // env slots scanned per block
-constexpr int kGen = 32;              // scenes generated concurrently per block (624 * kGen * 4 B = 78 KB shared memory)
+constexpr int kSlotsPerBlock = 128;   // env slots scanned per block of the draws kernel
+constexpr int kGen = 32;              // streams regenerated concurrently per draws block (624 * kGen * 4 B = 78 KB shared memory)
 
 // Compact the slots of this block that need a scene; returns the count (block-uniform). s_list[0..count) = env ids.
 __device__ __forceinline__ int compact_block(bool need, int e, int *s_list, int *s_count)

@@ -304,8 +304,11 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
         if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream, rec_rot); }
-        #define CS_MULTI_LAUNCH(NN) do { if (A.k.robot_visible) step_multi_kernel<NN, true, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); \
-                                         else step_multi_kernel<NN, false, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } while (0)
+        #define CS_MULTI_LAUNCH(NN) do { cudaError_t err_;                                                                \
+            if (A.k.robot_visible) { if ((err_ = set_carveout<step_multi_kernel<NN, true, false>>())) return (int)err_;         \
+                                     step_multi_kernel<NN, true, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); }          \
+            else { if ((err_ = set_carveout<step_multi_kernel<NN, false, false>>())) return (int)err_;                          \
+                   step_multi_kernel<NN, false, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } } while (0)
         switch (N) {
             case 2: CS_MULTI_LAUNCH(2); break;
             case 3: CS_MULTI_LAUNCH(3); break;
@@ -469,6 +472,11 @@ extern "C" int crowdsim_phase_probe(unsigned long long *out, int reset)
     }
     return (int)e;
 }
+#endif
+
+#ifdef CS_RESIDENCY_PROBE
+// Probe builds only: crowdsim_step_n's multi-step blocks' records (crowdsim_common.cuh, CS_RESIDENCY_PROBE).
+extern "C" int crowdsim_residency_probe_step(cs::ResRec *out, unsigned cap, unsigned *n) { return cs::res_read(out, cap, n); }
 #endif
 
 extern "C" int crowdsim_device_check(int *sm_count, int *cc_major, int *cc_minor)

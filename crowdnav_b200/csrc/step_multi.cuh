@@ -184,6 +184,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     static_assert(REC || !ROT, "unicycle rows are a recording variant");
     static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
     using namespace orca;
+    CS_RES_BEGIN
     constexpr int E = 32, L = N + 1, T = 32 * L;
     constexpr int MH = VIS ? N : N - 1;                     // lines of a human solve
     constexpr int SUB = N - 1;                              // lanes per queued lp3 item (sub-problems i = 1 .. N-1)
@@ -538,6 +539,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             }
         }
     }
+    CS_RES_END(CS_RES_STEP);
 }
 
 }  // namespace cs

@@ -219,6 +219,10 @@ typedef struct crowdsim_reset_args {
      * case_wrap = 0: seed_base + c. */
     int32_t case_first;
     int32_t case_wrap;
+    /* [624][B] words of scratch (B * 624 < 2^31): the MT19937 state of the scene generated for slot e lives in column e
+     * while crowdsim_reset / crowdsim_prefetch_scenes run (required by those two; crowdsim_policy_draws and
+     * crowdsim_mt_streams ignore it). Calls that may run at the same time need scratch of their own. */
+    uint32_t *scene_mt;
 } crowdsim_reset_args;
 
 /* Library / device probing (host only, no kernel launch). */
