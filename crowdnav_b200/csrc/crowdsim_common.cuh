@@ -14,7 +14,7 @@ extern unsigned long long g_launches;
 #define CS_PI 3.141592653589793
 
 // np.linalg.norm((a, b)): BLAS ddot accumulates a*a, then fma(b, b, .) (see oracle/crowdsim_oracle.c header).
-__device__ __forceinline__ double norm2(double a, double b) { return sqrt(fma(b, b, a * a)); }
+__host__ __device__ __forceinline__ double norm2(double a, double b) { return sqrt(fma(b, b, a * a)); }
 
 // crowd_sim/envs/utils/utils.py:4-26 with (x3, y3) = (0, 0)
 __device__ __forceinline__ double point_to_segment_dist0(double x1, double y1, double x2, double y2)

@@ -6,6 +6,8 @@
 // (sample_random_attributes). float64 arithmetic in the reference's expression order; cos/sin are CUDA's (<= 1-2 ulp from
 // glibc's, which numpy uses): initial coordinates can differ from the CPU reference by ~1e-15 (tests bound it at 4e-15).
 // The draws themselves do not depend on cos/sin, so the stream after a scene is numpy's word for word.
+// MT, MTScene and generate_scene are also host functions: tests/native/mt_scene_check.cu compiles them for the CPU (glibc's
+// cos/sin there) and compares them with the CPU oracle word for word and bit for bit.
 #pragma once
 #include "crowdsim_common.cuh"
 
@@ -22,12 +24,12 @@ struct MT {
     uint32_t *mt;      // this generator's column of the state array
     int stride;        // columns of the state array
     int pos;           // next word to produce, 0..623 (wraps)
-    __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
-    __device__ void seed(uint32_t s) {
+    __host__ __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
+    __host__ __device__ void seed(uint32_t s) {
         for (int i = 0; i < 624; ++i) { w(i) = s; s = 1812433253u * (s ^ (s >> 30)) + (uint32_t)i + 1u; }
         pos = 0;
     }
-    __device__ __forceinline__ uint32_t next() {
+    __host__ __device__ __forceinline__ uint32_t next() {
         const int i = pos;
         const int i1 = (i == 623) ? 0 : i + 1;
         const int im = (i < 227) ? i + 397 : i - 227;
@@ -38,13 +40,13 @@ struct MT {
         y ^= (y >> 11); y ^= (y << 7) & 0x9d2c5680u; y ^= (y << 15) & 0xefc60000u; y ^= (y >> 18);
         return y;
     }
-    __device__ __forceinline__ double next_double() {          // genrand_res53
+    __host__ __device__ __forceinline__ double next_double() { // genrand_res53
         const uint32_t a = next() >> 5, b = next() >> 6;
         return (a * 67108864.0 + b) / 9007199254740992.0;
     }
     // RandomState.choice(A) for 1 <= A <= 2^31: legacy randint(0, A) by masked rejection, one 32-bit word per try, with
     // the smallest mask 2^k - 1 >= A - 1; A == 1 draws no word.
-    __device__ __forceinline__ int next_index(uint32_t A) {
+    __host__ __device__ __forceinline__ int next_index(uint32_t A) {
         const uint32_t rng = A - 1u;
         if (rng == 0u) return 0;
         uint32_t mask = rng;
@@ -68,15 +70,15 @@ struct MTScene {
     int pos;           // next word to produce, 0..623 (wraps)
     bool first;        // still in the first block after seeding
     uint32_t a, a1, m; // first block: seeded words s[pos], s[pos + 1], s[pos + 397]
-    __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
-    static __device__ __forceinline__ uint32_t init_step(uint32_t s, int k) { return 1812433253u * (s ^ (s >> 30)) + (uint32_t)k; }
-    __device__ void seed(uint32_t s) {
+    __host__ __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
+    static __host__ __device__ __forceinline__ uint32_t init_step(uint32_t s, int k) { return 1812433253u * (s ^ (s >> 30)) + (uint32_t)k; }
+    __host__ __device__ void seed(uint32_t s) {
         a = s; a1 = init_step(s, 1);
         m = a1;
         for (int k = 2; k <= 397; ++k) m = init_step(m, k);
         pos = 0; first = true;
     }
-    __device__ __forceinline__ uint32_t next() {
+    __host__ __device__ __forceinline__ uint32_t next() {
         const int i = pos;
         const int i1 = (i == 623) ? 0 : i + 1;
         const int im = (i < 227) ? i + 397 : i - 227;
@@ -94,7 +96,7 @@ struct MTScene {
         y ^= (y >> 11); y ^= (y << 7) & 0x9d2c5680u; y ^= (y << 15) & 0xefc60000u; y ^= (y >> 18);
         return y;
     }
-    __device__ __forceinline__ double next_double() {          // genrand_res53, as MT::next_double
+    __host__ __device__ __forceinline__ double next_double() { // genrand_res53, as MT::next_double
         const uint32_t a_ = next() >> 5, b_ = next() >> 6;
         return (a_ * 67108864.0 + b_) / 9007199254740992.0;
     }
@@ -106,7 +108,7 @@ struct MTScene {
 // the fixed-N layout are PARKED: position = goal = (CROWDSIM_PARKED_X + 100 i, CROWDSIM_PARKED_X), i.e. outside every
 // neighbour range and far from the robot, so they take no part in any solve, collision test or minimum distance.
 template <class RNG>
-__device__ __forceinline__ void generate_scene(RNG &rng, const crowdsim_reset_args &a, int N, double *hp, double *hg, double *ha)
+__host__ __device__ __forceinline__ void generate_scene(RNG &rng, const crowdsim_reset_args &a, int N, double *hp, double *hg, double *ha)
 {
     const double rpx = 0.0, rpy = -a.circle_radius, rgx = 0.0, rgy = a.circle_radius;
     auto put = [&](int i, double px, double py, double gx, double gy, double radius, double v_pref) {

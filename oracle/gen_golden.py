@@ -237,6 +237,72 @@ def run_resets(out_name='reset_scenes', blocks=None):
     print(out_name, 'written')
 
 
+# Scenes that outlast the generator's first MT19937 block (624 words). Besides seeds 0, 1, 2^32 - 1 and a run of plain
+# seeds, each block lists seeds whose scene ends exactly on a block edge (624 or 1248 words, numpy pos 624) or one draw
+# beside it: a square-crossing human draws in steps of 4 words, a circle-crossing try in steps of 6, so a square scene of
+# 63 humans (2 mod 4 words) cannot end on an edge and its seeds end 2 words either side of 1248 instead.
+# (word counts: tests/explore_oracle.scene_words; the fixture records them too)
+RESETS_LONG = [
+    ('square40', dict(human_num=40, test_sim='square_crossing'),
+     [19, 33, 71, 16, 35, 28, 89] + [2000 + i for i in range(8)]),
+    ('square40_envcfg', dict(human_num=40, test_sim='square_crossing', profile='env_config'),
+     [474, 1899, 2153, 1034, 2506] + [2000 + i for i in range(6)]),
+    ('square63', dict(human_num=63, test_sim='square_crossing'),
+     [536, 563, 332, 588, 1932, 834] + [2000 + i for i in range(4)]),
+    ('square63_envcfg', dict(human_num=63, test_sim='square_crossing', profile='env_config'),
+     [1068, 2327, 1464] + [2000 + i for i in range(4)]),
+    ('square32_random_attr', dict(human_num=32, test_sim='square_crossing', randomize=True),
+     [511, 50, 143, 30, 3, 88, 2227, 15257] + [2000 + i for i in range(6)]),
+    ('circle15', dict(human_num=15, test_sim='circle_crossing'),
+     [133, 166, 232, 971, 127, 65, 792, 672] + [2000 + i for i in range(6)]),
+]
+
+
+def words_drawn(seed, key, pos):
+    """MT19937 words between np.random.seed(seed) and the state (key, pos), from numpy's own MT19937.random_raw: whole
+    blocks are drawn until the key matches (the key changes only when a block is twisted), then the count is checked by
+    drawing exactly that many words from a fresh generator."""
+    seeded = np.random.RandomState(seed).get_state()
+    bg = np.random.MT19937()
+    bg.state = {'bit_generator': 'MT19937', 'state': {'key': seeded[1], 'pos': seeded[2]}}
+    blocks = 0
+    while not np.array_equal(bg.state['state']['key'], key):
+        bg.random_raw(624)
+        blocks += 1
+        assert blocks < 1000
+    words = 0 if blocks == 0 else 624 * (blocks - 1) + pos
+    bg.state = {'bit_generator': 'MT19937', 'state': {'key': seeded[1], 'pos': seeded[2]}}
+    if words:
+        bg.random_raw(words)
+    assert np.array_equal(bg.state['state']['key'], key) and bg.state['state']['pos'] == pos
+    return words
+
+
+def run_resets_long():
+    """Initial scenes that draw more than one MT19937 block, and numpy's state after each (val phase: seed = case)."""
+    import hashlib
+    out = {}
+    for name, kw, seeds in RESETS_LONG:
+        env, robot, _ = make_env(**kw)
+        robot.policy.multiagent_training = True
+        env.train_val_sim = kw['test_sim']
+        rows = []
+        for seed in [0, 1, 2 ** 32 - 1] + seeds:
+            env.reset('val', seed)
+            st = np.random.get_state()
+            nxt = np.random.RandomState()
+            nxt.set_state(st)
+            rows.append({'seed': seed, 'scene': scene(env), 'pos': int(st[2]),
+                         'key_sha256': hashlib.sha256(np.ascontiguousarray(st[1], dtype='<u4').tobytes()).hexdigest(),
+                         'next_words': [int(w) for w in np.frombuffer(nxt.bytes(64), dtype='<u4')],
+                         'words': words_drawn(seed, st[1], int(st[2]))})
+        out[name] = {'config': kw, 'phase': 'val', 'rows': rows}
+        print(name, [r['words'] for r in rows])
+    with gzip.open(os.path.join(OUT, 'reset_scenes_long.json.gz'), 'wt') as f:
+        json.dump(out, f, separators=(',', ':'))
+    print('reset_scenes_long written')
+
+
 def run_rotate(out_name='rotate_lookahead', profile=None, cases=(0, 3, 7), steps=12, every=4):
     """CADRL.rotate and the inner loop of MultiHumanRL.predict (multi_human_rl.py:35-45), reference code only."""
     pcfg = configparser.RawConfigParser()
@@ -675,6 +741,7 @@ ONLY = {
     'il_safety': run_il_safety,
     'envcfg': run_envcfg,
     'resets_envcfg': run_resets_envcfg,
+    'resets_long': run_resets_long,
     'human_times_envcfg': lambda: run_human_times('human_times_envcfg', HUMAN_TIMES_ENVCFG),
     'rotate_envcfg': lambda: run_rotate('rotate_lookahead_envcfg', 'env_config', cases=(0, 3, 11), steps=16, every=4),
     'rotate_unicycle': run_rotate_unicycle,

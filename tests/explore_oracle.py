@@ -23,16 +23,21 @@ def lib():
     global _lib
     if _lib is None:
         import build as oracle_build                       # oracle/build.py: the CPU oracle's compiler flags
-        h = hashlib.sha256(open(SRC, 'rb').read() + open(ORACLE_SRC, 'rb').read() + ' '.join(oracle_build.CFLAGS).encode())
+        # -fopenmp as oracle/build.py: the oracle's batch loops call omp_get_thread_num, which must resolve even in a
+        # process that has not loaded libgomp through torch
+        flags = oracle_build.CFLAGS + ['-fopenmp']
+        h = hashlib.sha256(open(SRC, 'rb').read() + open(ORACLE_SRC, 'rb').read() + ' '.join(flags).encode())
         so = os.path.join(tempfile.gettempdir(), 'crowdnav_stream_oracle_%d_%s.so' % (os.getuid(), h.hexdigest()[:16]))
         if not os.path.exists(so):
             tmp = so + '.%d.tmp' % os.getpid()
-            subprocess.check_call(['gcc'] + oracle_build.CFLAGS + ['-Wno-unknown-pragmas', SRC, '-o', tmp, '-lm'])
+            subprocess.check_call(['gcc'] + flags + [SRC, '-o', tmp, '-lm'])
             os.replace(tmp, so)
         from crowdnav_b200 import _abi
         _lib = C.CDLL(so)
         _lib.so_post_generation.restype = None
         _lib.so_post_generation.argtypes = [C.POINTER(_abi.ResetArgs), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p]
+        _lib.so_scene_words.restype = C.c_long
+        _lib.so_scene_words.argtypes = [C.POINTER(_abi.ResetArgs), C.c_int, C.c_uint32]
     return _lib
 
 
@@ -49,6 +54,12 @@ def post_generation(args, N, seed):
     pos = np.zeros(1, dtype=np.int32)
     lib().so_post_generation(C.byref(args), int(N), int(seed) % 2 ** 32, key.ctypes.data, pos.ctypes.data)
     return ('MT19937', key, int(pos[0]), 0, 0.0)
+
+
+def scene_words(args, N, seed):
+    """MT19937 words the scene generator of `args` draws at N humans after np.random.seed(seed). A scene of w words
+    leaves numpy's pos at w - 624 (ceil(w / 624) - 1), so pos 624 (the device's pos 0) means it ended on a block edge."""
+    return int(lib().so_scene_words(C.byref(args), int(N), int(seed) % 2 ** 32))
 
 
 def key_digest(key):
