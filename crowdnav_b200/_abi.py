@@ -147,6 +147,9 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
     f.restype, f.argtypes = C.c_int, [P(ResetArgs), C.c_int, C.c_int, P(State), P(Episodes)] + s
     f = getattr(lib, prefix + 'pack_joint')
     f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(State), C.c_int, C.c_void_p] + s
+    if hasattr(lib, prefix + 'pack_joint_sorted'):
+        f = getattr(lib, prefix + 'pack_joint_sorted')
+        f.restype, f.argtypes = C.c_int, [C.c_int, C.c_int, P(State), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p] + s
     f = getattr(lib, prefix + 'lookahead_pack')
     f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), C.c_void_p, C.c_int, C.c_int,
                                       C.c_void_p, C.c_void_p] + s
@@ -161,7 +164,7 @@ EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_cou
            'crowdsim_event_wait', 'crowdsim_host_pump', 'crowdsim_step', 'crowdsim_step_n', 'crowdsim_step_n_record', 'crowdsim_record_flush',
            'crowdsim_step_n_record_ex', 'crowdsim_step_n_record_rot', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
            'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes',
-           'crowdsim_policy_draws', 'crowdsim_mt_streams', 'crowdsim_pack_joint', 'crowdsim_lookahead_pack',
+           'crowdsim_policy_draws', 'crowdsim_mt_streams', 'crowdsim_pack_joint', 'crowdsim_pack_joint_sorted', 'crowdsim_lookahead_pack',
            'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
 
 # CROWDSIM_B200_LIB selects another build of the SAME library (A/B runs of kernel variants built into build_probe/);

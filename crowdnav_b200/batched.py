@@ -404,7 +404,8 @@ class BatchedCrowdSim(object):
         tracking and auto-reset (ValueError otherwise).
         record: a memory.DeviceRLRecorder -- with an ORCA robot the same n_steps steps through crowdsim_step_n_record_ex
         (no actions); with an external robot one step with `actions` (n_steps = 1), booked around it by crowdsim_record_book
-        and its rows staged by pack_joint. The recorder flushes its reinforcement-learning pairs when its staging is full."""
+        and its rows staged by pack_joint (a recorder with sort_humans=True: LSTM-RL's sorted rows and, with maps, the
+        sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full."""
         if record is not None and getattr(record, 'rl', False):
             return self._step_record_rl(actions, int(n_steps), record)
         if record is not None:
@@ -461,6 +462,8 @@ class BatchedCrowdSim(object):
         if self.robot_policy == _abi.ROBOT_ORCA:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
+            if getattr(record, 'sort_humans', False):
+                raise ValueError('sorted rows are staged only for robots stepped with external actions')
             if not 1 <= n_steps <= record.n_max:
                 raise ValueError('n_steps must be between 1 and the recorder\'s n_max')
             if record.s + n_steps > record.n_max:
@@ -486,7 +489,12 @@ class BatchedCrowdSim(object):
             rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
                                                -1, s, self._stream())
         _abi.check(rc, 'crowdsim_record_book')
-        self.pack_joint(unicycle=record.unicycle, out=record.rows[s])       # TrajectoryRecorder.before_step's rows
+        if getattr(record, 'sort_humans', False):
+            # LSTM-RL's rows, and the sorted human state over the env-order state the booking staged for the maps
+            self.pack_joint(unicycle=record.unicycle, out=record.rows[s], order_by_distance=True,
+                            out_pos=record.h_pos[s] if record.om else None, out_vel=record.h_vel[s] if record.om else None)
+        else:
+            self.pack_joint(unicycle=record.unicycle, out=record.rows[s])   # TrajectoryRecorder.before_step's rows
         self.step(actions)
         with torch.cuda.device(self.device):
             rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
@@ -513,14 +521,33 @@ class BatchedCrowdSim(object):
         return s.h_pos, s.h_vel, s.h_attr[..., 0]
 
     # ---- value-network support -----------------------------------------------------------------------------------
-    def pack_joint(self, unicycle=False, out=None):
+    def pack_joint(self, unicycle=False, out=None, order_by_distance=False, return_state=False, out_order=None, out_pos=None,
+                   out_vel=None):
+        """The rotated joint state of the current state, [B][N][13] float32 (transform(state) of a value-network policy).
+        order_by_distance: the rows of LSTM-RL's last_state (crowdsim_pack_joint_sorted), humans by decreasing distance to
+        the robot (lstm_rl.py:99-104); with return_state the result is (rows, order [B][N] int32, h_pos, h_vel [B][N][2]
+        float64 in row order: row i of env e is human order[e][i]). out_order / out_pos / out_vel are written when given."""
+        if return_state and not order_by_distance:
+            raise ValueError('return_state needs order_by_distance')
+        B, N = self.B, self.human_num
         if out is None:
-            out = torch.empty((self.B, self.human_num, 13), dtype=torch.float32, device=self.device)
+            out = torch.empty((B, N, 13), dtype=torch.float32, device=self.device)
         st = self.state.struct()
+        if not order_by_distance:
+            with torch.cuda.device(self.device):
+                rc = self.lib.crowdsim_pack_joint(B, N, C.byref(st), int(unicycle), _ptr(out), self._stream())
+            _abi.check(rc, 'crowdsim_pack_joint')
+            return out
+        if return_state:
+            f = lambda t, shape, dtype: torch.empty(shape, dtype=dtype, device=self.device) if t is None else t  # noqa: E731
+            out_order = f(out_order, (B, N), torch.int32)
+            out_pos = f(out_pos, (B, N, 2), torch.float64)
+            out_vel = f(out_vel, (B, N, 2), torch.float64)
         with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_pack_joint(self.B, self.human_num, C.byref(st), int(unicycle), _ptr(out), self._stream())
-        _abi.check(rc, 'crowdsim_pack_joint')
-        return out
+            rc = self.lib.crowdsim_pack_joint_sorted(B, N, C.byref(st), int(unicycle), _ptr(out), _ptr(out_order),
+                                                     _ptr(out_pos), _ptr(out_vel), self._stream())
+        _abi.check(rc, 'crowdsim_pack_joint_sorted')
+        return (out, out_order, out_pos, out_vel) if return_state else out
 
     def lookahead_pack(self, actions, unicycle=False, out_states=None, out_reward=None):
         """actions [A][2] float64 device tensor -> (states [B][A][N][13] f32, reward [B][A] f64)."""

@@ -3,6 +3,8 @@
 // crowdsim_pack_joint      current state -> rotate(self_state + human_state) rows, [B][N][13] float32:
 //                          crowd_sim/envs/utils/state.py:17-18,36-37 (14-tuple), crowd_nav/policy/multi_human_rl.py:98-107
 //                          (transform: float32 cast) and crowd_nav/policy/cadrl.py:187-222 (rotate).
+// crowdsim_pack_joint_sorted  the same rows with LSTM-RL's human order (lstm_rl.py:99-104: decreasing distance to the robot),
+//                          what LstmRL's last_state holds, plus the order and the permuted float64 human state
 // crowdsim_lookahead_pack  the inner loop of MultiHumanRL.predict / CADRL.predict (multi_human_rl.py:35-45, query_env=true):
 //                          for each of A candidate actions, env.onestep_lookahead(action) (crowd_sim.py:314-315,414-416,
 //                          agent.py:63-74), CADRL.propagate (cadrl.py:104-129) and rotate. The reference re-solves the N human
@@ -39,6 +41,49 @@ __global__ void __launch_bounds__(128) pack_joint_kernel(const __grid_constant__
     float *o = A.out + idx * 13;
     #pragma unroll
     for (int i = 0; i < 13; ++i) o[i] = row[i];
+}
+
+// ---- crowdsim_pack_joint_sorted: LstmRL.predict sorts state.human_states in place by decreasing distance to the robot
+// (lstm_rl.py:99-104) before MultiHumanRL.predict stores last_state = transform(state) (multi_human_rl.py:60-61). One warp
+// per env: the keys go to shared memory, each lane ranks its humans by comparison (ties: lower index first, the stability of
+// sorted(..., reverse=True); the rank of propagate_pack_kernel) and writes each human's pack_joint row at its rank. ----
+constexpr int PS_WARPS = 4;
+
+struct PackSortedArgs { int B, N, unicycle; crowdsim_state st; float *out; int32_t *order; double *h_pos, *h_vel; };
+
+__global__ void __launch_bounds__(32 * PS_WARPS) pack_joint_sorted_kernel(const __grid_constant__ PackSortedArgs A)
+{
+    __shared__ double s_key[PS_WARPS][CROWDSIM_MAX_HUMANS];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int e = blockIdx.x * PS_WARPS + w, N = A.N;
+    if (e >= A.B) return;                                  // whole warps: only __syncwarp below
+    double *key = s_key[w];
+    const double2 rp = ld2(A.st.r_pos, e), rv = ld2(A.st.r_vel, e), rg = ld2(A.st.r_goal, e), ra = ld2(A.st.r_attr, e);
+    for (int i = lane; i < N; i += 32) {
+        const double2 hp = ld2(A.st.h_pos, (size_t)e * N + i);
+        key[i] = norm2(hp.x - rp.x, hp.y - rp.y);
+    }
+    __syncwarp();
+    // the row of pack_joint_kernel, term for term
+    const float th = A.unicycle ? (float)A.st.r_theta[e] : 0.f;
+    float c, s, rot, dg, rvx, rvy;
+    rotate_self((float)rp.x, (float)rp.y, (float)rv.x, (float)rv.y, (float)rg.x, (float)rg.y, c, s, rot, dg, rvx, rvy);
+    for (int i = lane; i < N; i += 32) {
+        const double k = key[i];
+        int r = 0;
+        for (int j = 0; j < N; ++j) { const double kj = key[j]; r += (kj > k) || (kj == k && j < i); }
+        const size_t src = (size_t)e * N + i, dst = (size_t)e * N + r;
+        const double2 hp = ld2(A.st.h_pos, src), hv = ld2(A.st.h_vel, src), ha = ld2(A.st.h_attr, src);
+        float row[13];
+        rotate_row(row, (float)rp.x, (float)rp.y, (float)ra.x, (float)ra.y, A.unicycle ? (th - rot) : 0.f, dg, rvx, rvy, c, s,
+                   (float)hp.x, (float)hp.y, (float)hv.x, (float)hv.y, (float)ha.x);
+        float *o = A.out + dst * 13;
+        #pragma unroll
+        for (int q = 0; q < 13; ++q) o[q] = row[q];
+        if (A.order) A.order[dst] = i;
+        if (A.h_pos) st2(A.h_pos, dst, hp);
+        if (A.h_vel) st2(A.h_vel, dst, hv);
+    }
 }
 
 struct LookArgs {
@@ -285,6 +330,22 @@ extern "C" int crowdsim_pack_joint(int B, int N, const crowdsim_state *st, int k
     cs::PackArgs A; A.B = B; A.N = N; A.unicycle = kinematics_unicycle; A.st = *st; A.out = out;
     const size_t n = (size_t)B * N; const int threads = 128; const int blocks = (int)((n + threads - 1) / threads);
     cs::pack_joint_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(A);
+    ++cs::g_launches;
+    return (int)cudaGetLastError();
+}
+
+extern "C" int crowdsim_pack_joint_sorted(int B, int N, const crowdsim_state *st, int kinematics_unicycle, float *out,
+                                          int32_t *order, double *h_pos_out, double *h_vel_out, void *stream)
+{
+    if (!st || !out || B < 0 || N < 0) return CROWDSIM_EINVAL;
+    if (!st->h_pos || !st->h_vel || !st->h_attr || !st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr) return CROWDSIM_EINVAL;
+    if (kinematics_unicycle && !st->r_theta) return CROWDSIM_EINVAL;
+    if (N > CROWDSIM_MAX_HUMANS) return CROWDSIM_EUNSUPPORTED;
+    if (B == 0 || N == 0) return CROWDSIM_OK;
+    cs::PackSortedArgs A; A.B = B; A.N = N; A.unicycle = kinematics_unicycle ? 1 : 0; A.st = *st; A.out = out;
+    A.order = order; A.h_pos = h_pos_out; A.h_vel = h_vel_out;
+    const int blocks = (B + cs::PS_WARPS - 1) / cs::PS_WARPS;
+    cs::pack_joint_sorted_kernel<<<blocks, 32 * cs::PS_WARPS, 0, (cudaStream_t)stream>>>(A);
     ++cs::g_launches;
     return (int)cudaGetLastError();
 }

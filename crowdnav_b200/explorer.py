@@ -19,8 +19,11 @@ inside the multi-step kernel at 2 <= N <= 5 -- plus a flush).
 Reinforcement learning with a target model records on device too, for the ORCA robot (steps_per_launch steps per launch)
 and for act_batch policies (one step per call), flushing every steps_per_launch steps with one target-network forward
 (memory.DeviceRLRecorder); without a target model, or with any other policy, the rollout records step by step
-(memory.TrajectoryRecorder). All of them push the same pairs in the same order. In imitation learning the rows are what target_policy.transform stores (explorer.py:102): its occupancy-map
-settings (with_om, cell_num, cell_size, om_channel_size) when target_policy is given.
+(memory.TrajectoryRecorder). All of them push the same pairs in the same order. In reinforcement learning the rows are
+the robot policy's last_state: a policy whose sort_last_state is set (LSTM-RL, policy.make_lstm_rl) has its humans sorted
+by decreasing distance to the robot (lstm_rl.py:99-104), and its rows and maps are recorded in that order.
+In imitation learning the rows are what target_policy.transform stores (explorer.py:102): its occupancy-map settings
+(with_om, cell_num, cell_size, om_channel_size) when target_policy is given.
 
 Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous ranges per rank; there is no data-path
 collective; ONE gather of the per-case result rows (48 B per episode: 6 float64 columns; NCCL on GPU tensors, gloo in the CPU tests) brings
@@ -181,17 +184,22 @@ class BatchedExplorer(object):
             else:
                 om = getattr(self.robot_policy, 'om', None) if getattr(self.robot_policy, 'with_om', False) else None
                 rows_unicycle = unicycle
+            # RL rows are the robot policy's own last_state: LSTM-RL's are sorted by decreasing distance to the robot
+            # (lstm_rl.py:99-104); imitation learning stores target_policy.transform(ORCA's state), never sorted
+            sort_humans = (not imitation_learning and self.robot_policy != 'orca'
+                           and bool(getattr(self.robot_policy, 'sort_last_state', False)))
             if self.robot_policy == 'orca' and imitation_learning:
                 dev_rec = DeviceILRecorder(env, self.memory, self.gamma, chunk, om=om, unicycle=rows_unicycle)
                 dev_rec.begin()
             elif not imitation_learning and self.target_model is not None and (
                     self.robot_policy == 'orca' or hasattr(self.robot_policy, 'act_batch')):
                 # RL targets: staged on device, the target network runs once per flush of `chunk` steps
-                dev_rec = DeviceRLRecorder(env, self.memory, self.gamma, self.target_model, chunk, om=om, unicycle=unicycle)
+                dev_rec = DeviceRLRecorder(env, self.memory, self.gamma, self.target_model, chunk, om=om, unicycle=unicycle,
+                                           sort_humans=sort_humans)
                 dev_rec.begin()
             else:
                 recorder = TrajectoryRecorder(env, self.memory, self.gamma, imitation_learning, self.target_model, om=om,
-                                              unicycle=rows_unicycle)
+                                              unicycle=rows_unicycle, sort_humans=sort_humans)
         side = torch.cuda.Stream(device=env.device)
         main = torch.cuda.current_stream(env.device)
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per

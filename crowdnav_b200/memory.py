@@ -14,6 +14,8 @@
   DeviceRLRecorder     the same for reinforcement learning (target-network values), for the ORCA robot and for robots
                        stepped with external actions (holonomic or unicycle): same pairs, same order and same rows as
                        TrajectoryRecorder; the values differ only by how the batch a target network sees rounds
+With sort_humans=True, TrajectoryRecorder and DeviceRLRecorder store LSTM-RL's last_state: rows (and maps) of the humans sorted by decreasing
+distance to the robot, as LstmRL.predict sorts them before MultiHumanRL.predict stores transform(state).
 The IL return is accumulated forward in t (G_i += pow(...) * r_t as each reward arrives), i.e. in the same order and
 with the same pow() factors as the reference's sum(). That is the project's summation rule for every discounted return: a
 plain left fold from +0.0, one rounding per product and per sum, which is sum() before CPython 3.12. CPython 3.12's
@@ -62,12 +64,15 @@ class DeviceReplayMemory(object):
 
 
 class TrajectoryRecorder(object):
-    def __init__(self, env, memory, gamma, imitation_learning=True, target_model=None, max_steps=None, om=None, unicycle=False):
+    def __init__(self, env, memory, gamma, imitation_learning=True, target_model=None, max_steps=None, om=None, unicycle=False,
+                 sort_humans=False):
         """om = None or (cell_num, cell_size, om_channel_size): append the occupancy maps of the current human states to
         every recorded row, as MultiHumanRL.transform does with with_om (multi_human_rl.py:98-104). unicycle: the rows of a
-        unicycle robot (pack_joint's theta column, cadrl.py:205-209)."""
+        unicycle robot (pack_joint's theta column, cadrl.py:205-209). sort_humans: LSTM-RL's last_state, whose humans
+        LstmRL.predict sorted by decreasing distance to the robot (lstm_rl.py:99-104): the sorted rows, and the maps of the
+        sorted human state."""
         self.env, self.memory = env, memory
-        self.unicycle = bool(unicycle)
+        self.unicycle, self.sort_humans = bool(unicycle), bool(sort_humans)
         self.om = om
         F = 13 + (om[0] * om[0] * om[2] if om else 0)
         self.il, self.target_model = imitation_learning, target_model
@@ -90,9 +95,12 @@ class TrajectoryRecorder(object):
         env = self.env
         self._t = env.episodes.ep_steps.long().clamp_(max=self.T - 1)
         self._live = env.state.active.bool()
-        packed = env.pack_joint(unicycle=self.unicycle)
+        if self.sort_humans:
+            packed, _, h_pos, h_vel = env.pack_joint(unicycle=self.unicycle, order_by_distance=True, return_state=True)
+        else:
+            packed, h_pos, h_vel = env.pack_joint(unicycle=self.unicycle), None, None
         if self.om:
-            packed = torch.cat([packed, env.occupancy_maps(None, None, *self.om)], dim=2)
+            packed = torch.cat([packed, env.occupancy_maps(h_pos, h_vel, *self.om)], dim=2)
         rows = torch.arange(env.B, device=env.device)
         self.states[rows, self._t] = torch.where(self._live.view(-1, 1, 1), packed, self.states[rows, self._t])
 
@@ -220,12 +228,14 @@ class DeviceRLRecorder(object):
                        multi-step kernel at 2 <= N <= 5, around each single-step launch otherwise)
       external robot   one step per call with the caller's actions: crowdsim_record_book books the step, env.pack_joint stages
                        its rows (unicycle: the rows of a unicycle robot, as TrajectoryRecorder(unicycle=True) packs them)
+    sort_humans=True (external robots only): LSTM-RL's rows, as TrajectoryRecorder(sort_humans=True) records them; the
+    pack stages the sorted human state for the maps too (crowdsim_pack_joint_sorted).
     It flushes when its staging is full and at finish(). The ring's write position and size live on the device during a run:
     call begin() before the first step and finish() after the last (one host read)."""
 
     rl = True
 
-    def __init__(self, env, memory, gamma, target_model, n_max, om=None, unicycle=False):
+    def __init__(self, env, memory, gamma, target_model, n_max, om=None, unicycle=False, sort_humans=False):
         from .batched import max_episode_steps
         B, N, dev = env.B, env.human_num, env.device
         if om is not None and N < 2:
@@ -236,7 +246,7 @@ class DeviceRLRecorder(object):
         if int(n_max) < 1:
             raise ValueError('n_max must be at least 1')
         self.env, self.memory, self.target_model, self.n_max = env, memory, target_model, int(n_max)
-        self.om, self.unicycle = om, bool(unicycle)
+        self.om, self.unicycle, self.sort_humans = om, bool(unicycle), bool(sort_humans)
         self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
         self.gamma_bar = pow(gamma, env.time_step * env.robot_v_pref)              # TrajectoryRecorder.gamma_bar
         n = self.n_max

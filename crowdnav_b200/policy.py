@@ -134,8 +134,10 @@ class BatchedValuePolicy(object):
     decisions and the env's reward); False extrapolates every human at its own velocity and uses the policy's compute_reward
     (multi_human_rl.py:38-42: propagate_pack). CADRL always queries the env (cadrl.py:156-170), so joint=False with
     query_env=False is refused. order_by_distance: with query_env=False the rows follow LSTM-RL's sort by decreasing
-    distance to the robot (lstm_rl.py:99-103). kinematics 'holonomic' or 'unicycle': the action space of
-    build_action_space and the robot's propagate; the env's robot must step the same kinematics (external_xy / external_rot)."""
+    distance to the robot (lstm_rl.py:99-103). sort_last_state: the policy's stored last_state (the rows of its replay
+    pairs) has that sort too, with either query_env (LSTM-RL); lookahead rows with query_env=True stay in env order.
+    kinematics 'holonomic' or 'unicycle': the action space of build_action_space and the robot's propagate; the env's robot
+    must step the same kinematics (external_xy / external_rot)."""
 
     name = 'BatchedValuePolicy'
     trainable = True
@@ -143,7 +145,7 @@ class BatchedValuePolicy(object):
 
     def __init__(self, model, gamma=0.9, v_pref=1.0, time_step=0.25, joint=True, speed_samples=5, rotation_samples=16,
                  with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3, query_env=True, kinematics='holonomic',
-                 order_by_distance=False, exploration='torch'):
+                 order_by_distance=False, exploration='torch', sort_last_state=False):
         if kinematics not in ('holonomic', 'unicycle'):
             raise ValueError('kinematics must be holonomic or unicycle, not %r' % (kinematics,))
         if exploration not in ('torch', 'numpy'):
@@ -153,6 +155,9 @@ class BatchedValuePolicy(object):
             raise ValueError('CADRL always queries the env (cadrl.py:156-170): query_env=False needs a joint policy')
         self.model = model
         self.query_env, self.kinematics, self.order_by_distance = bool(query_env), kinematics, bool(order_by_distance)
+        # the rows the reference stores as last_state in the train phase have their humans sorted by decreasing distance
+        # to the robot (LSTM-RL: lstm_rl.py:99-104, whatever query_env is); BatchedExplorer records RL pairs in that order
+        self.sort_last_state = bool(sort_last_state)
         # policy.config [om] + with_om: occupancy maps of the NEXT human states are appended to every row
         # (multi_human_rl.py:46-49; they do not depend on the action, so they are built once per env and broadcast)
         self.with_om = with_om
@@ -277,14 +282,19 @@ def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='hol
 
 
 def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interaction_module=False, query_env=True,
-                 kinematics='holonomic', exploration='torch'):
+                 kinematics='holonomic', exploration='torch', with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3):
     """LSTM-RL with the reference's default sizes (crowd_nav/configs/policy.config:24-31). With query_env=False its rows
-    follow the reference's sort of the humans by decreasing distance to the robot (lstm_rl.py:99-103)."""
+    follow the reference's sort of the humans by decreasing distance to the robot (lstm_rl.py:99-103); its last_state,
+    the rows of its replay pairs, always does (sort_last_state). with_om=True gives OM-LSTM-RL ([lstm_rl] with_om,
+    lstm_rl.py:79-88): input_dim grows by cell_num^2 * om_channel_size (multi_human_rl.py:106-107), the LSTM's input or,
+    with the interaction module, mlp1's."""
     if seed is not None:
         torch.manual_seed(seed)
-    net = LSTMRLValueNetwork(mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
+    net = LSTMRLValueNetwork(input_dim=13 + (cell_num * cell_num * om_channel_size if with_om else 0),
+                             mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
                              mlp1_dims=(150, 100, 100, 50) if with_interaction_module else None)
-    p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True, query_env=query_env, kinematics=kinematics,
-                           order_by_distance=not query_env, exploration=exploration)
-    p.name = 'LSTM-RL'
+    p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True, with_om=with_om, cell_num=cell_num,
+                           cell_size=cell_size, om_channel_size=om_channel_size, query_env=query_env, kinematics=kinematics,
+                           order_by_distance=not query_env, exploration=exploration, sort_last_state=True)
+    p.name = 'OM-LSTM-RL' if with_om else 'LSTM-RL'
     return p

@@ -40,6 +40,7 @@
  *   crowdsim_propagate_pack  the same loop with query_env=false: CADRL.propagate of the robot and of every human at its
  *                            own velocity, MultiHumanRL.compute_reward (multi_human_rl.py:65-88), rotate, fused
  *   crowdsim_pack_joint      crowd_sim/envs/utils/state.py:17-18,36-37 (14-tuple) + cadrl.py:187-222 (rotate)
+ *   crowdsim_pack_joint_sorted  the same rows in LSTM-RL's order (lstm_rl.py:99-104), with the order and permuted state
  *   crowdsim_lookahead_humans  the observation of env.onestep_lookahead (crowd_sim.py:314-315,414-416; agent.py:63-74)
  *   crowdsim_occupancy_maps  crowd_nav/policy/multi_human_rl.py:109-163 (MultiHumanRL.build_occupancy_maps)
  *   crowdsim_onestep_lookahead  crowd_sim/envs/crowd_sim.py:314-315 (step(action, update=False)), one action per env
@@ -465,6 +466,21 @@ int crowdsim_mt_streams(const crowdsim_reset_args *args, int B, int N, const cro
  * multi_human_rl.py:43). kinematics_unicycle selects theta handling (cadrl.py:205-209).
  */
 int crowdsim_pack_joint(int B, int N, const crowdsim_state *st, int kinematics_unicycle, float *out, void *stream);
+
+/*
+ * crowdsim_pack_joint with LSTM-RL's row order: LstmRL.predict sorts state.human_states by decreasing distance to the robot
+ * (lstm_rl.py:99-104) before MultiHumanRL.predict stores last_state = transform(state) (multi_human_rl.py:60-61).
+ *   out       [B][N][13] float32  row i of env e is, bit for bit, the crowdsim_pack_joint row of human order[e][i]
+ *   order     [B][N] int32        humans ranked by decreasing norm(h_pos - r_pos) at the current state; equal distances
+ *                                 keep env order (the stability of sorted(..., reverse=True)). NULL: not written
+ *   h_pos_out, h_vel_out [B][N][2] float64  the human positions / velocities in row order, the input of
+ *                                 crowdsim_occupancy_maps for the sorted state's maps. NULL: not written
+ * Every env is written, live or not (st->active is not read). Reads h_pos, h_vel, h_attr, r_pos, r_vel, r_goal, r_attr
+ * and r_theta (kinematics_unicycle only: required, CROWDSIM_EINVAL without it). N > CROWDSIM_MAX_HUMANS returns
+ * CROWDSIM_EUNSUPPORTED; B = 0 or N = 0 returns CROWDSIM_OK without a launch. Nothing is mutated.
+ */
+int crowdsim_pack_joint_sorted(int B, int N, const crowdsim_state *st, int kinematics_unicycle, float *out, int32_t *order,
+                               double *h_pos_out, double *h_vel_out, void *stream);
 
 /*
  * One-step lookahead for A candidate robot actions per env (multi_human_rl.py:35-45 with query_env=true):

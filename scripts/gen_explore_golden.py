@@ -40,13 +40,21 @@ def key_digest(state):
     return hashlib.sha256(np.ascontiguousarray(state[1], dtype='<u4').tobytes()).hexdigest()
 
 
-def policy_config(rotation_samples=None, speed_samples=None):
+def policy_config(rotation_samples=None, speed_samples=None, overrides=None):
+    """The reference's policy.config; overrides: {(section, key): value} written over it."""
     pcfg = configparser.RawConfigParser()
     pcfg.read(os.path.join(REF, 'crowd_nav', 'configs', 'policy.config'))
     if rotation_samples is not None:
         pcfg.set('action_space', 'rotation_samples', str(rotation_samples))
         pcfg.set('action_space', 'speed_samples', str(speed_samples))
+    for (sec, key), v in (overrides or {}).items():
+        pcfg.set(sec, key, str(v))
     return pcfg
+
+
+def value_layer(policy, model):
+    """The last layer of a policy's value network, zeroed for a constant value."""
+    return {'cadrl': lambda: model.value_network[-1], 'lstm_rl': lambda: model.mlp[-1]}.get(policy, lambda: model.mlp3[-1])()
 
 
 def next_words(state, n=16):
@@ -61,8 +69,12 @@ class ListMemory(list):
 
 
 def run_block(tag, policy, N, rule, k, epsilon, randomize=False, profile=None, rotation_samples=None, speed_samples=None,
-              steps=True, seed=None, pairs_target_seed=None, kinematics='holonomic'):
-    pcfg = policy_config(rotation_samples, speed_samples)
+              steps=True, seed=None, pairs_target_seed=None, kinematics='holonomic', config=None, target_config=None,
+              on_predict=None):
+    """config: policy.config overrides of the robot's policy and of the pairs' target network; target_config: further
+    overrides of the target's alone. on_predict(state, rec): called with each decision's state before the policy sees it,
+    to add fields to the decision's record."""
+    pcfg = policy_config(rotation_samples, speed_samples, config)
     pcfg.set('action_space', 'kinematics', kinematics)
     torch.manual_seed(0 if seed is None else seed)
     env, robot, _ = make_env(human_num=N, randomize=randomize, profile=profile, policy_name=policy, policy_config=pcfg)
@@ -70,14 +82,14 @@ def run_block(tag, policy, N, rule, k, epsilon, randomize=False, profile=None, r
     pol = robot.policy
     assert robot.kinematics == kinematics
     if seed is None:
-        last = pol.model.value_network[-1] if policy == 'cadrl' else pol.model.mlp3[-1]
+        last = value_layer(policy, pol.model)
         with torch.no_grad():                              # constant value 0: the greedy choice is the reward's argmax
             last.weight.zero_(); last.bias.zero_()
     pol.set_epsilon(epsilon)
     mem, target = None, None
     if pairs_target_seed is not None:
         torch.manual_seed(pairs_target_seed)
-        tp = policy_config(); tpol = type(pol)(); tpol.configure(tp)
+        tp = policy_config(overrides={**(config or {}), **(target_config or {})}); tpol = type(pol)(); tpol.configure(tp)
         target, mem = tpol.get_model(), ListMemory()
     resets, episodes = [], []
     rnd, cho = np.random.random, np.random.choice
@@ -104,12 +116,16 @@ def run_block(tag, policy, N, rule, k, epsilon, randomize=False, profile=None, r
 
     def predict(state):
         draw.clear()
+        extra = {}
+        if on_predict is not None:
+            on_predict(state, extra)
         action = pol_predict(state)
         idx = next((i for i, a in enumerate(pol.action_space or []) if a is action), -1)
         rec = {'u': R(draw['u']) if 'u' in draw else None, 'explored': int('index' in draw), 'index': idx if 'u' in draw else -1}
         if 'u' in draw and 'index' not in draw:            # greedy: the margin between the two best action values
             top = sorted(pol.action_values, reverse=True)
             rec['margin'] = top[0] - top[1]
+        rec.update(extra)
         episodes[-1]['steps'].append(rec)
         if 'index' in draw:
             assert idx == draw['index']

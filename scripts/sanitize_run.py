@@ -4,7 +4,7 @@
 Covers: small-crowd step kernel (per-warp and per-block lp3 queue), multi-step kernel with auto-reset and a CONCURRENT scene
 prefetch on a side stream (the release / acquire slot hand-over), crowd kernel (N = 12), generic kernel, scene generation,
 lookahead pack / humans / onestep_lookahead, propagate pack (query_env = false; N = 63 and 200 actions: several action and
-row tiles), occupancy maps, human_times, the recording multi-step kernel with its flush
+row tiles), LSTM-RL's sorted pack (crowdsim_pack_joint_sorted at N = 5 and 63), occupancy maps, human_times, the recording multi-step kernel with its flush
 (crowdsim_step_n_record, crowdsim_record_flush) through a small memory ring that wraps, and both routes of
 crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the launch loop's recording at N = 1 and N = 20, and occupancy-map rows
 at N = 5 (the map staging of the multi-step kernel, the map kernel of the flush), both routes of crowdsim_step_n_record_rot
@@ -98,6 +98,7 @@ for N, robot, om in ((5, 'orca', (4, 1.0, 3)), (20, 'orca', None), (5, 'external
 env = make(64, 5, policy='external_xy'); env.reset_seeds(torch.arange(64) + 1000)
 acts = torch.tensor([[0.0, 0.0], [1.0, 0.0], [0.0, 1.0]], dtype=torch.float64, device=env.device)
 env.lookahead_pack(acts); env.lookahead_humans(); env.pack_joint(); env.occupancy_maps()
+env.pack_joint(order_by_distance=True, return_state=True); env.pack_joint(unicycle=True, order_by_distance=True)
 env.propagate_pack(acts, unicycle=True, order_by_distance=True)
 env.onestep_lookahead(torch.zeros((64, 2), dtype=torch.float64, device=env.device))
 env.human_times(max_steps=60)
@@ -105,6 +106,7 @@ env = make(16, 20, policy='external_xy', rule='square_crossing'); env.reset_seed
 env.lookahead_pack(acts); env.human_times(max_steps=20)
 env = make(3, 63, policy='external_xy', rule='square_crossing'); env.reset_seeds(torch.arange(3) + 1000, rule='square_crossing')
 env.propagate_pack(torch.rand((200, 2), dtype=torch.float64, device=env.device), order_by_distance=True)   # several tiles
+env.pack_joint(order_by_distance=True, return_state=True)
 # exploration draws from numpy's stream: the post-generation streams, then decisions with episodes starting and running
 env = make(200, 63, policy='external_xy', rule='square_crossing'); env.track_episodes(200)
 env.reset_seeds(torch.arange(200) + 2000, rule='square_crossing'); env.mt_streams(rule='square_crossing')

@@ -5,13 +5,14 @@ reward + gamma_bar * target_model(next state)) through both recorders:
   device    memory.DeviceRLRecorder: env.step(..., record=...) and a flush with one target-network forward every
             --steps-per-launch steps (the ORCA robot: that many steps per recording launch)
 alternated in one process. Workloads: a SARL robot at epsilon = 1 (act_batch every step, its own lookahead and network) and
-the ORCA robot, both with a SARL target network, at every --B and --N. Reports the CUDA-event wall time per env-step
+the ORCA robot, both with a SARL target network, and an LSTM-RL robot at epsilon = 1 with an LSTM-RL target network, whose
+rows are sorted by decreasing distance to the robot (sort_humans, crowdsim_pack_joint_sorted), at every --B and --N. Reports the CUDA-event wall time per env-step
 (one lockstep step of all B envs) and the host synchronisations per step that torch counts (sync debug mode 'warn': every
 synchronising call it sees, such as .item(), bool() of a device tensor or a boolean-mask gather; the library's own calls
 never synchronise), and prints the card's name and power limit.
 
   python scripts/time_rl_rollout.py [--B 1024 4096] [--N 5 20] [--steps 192] [--reps 3] [--steps-per-launch 8]
-                                    [--robots sarl orca]
+                                    [--robots sarl orca lstm_rl]
 """
 import argparse
 import json
@@ -25,7 +26,7 @@ import torch  # noqa: E402
 
 from crowdnav_b200.batched import BatchedCrowdSim, default_config  # noqa: E402
 from crowdnav_b200.memory import DeviceReplayMemory, DeviceRLRecorder, TrajectoryRecorder  # noqa: E402
-from crowdnav_b200.policy import make_sarl  # noqa: E402
+from crowdnav_b200.policy import make_lstm_rl, make_sarl  # noqa: E402
 
 GAMMA, CAPACITY = 0.9, 100000
 
@@ -45,9 +46,10 @@ def make_env(B, N, robot):
 def rollout(env, robot, policy, target, path, steps, n):
     """`steps` env-steps of one path; returns the recorder (the device one is finished)."""
     mem = DeviceReplayMemory(CAPACITY, env.human_num, env.device)
+    sort = bool(getattr(policy, 'sort_last_state', False))
     side = torch.cuda.Stream(device=env.device); main = torch.cuda.current_stream(env.device)
     if path == 'per_step':
-        rec = TrajectoryRecorder(env, mem, GAMMA, False, target)
+        rec = TrajectoryRecorder(env, mem, GAMMA, False, target, sort_humans=sort)
         for it in range(steps):
             if it % 2 == 0:
                 side.wait_stream(main)
@@ -57,7 +59,7 @@ def rollout(env, robot, policy, target, path, steps, n):
             env.step() if robot == 'orca' else env.step(policy.act_batch(env))
             rec.after_step()
     else:
-        rec = DeviceRLRecorder(env, mem, GAMMA, target, n)
+        rec = DeviceRLRecorder(env, mem, GAMMA, target, n, sort_humans=sort)
         rec.begin()
         chunk = n if robot == 'orca' else 1
         for it in range(steps // chunk):
@@ -114,10 +116,11 @@ def main():
     for robot in args.robots:
         for N in args.N:
             for B in args.B:
-                target = make_sarl(seed=1); target.set_device('cuda')
+                make = make_lstm_rl if robot == 'lstm_rl' else make_sarl
+                target = make(seed=1); target.set_device('cuda')
                 policy = None
-                if robot == 'sarl':
-                    policy = make_sarl(seed=0); policy.set_device('cuda'); policy.set_phase('train'); policy.set_epsilon(1.0)
+                if robot != 'orca':
+                    policy = make(seed=0); policy.set_device('cuda'); policy.set_phase('train'); policy.set_epsilon(1.0)
                 paths = ('per_step', 'device')
                 for path in paths:                           # warm-up: every kernel and allocation of the path
                     rollout(make_env(B, N, robot), robot, policy, target.model, path, 2 * n, n)
