@@ -68,6 +68,12 @@ class AutoReset(C.Structure):
 SLOT_EMPTY, SLOT_READY, SLOT_EXHAUSTED, SLOT_CLAIMED = 0, 1, 2, 3
 
 
+class Arrivals(C.Structure):
+    """crowdsim_arrivals: the humans' arrival times and the end snapshots of finished episodes (crowdsim_step_n_arrivals)."""
+    _fields_ = [(n, C.c_void_p) for n in ('h_arrival', 'snap_r_vel', 'snap_h_pos', 'snap_h_vel', 'snap_h_goal', 'snap_h_attr',
+                                          'snap_arrival')]
+
+
 class MTStream(C.Structure):
     """crowdsim_mt_stream: per-env MT19937 state of the policy's exploration draws ([624][B] words, [B] positions)."""
     _fields_ = [('mt', C.c_void_p), ('pos', C.c_void_p)]
@@ -110,6 +116,10 @@ def declare(lib, prefix='crowdsim_', with_stream=True):
     if hasattr(lib, prefix + 'step_n'):
         f = getattr(lib, prefix + 'step_n')
         f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int] + s
+    if hasattr(lib, prefix + 'step_n_arrivals'):
+        f = getattr(lib, prefix + 'step_n_arrivals')
+        f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int,
+                                          P(Arrivals)] + s
     if hasattr(lib, prefix + 'step_n_record'):
         f = getattr(lib, prefix + 'step_n_record')
         f.restype, f.argtypes = C.c_int, [P(Params), C.c_int, C.c_int, P(State), P(StepIO), P(Episodes), P(AutoReset), C.c_int,
@@ -165,7 +175,8 @@ EXPORTS = ('crowdsim_abi_version', 'crowdsim_device_check', 'crowdsim_launch_cou
            'crowdsim_step_n_record_ex', 'crowdsim_step_n_record_rot', 'crowdsim_record_flush_ex', 'crowdsim_record_book', 'crowdsim_record_flush_maps',
            'crowdsim_record_flush_rl', 'crowdsim_orca_act', 'crowdsim_reset', 'crowdsim_prefetch_scenes',
            'crowdsim_policy_draws', 'crowdsim_mt_streams', 'crowdsim_pack_joint', 'crowdsim_pack_joint_sorted', 'crowdsim_lookahead_pack',
-           'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead')
+           'crowdsim_propagate_pack', 'crowdsim_lookahead_humans', 'crowdsim_occupancy_maps', 'crowdsim_human_times', 'crowdsim_onestep_lookahead',
+           'crowdsim_step_n_arrivals')
 
 # CROWDSIM_B200_LIB selects another build of the SAME library (A/B runs of kernel variants built into build_probe/);
 # it is never a fallback: the named file must exist.

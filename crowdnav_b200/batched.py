@@ -153,6 +153,26 @@ class AutoResetBuffers(object):
         return {f: getattr(self, f).cpu().numpy() for f in self.FIELDS}
 
 
+class ArrivalBuffers(object):
+    """crowdsim_arrivals: each human's arrival time in the running episode (crowd_sim.py:404-407) and, with k > 0, the end
+    state of every finished episode with a result row, as CrowdSim.get_human_times starts from it."""
+
+    def __init__(self, B, N, k, device):
+        f64 = lambda *s: torch.zeros(s, dtype=torch.float64, device=device)  # noqa: E731
+        self.h_arrival = f64(B, N)
+        self.k = k
+        if k > 0:
+            self.snap_r_vel = f64(k, 2)
+            self.snap_h_pos, self.snap_h_vel, self.snap_h_goal, self.snap_h_attr = f64(k, N, 2), f64(k, N, 2), f64(k, N, 2), f64(k, N, 2)
+            self.snap_arrival = f64(k, N)
+        else:
+            self.snap_r_vel = self.snap_h_pos = self.snap_h_vel = self.snap_h_goal = self.snap_h_attr = self.snap_arrival = None
+
+    def struct(self):
+        return _abi.Arrivals(*[_ptr(getattr(self, f)) for f in ('h_arrival', 'snap_r_vel', 'snap_h_pos', 'snap_h_vel',
+                                                                  'snap_h_goal', 'snap_h_attr', 'snap_arrival')])
+
+
 class BatchedCrowdSim(object):
     def __init__(self, num_envs, device='cuda:0'):
         self.lib = _abi.load()
@@ -175,6 +195,7 @@ class BatchedCrowdSim(object):
         # ORCA constants (orca.py:61-64)
         self.neighbor_dist = 10.0; self.max_neighbors = 10; self.time_horizon = 5.0
         self.state = None; self.episodes = None; self.autoreset = None
+        self.arrivals = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
         self._scene_src = None                      # (rule, from the case queue?) of the scenes the envs now hold
@@ -228,6 +249,7 @@ class BatchedCrowdSim(object):
         # MT19937 state of the scene being generated for each slot (crowdsim_reset_args.scene_mt): reset and prefetch
         # run on this batch's streams one after the other, so they share it
         self._scene_mt = torch.empty((624, B), dtype=torch.int32, device=self.device)
+        self.arrivals = None
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -246,7 +268,59 @@ class BatchedCrowdSim(object):
     def track_episodes(self, k, gamma=0.9):
         self.episodes = EpisodeBuffers(self.B, k, self.device, gamma, self.time_step, self.robot_v_pref,
                                        max_steps=max_episode_steps(self.time_limit, self.time_step))
+        self.fit_arrival_snapshots()
         return self.episodes
+
+    def fit_arrival_snapshots(self):
+        """The end snapshots of track_arrivals(snapshots=True) are indexed by result row: after the episode rows change
+        (track_episodes), give them as many rows, keeping the running stamps."""
+        arr = self.arrivals
+        if arr is not None and arr.k > 0 and self.episodes is not None and arr.k != self.episodes.k:
+            self.arrivals = ArrivalBuffers(self.B, self.human_num, self.episodes.k, self.device)
+            self.arrivals.h_arrival.copy_(arr.h_arrival)
+
+    # ---- human arrival times --------------------------------------------------------------------------------------
+    def track_arrivals(self, snapshots=False):
+        """Stamp the humans' arrival times from now on (crowdsim_step_n_arrivals): human_times_arrived [B][N] float64 holds
+        the global_time after the first step that ended with the human within its radius of its goal, 0 before
+        (crowd_sim.py:404-407); reset and auto-reset installs zero an env's row. snapshots=True (needs track_episodes):
+        every finished episode also leaves its end state in its result row, for case_human_times()."""
+        if snapshots and self.episodes is None:
+            raise ValueError('end snapshots are kept per result row: track_episodes first')
+        self.arrivals = ArrivalBuffers(self.B, self.human_num, self.episodes.k if snapshots else 0, self.device)
+        return self.arrivals
+
+    @property
+    def human_times_arrived(self):
+        """[B][N] float64 device tensor of the arrival times stamped so far (None unless track_arrivals was called)."""
+        return None if self.arrivals is None else self.arrivals.h_arrival
+
+    def case_human_times(self, cases, max_steps=4000):
+        """CrowdSim.get_human_times (crowdsim_human_times) from the end snapshots of the given result rows (episodes that
+        ended at the goal; track_arrivals(snapshots=True)): (human_times [k][N], global_time [k], final positions [k][N+1][2]
+        robot first). The robot's position and time are the rows' res_final_rpos / res_time, its goal and attributes those
+        every episode starts with (crowd_sim.py:274)."""
+        arr, ep = self.arrivals, self.episodes
+        if arr is None or arr.k == 0 or ep is None:
+            raise ValueError('case_human_times needs track_arrivals(snapshots=True)')
+        idx = torch.as_tensor(cases, dtype=torch.int64, device=self.device)
+        k, N = int(idx.numel()), self.human_num
+        ht = arr.snap_arrival[idx].contiguous()
+        gt = torch.empty((k,), dtype=torch.float64, device=self.device)
+        fp = torch.empty((k, N + 1, 2), dtype=torch.float64, device=self.device)
+        if k == 0:
+            return ht, gt, fp
+        f64 = lambda vals: torch.tensor(vals, dtype=torch.float64, device=self.device).expand(k, len(vals)).contiguous()  # noqa: E731
+        snap = [arr.snap_h_pos[idx].contiguous(), arr.snap_h_vel[idx].contiguous(), arr.snap_h_goal[idx].contiguous(),
+                arr.snap_h_attr[idx].contiguous(), ep.res_final_rpos[idx].contiguous(), arr.snap_r_vel[idx].contiguous(),
+                f64([0.0, self.circle_radius]), f64([self.robot_radius, self.robot_v_pref]),
+                torch.full((k,), np.pi / 2, dtype=torch.float64, device=self.device), ep.res_time[idx].contiguous()]
+        st = _abi.State(*[_ptr(t) for t in snap], None)
+        prm = self.params()
+        with torch.cuda.device(self.device):
+            rc = self.lib.crowdsim_human_times(C.byref(prm), k, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps), self._stream())
+        _abi.check(rc, 'crowdsim_human_times')
+        return ht, gt, fp
 
     # ---- reset ---------------------------------------------------------------------------------------------------
     def reset(self, phase='test', cases=None, mask=None, rule=None):
@@ -300,6 +374,11 @@ class BatchedCrowdSim(object):
                                          C.byref(ep) if ep is not None else None, self._stream())
         _abi.check(rc, 'crowdsim_reset')
         self._keep = (mask, a)
+        if self.arrivals is not None:                   # crowd_sim.py:263-265
+            if mask is None:
+                self.arrivals.h_arrival.zero_()
+            else:
+                self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
 
     # ---- auto-reset with prefetched scenes -------------------------------------------------------------------------
     def set_case_queue(self, first_case, total, phase='test'):
@@ -408,6 +487,12 @@ class BatchedCrowdSim(object):
         sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full."""
         if record is not None and getattr(record, 'rl', False):
             return self._step_record_rl(actions, int(n_steps), record)
+        if record is not None and self.arrivals is not None:
+            raise ValueError('recorded rollouts do not stamp arrival times: track_arrivals is for rollouts without a recorder')
+        if self.arrivals is not None and self.arrivals.k not in (0, self.episodes.k if self.episodes is not None else 0):
+            # the kernels write a snapshot at row ep_case of arrays the C struct does not size: never past their end
+            raise ValueError('arrival snapshots have %d rows, the episode results %s'
+                             % (self.arrivals.k, None if self.episodes is None else self.episodes.k))
         if record is not None:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
@@ -439,7 +524,14 @@ class BatchedCrowdSim(object):
                          _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
         ep = self.episodes.struct() if self.episodes is not None else None
         ar = self.autoreset.struct() if self.autoreset is not None else None
-        if n_steps == 1:
+        if self.arrivals is not None:
+            arr = self.arrivals.struct()
+            with torch.cuda.device(self.device):
+                rc = self.lib.crowdsim_step_n_arrivals(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
+                                                       C.byref(ep) if ep is not None else None,
+                                                       C.byref(ar) if ar is not None else None, int(n_steps), C.byref(arr),
+                                                       self._stream())
+        elif n_steps == 1:
             with torch.cuda.device(self.device):
                 rc = self.lib.crowdsim_step(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
                                             C.byref(ep) if ep is not None else None, C.byref(ar) if ar is not None else None,
@@ -621,9 +713,15 @@ class BatchedCrowdSim(object):
 
     def human_times(self, human_times=None, max_steps=4000):
         """CrowdSim.get_human_times for every env (crowdsim_human_times): (human_times [B][N], global_time [B], final
-        positions [B][N+1][2] robot first). `human_times`: arrivals recorded during the episode (0 = not yet)."""
+        positions [B][N+1][2] robot first). `human_times`: arrivals recorded during the episode (0 = not yet); default: the
+        stamps of track_arrivals (human_times_arrived, copied), or zeros when arrivals are not tracked."""
         B, N = self.B, self.human_num
-        ht = torch.zeros((B, N), dtype=torch.float64, device=self.device) if human_times is None else human_times.to(self.device, torch.float64).contiguous()
+        if human_times is not None:
+            ht = human_times.to(self.device, torch.float64).contiguous()
+        elif self.arrivals is not None:
+            ht = self.arrivals.h_arrival.clone()
+        else:
+            ht = torch.zeros((B, N), dtype=torch.float64, device=self.device)
         gt = torch.empty((B,), dtype=torch.float64, device=self.device)
         fp = torch.empty((B, N + 1, 2), dtype=torch.float64, device=self.device)
         prm = self.params(); st = self.state.struct()

@@ -144,6 +144,7 @@ class CrowdSim(object):
             self.human_num = 3
         self.humans = [Human(self.config, 'humans') for _ in range(n)]
         self.human_times = [0] * n
+        eng.track_arrivals()                                  # the step kernel stamps arrivals from here on (crowd_sim.py:404-407)
         self._pull(scene=True)
         for h in self.humans:
             h.theta = 0 if case >= 0 else np.pi / 2
@@ -185,9 +186,7 @@ class CrowdSim(object):
         v = self._np
         reward = float(v['reward'][0]); done = bool(v['done'][0]); code = int(v['info'][0])
         info = info_from_code(code, float(v['dmin'][0]))
-        for i, h in enumerate(self.humans):
-            if self.human_times[i] == 0 and h.reached_destination():
-                self.human_times[i] = self.global_time
+        self.human_times = eng.human_times_arrived[0, :len(self.humans)].tolist()
         ob = [h.get_observable_state() for h in self.humans]
         return ob, reward, done, info
 

@@ -23,7 +23,26 @@ struct StepArgs {
                            // other fields keep their offsets)
     crowdsim_record_maps recm;   // crowdsim_step_n_record_ex with occupancy-map rows (h_pos == NULL: none); after rec for
                                  // the same reason
+    crowdsim_arrivals arr;       // crowdsim_step_n_arrivals: read only by the ARR instantiations; last for the same reason
 };
+
+// ARR = true (crowdsim_step_n_arrivals): human a of env e after its float64 integration to np_ (crowd_sim.py:404-407,
+// agent.py:137-138): stamps its arrival with the env's post-step global_time ntime if it has none yet, and returns the stamp.
+__device__ __forceinline__ double arr_stamp(const StepArgs &A, size_t hi, double2 np_, double2 goal, double radius, double ntime)
+{
+    double t = A.arr.h_arrival[hi];
+    if (t == 0.0 && norm2(np_.x - goal.x, np_.y - goal.y) < radius) { t = ntime; A.arr.h_arrival[hi] = t; }
+    return t;
+}
+// ARR = true: human a's part of the end snapshot of the episode with result row c (crowdsim_arrivals).
+__device__ __forceinline__ void arr_snap_human(const StepArgs &A, int c, int N, int a, double2 np_, double2 nv, double2 goal,
+                                               double2 attr, double t)
+{
+    if (!A.arr.snap_h_pos) return;
+    const size_t j = (size_t)c * N + a;
+    st2(A.arr.snap_h_pos, j, np_); st2(A.arr.snap_h_vel, j, nv); st2(A.arr.snap_h_goal, j, goal); st2(A.arr.snap_h_attr, j, attr);
+    A.arr.snap_arrival[j] = t;
+}
 
 // ---- auto-reset protocol, consumer side (include/crowdsim_b200.h: crowdsim_autoreset) ----
 // Robot lane: an env that just finished (or is parked waiting) looks at its next-scene slot. Returns 1 = install now.
@@ -60,6 +79,15 @@ __device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
         A.ep.ep_case[e] = __ldcg(A.ar.n_case + e);
     }
     A.st.active[e] = 1; A.ar.want[e] = 0;
+}
+
+// crowdsim_step_n_arrivals' argument rules (include/crowdsim_b200.h).
+static inline int check_arrivals(const crowdsim_arrivals *r, const crowdsim_episodes *ep)
+{
+    if (!r->h_arrival) return CROWDSIM_EINVAL;
+    const int snaps = !!r->snap_r_vel + !!r->snap_h_pos + !!r->snap_h_vel + !!r->snap_h_goal + !!r->snap_h_attr + !!r->snap_arrival;
+    if (snaps != 0 && (snaps != 6 || !ep)) return CROWDSIM_EINVAL;
+    return CROWDSIM_OK;
 }
 
 // crowdsim_step_n_record_ex / crowdsim_record_flush_ex: the occupancy-map arguments, checked as crowdsim_occupancy_maps

@@ -41,6 +41,8 @@ namespace cs {
 // A/B builds.
 // ROT: the robot is a unicycle (CROWDSIM_ROBOT_EXTERNAL_ROT, agent.py:115-135). A template parameter so that the double
 // precision cos / sin / fmod code (12 % of the round-1 kernel's SASS) is only present in the kernels that execute it.
+// ARR: crowdsim_step_n_arrivals -- the humans stamp their arrivals and write the end snapshot of a finished episode
+// (step_args.cuh); ARR = false compiles to the SASS the kernel had before ARR.
 #ifndef CS_FLAT_WPB
 #define CS_FLAT_WPB 4
 #endif
@@ -59,7 +61,7 @@ struct RobotRec {
     uint8_t want, o_done, any_live, dirty_ep, new_case;
 };
 
-template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false>
+template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false>
 __global__ void __launch_bounds__(32 * CS_FLAT_WPB, CS_FLAT_MINBLOCKS * 4 / CS_FLAT_WPB)
 step_flat_kernel(const __grid_constant__ StepArgs A)
 {
@@ -307,6 +309,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     // ---- robot lane: ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72);
     // decides about auto-reset ----
     int install = 0;
+    int snap_c = -1;                                         // ARR: the result row of the episode that ended this step
     if (is_robot && env_ok) {
         bool done = false;
         if (live) {
@@ -338,6 +341,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                         ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
                         if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
+                        if constexpr (ARR) { snap_c = ep_c; if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, ep_c, vel); }
                     }
                     if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                 }
@@ -358,6 +362,16 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             }
         }
     }
+    if constexpr (ARR) {
+        // the humans' post-step positions, stamped and, when the episode ended, snapshotted before an install replaces them
+        const double ntime = __shfl_sync(CS_FULL, rr.gtime, rl);
+        const int snap = __shfl_sync(CS_FULL, snap_c, rl);
+        if (live && !is_robot) {
+            const double2 np_ = make_double2(pos.x + (double)nv.x * dt, pos.y + (double)nv.y * dt);
+            const double t = arr_stamp(A, hi, np_, goal, attr.x, ntime);
+            if (snap >= 0) arr_snap_human(A, snap, N, a, np_, make_double2((double)nv.x, (double)nv.y), goal, attr, t);
+        }
+    }
     if (A.has_ar) {                                          // warp-uniform
         install = __shfl_sync(CS_FULL, install, rl) && env_ok;
         // the scene goes straight from the slot to the live state (ar_install_*: acquire on the slot flag, copy)
@@ -365,6 +379,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             if (is_robot) ar_install_robot(A, e);
             else {
                 ar_install_human(A, e, N, a);
+                if constexpr (ARR) A.arr.h_arrival[hi] = 0.0;                       // crowd_sim.py:263-265
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, hi); reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
             }
         }

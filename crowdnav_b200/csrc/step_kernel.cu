@@ -36,7 +36,9 @@ namespace cs {
 // MID = false: the generic kernel of round 1 (RVO2's sequential code on per-thread shared-memory columns; any
 // max_neighbors <= 10; kept as the A/B partner of the two fast kernels in the tests: crowdsim_debug_force_generic).
 // MID = true: the crowd kernel for N > 5 (step_mid.cuh: register-resident lines, speculative LPs, compacted lp3).
-template <bool MID>
+// ARR = true: crowdsim_step_n_arrivals (the humans stamp their arrivals and write a finished episode's end snapshot,
+// step_args.cuh); ARR = false compiles to the SASS the kernel had before ARR.
+template <bool MID, bool ARR = false>
 __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgs A)
 {
     extern __shared__ __align__(16) unsigned char smem[];
@@ -102,6 +104,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
     // ---- robot lane: reduce clearances, ladder, update, bookkeeping; decides about auto-reset ----
     const bool env_ok = (e < A.B);
     int install = 0;
+    int snap_c = -1;                                         // ARR: the result row of the episode that ended this step
     if (is_robot && env_ok) {
         bool done = false;
         if (live) {
@@ -144,12 +147,24 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
                         ep.res_time[c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[c] = ret; ep.res_too_close[c] = tc; ep.res_min_dist_sum[c] = mds;
                         if (ep.res_final_rpos) st2(ep.res_final_rpos, c, npos);
+                        if constexpr (ARR) { snap_c = c; if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, c, nvel); }
                     }
                     if (A.st.active && !A.has_ar) A.st.active[e] = 0;
                 }
             }
+            if constexpr (ARR) s.act[le] = make_double2(ntime, (double)snap_c);   // (the humans read s.act[le] before the last barrier)
         }
         if (A.has_ar) install = ar_decide(A, e, ld_relaxed_u8(A.ar.n_state + e), live && done, !live && A.ar.want[e] != 0);
+    }
+    if constexpr (ARR) {
+        // the humans' post-step positions, stamped and, when the episode ended, snapshotted before an install replaces them
+        __syncthreads();
+        if (live && !is_robot) {
+            const double2 tc = s.act[le];                            // (post-step global_time, result row or -1)
+            const double2 np_ = make_double2(pos.x + (double)nv.x * dt, pos.y + (double)nv.y * dt);
+            const double t = arr_stamp(A, (size_t)e * N + a, np_, goal, attr.x, tc.x);
+            if (tc.y >= 0) arr_snap_human(A, (int)tc.y, N, a, np_, make_double2((double)nv.x, (double)nv.y), goal, attr, t);
+        }
     }
     if (A.has_ar) {
         if (is_robot) s.closest[le * L + N] = (double)install;     // the robot's own clearance slot is unused: env-wide flag
@@ -159,6 +174,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
             if (is_robot) ar_install_robot(A, e);
             else {
                 ar_install_human(A, e, N, a);
+                if constexpr (ARR) A.arr.h_arrival[(size_t)e * N + a] = 0.0;      // crowd_sim.py:263-265
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, (size_t)e * N + a); reinterpret_cast<float4 *>(A.io.obs32)[(size_t)e * N + a] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
             }
         }
@@ -244,9 +260,11 @@ static int sm_count()
 static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
                   const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int act_only, int n_steps, cudaStream_t stream,
                   double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr,
-                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr, bool rec_rot = false)
+                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr, bool rec_rot = false,
+                  const crowdsim_arrivals *arr = nullptr)
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
+    if (arr) { const int rc = check_arrivals(arr, ep); if (rc != CROWDSIM_OK) return rc; }
     if (rec) {
         // crowdsim_step_n_record: only the recording instantiation of the multi-step kernel records. crowdsim_step_n_record_ex
         // (rec_any_route): every N >= 1, through the launch loop where the multi-step kernel does not run
@@ -284,6 +302,8 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if (A.has_ar) A.ar = *ar; else memset(&A.ar, 0, sizeof(A.ar));
     if (rec) A.rec = *rec; else memset(&A.rec, 0, sizeof(A.rec));
     if (recm) A.recm = *recm; else memset(&A.recm, 0, sizeof(A.recm));
+    if (arr) A.arr = *arr; else memset(&A.arr, 0, sizeof(A.arr));
+    const bool ar_on = (arr != nullptr);                     // crowdsim_step_n_arrivals: the ARR instantiations
     if (act_only && N >= 1 && N <= 5 && !g_force_generic) {
         const int blocks = (B + 127) / 128;
         switch (N) {
@@ -304,16 +324,25 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
         if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream, rec_rot); }
-        #define CS_MULTI_LAUNCH(NN) do { cudaError_t err_;                                                                \
-            if (A.k.robot_visible) { if ((err_ = set_carveout<step_multi_kernel<NN, true, false>>())) return (int)err_;         \
-                                     step_multi_kernel<NN, true, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); }          \
-            else { if ((err_ = set_carveout<step_multi_kernel<NN, false, false>>())) return (int)err_;                          \
-                   step_multi_kernel<NN, false, false><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } } while (0)
-        switch (N) {
-            case 2: CS_MULTI_LAUNCH(2); break;
-            case 3: CS_MULTI_LAUNCH(3); break;
-            case 4: CS_MULTI_LAUNCH(4); break;
-            default: CS_MULTI_LAUNCH(5); break;
+        #define CS_MULTI_LAUNCH(NN, AR) do { cudaError_t err_;                                                            \
+            if (A.k.robot_visible) { if ((err_ = set_carveout<step_multi_kernel<NN, true, false, false, AR>>())) return (int)err_; \
+                                     step_multi_kernel<NN, true, false, false, AR><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } \
+            else { if ((err_ = set_carveout<step_multi_kernel<NN, false, false, false, AR>>())) return (int)err_;                 \
+                   step_multi_kernel<NN, false, false, false, AR><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } } while (0)
+        if (ar_on) {
+            switch (N) {
+                case 2: CS_MULTI_LAUNCH(2, true); break;
+                case 3: CS_MULTI_LAUNCH(3, true); break;
+                case 4: CS_MULTI_LAUNCH(4, true); break;
+                default: CS_MULTI_LAUNCH(5, true); break;
+            }
+        } else {
+            switch (N) {
+                case 2: CS_MULTI_LAUNCH(2, false); break;
+                case 3: CS_MULTI_LAUNCH(3, false); break;
+                case 4: CS_MULTI_LAUNCH(4, false); break;
+                default: CS_MULTI_LAUNCH(5, false); break;
+            }
         }
         #undef CS_MULTI_LAUNCH
         ++g_launches;
@@ -328,17 +357,27 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         // block barrier), per block when the chip is full (issue-bound: one warp runs the pass for the whole block).
         // The threshold scales with the device's SM count; scripts/latency_probe.cu times both.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        #define CS_FLAT_LAUNCH(NN) do { if (rot) step_flat_kernel<NN, 99, true, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                        else if (warpq) step_flat_kernel<NN, 99, false, true><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                        else step_flat_kernel<NN, 99, false, false><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
+        #define CS_FLAT_LAUNCH(NN, AR) do { if (rot) step_flat_kernel<NN, 99, true, true, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
+                                            else if (warpq) step_flat_kernel<NN, 99, false, true, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
+                                            else step_flat_kernel<NN, 99, false, false, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
         for (int rep = 0; rep < n_steps; ++rep) {
             if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);   // (crowdsim_step_n_record_ex at N = 1)
-            switch (N) {
-                case 1: CS_FLAT_LAUNCH(1); break;
-                case 2: CS_FLAT_LAUNCH(2); break;
-                case 3: CS_FLAT_LAUNCH(3); break;
-                case 4: CS_FLAT_LAUNCH(4); break;
-                default: CS_FLAT_LAUNCH(5); break;
+            if (ar_on) {
+                switch (N) {
+                    case 1: CS_FLAT_LAUNCH(1, true); break;
+                    case 2: CS_FLAT_LAUNCH(2, true); break;
+                    case 3: CS_FLAT_LAUNCH(3, true); break;
+                    case 4: CS_FLAT_LAUNCH(4, true); break;
+                    default: CS_FLAT_LAUNCH(5, true); break;
+                }
+            } else {
+                switch (N) {
+                    case 1: CS_FLAT_LAUNCH(1, false); break;
+                    case 2: CS_FLAT_LAUNCH(2, false); break;
+                    case 3: CS_FLAT_LAUNCH(3, false); break;
+                    case 4: CS_FLAT_LAUNCH(4, false); break;
+                    default: CS_FLAT_LAUNCH(5, false); break;
+                }
             }
             ++g_launches;
         }
@@ -351,14 +390,20 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     const bool mid = !g_force_generic && N > 5;              // (N = 0 and the forced A/B route stay on the generic kernel)
     const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
     if (smem > 48 * 1024) {                                  // (a per-device attribute; setting it again is cheap)
-        cudaError_t err = mid ? cudaFuncSetAttribute(step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                              : cudaFuncSetAttribute(step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        const void *fn = mid ? (ar_on ? (const void *)step_kernel<true, true> : (const void *)step_kernel<true>)
+                             : (ar_on ? (const void *)step_kernel<false, true> : (const void *)step_kernel<false>);
+        cudaError_t err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (err != cudaSuccess) return (int)err;
     }
     for (int rep = 0; rep < n_steps; ++rep) {
         if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);       // (crowdsim_step_n_record_ex)
-        if (mid) step_kernel<true><<<blocks, threads, smem, stream>>>(A);
-        else step_kernel<false><<<blocks, threads, smem, stream>>>(A);
+        if (ar_on) {
+            if (mid) step_kernel<true, true><<<blocks, threads, smem, stream>>>(A);
+            else step_kernel<false, true><<<blocks, threads, smem, stream>>>(A);
+        } else {
+            if (mid) step_kernel<true><<<blocks, threads, smem, stream>>>(A);
+            else step_kernel<false><<<blocks, threads, smem, stream>>>(A);
+        }
         ++g_launches;
     }
     if (rec) launch_record_between(A, n_steps - 1, -1, stream, rec_rot);
@@ -377,6 +422,15 @@ extern "C" int crowdsim_step_n(const crowdsim_params *prm, int B, int N, crowdsi
                                crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream)
 {
     return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream);
+}
+
+extern "C" int crowdsim_step_n_arrivals(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                        crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps,
+                                        const crowdsim_arrivals *arr, void *stream)
+{
+    if (!arr) return CROWDSIM_EINVAL;
+    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, nullptr, false, nullptr,
+                      false, arr);
 }
 
 extern "C" int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,

@@ -177,11 +177,15 @@ __device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int
 // ROT = true (REC only, crowdsim_step_n_record_rot): the rows of a unicycle robot, crowdsim_pack_joint(kinematics_unicycle = 1).
 // The robot's heading comes from st.r_theta at the launch's start; its ORCA step leaves it as it is, and an auto-reset
 // install carries on with the value the install writes to r_theta. ROT = false compiles to the SASS it had before ROT.
-template <int N, bool VIS, bool REC, bool ROT = false>
+// ARR = true (crowdsim_step_n_arrivals, not with REC): every human stamps its arrival (step_args.cuh) when it happens, from
+// one "arrived" bit kept across the steps, and writes its part of a finished episode's end snapshot before an install
+// replaces it; the robot writes its velocity's. ARR = false compiles to the SASS the kernel had before ARR.
+template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
 step_multi_kernel(const __grid_constant__ StepArgs A)
 {
     static_assert(REC || !ROT, "unicycle rows are a recording variant");
+    static_assert(!(REC && ARR), "arrivals are stamped by the rollout kernels only");
     static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
     using namespace orca;
     CS_RES_BEGIN
@@ -245,6 +249,8 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     }
     s_goal[tid] = goal;
     RobotRec &rr = s_rr[le];                                 // robot threads of valid envs only
+    bool arrived = false;                                    // ARR: my h_arrival is non-zero
+    if constexpr (ARR) { if (env_ok && !is_robot) arrived = A.arr.h_arrival[hi] != 0.0; }
 
     // what this launch changed on this thread (decides the stores at the end)
     bool dirty_kin = false, dirty_scene = false;
@@ -383,6 +389,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     // read their env's clearances after the barrier below without another one
     double *const s_cl = reinterpret_cast<double *>(&s_r2[0][0]);     // [E * N]: the humans' clearances
     bool timeout = false, reaching_goal = false;                       // robot lanes of live envs
+    int arr_c = -1;                                                    // ARR: my env's result row, read before the robot's tail
     if (!is_robot) {
         if (live) {
             // swept-segment clearance against the robot's velocity of this step
@@ -393,6 +400,12 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             const double hx = (double)nv.x, hy = (double)nv.y;
             pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
             dirty_kin = true;
+            if constexpr (ARR) {
+                // crowd_sim.py:404-407 with the robot's post-step time (rr.gtime + dt: the tail's ntime, the same operation)
+                arr_c = rr.ep_c;
+                const double2 g = s_goal[tid];
+                if (!arrived && norm2(pos.x - g.x, pos.y - g.y) < attr.x) { A.arr.h_arrival[hi] = rr.gtime + dt; arrived = true; }
+            }
         }
     } else if (env_ok) {
         // meanwhile the robot publishes everything else the env's ending depends on (PRE_*), so that after the barrier its
@@ -428,6 +441,9 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 for (int i = 0; i < N; ++i) collision |= s_cl[le * N + i] < 0;
                 done = (pf & PRE_TIMEOUT) || collision || (pf & PRE_GOAL);
                 if (done && A.has_ep && A.st.active && !A.has_ar) act_flag = 0;          // frozen
+                if constexpr (ARR) {
+                    if (done && arr_c >= 0) arr_snap_human(A, arr_c, N, a, pos, vel, s_goal[tid], attr, arrived ? A.arr.h_arrival[hi] : 0.0);
+                }
             }
             if (A.has_ar && ((live && done) || (!live && (pf & PRE_WANT)))) {
                 act_flag = (pf & PRE_READY) ? 1 : 0;                                      // install, or park
@@ -435,6 +451,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                     (void)ld_acquire_u8(A.ar.n_state + e);
                     pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); s_goal[tid] = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
                     dirty_kin = true; dirty_scene = true;
+                    if constexpr (ARR) { A.arr.h_arrival[hi] = 0.0; arrived = false; }       // crowd_sim.py:263-265
                 }
             }
         }
@@ -477,6 +494,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                             ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                             ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
                             if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
+                            if constexpr (ARR) { if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, ep_c, vel); }
                         }
                         if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                     }

@@ -28,6 +28,11 @@ In imitation learning the rows are what target_policy.transform stores (explorer
 Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous ranges per rank; there is no data-path
 collective; ONE gather of the per-case result rows (48 B per episode: 6 float64 columns; NCCL on GPU tensors, gloo in the CPU tests) brings
 them to rank 0, which prints the log lines.
+
+BatchedExplorer(..., human_times=True): the humans' time to goal after every successful episode (crowd_nav/test.py:105-107,
+"Average time for humans to reach goal"). The step kernels stamp the arrivals and keep each episode's end state
+(BatchedCrowdSim.track_arrivals); after the rollout CrowdSim.get_human_times runs once on device over every ReachGoal case
+(BatchedCrowdSim.case_human_times). The result rows then carry N more columns, the case's human times (0 for other endings).
 """
 import logging
 
@@ -53,11 +58,15 @@ def shard_range(k, rank, world):
     return start, base + (1 if rank < extra else 0)
 
 
-def pack_results(ep, n):
-    """Per-case result rows of an EpisodeBuffers as one [n][6] float64 tensor (exact for the integer columns)."""
+def pack_results(ep, n, human_times=None):
+    """Per-case result rows of an EpisodeBuffers as one [n][6] float64 tensor (exact for the integer columns); with
+    human_times ([n][N] float64) the rows are [n][6 + N]."""
     cols = [ep.res_info[:n].double(), ep.res_steps[:n].double(), ep.res_time[:n], ep.res_return[:n],
             ep.res_too_close[:n].double(), ep.res_min_dist_sum[:n]]
-    return torch.stack(cols, dim=1).contiguous()
+    rows = torch.stack(cols, dim=1)
+    if human_times is not None:
+        rows = torch.cat([rows, human_times[:n].to(rows.device, torch.float64)], dim=1)
+    return rows.contiguous()
 
 
 def gather_results(local_rows, k, rank, world, group=None):
@@ -75,9 +84,12 @@ def gather_results(local_rows, k, rank, world, group=None):
 
 
 def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info):
-    """explorer.py:52-90 on gathered per-case rows ([k][6]: info, steps, time, return, too_close, min_dist_sum).
-    Returns the statistics as a dict and emits the reference's log lines through `log`."""
+    """explorer.py:52-90 on gathered per-case rows ([k][6]: info, steps, time, return, too_close, min_dist_sum; [k][6 + N]
+    with the human times of BatchedExplorer(human_times=True)). Returns the statistics as a dict and emits the reference's
+    log lines through `log`."""
     rows = rows.cpu().tolist()
+    human_times = [list(r[6:]) if int(r[0]) == _abi.INFO_REACHGOAL else None for r in rows] if rows and len(rows[0]) > 6 else None
+    rows = [r[:6] for r in rows]
     success_times, collision_times, timeout_times = [], [], []
     collision_cases, timeout_cases = [], []
     cumulative_rewards = []
@@ -113,6 +125,12 @@ def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure
             % (too_close / num_step, avg_min_dist))
         stats['danger_frequency'] = too_close / num_step
         stats['avg_min_dist'] = avg_min_dist
+    if human_times is not None:
+        # crowd_nav/test.py:106-107 per successful case, averaged over the successful cases
+        per_case = [sum(ht) / len(ht) for ht in human_times if ht is not None]
+        stats['human_times'] = human_times
+        stats['avg_human_time'] = average(per_case)
+        log('Average time for humans to reach goal: %.2f' % stats['avg_human_time'])
     if print_failure:
         log('Collision cases: ' + ' '.join([str(x) for x in collision_cases]))
         log('Timeout cases: ' + ' '.join([str(x) for x in timeout_cases]))
@@ -137,8 +155,9 @@ def _unicycle_rows(policy):
 
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
-                 rank=0, world=1, group=None):
+                 rank=0, world=1, group=None, human_times=False):
         self.env = env
+        self.human_times = bool(human_times)
         self.robot_policy = robot_policy
         self.device = device or env.device
         self.memory = memory
@@ -158,11 +177,31 @@ class BatchedExplorer(object):
         env = self.env
         if update_memory and (self.memory is None or self.gamma is None):
             raise ValueError('Memory or gamma value is not set!')            # explorer.py:93-94
+        rule = env.test_sim if phase == 'test' else env.train_val_sim
+        if self.human_times and rule == 'mixed':
+            # the reference's own step raises IndexError there (crowd_sim.py:404-407 over a stale human_times, DESIGN §8)
+            raise ValueError('human times are not defined for rule mixed')
+        if self.human_times and update_memory:
+            raise ValueError('human times are measured by rollouts that do not record (update_memory=False)')
         first_case = env.case_counter[phase]
         start, n_local = shard_range(k, self.rank, self.world)
         gamma = self.gamma if self.gamma is not None else 0.9
+        args = (env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
+                steps_per_launch, first_case, start, n_local, gamma, rule)
+        if not self.human_times:
+            return self._run(*args)
+        prev_arrivals = env.arrivals                   # the caller's arrival tracking, back in place after the run
+        try:
+            return self._run(*args)
+        finally:
+            env.arrivals = prev_arrivals
+            env.fit_arrival_snapshots()                # (the run replaced the episode rows)
+
+    def _run(self, env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
+             steps_per_launch, first_case, start, n_local, gamma, rule):
         ep = env.track_episodes(max(n_local, 1), gamma)
-        rule = env.test_sim if phase == 'test' else env.train_val_sim
+        if self.human_times:
+            env.track_arrivals(snapshots=True)
         env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
         env.enable_autoreset(rule)
         unicycle = self.robot_policy != 'orca' and getattr(self.robot_policy, 'kinematics', 'holonomic') == 'unicycle'
@@ -237,7 +276,14 @@ class BatchedExplorer(object):
         main.wait_stream(side)
         if dev_rec is not None:
             dev_rec.finish()
-        rows = gather_results(pack_results(ep, n_local), k, self.rank, self.world, self.group)
+        local_times = None
+        if self.human_times:
+            # get_human_times once over every case of this rank that ended at the goal, from its end snapshot
+            local_times = torch.zeros((n_local, env.human_num), dtype=torch.float64, device=env.device)
+            ok = torch.nonzero(ep.res_info[:n_local] == _abi.INFO_REACHGOAL).flatten()
+            if ok.numel():
+                local_times[ok] = env.case_human_times(ok)[0]
+        rows = gather_results(pack_results(ep, n_local, local_times), k, self.rank, self.world, self.group)
         env.case_counter[phase] = (first_case + k) % env.case_size[phase]
         env.autoreset = None
         self.last_rows = rows

@@ -15,6 +15,8 @@
  *                            per-step part of Explorer.run_k_episodes (explorer.py:41-72)
  *   crowdsim_step_n          the inner loop of Explorer.run_k_episodes for a robot that decides on device
  *                            (crowd_nav/utils/explorer.py:41-43: robot.act -> env.step, n times), closed on the GPU
+ *   crowdsim_step_n_arrivals crowdsim_step_n that also stamps the humans' arrival times (crowd_sim.py:404-407) and keeps
+ *                            each finished episode's end state for get_human_times
  *   crowdsim_step_n_record   crowdsim_step_n that also stages one launch's imitation-learning demonstrations
  *   crowdsim_record_flush    ... and turns them into (state, value) pairs of the replay memory: Explorer.run_k_episodes
  *                            (update_memory=True, imitation_learning=True) with an ORCA robot (explorer.py:41-43,66-69,
@@ -269,6 +271,36 @@ int crowdsim_step(const crowdsim_params *prm, int B, int N, crowdsim_state *st, 
  */
 int crowdsim_step_n(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
                     crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream);
+
+/*
+ * Human arrival times of CrowdSim.step (crowd_sim.py:404-407): after every step that moves the agents (the terminal step
+ * included), human i of env e whose h_arrival[e][i] is 0 and who is within its radius of its goal (agent.py:137-138,
+ * norm(p - g) < radius in float64) gets h_arrival[e][i] = the env's global_time after the step. An auto-reset install
+ * zeroes the env's row, as CrowdSim.reset does (crowd_sim.py:263-265).
+ * When `ep` is given and an episode with a result row c = ep_case[e] >= 0 ends, the state CrowdSim.get_human_times starts
+ * from is written to row c of the snapshot arrays, before an install overwrites it: with ep->res_final_rpos (the robot's
+ * position) and ep->res_time (its global_time for ReachGoal), they form a crowdsim_state of k envs for
+ * crowdsim_human_times, whose human_times input is snap_arrival. The snapshot arrays are all given or all NULL (none
+ * written).
+ */
+typedef struct crowdsim_arrivals {
+    double *h_arrival;     /* [B][N] required, in/out: 0 = not arrived in the running episode */
+    double *snap_r_vel;    /* [k][2]    robot velocity after the terminal step */
+    double *snap_h_pos;    /* [k][N][2] human positions after the terminal step */
+    double *snap_h_vel;    /* [k][N][2] ... velocities */
+    double *snap_h_goal;   /* [k][N][2] ... goals */
+    double *snap_h_attr;   /* [k][N][2] ... radius, v_pref */
+    double *snap_arrival;  /* [k][N]    ... arrival times, the terminal step's stamps included */
+} crowdsim_arrivals;
+
+/*
+ * crowdsim_step_n(prm, B, N, st, io, ep, ar, n_steps) that also stamps arrivals (crowdsim_arrivals above), on every route
+ * crowdsim_step_n takes for n_steps = 1 and n_steps > 1; the states, outputs and episode rows are those of crowdsim_step_n.
+ * CROWDSIM_EINVAL without arr->h_arrival, with some but not all snapshot arrays, or with snapshot arrays and no `ep`.
+ */
+int crowdsim_step_n_arrivals(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                             crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const crowdsim_arrivals *arr,
+                             void *stream);
 
 /*
  * Imitation-learning demonstrations recorded on device: Explorer.run_k_episodes(update_memory=True,
