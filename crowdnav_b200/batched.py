@@ -24,6 +24,16 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
+def _ref(s):
+    """A ctypes struct by reference, or NULL."""
+    return None if s is None else C.byref(s)
+
+
+def _struct(buffers):
+    """The C struct of optional buffers (EpisodeBuffers, AutoResetBuffers, ...), or None."""
+    return None if buffers is None else buffers.struct()
+
+
 def max_episode_steps(time_limit, time_step):
     """Steps an episode can last: the timeout fires on the first step with global_time >= time_limit - 1
     (crowd_sim.py:368; 97 with the default 25 s / 0.25 s). +2 of slack."""
@@ -367,11 +377,9 @@ class BatchedCrowdSim(object):
                 self._scene_seed32.copy_(self._seed32)
             else:
                 self._scene_seed32.copy_(torch.where(mask != 0, self._seed32, self._scene_seed32))
-        st = self.state.struct()
-        ep = self.episodes.struct() if self.episodes is not None else None
+        st, ep = self.state.struct(), _struct(self.episodes)
         with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_reset(C.byref(a), self.B, self.human_num, C.byref(st),
-                                         C.byref(ep) if ep is not None else None, self._stream())
+            rc = self.lib.crowdsim_reset(C.byref(a), self.B, self.human_num, C.byref(st), _ref(ep), self._stream())
         _abi.check(rc, 'crowdsim_reset')
         self._keep = (mask, a)
         if self.arrivals is not None:                   # crowd_sim.py:263-265
@@ -496,21 +504,10 @@ class BatchedCrowdSim(object):
         if record is not None:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
-            prm = self.params(); st = self.state.struct()
-            io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
-                             _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
-            ep = self.episodes.struct() if self.episodes is not None else None
-            ar = self.autoreset.struct() if self.autoreset is not None else None
             rec, maps = record.struct(), record.maps_struct()
-            mp = C.byref(maps) if maps is not None else None
-            name = 'crowdsim_step_n_record_rot' if getattr(record, 'unicycle', False) else 'crowdsim_step_n_record_ex'
+            self._step_record_orca(int(n_steps), rec, maps, getattr(record, 'unicycle', False))
             with torch.cuda.device(self.device):
-                rc = getattr(self.lib, name)(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                             C.byref(ep) if ep is not None else None,
-                                             C.byref(ar) if ar is not None else None, int(n_steps), C.byref(rec),
-                                             mp, self._stream())
-                _abi.check(rc, name)
-                rc = self.lib.crowdsim_record_flush_ex(self.B, self.human_num, C.byref(rec), mp, int(n_steps), self._stream())
+                rc = self.lib.crowdsim_record_flush_ex(self.B, self.human_num, C.byref(rec), _ref(maps), int(n_steps), self._stream())
             _abi.check(rc, 'crowdsim_record_flush_ex')
             return self.observation(), self.reward, self.done, self.info
         if self.robot_policy != _abi.ROBOT_ORCA:
@@ -518,39 +515,38 @@ class BatchedCrowdSim(object):
                 raise ValueError('robot policy is external: actions required')
             if actions.data_ptr() != self.action.data_ptr():
                 self.action.copy_(actions, non_blocking=True)
-        prm = self.params()
-        st = self.state.struct()
-        io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
-                         _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
-        ep = self.episodes.struct() if self.episodes is not None else None
-        ar = self.autoreset.struct() if self.autoreset is not None else None
-        if self.arrivals is not None:
-            arr = self.arrivals.struct()
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step_n_arrivals(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                                       C.byref(ep) if ep is not None else None,
-                                                       C.byref(ar) if ar is not None else None, int(n_steps), C.byref(arr),
-                                                       self._stream())
-        elif n_steps == 1:
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                            C.byref(ep) if ep is not None else None, C.byref(ar) if ar is not None else None,
-                                            self._stream())
-        else:
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step_n(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                              C.byref(ep) if ep is not None else None, C.byref(ar) if ar is not None else None,
-                                              int(n_steps), self._stream())
+        prm, st, io = self.params(), self.state.struct(), self._io()
+        head = (C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(_struct(self.episodes)),
+                _ref(_struct(self.autoreset)), int(n_steps))
+        with torch.cuda.device(self.device):
+            if self.arrivals is not None:
+                arr = self.arrivals.struct()
+                rc = self.lib.crowdsim_step_n_arrivals(*head, C.byref(arr), self._stream())
+            else:
+                rc = self.lib.crowdsim_step_n(*head, self._stream())
         _abi.check(rc, 'crowdsim_step')
         return self.observation(), self.reward, self.done, self.info
 
+    def _io(self, obs32=True):
+        """crowdsim_step_io on this env's buffers, with the float32 observation when write_obs32 is set and obs32 allows it."""
+        return _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin), _ptr(self.done),
+                           _ptr(self.info), _ptr(self.obs32) if obs32 and self.write_obs32 else None)
+
+    def _step_record_orca(self, n_steps, rec, maps, unicycle):
+        """n_steps closed-loop steps of the ORCA robot, staged at `rec` / `maps` for a recorder: crowdsim_step_n_record_ex,
+        or crowdsim_step_n_record_rot for a unicycle target's rows."""
+        name = 'crowdsim_step_n_record_rot' if unicycle else 'crowdsim_step_n_record_ex'
+        prm, st, io = self.params(), self.state.struct(), self._io()
+        ep, ar = _struct(self.episodes), _struct(self.autoreset)
+        with torch.cuda.device(self.device):
+            rc = getattr(self.lib, name)(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(ep), _ref(ar),
+                                         n_steps, C.byref(rec), _ref(maps), self._stream())
+        _abi.check(rc, name)
+
     def _step_record_rl(self, actions, n_steps, record):
         """step(actions, n_steps, record=DeviceRLRecorder): stage the steps at the recorder's next free staging slots."""
-        ep = self.episodes.struct() if self.episodes is not None else None
-        if ep is None or self.autoreset is None:
+        if self.episodes is None or self.autoreset is None:
             raise ValueError('a recorded rollout needs episode tracking and auto-reset')
-        io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
-                         _ptr(self.done), _ptr(self.info), _ptr(self.obs32) if self.write_obs32 else None)
         if self.robot_policy == _abi.ROBOT_ORCA:
             if actions is not None:
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
@@ -560,13 +556,8 @@ class BatchedCrowdSim(object):
                 raise ValueError('n_steps must be between 1 and the recorder\'s n_max')
             if record.s + n_steps > record.n_max:
                 record.flush()
-            rec, maps = record.struct(record.s), record.maps_struct(record.s)
-            prm = self.params(); st = self.state.struct(); ar = self.autoreset.struct()
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_step_n_record_ex(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io),
-                                                        C.byref(ep), C.byref(ar), n_steps, C.byref(rec),
-                                                        C.byref(maps) if maps is not None else None, self._stream())
-            _abi.check(rc, 'crowdsim_step_n_record_ex')
+            # (the rows are the ORCA robot's own, holonomic ones, whatever the recorder's unicycle)
+            self._step_record_orca(n_steps, record.struct(record.s), record.maps_struct(record.s), False)
             record.staged(n_steps)
             return self.observation(), self.reward, self.done, self.info
         if actions is None:
@@ -575,11 +566,10 @@ class BatchedCrowdSim(object):
             raise ValueError('an external robot records one step per call')
         s = record.s
         rec, maps = record.struct(), record.maps_struct()
-        mp = C.byref(maps) if maps is not None else None
-        st = self.state.struct()
+        st, io, ep = self.state.struct(), self._io(), self.episodes.struct()
         with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
-                                               -1, s, self._stream())
+            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec),
+                                               _ref(maps), -1, s, self._stream())
         _abi.check(rc, 'crowdsim_record_book')
         if getattr(record, 'sort_humans', False):
             # LSTM-RL's rows, and the sorted human state over the env-order state the booking staged for the maps
@@ -589,8 +579,8 @@ class BatchedCrowdSim(object):
             self.pack_joint(unicycle=record.unicycle, out=record.rows[s])   # TrajectoryRecorder.before_step's rows
         self.step(actions)
         with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), mp,
-                                               s, -1, self._stream())
+            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec),
+                                               _ref(maps), s, -1, self._stream())
         _abi.check(rc, 'crowdsim_record_book')
         record.staged(1)
         return self.observation(), self.reward, self.done, self.info
@@ -704,8 +694,7 @@ class BatchedCrowdSim(object):
         out_vel = torch.empty((B, N, 2), dtype=torch.float64, device=self.device) if out_vel is None else out_vel
         if actions.data_ptr() != self.action.data_ptr():
             self.action.copy_(actions, non_blocking=True)
-        prm = self.params(); st = self.state.struct()
-        io = _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin), _ptr(self.done), _ptr(self.info), None)
+        prm, st, io = self.params(), self.state.struct(), self._io(obs32=False)
         with torch.cuda.device(self.device):
             rc = self.lib.crowdsim_onestep_lookahead(C.byref(prm), B, N, C.byref(st), C.byref(io), _ptr(out_pos), _ptr(out_vel), self._stream())
         _abi.check(rc, 'crowdsim_onestep_lookahead')

@@ -1,8 +1,9 @@
 // record_kernel.cu -- imitation-learning demonstrations recorded on device (sm_90a):
 //   launch_multi_record  the recording instantiations of the multi-step kernel (step_multi.cuh, REC = true), launched by
-//                        crowdsim_step_n_record and crowdsim_step_n_record_ex at 2 <= N <= 5 (step_kernel.cu)
-//   launch_record_between  the recording around each single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1,
-//                        N > 5, the forced generic kernel): the same staging, from the state between two launches
+//                        crowdsim_step_n_record and crowdsim_step_n_record_ex on the multi-step route (step_kernel.cu: route)
+//   launch_record_between  the recording around each single-step launch of the launch loop, for crowdsim_step_n_record_ex
+//                        on the other routes (N = 1, N > 5, the forced generic kernel): the same staging, from the state
+//                        between two launches
 //   (both with rot: crowdsim_step_n_record_rot, the rows of a unicycle robot -- step_multi_kernel<N, VIS, true, true> and
 //                        record_between_rot_kernel, the theta column (float)r_theta - rot)
 //   crowdsim_record_flush  one launch's staging -> per-slot trajectories -> (state, value) pairs of the replay memory ring
@@ -33,23 +34,9 @@ namespace cs {
 
 int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot)
 {
-    #define CS_MULTI_REC_RUN(...) do { if (cudaError_t err_ = set_carveout<step_multi_kernel<__VA_ARGS__>>()) return (int)err_; \
-                                       step_multi_kernel<__VA_ARGS__><<<blocks, 32 * (A.N + 1), 0, stream>>>(A); } while (0)
-    #define CS_MULTI_REC_LAUNCH(NN) do {                                                                                    \
-        if (rot) { if (A.k.robot_visible) CS_MULTI_REC_RUN(NN, true, true, true);                                           \
-                   else CS_MULTI_REC_RUN(NN, false, true, true); }                                                          \
-        else if (A.k.robot_visible) CS_MULTI_REC_RUN(NN, true, true);                                                       \
-        else CS_MULTI_REC_RUN(NN, false, true); } while (0)
-    switch (A.N) {
-        case 2: CS_MULTI_REC_LAUNCH(2); break;
-        case 3: CS_MULTI_REC_LAUNCH(3); break;
-        case 4: CS_MULTI_REC_LAUNCH(4); break;
-        case 5: CS_MULTI_REC_LAUNCH(5); break;
-        default: return CROWDSIM_EUNSUPPORTED;
-    }
-    #undef CS_MULTI_REC_LAUNCH
-    #undef CS_MULTI_REC_RUN
-    return (int)cudaGetLastError();
+    const int rc = with_int<2, 5>(A.N, [&](auto n) { return with_bool(A.k.robot_visible, [&](auto vis) { return with_bool(rot, [&](auto r) {
+        return launch_carved<step_multi_kernel<n, vis, true, r>>(A, blocks, 32 * (n + 1), stream); }); }); });
+    return rc != CROWDSIM_OK ? rc : (int)cudaGetLastError();
 }
 
 // The launch loop's recording (crowdsim_step_n_record_ex at N = 1, N > 5 or with the forced generic kernel): between two

@@ -1,9 +1,29 @@
 // step_args.cuh -- the argument block of the step kernels and the consumer side of the auto-reset protocol, shared by
 // step_kernel.cu (every step kernel) and record_kernel.cu (the recording instantiations of the multi-step kernel).
 #pragma once
+#include <type_traits>
 #include "crowdsim_common.cuh"
 
 namespace cs {
+
+// Runtime -> template arguments: with_int<Lo, Hi>(n, f) calls f(std::integral_constant<int, n>) for Lo <= n < Hi and
+// with Hi otherwise; with_bool(b, f) calls f(std::true_type / std::false_type). Each instantiates f at every value it
+// can pass, so a kernel set that is not a full product (no multi-step kernel with N = 1, no flat kernel with ROT && !WARPQ,
+// no recording multi-step kernel with ARR) keeps its exceptions out of the dispatched arguments.
+template <int Lo, int Hi, class F>
+inline auto with_int(int n, F &&f)
+{
+    if constexpr (Lo == Hi) return f(std::integral_constant<int, Lo>());
+    else {
+        if (n == Lo) return f(std::integral_constant<int, Lo>());
+        return with_int<Lo + 1, Hi>(n, f);
+    }
+}
+template <class F>
+inline auto with_bool(bool b, F &&f)
+{
+    return b ? f(std::true_type()) : f(std::false_type());
+}
 
 struct StepArgs {
     KParams k;
@@ -25,6 +45,16 @@ struct StepArgs {
                                  // the same reason
     crowdsim_arrivals arr;       // crowdsim_step_n_arrivals: read only by the ARR instantiations; last for the same reason
 };
+
+// Launch a multi-step kernel after setting its shared-memory carve-out (crowdsim_common.cuh). A carve-out error is
+// returned before anything is launched.
+template <auto Kernel>
+inline int launch_carved(const StepArgs &A, int blocks, int threads, cudaStream_t stream)
+{
+    if (const cudaError_t err = set_carveout<Kernel>()) return (int)err;
+    Kernel<<<blocks, threads, 0, stream>>>(A);
+    return CROWDSIM_OK;
+}
 
 // ARR = true (crowdsim_step_n_arrivals): human a of env e after its float64 integration to np_ (crowd_sim.py:404-407,
 // agent.py:137-138): stamps its arrival with the env's post-step global_time ntime if it has none yet, and returns the stamp.
@@ -101,14 +131,15 @@ static inline int check_record_maps(int N, const crowdsim_record_maps *m)
     return CROWDSIM_OK;
 }
 
-// record_kernel.cu: launch step_multi_kernel<N, VIS, true> (crowdsim_step_n_record) for 2 <= A.N <= 5. The recording
-// instantiations live in a unit of their own: their rows use CUDA's float32 atan2f / cosf / sinf (rotate.cuh), whose
-// library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code. rot: the unicycle-row
-// instantiation step_multi_kernel<N, VIS, true, true> (crowdsim_step_n_record_rot).
-int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot = false);
-// record_kernel.cu: the recording around one single-step launch of crowdsim_step_n_record_ex's launch loop (N = 1, N > 5, the
-// forced generic kernel). post >= 0: book step `post`'s reward and ending (TrajectoryRecorder.after_step); pre >= 0: stage
-// step `pre`'s rows of the envs live now (before_step). One launch. rot: the rows of a unicycle robot.
-void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream, bool rot = false);
+// record_kernel.cu: launch step_multi_kernel<N, VIS, true> (crowdsim_step_n_record) for 2 <= A.N <= 5; the caller has
+// checked N. The recording instantiations live in a unit of their own: their rows use CUDA's float32 atan2f / cosf / sinf
+// (rotate.cuh), whose library code contains explicit fma, and step_kernel.cu holds only FMA-free solver code. rot: the
+// unicycle-row instantiation step_multi_kernel<N, VIS, true, true> (crowdsim_step_n_record_rot).
+int launch_multi_record(const StepArgs &A, int blocks, cudaStream_t stream, bool rot);
+// record_kernel.cu: the recording around one single-step launch of the launch loop (step_kernel.cu: launch_loop) for
+// crowdsim_step_n_record_ex off the multi-step route (N = 1, N > 5, the forced generic kernel). post >= 0: book step
+// `post`'s reward and ending (TrajectoryRecorder.after_step); pre >= 0: stage step `pre`'s rows of the envs live now
+// (before_step). One launch. rot: the rows of a unicycle robot.
+void launch_record_between(const StepArgs &A, int post, int pre, cudaStream_t stream, bool rot);
 
 }  // namespace cs

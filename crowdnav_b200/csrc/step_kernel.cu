@@ -257,157 +257,150 @@ static int sm_count()
     return cache[dev];
 }
 
-static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
-                  const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int act_only, int n_steps, cudaStream_t stream,
-                  double *la_pos = nullptr, double *la_vel = nullptr, const crowdsim_record *rec = nullptr,
-                  bool rec_any_route = false, const crowdsim_record_maps *recm = nullptr, bool rec_rot = false,
-                  const crowdsim_arrivals *arr = nullptr)
+// What a step entry point asks for beyond the arguments every one of them takes. The defaults are crowdsim_step_n.
+struct StepMode {
+    bool act_only = false;                          // crowdsim_orca_act: the robot's ORCA decision only, nothing mutated
+    double *la_pos = nullptr, *la_vel = nullptr;    // crowdsim_onestep_lookahead: the humans' next states go here
+    const crowdsim_arrivals *arr = nullptr;         // crowdsim_step_n_arrivals: the ARR instantiations
+    const crowdsim_record *rec = nullptr;           // crowdsim_step_n_record*: stage the steps for an IL recorder
+    bool rec_any_route = false;                     // _ex / _rot: every N >= 1, through the launch loop off the multi route
+    bool rec_rot = false;                           // _rot: the rows of a unicycle robot
+    const crowdsim_record_maps *recm = nullptr;     // _ex / _rot: occupancy-map staging (NULL: none)
+};
+
+// The argument rules of every step entry point (include/crowdsim_b200.h), all decided before any CUDA call.
+static int check(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
+                 const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, const StepMode &m)
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
-    if (arr) { const int rc = check_arrivals(arr, ep); if (rc != CROWDSIM_OK) return rc; }
-    if (rec) {
+    if (m.arr) { const int rc = check_arrivals(m.arr, ep); if (rc != CROWDSIM_OK) return rc; }
+    if (const crowdsim_record *rec = m.rec) {
         // crowdsim_step_n_record: only the recording instantiation of the multi-step kernel records. crowdsim_step_n_record_ex
         // (rec_any_route): every N >= 1, through the launch loop where the multi-step kernel does not run
-        if (rec_any_route ? (N < 1 || N > CROWDSIM_MAX_HUMANS) : (N < 2 || N > 5 || g_force_generic)) return CROWDSIM_EUNSUPPORTED;
+        if (m.rec_any_route ? (N < 1 || N > CROWDSIM_MAX_HUMANS) : (N < 2 || N > 5 || g_force_generic)) return CROWDSIM_EUNSUPPORTED;
         if (prm->robot_policy != CROWDSIM_ROBOT_ORCA) return CROWDSIM_EUNSUPPORTED;
         if (!ep || !ar || !rec->rows || !rec->reward || !rec->t || !rec->code || n_steps > rec->n_max) return CROWDSIM_EINVAL;
-        if (rec_rot && !st->r_theta) return CROWDSIM_EINVAL;   // crowdsim_step_n_record_rot: the rows' heading
-        const int rc = check_record_maps(N, recm);
+        if (m.rec_rot && !st->r_theta) return CROWDSIM_EINVAL;   // crowdsim_step_n_record_rot: the rows' heading
+        const int rc = check_record_maps(N, m.recm);
         if (rc != CROWDSIM_OK) return rc;
     }
     if (N > CROWDSIM_MAX_HUMANS || prm->max_neighbors > CROWDSIM_MAX_NEIGHBORS) return CROWDSIM_EUNSUPPORTED;
     if (N > 0 && (!st->h_pos || !st->h_vel || !st->h_goal || !st->h_attr)) return CROWDSIM_EINVAL;
     if (!st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr || !st->g_time) return CROWDSIM_EINVAL;
     if (prm->robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT && !st->r_theta) return CROWDSIM_EINVAL;
-    if (act_only) { if (!io->action_out) return CROWDSIM_EINVAL; }
+    if (m.act_only) { if (!io->action_out) return CROWDSIM_EINVAL; }
     else {
         if (!io->reward || !io->dmin || !io->done || !io->info) return CROWDSIM_EINVAL;
         if (prm->robot_policy != CROWDSIM_ROBOT_ORCA && !io->action) return CROWDSIM_EINVAL;
     }
-    if (ep && !act_only && (!ep->ep_case || !ep->ep_steps || !ep->ep_return || !ep->ep_too_close || !ep->ep_min_dist_sum ||
-                            !ep->discount || !ep->res_info || !ep->res_steps || !ep->res_time || !ep->res_return ||
-                            !ep->res_too_close || !ep->res_min_dist_sum)) return CROWDSIM_EINVAL;
-    if (ar && !act_only) {
+    if (ep && !m.act_only && (!ep->ep_case || !ep->ep_steps || !ep->ep_return || !ep->ep_too_close || !ep->ep_min_dist_sum ||
+                              !ep->discount || !ep->res_info || !ep->res_steps || !ep->res_time || !ep->res_return ||
+                              !ep->res_too_close || !ep->res_min_dist_sum)) return CROWDSIM_EINVAL;
+    if (ar && !m.act_only) {
         if (!st->active || !ar->n_state || !ar->n_case || !ar->want || (N > 0 && (!ar->n_h_pos || !ar->n_h_goal || !ar->n_h_attr))) return CROWDSIM_EINVAL;
     }
-    if (B == 0) return CROWDSIM_OK;
+    return CROWDSIM_OK;
+}
+
+enum class Route { act, multi, flat, loop };
+
+// The kernel a step call runs: the first row that matches. F = crowdsim_debug_force_generic(1).
+//   act    crowdsim_orca_act, 1 <= N <= 5, !F                      orca_act_kernel<N>, one launch
+//   multi  (n_steps > 1 or rec), 2 <= N <= 5, ORCA robot, !F,      step_multi_kernel<N, VIS, REC, ROT, ARR>, n_steps in one
+//          not lookahead                                            launch with the state in registers (step_multi.cuh)
+//   flat   1 <= N <= 5, !F, not lookahead                          step_flat_kernel<N, 99, ROT, WARPQ, ARR> in the launch loop
+//   loop   everything else                                         step_kernel<MID, ARR> in the launch loop: the crowd kernel
+//                                                                   (MID) iff !F and N > 5, else the generic kernel
+// The multi-step kernel takes no external actions (the robot decides on device), and not N = 1: ptxas (CUDA 12.9, sm_90a,
+// -O1 and above) miscompiled that instantiation of the previous multi-step kernel -- its humans stored the position of the
+// step before the last one -- so N = 1 runs n single-step launches. Its recording instantiation runs for any n_steps.
+static Route route(const StepArgs &A, int n_steps, bool rec)
+{
+    const bool small = A.N >= 1 && A.N <= 5 && !g_force_generic;
+    if (A.act_only) return small ? Route::act : Route::loop;
+    if (!small || A.lookahead) return Route::loop;
+    if ((n_steps > 1 || rec) && A.N >= 2 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA) return Route::multi;
+    return Route::flat;
+}
+
+// n_steps single-step launches, each staged and booked by the recording around it when m.rec is set.
+template <class StepOnce>
+static int launch_loop(const StepArgs &A, int n_steps, const StepMode &m, cudaStream_t stream, StepOnce &&step_once)
+{
+    for (int rep = 0; rep < n_steps; ++rep) {
+        if (m.rec) launch_record_between(A, rep - 1, rep, stream, m.rec_rot);
+        step_once();
+        ++g_launches;
+    }
+    if (m.rec) launch_record_between(A, n_steps - 1, -1, stream, m.rec_rot);
+    return (int)cudaGetLastError();
+}
+
+static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, const crowdsim_step_io *io,
+                  const crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream_, const StepMode &m = {})
+{
+    const int rc = check(prm, B, N, st, io, ep, ar, n_steps, m);
+    if (rc != CROWDSIM_OK || B == 0) return rc;
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    const bool act_only = m.act_only;
     StepArgs A;
     A.k = make_kparams(prm, N);
     if (act_only) A.k.robot_policy = CROWDSIM_ROBOT_ORCA;
     A.B = B; A.N = N; A.L = N + 1; A.EPB = envs_per_block(A.L, 128);
     A.st = *st; A.io = *io; A.has_ep = (ep != nullptr && !act_only); A.act_only = act_only; A.n_steps = 1;
-    A.lookahead = (la_pos != nullptr); A.la_pos = la_pos; A.la_vel = la_vel;
+    A.lookahead = (m.la_pos != nullptr); A.la_pos = m.la_pos; A.la_vel = m.la_vel;
     if (A.has_ep) A.ep = *ep; else memset(&A.ep, 0, sizeof(A.ep));
     A.has_ar = (ar != nullptr && !act_only);
     if (A.has_ar) A.ar = *ar; else memset(&A.ar, 0, sizeof(A.ar));
-    if (rec) A.rec = *rec; else memset(&A.rec, 0, sizeof(A.rec));
-    if (recm) A.recm = *recm; else memset(&A.recm, 0, sizeof(A.recm));
-    if (arr) A.arr = *arr; else memset(&A.arr, 0, sizeof(A.arr));
-    const bool ar_on = (arr != nullptr);                     // crowdsim_step_n_arrivals: the ARR instantiations
-    if (act_only && N >= 1 && N <= 5 && !g_force_generic) {
-        const int blocks = (B + 127) / 128;
-        switch (N) {
-            case 1: orca_act_kernel<1><<<blocks, 128, 0, stream>>>(A); break;
-            case 2: orca_act_kernel<2><<<blocks, 128, 0, stream>>>(A); break;
-            case 3: orca_act_kernel<3><<<blocks, 128, 0, stream>>>(A); break;
-            case 4: orca_act_kernel<4><<<blocks, 128, 0, stream>>>(A); break;
-            default: orca_act_kernel<5><<<blocks, 128, 0, stream>>>(A); break;
-        }
+    if (m.rec) A.rec = *m.rec; else memset(&A.rec, 0, sizeof(A.rec));
+    if (m.recm) A.recm = *m.recm; else memset(&A.recm, 0, sizeof(A.recm));
+    if (m.arr) A.arr = *m.arr; else memset(&A.arr, 0, sizeof(A.arr));
+    const bool arr = (m.arr != nullptr);
+    switch (route(A, n_steps, m.rec != nullptr)) {
+    case Route::act:
+        with_int<1, 5>(N, [&](auto n) { orca_act_kernel<n><<<(B + 127) / 128, 128, 0, stream>>>(A); });
         ++g_launches;
         return (int)cudaGetLastError();
-    }
-    // n steps in one launch with the state in registers (step_multi.cuh): closed-loop only (the robot decides on device).
-    // Not for N = 1: ptxas (CUDA 12.9, sm_90a, -O1 and above) miscompiled that instantiation of the previous multi-step
-    // kernel -- its humans stored the position of the step before the last one -- so N = 1 runs n single-step launches.
-    // The recording instantiation runs for any n_steps (one step included).
-    if ((n_steps > 1 || rec) && N >= 2 && N <= 5 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA && !g_force_generic && !A.lookahead) {
+    case Route::multi: {
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
-        if (rec) { ++g_launches; return launch_multi_record(A, blocks, stream, rec_rot); }
-        #define CS_MULTI_LAUNCH(NN, AR) do { cudaError_t err_;                                                            \
-            if (A.k.robot_visible) { if ((err_ = set_carveout<step_multi_kernel<NN, true, false, false, AR>>())) return (int)err_; \
-                                     step_multi_kernel<NN, true, false, false, AR><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } \
-            else { if ((err_ = set_carveout<step_multi_kernel<NN, false, false, false, AR>>())) return (int)err_;                 \
-                   step_multi_kernel<NN, false, false, false, AR><<<blocks, 32 * (NN + 1), 0, stream>>>(A); } } while (0)
-        if (ar_on) {
-            switch (N) {
-                case 2: CS_MULTI_LAUNCH(2, true); break;
-                case 3: CS_MULTI_LAUNCH(3, true); break;
-                case 4: CS_MULTI_LAUNCH(4, true); break;
-                default: CS_MULTI_LAUNCH(5, true); break;
-            }
-        } else {
-            switch (N) {
-                case 2: CS_MULTI_LAUNCH(2, false); break;
-                case 3: CS_MULTI_LAUNCH(3, false); break;
-                case 4: CS_MULTI_LAUNCH(4, false); break;
-                default: CS_MULTI_LAUNCH(5, false); break;
-            }
-        }
-        #undef CS_MULTI_LAUNCH
+        if (m.rec) { ++g_launches; return launch_multi_record(A, blocks, stream, m.rec_rot); }
+        const int err = with_int<2, 5>(N, [&](auto n) { return with_bool(A.k.robot_visible, [&](auto vis) { return with_bool(arr, [&](auto ar_on) {
+            return launch_carved<step_multi_kernel<n, vis, false, false, ar_on>>(A, blocks, 32 * (n + 1), stream); }); }); });
+        if (err != CROWDSIM_OK) return err;
         ++g_launches;
         return (int)cudaGetLastError();
     }
-    if (N >= 1 && N <= 5 && !g_force_generic && !A.lookahead) {
+    case Route::flat: {
         // small crowds: register-resident solver, 32 / (N + 1) whole envs per warp (step_flat.cuh)
         const int epb = CS_FLAT_WPB * (32 / (N + 1));
         const int blocks = (B + epb - 1) / epb;
         const bool rot = A.k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT;
         // linearProgram3 queue of the single-step kernel: per warp when the launch leaves SMs mostly empty (latency-bound: no
         // block barrier), per block when the chip is full (issue-bound: one warp runs the pass for the whole block).
-        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both.
+        // The threshold scales with the device's SM count; scripts/latency_probe.cu times both. The unicycle robot's
+        // kernel exists with the per-warp queue only.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        #define CS_FLAT_LAUNCH(NN, AR) do { if (rot) step_flat_kernel<NN, 99, true, true, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                            else if (warpq) step_flat_kernel<NN, 99, false, true, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); \
-                                            else step_flat_kernel<NN, 99, false, false, AR><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); } while (0)
-        for (int rep = 0; rep < n_steps; ++rep) {
-            if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);   // (crowdsim_step_n_record_ex at N = 1)
-            if (ar_on) {
-                switch (N) {
-                    case 1: CS_FLAT_LAUNCH(1, true); break;
-                    case 2: CS_FLAT_LAUNCH(2, true); break;
-                    case 3: CS_FLAT_LAUNCH(3, true); break;
-                    case 4: CS_FLAT_LAUNCH(4, true); break;
-                    default: CS_FLAT_LAUNCH(5, true); break;
-                }
-            } else {
-                switch (N) {
-                    case 1: CS_FLAT_LAUNCH(1, false); break;
-                    case 2: CS_FLAT_LAUNCH(2, false); break;
-                    case 3: CS_FLAT_LAUNCH(3, false); break;
-                    case 4: CS_FLAT_LAUNCH(4, false); break;
-                    default: CS_FLAT_LAUNCH(5, false); break;
-                }
+        return launch_loop(A, n_steps, m, stream, [&] { with_int<1, 5>(N, [&](auto n) { with_bool(arr, [&](auto ar_on) {
+            if (rot) step_flat_kernel<n, 99, true, true, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else step_flat_kernel<n, 99, false, false, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); }); }); });
+    }
+    case Route::loop: {
+        const int threads = A.EPB * A.L;
+        const int blocks = (B + A.EPB - 1) / A.EPB;
+        const bool mid = !g_force_generic && N > 5;          // (N = 0 and the forced A/B route stay on the generic kernel)
+        const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
+        return with_bool(mid, [&](auto mid_) { return with_bool(arr, [&](auto ar_on) {
+            constexpr auto kernel = step_kernel<mid_, ar_on>;
+            if (smem > 48 * 1024) {                          // (a per-device attribute; setting it again is cheap)
+                const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                if (err != cudaSuccess) return (int)err;
             }
-            ++g_launches;
-        }
-        #undef CS_FLAT_LAUNCH
-        if (rec) launch_record_between(A, n_steps - 1, -1, stream, rec_rot);
-        return (int)cudaGetLastError();
+            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(A); }); }); });
     }
-    const int threads = A.EPB * A.L;
-    const int blocks = (B + A.EPB - 1) / A.EPB;
-    const bool mid = !g_force_generic && N > 5;              // (N = 0 and the forced A/B route stay on the generic kernel)
-    const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
-    if (smem > 48 * 1024) {                                  // (a per-device attribute; setting it again is cheap)
-        const void *fn = mid ? (ar_on ? (const void *)step_kernel<true, true> : (const void *)step_kernel<true>)
-                             : (ar_on ? (const void *)step_kernel<false, true> : (const void *)step_kernel<false>);
-        cudaError_t err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (err != cudaSuccess) return (int)err;
     }
-    for (int rep = 0; rep < n_steps; ++rep) {
-        if (rec) launch_record_between(A, rep - 1, rep, stream, rec_rot);       // (crowdsim_step_n_record_ex)
-        if (ar_on) {
-            if (mid) step_kernel<true, true><<<blocks, threads, smem, stream>>>(A);
-            else step_kernel<false, true><<<blocks, threads, smem, stream>>>(A);
-        } else {
-            if (mid) step_kernel<true><<<blocks, threads, smem, stream>>>(A);
-            else step_kernel<false><<<blocks, threads, smem, stream>>>(A);
-        }
-        ++g_launches;
-    }
-    if (rec) launch_record_between(A, n_steps - 1, -1, stream, rec_rot);
-    return (int)cudaGetLastError();
+    return CROWDSIM_EINVAL;   // (unreachable: route() returns one of the four)
 }
 
 }  // namespace cs
@@ -415,13 +408,13 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
 extern "C" int crowdsim_step(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
                              crowdsim_episodes *ep, const crowdsim_autoreset *ar, void *stream)
 {
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, 1, (cudaStream_t)stream);
+    return cs::launch(prm, B, N, st, io, ep, ar, 1, stream);
 }
 
 extern "C" int crowdsim_step_n(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
                                crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps, void *stream)
 {
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream);
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream);
 }
 
 extern "C" int crowdsim_step_n_arrivals(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
@@ -429,8 +422,8 @@ extern "C" int crowdsim_step_n_arrivals(const crowdsim_params *prm, int B, int N
                                         const crowdsim_arrivals *arr, void *stream)
 {
     if (!arr) return CROWDSIM_EINVAL;
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, nullptr, false, nullptr,
-                      false, arr);
+    cs::StepMode m; m.arr = arr;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 
 extern "C" int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
@@ -438,7 +431,8 @@ extern "C" int crowdsim_step_n_record(const crowdsim_params *prm, int B, int N, 
                                       void *stream)
 {
     if (!rec) return CROWDSIM_EINVAL;
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec);
+    cs::StepMode m; m.rec = rec;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 
 extern "C" int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
@@ -446,7 +440,8 @@ extern "C" int crowdsim_step_n_record_ex(const crowdsim_params *prm, int B, int 
                                          const crowdsim_record_maps *maps, void *stream)
 {
     if (!rec) return CROWDSIM_EINVAL;
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec, true, maps);
+    cs::StepMode m; m.rec = rec; m.rec_any_route = true; m.recm = maps;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 
 extern "C" int crowdsim_step_n_record_rot(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
@@ -454,7 +449,8 @@ extern "C" int crowdsim_step_n_record_rot(const crowdsim_params *prm, int B, int
                                           const crowdsim_record_maps *maps, void *stream)
 {
     if (!rec) return CROWDSIM_EINVAL;
-    return cs::launch(prm, B, N, st, io, ep, ar, 0, n_steps, (cudaStream_t)stream, nullptr, nullptr, rec, true, maps, true);
+    cs::StepMode m; m.rec = rec; m.rec_any_route = true; m.rec_rot = true; m.recm = maps;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 
 extern "C" int crowdsim_onestep_lookahead(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, crowdsim_step_io *io,
@@ -462,14 +458,16 @@ extern "C" int crowdsim_onestep_lookahead(const crowdsim_params *prm, int B, int
 {
     if (!next_h_pos || !next_h_vel || !st) return CROWDSIM_EINVAL;
     if (io && io->obs32) return CROWDSIM_EINVAL;
-    return cs::launch(prm, B, N, st, io, nullptr, nullptr, 0, 1, (cudaStream_t)stream, next_h_pos, next_h_vel);
+    cs::StepMode m; m.la_pos = next_h_pos; m.la_vel = next_h_vel;
+    return cs::launch(prm, B, N, st, io, nullptr, nullptr, 1, stream, m);
 }
 
 extern "C" int crowdsim_orca_act(const crowdsim_params *prm, int B, int N, const crowdsim_state *st, double *action_out,
                                  void *stream)
 {
     crowdsim_step_io io; memset(&io, 0, sizeof(io)); io.action_out = action_out;
-    return cs::launch(prm, B, N, st, &io, nullptr, nullptr, 1, 1, (cudaStream_t)stream);
+    cs::StepMode m; m.act_only = true;
+    return cs::launch(prm, B, N, st, &io, nullptr, nullptr, 1, stream, m);
 }
 
 extern "C" int crowdsim_graph_launch(void *graph_exec, void *stream, void *done_event)

@@ -140,23 +140,13 @@ def il_discounts(gamma, time_step, v_pref, T):
     return [pow(gamma, k * expo) for k in range(T)]
 
 
-class DeviceILRecorder(object):
-    """Imitation-learning demonstrations of an ORCA robot recorded on device (include/crowdsim_b200.h: crowdsim_record).
+class _DeviceRecorder(object):
+    """What DeviceILRecorder and DeviceRLRecorder share: the argument checks, the staging of up to n_max steps
+    (include/crowdsim_b200.h: crowdsim_record, with crowdsim_record_maps for occupancy maps), the per-slot trajectories,
+    and the ring's write position and size, which live on the device during a run: call begin() before the first step
+    and finish() after the last (one host read)."""
 
-    env.step(None, n_steps, record=self) runs n_steps closed-loop steps in one launch that also stages, per step and live
-    env, the rotated joint state, the reward, the episode step and how the step ended; a flush launch then appends them to
-    per-slot trajectories and writes the pairs of every episode that ends in ReachGoal or Collision to the memory ring, in
-    the order TrajectoryRecorder pushes them. The ring's write position and size live on the device during a run: call
-    begin() before the first step and finish() after the last (one host read).
-    At 2 <= N <= 5 the steps run in the recording multi-step kernel (one launch); at N = 1 and N > 5 they run one launch
-    each, between launches that stage the rows and book the rewards (include/crowdsim_b200.h: crowdsim_step_n_record_ex).
-    om = (cell_num, cell_size, om_channel_size): every row is followed by the occupancy map of the pre-step human state, as
-    TrajectoryRecorder(om=...) records it (MultiHumanRL.transform with with_om); the memory holds [N][13 + cell_num^2 *
-    om_channel_size] rows. unicycle: the rows of a unicycle target policy (crowdsim_step_n_record_rot: the theta column
-    r_theta - rot, cadrl.py:205-209), as TrajectoryRecorder(unicycle=True) packs them; the robot still runs ORCA and keeps
-    the heading its reset gave it. Only for an ORCA robot; RL targets use DeviceRLRecorder."""
-
-    def __init__(self, env, memory, gamma, n_max, om=None, unicycle=False):
+    def __init__(self, env, memory, n_max, om):
         from .batched import max_episode_steps
         B, N, dev = env.B, env.human_num, env.device
         if om is not None and N < 2:
@@ -164,24 +154,25 @@ class DeviceILRecorder(object):
         F = 13 + (om[0] * om[0] * om[2] if om else 0)
         if tuple(memory.states.shape[1:]) != (N, F):
             raise ValueError('memory rows must be [N][%d] joint states%s' % (F, ' with occupancy maps' if om else ''))
+        if int(n_max) < 1:
+            raise ValueError('n_max must be at least 1')
         self.env, self.memory, self.n_max, self.om = env, memory, int(n_max), om
-        self.unicycle = bool(unicycle)
         self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
-        self.g = torch.tensor(il_discounts(gamma, env.time_step, env.robot_v_pref, self.T), dtype=torch.float64, device=dev)
         n = self.n_max
-        self.rows = torch.empty((n, B, N, 13), dtype=torch.float32, device=dev)
-        self.reward = torch.empty((n, B), dtype=torch.float64, device=dev)
-        self.t = torch.empty((n, B), dtype=torch.int32, device=dev)
+        self.rows = torch.zeros((n, B, N, 13), dtype=torch.float32, device=dev)
+        self.reward = torch.zeros((n, B), dtype=torch.float64, device=dev)
+        self.t = torch.zeros((n, B), dtype=torch.int32, device=dev)
         self.code = torch.zeros((n, B), dtype=torch.uint8, device=dev)
         self.traj_rows = torch.zeros((B, self.T, N, F), dtype=torch.float32, device=dev)
         self.traj_reward = torch.zeros((B, self.T), dtype=torch.float64, device=dev)
         self.pushed = torch.zeros(1, dtype=torch.int64, device=dev)
         self.scan = torch.empty(n * B + 2, dtype=torch.int64, device=dev)
         self.position0 = memory.position
+        self.g = None                               # the IL discounts (DeviceILRecorder)
         if om:
-            self.h_pos = torch.empty((n, B, N, 2), dtype=torch.float64, device=dev)
-            self.h_vel = torch.empty((n, B, N, 2), dtype=torch.float64, device=dev)
-            self.maps = torch.empty((n, B, N, F - 13), dtype=torch.float32, device=dev)
+            self.h_pos = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.h_vel = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
+            self.maps = torch.zeros((n, B, N, F - 13), dtype=torch.float32, device=dev)
 
     def begin(self):
         """Start counting pushes at the memory's current write position."""
@@ -198,23 +189,47 @@ class DeviceILRecorder(object):
         self.pushed.zero_()
         return n
 
-    def struct(self):
+    def struct(self, s=0):
+        """crowdsim_record with its staging starting at step s of the window."""
         m = self.memory
         p = lambda t: t.data_ptr()  # noqa: E731
-        return _abi.Record(p(self.rows), p(self.reward), p(self.t), p(self.code), self.n_max, p(self.traj_rows),
-                           p(self.traj_reward), self.T, p(self.g), p(m.states), p(m.values), m.capacity, self.position0,
-                           p(self.pushed), p(self.scan))
+        return _abi.Record(p(self.rows[s]), p(self.reward[s]), p(self.t[s]), p(self.code[s]), self.n_max - s,
+                           p(self.traj_rows), p(self.traj_reward), self.T, None if self.g is None else p(self.g), p(m.states),
+                           p(m.values), m.capacity, self.position0, p(self.pushed), p(self.scan))
 
-    def maps_struct(self):
-        """The occupancy-map staging (include/crowdsim_b200.h: crowdsim_record_maps), or None without maps."""
+    def maps_struct(self, s=0):
+        """crowdsim_record_maps with its staging starting at step s, or None without maps."""
         if not self.om:
             return None
         cell_num, cell_size, channels = self.om
-        return _abi.RecordMaps(self.h_pos.data_ptr(), self.h_vel.data_ptr(), self.maps.data_ptr(), int(cell_num),
+        return _abi.RecordMaps(self.h_pos[s].data_ptr(), self.h_vel[s].data_ptr(), self.maps[s].data_ptr(), int(cell_num),
                                int(channels), float(cell_size))
 
 
-class DeviceRLRecorder(object):
+class DeviceILRecorder(_DeviceRecorder):
+    """Imitation-learning demonstrations of an ORCA robot recorded on device (include/crowdsim_b200.h: crowdsim_record).
+
+    env.step(None, n_steps, record=self) runs n_steps closed-loop steps in one launch that also stages, per step and live
+    env, the rotated joint state, the reward, the episode step and how the step ended; a flush launch then appends them to
+    per-slot trajectories and writes the pairs of every episode that ends in ReachGoal or Collision to the memory ring, in
+    the order TrajectoryRecorder pushes them. The ring's write position and size live on the device during a run: call
+    begin() before the first step and finish() after the last (one host read).
+    At 2 <= N <= 5 the steps run in the recording multi-step kernel (one launch); at N = 1 and N > 5 they run one launch
+    each, between launches that stage the rows and book the rewards (include/crowdsim_b200.h: crowdsim_step_n_record_ex).
+    om = (cell_num, cell_size, om_channel_size): every row is followed by the occupancy map of the pre-step human state, as
+    TrajectoryRecorder(om=...) records it (MultiHumanRL.transform with with_om); the memory holds [N][13 + cell_num^2 *
+    om_channel_size] rows. unicycle: the rows of a unicycle target policy (crowdsim_step_n_record_rot: the theta column
+    r_theta - rot, cadrl.py:205-209), as TrajectoryRecorder(unicycle=True) packs them; the robot still runs ORCA and keeps
+    the heading its reset gave it. Only for an ORCA robot; RL targets use DeviceRLRecorder."""
+
+    def __init__(self, env, memory, gamma, n_max, om=None, unicycle=False):
+        super().__init__(env, memory, n_max, om)
+        self.unicycle = bool(unicycle)
+        self.g = torch.tensor(il_discounts(gamma, env.time_step, env.robot_v_pref, self.T), dtype=torch.float64,
+                              device=env.device)
+
+
+class DeviceRLRecorder(_DeviceRecorder):
     """Reinforcement-learning transitions recorded on device: TrajectoryRecorder(imitation_learning=False) with the same
     pairs in the same order and no host synchronisation between steps (include/crowdsim_b200.h: crowdsim_record_flush_rl).
 
@@ -236,69 +251,19 @@ class DeviceRLRecorder(object):
     rl = True
 
     def __init__(self, env, memory, gamma, target_model, n_max, om=None, unicycle=False, sort_humans=False):
-        from .batched import max_episode_steps
-        B, N, dev = env.B, env.human_num, env.device
-        if om is not None and N < 2:
-            raise ValueError('need at least one array to concatenate')      # what env.occupancy_maps raises
-        F = 13 + (om[0] * om[0] * om[2] if om else 0)
-        if tuple(memory.states.shape[1:]) != (N, F):
-            raise ValueError('memory rows must be [N][%d] joint states%s' % (F, ' with occupancy maps' if om else ''))
-        if int(n_max) < 1:
-            raise ValueError('n_max must be at least 1')
-        self.env, self.memory, self.target_model, self.n_max = env, memory, target_model, int(n_max)
-        self.om, self.unicycle, self.sort_humans = om, bool(unicycle), bool(sort_humans)
-        self.T = max(128, max_episode_steps(env.time_limit, env.time_step))       # covers the longest episode
+        super().__init__(env, memory, n_max, om)
+        B, dev = env.B, env.device
+        self.target_model, self.unicycle, self.sort_humans = target_model, bool(unicycle), bool(sort_humans)
         self.gamma_bar = pow(gamma, env.time_step * env.robot_v_pref)              # TrajectoryRecorder.gamma_bar
-        n = self.n_max
-        self.rows = torch.zeros((n, B, N, 13), dtype=torch.float32, device=dev)
-        self.reward = torch.zeros((n, B), dtype=torch.float64, device=dev)
-        self.t = torch.zeros((n, B), dtype=torch.int32, device=dev)
-        self.code = torch.zeros((n, B), dtype=torch.uint8, device=dev)
-        self.boot = torch.zeros((n, B), dtype=torch.float32, device=dev)
-        self.traj_rows = torch.zeros((B, self.T, N, F), dtype=torch.float32, device=dev)
-        self.traj_reward = torch.zeros((B, self.T), dtype=torch.float64, device=dev)
+        self.boot = torch.zeros((self.n_max, B), dtype=torch.float32, device=dev)
         self.traj_boot = torch.zeros((B, self.T), dtype=torch.float32, device=dev)
-        self.pushed = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.scan = torch.empty(n * B + 2, dtype=torch.int64, device=dev)
-        self.position0 = memory.position
-        if om:
-            self.h_pos = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
-            self.h_vel = torch.zeros((n, B, N, 2), dtype=torch.float64, device=dev)
-            self.maps = torch.zeros((n, B, N, F - 13), dtype=torch.float32, device=dev)
         self.s = 0                                  # steps staged since the last flush
-
-    def begin(self):
-        """Start counting pushes at the memory's current write position."""
-        self.pushed.zero_()
-        self.position0 = self.memory.position
 
     def finish(self):
         """Flush what is staged, then move the memory's write position and size by what the flushes pushed since begin()
         (reads the counter)."""
         self.flush()
-        n = int(self.pushed.item())
-        m = self.memory
-        m.position = (self.position0 + n) % m.capacity
-        m.size = min(m.capacity, m.size + n)
-        self.position0 = m.position
-        self.pushed.zero_()
-        return n
-
-    def struct(self, s=0):
-        """crowdsim_record with its staging starting at step s of the window."""
-        m = self.memory
-        p = lambda t: t.data_ptr()  # noqa: E731
-        return _abi.Record(p(self.rows[s]), p(self.reward[s]), p(self.t[s]), p(self.code[s]), self.n_max - s,
-                           p(self.traj_rows), p(self.traj_reward), self.T, None, p(m.states), p(m.values), m.capacity,
-                           self.position0, p(self.pushed), p(self.scan))
-
-    def maps_struct(self, s=0):
-        """crowdsim_record_maps with its staging starting at step s, or None without maps."""
-        if not self.om:
-            return None
-        cell_num, cell_size, channels = self.om
-        return _abi.RecordMaps(self.h_pos[s].data_ptr(), self.h_vel[s].data_ptr(), self.maps[s].data_ptr(), int(cell_num),
-                               int(channels), float(cell_size))
+        return super().finish()
 
     def rl_struct(self):
         return _abi.RecordRL(self.boot.data_ptr(), self.traj_boot.data_ptr(), float(self.gamma_bar))
