@@ -781,7 +781,8 @@ class HostStepper(object):
 
         # The refill of the consumed next-scene slots only has to come round before the same slot's NEXT episode ends, and
         # an episode lasts at least ~7 steps: a refill launch on every prefetch_every-th step (default 4) loses nothing, while
-        # one per step keeps 32 blocks x 78 KB of shared memory busy for ~76 us on every step of every batch in flight.
+        # one per step adds the case assigner's launch and a grid of one-warp scene blocks beside every step of every batch
+        # in flight.
         self.prefetch_every = max(1, int(prefetch_every))
         self._n_launched = 0
 

@@ -7,10 +7,9 @@
 // Each env keeps that stream in a global [624][B] column (crowdsim_mt_stream) between decisions.
 //
 // At the first decision of an episode (ep_steps == 0) the stream is re-derived rather than carried over from the scene
-// kernels: the env's scene seed is seeded again and scene.cuh's generator runs on scratch to consume exactly its draws.
-// Like scene_kernel, each 128-slot block compacts the starting envs and its first kGen threads regenerate them in
-// shared-memory columns; the state then goes to the env's global column. After a block barrier every live env makes its
-// decision's draws from its global column.
+// kernels: the env's thread seeds scene.cuh's generator on the env's own column, runs the scene generator on its slice of
+// shared-memory scratch to consume exactly the scene's draws, and goes on to the decision's draws with the same generator.
+// One thread per env, one warp per block: no barrier, no shared generator state.
 #include "scene.cuh"
 
 namespace cs {
@@ -24,74 +23,59 @@ struct DrawKArgs {
     int B, N;
 };
 
-// The scene of env e again, from the seed that generated it, and the stream it leaves behind into e's global column.
-__device__ __forceinline__ void regenerate_stream(const DrawKArgs &K, int e, MT &rng, double *scratch, bool queue)
-{
-    const uint32_t seed = queue ? queue_seed(K.a, K.ep.ep_case[e]) : K.a.seed[e];
-    rng.seed(seed);
-    generate_scene(rng, K.a, K.N, scratch, scratch + 2 * K.N, scratch + 4 * K.N);
-    for (int i = 0; i < 624; ++i) K.ms.mt[(size_t)i * K.B + e] = rng.w(i);
-    K.ms.pos[e] = rng.pos;
-}
-
 // DRAW = false: write the post-generation stream of every (masked) env from its per-slot seed. DRAW = true: one policy
 // decision per live env, the stream re-derived first where the episode starts.
 template <bool DRAW>
-__global__ void __launch_bounds__(kSlotsPerBlock) policy_draws_kernel(const __grid_constant__ DrawKArgs K)
+__global__ void __launch_bounds__(32) policy_draws_kernel(const __grid_constant__ DrawKArgs K)
 {
-    extern __shared__ uint32_t s_mt[];                     // [624][kGen] words, then kGen x [3][N][2] doubles of scratch
-    __shared__ int s_list[kSlotsPerBlock];
-    __shared__ int s_count;
-    const int e = blockIdx.x * kSlotsPerBlock + threadIdx.x;
-    const bool queue = DRAW && K.a.case_counter != nullptr;
-    bool live = false, start = false;
-    if (e < K.B) {
-        if (DRAW) { live = K.st.active[e] != 0; start = live && K.ep.ep_steps[e] == 0; }
-        else start = !(K.a.mask && !K.a.mask[e]);
-    }
-    const int count = compact_block(start, e, s_list, &s_count);
-    if (threadIdx.x < kGen) {
-        MT rng; rng.mt = s_mt + threadIdx.x; rng.stride = kGen;
-        double *scratch = reinterpret_cast<double *>(s_mt + 624 * kGen) + (size_t)threadIdx.x * 6 * K.N;
-        for (int base = 0; base + (int)threadIdx.x < count; base += kGen)
-            regenerate_stream(K, s_list[base + threadIdx.x], rng, scratch, queue);
-    }
-    if (!DRAW) return;
-    __syncthreads();                                       // the regenerated columns are visible to their envs' threads
+    // [32][3][N][2]: each thread's scene scratch (hp, hg, ha). Not a local array: its ~3 KB at N = 63 would be stack
+    // reserved for every resident thread of the device, whichever kernel it runs.
+    extern __shared__ double s_scene[];
+    const int e = blockIdx.x * 32 + threadIdx.x;
     if (e >= K.B) return;
-    const crowdsim_policy_draw &d = K.d;
-    double u = -1.0; uint8_t explored = 0; int index = 0; uint8_t reached = 0;
-    if (live) {
-        // policy.py:41-48 reach_destination, with act_batch's expression: sqrt(dy * dy + dx * dx) < radius
-        const double2 p = ld2(K.st.r_pos, e), g = ld2(K.st.r_goal, e);
-        const double dy = p.y - g.y, dx = p.x - g.x;
-        reached = sqrt(dy * dy + dx * dx) < K.st.r_attr[2 * e];
-        if (!reached) {
-            MT rng; rng.mt = K.ms.mt + e; rng.stride = K.B; rng.pos = K.ms.pos[e];
-            u = rng.next_double();
-            if (d.train && u < d.epsilon) { explored = 1; index = rng.next_index((uint32_t)d.A); }
-            K.ms.pos[e] = rng.pos;
-        }
+    bool live = false, start;
+    if (DRAW) { live = K.st.active[e] != 0; start = live && K.ep.ep_steps[e] == 0; }
+    else start = !(K.a.mask && !K.a.mask[e]);
+    MT rng; rng.mt = K.ms.mt + e; rng.stride = K.B;
+    if (start) {                                           // the scene of env e again, from the seed that generated it
+        const bool queue = DRAW && K.a.case_counter != nullptr;
+        rng.seed(queue ? queue_seed(K.a, K.ep.ep_case[e]) : K.a.seed[e]);
+        double *scratch = s_scene + (size_t)threadIdx.x * 6 * K.N;
+        generate_scene(rng, K.a, K.N, scratch, scratch + 2 * K.N, scratch + 4 * K.N);
     }
-    d.u[e] = u; d.explored[e] = explored; d.index[e] = index; d.reached[e] = reached;
+    bool drew = false;
+    if (DRAW) {
+        const crowdsim_policy_draw &d = K.d;
+        double u = -1.0; uint8_t explored = 0; int index = 0; uint8_t reached = 0;
+        if (live) {
+            // policy.py:41-48 reach_destination, with act_batch's expression: sqrt(dy * dy + dx * dx) < radius
+            const double2 p = ld2(K.st.r_pos, e), g = ld2(K.st.r_goal, e);
+            const double dy = p.y - g.y, dx = p.x - g.x;
+            reached = sqrt(dy * dy + dx * dx) < K.st.r_attr[2 * e];
+            if (!reached) {
+                if (!start) rng.resume(K.ms.pos[e]);
+                u = rng.next_double();
+                if (d.train && u < d.epsilon) { explored = 1; index = rng.next_index((uint32_t)d.A); }
+                drew = true;
+            }
+        }
+        d.u[e] = u; d.explored[e] = explored; d.index[e] = index; d.reached[e] = reached;
+    }
+    if (start || drew) {
+        rng.store_seeded();
+        K.ms.pos[e] = rng.pos;
+    }
 }
-
-static size_t draws_smem(int N) { return (size_t)624 * kGen * sizeof(uint32_t) + (size_t)kGen * 6 * N * sizeof(double); }
 
 template <bool DRAW>
 static int launch_policy_draws(const DrawKArgs &K, cudaStream_t stream)
 {
-    static bool attr_set_dev[2][64];                       // the attribute is per DEVICE: cache keyed by the current device
-    int dev = 0; cudaGetDevice(&dev);
-    bool dummy = false; bool &attr_done = (dev >= 0 && dev < 64) ? attr_set_dev[DRAW][dev] : dummy;
-    if (!attr_done) {
-        cudaError_t err = cudaFuncSetAttribute(policy_draws_kernel<DRAW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)draws_smem(CROWDSIM_MAX_HUMANS));
+    const size_t smem = (size_t)32 * 6 * K.N * sizeof(double);
+    if (smem > 48 * 1024) {                                // (a per-device attribute; setting it again is cheap)
+        const cudaError_t err = cudaFuncSetAttribute(policy_draws_kernel<DRAW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (err != cudaSuccess) return (int)err;
-        attr_done = true;
     }
-    const int blocks = (K.B + kSlotsPerBlock - 1) / kSlotsPerBlock;
-    policy_draws_kernel<DRAW><<<blocks, kSlotsPerBlock, draws_smem(K.N), stream>>>(K);
+    policy_draws_kernel<DRAW><<<(K.B + 31) / 32, 32, smem, stream>>>(K);
     ++g_launches;
     return (int)cudaGetLastError();
 }

@@ -6,7 +6,7 @@
 // The refill kernels run beside other batches' multi-step kernels (bench: 16 streams, each a batch's steps and then its
 // refill), so they are sized to fit in what five multi-step blocks leave of an SM (DESIGN §3.3): one-warp scene blocks
 // without shared memory, a two-warp case assigner, and the multi-step kernel's shared-memory carve-out. The generator
-// (MTScene, scene.cuh) keeps the seeded MT19937 words it needs in registers and writes only the twisted words, to the slot's
+// (MT, scene.cuh) keeps the seeded MT19937 words it needs in registers and writes only the twisted words, to the slot's
 // column of a global [624][B] scratch (crowdsim_reset_args.scene_mt), so a scene reads no memory for its draws.
 #include <limits.h>
 #include "scene.cuh"
@@ -40,7 +40,7 @@ struct ResetKArgs {
 };
 
 // Live-state reset of env e from its generated scene (crowd_sim.py:251-312).
-__device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MTScene &rng)
+__device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MT &rng)
 {
     const crowdsim_reset_args &a = A.a;
     const int N = A.N;
@@ -68,7 +68,7 @@ __device__ __forceinline__ void reset_env(const ResetKArgs &A, int e, MTScene &r
 
 // Generator side of the auto-reset protocol (include/crowdsim_b200.h): fill an EMPTY (case queue: CLAIMED) next-scene slot,
 // mark it READY.
-__device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MTScene &rng)
+__device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MT &rng)
 {
     const crowdsim_autoreset &ar = A.ar;
     const int N = A.N;
@@ -84,39 +84,27 @@ __device__ __forceinline__ void prefetch_env(const ResetKArgs &A, int e, MTScene
     st_release_u8(ar.n_state + e, CROWDSIM_SLOT_READY);    // scene visible before the flag (release at gpu scope)
 }
 
-// One warp per block, kSceneSlots slots per block: the lanes ballot which of the block's slots need a scene, and the k-th
-// of those (in slot order) goes to lane k % 32, so every lane generates scenes while any are left. The block holds 32
-// threads x <= 64 registers and no shared memory, so two fit in what five multi-step blocks leave of an SM and a refill
-// never waits for step blocks to drain. A lane's twisted MT19937 words go to column base + lane of the caller's [624][B]
-// scratch (base + lane < B whenever the lane has a scene), so the stores of lanes drawing in step are one 128-byte line.
-// 32 slots per block: at most one scene per lane, so a block lives one scene. 128 slots per block (two to three scenes in
-// a row per lane, four times fewer blocks) measured 1.34e9 against 1.48-1.50e9 env-steps/s at full chip (DESIGN §3.6).
-constexpr int kSceneSlots = 32;
+// One warp per block over 32 slots: the lanes ballot which slots need a scene, and the k-th of them (in slot order) goes to
+// lane k, so every lane generates while scenes are left. A lane's twisted MT19937 words go to column base + lane of the
+// caller's [624][B] scratch (base + lane < B whenever the lane has a scene), so the stores of lanes drawing in step are one
+// 128-byte line. The block holds 32 threads x <= 64 registers and no shared memory, so two fit in what five multi-step
+// blocks leave of an SM and a refill never waits for step blocks to drain; it lives one scene. 128 slots per block (two to
+// three scenes in a row per lane, four times fewer blocks) measured 1.34e9 against 1.48-1.50e9 env-steps/s at full chip,
+// and each slot on its own lane without the ballot (64 registers instead of 58) 1-2 % slower with one batch in flight
+// (DESIGN §3.3, §3.6).
 template <bool PREFETCH>
 __global__ void __launch_bounds__(32, 32) scene_kernel(const __grid_constant__ ResetKArgs A)
 {
     CS_RES_BEGIN
-    const int lane = threadIdx.x, base = blockIdx.x * kSceneSlots;
-    unsigned bal[kSceneSlots / 32];
-    int count = 0;
-    #pragma unroll
-    for (int j = 0; j < kSceneSlots / 32; ++j) {
-        const int e = base + 32 * j + lane;
-        // acquire: the consumer's reads of the previous scene happen-before the writes of the next one
-        const bool need = e < A.B && (PREFETCH ? ld_acquire_u8(A.ar.n_state + e) == (A.assigned ? CROWDSIM_SLOT_CLAIMED : CROWDSIM_SLOT_EMPTY)
-                                               : !(A.a.mask && !A.a.mask[e]));
-        bal[j] = __ballot_sync(0xffffffffu, need);
-        count += __popc(bal[j]);
-    }
-    MTScene rng; rng.mt = A.a.scene_mt + base + lane; rng.stride = A.B;
-    for (int k = lane; k < count; k += 32) {
-        int j = 0, r = k;                                    // the k-th slot that needs a scene: bit r of ballot j
-        unsigned bj = bal[0];
-        #pragma unroll
-        for (int jj = 1; jj < kSceneSlots / 32; ++jj)
-            if (j == jj - 1 && r >= __popc(bj)) { r -= __popc(bj); j = jj; bj = bal[jj]; }
-        const int e = base + 32 * j + (int)__fns(bj, 0, r + 1);
-        if (PREFETCH) prefetch_env(A, e, rng); else reset_env(A, e, rng);
+    const int lane = threadIdx.x, base = blockIdx.x * 32, e = base + lane;
+    // acquire: the consumer's reads of the previous scene happen-before the writes of the next one
+    const bool need = e < A.B && (PREFETCH ? ld_acquire_u8(A.ar.n_state + e) == (A.assigned ? CROWDSIM_SLOT_CLAIMED : CROWDSIM_SLOT_EMPTY)
+                                           : !(A.a.mask && !A.a.mask[e]));
+    const unsigned bal = __ballot_sync(0xffffffffu, need);
+    MT rng; rng.mt = A.a.scene_mt + base + lane; rng.stride = A.B;
+    for (int k = lane; k < __popc(bal); k += 32) {          // (at most one pass)
+        const int slot = base + (int)__fns(bal, 0, k + 1);
+        if (PREFETCH) prefetch_env(A, slot, rng); else reset_env(A, slot, rng);
     }
 #ifdef CS_RESIDENCY_PROBE
     __syncwarp();                                            // the block ends with its last lane
@@ -195,7 +183,7 @@ static int launch_scene_kernel(ResetKArgs A, int B, cudaStream_t stream)
         assign_cases_kernel<PREFETCH><<<1, kAssignThreads, 0, stream>>>(A);
         ++g_launches;
     }
-    scene_kernel<PREFETCH><<<(B + kSceneSlots - 1) / kSceneSlots, 32, 0, stream>>>(A);
+    scene_kernel<PREFETCH><<<(B + 31) / 32, 32, 0, stream>>>(A);
     ++g_launches;
     return (int)cudaGetLastError();
 }

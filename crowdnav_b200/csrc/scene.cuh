@@ -6,7 +6,7 @@
 // (sample_random_attributes). float64 arithmetic in the reference's expression order; cos/sin are CUDA's (<= 1-2 ulp from
 // glibc's, which numpy uses): initial coordinates can differ from the CPU reference by ~1e-15 (tests bound it at 4e-15).
 // The draws themselves do not depend on cos/sin, so the stream after a scene is numpy's word for word.
-// MT, MTScene and generate_scene are also host functions: tests/native/mt_scene_check.cu compiles them for the CPU (glibc's
+// MT and generate_scene are also host functions: tests/native/mt_scene_check.cu compiles them for the CPU (glibc's
 // cos/sin there) and compares them with the CPU oracle word for word and bit for bit.
 #pragma once
 #include "crowdsim_common.cuh"
@@ -14,61 +14,24 @@
 namespace cs {
 
 // One generator's 624-word state, addressed through a pointer and a stride: an env's column of a global [624][B] array
-// between policy decisions, a thread's column of a shared-memory [624][columns] array while the draws kernel regenerates a
-// stream (scene_kernel's generator is MTScene below).
+// (crowdsim_mt_stream between policy decisions, crowdsim_reset_args.scene_mt for the scene kernel).
 // The twist is done lazily, in place and in order (word i of the next block needs old words i, i+1 and word i+397 mod 624,
 // which is old for i < 227 and already-new afterwards -- exactly the dependency order of the classic in-place loop), so a
 // scene only pays for the words it actually draws. Words [0, pos) therefore belong to the current block and words
 // [pos, 624) to the previous one; pos == 0 is both "just seeded" and "a whole block consumed", which numpy writes as pos 624.
+// Seeding stores nothing. In the first block after seeding, word i is twisted from seeded words s[i], s[i + 1] and, for
+// i < 227, s[i + 397]; those are never rewritten before they are read, so two cursors of the seeding recurrence in registers
+// produce them as the draws need them (seeding = 397 recurrence steps to place the second cursor). Only the twisted words go
+// to the column: word i >= 227 of the first block reads twisted word i - 227, word 623 reads twisted word 0, and from the
+// second block on the column holds a whole block of twisted words and the generator is the lazy twist over it. A scene (tens
+// of words) therefore reads no memory at all; each draw writes its word, a store nobody waits for. store_seeded() writes
+// the seeded words the column still lacks, after which column and pos are the whole state (batched.numpy_state reads it)
+// and resume(pos) continues from them.
 struct MT {
     uint32_t *mt;      // this generator's column of the state array
     int stride;        // columns of the state array
     int pos;           // next word to produce, 0..623 (wraps)
-    __host__ __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
-    __host__ __device__ void seed(uint32_t s) {
-        for (int i = 0; i < 624; ++i) { w(i) = s; s = 1812433253u * (s ^ (s >> 30)) + (uint32_t)i + 1u; }
-        pos = 0;
-    }
-    __host__ __device__ __forceinline__ uint32_t next() {
-        const int i = pos;
-        const int i1 = (i == 623) ? 0 : i + 1;
-        const int im = (i < 227) ? i + 397 : i - 227;
-        const uint32_t y0 = (w(i) & 0x80000000u) | (w(i1) & 0x7fffffffu);
-        uint32_t y = w(im) ^ (y0 >> 1) ^ ((y0 & 1u) ? 0x9908b0dfu : 0u);
-        w(i) = y;
-        pos = i1;
-        y ^= (y >> 11); y ^= (y << 7) & 0x9d2c5680u; y ^= (y << 15) & 0xefc60000u; y ^= (y >> 18);
-        return y;
-    }
-    __host__ __device__ __forceinline__ double next_double() { // genrand_res53
-        const uint32_t a = next() >> 5, b = next() >> 6;
-        return (a * 67108864.0 + b) / 9007199254740992.0;
-    }
-    // RandomState.choice(A) for 1 <= A <= 2^31: legacy randint(0, A) by masked rejection, one 32-bit word per try, with
-    // the smallest mask 2^k - 1 >= A - 1; A == 1 draws no word.
-    __host__ __device__ __forceinline__ int next_index(uint32_t A) {
-        const uint32_t rng = A - 1u;
-        if (rng == 0u) return 0;
-        uint32_t mask = rng;
-        mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
-        uint32_t v;
-        do { v = next() & mask; } while (v > rng);
-        return (int)v;
-    }
-};
-
-// The same stream as MT for a generator that starts from a seed (scene_kernel), without storing the seeded state.
-// In the first block after seeding, word i is twisted from seeded words s[i], s[i + 1] and, for i < 227, s[i + 397];
-// those are never rewritten before they are read, so two cursors of the seeding recurrence in registers produce them as
-// the draws need them (seeding = 397 recurrence steps to place the second cursor, no stores). Only the twisted words go to
-// the column: word i >= 227 of the first block reads twisted word i - 227, word 623 reads twisted word 0, and from the
-// second block on the column holds a whole block of twisted words and the generator is MT's lazy twist. A scene (tens of
-// words) therefore reads no memory at all; each draw writes its word, a store nobody waits for.
-struct MTScene {
-    uint32_t *mt;      // this generator's column of the state array (twisted words)
-    int stride;        // columns of the state array
-    int pos;           // next word to produce, 0..623 (wraps)
-    bool first;        // still in the first block after seeding
+    bool first;        // still in the first block after seeding: words [pos, 624) of the column not yet written
     uint32_t a, a1, m; // first block: seeded words s[pos], s[pos + 1], s[pos + 397]
     __host__ __device__ __forceinline__ uint32_t &w(int i) { return mt[i * stride]; }
     static __host__ __device__ __forceinline__ uint32_t init_step(uint32_t s, int k) { return 1812433253u * (s ^ (s >> 30)) + (uint32_t)k; }
@@ -77,6 +40,14 @@ struct MTScene {
         m = a1;
         for (int k = 2; k <= 397; ++k) m = init_step(m, k);
         pos = 0; first = true;
+    }
+    // Continue from a column and pos that store_seeded() left behind.
+    __host__ __device__ __forceinline__ void resume(int p) { pos = p; first = false; }
+    // Write the seeded words [pos, 624) of the first block (nothing after it), so the column holds the whole state.
+    __host__ __device__ void store_seeded() {
+        if (!first) return;
+        for (int i = pos; i < 624; ++i) { w(i) = a; a = init_step(a, i + 1); }
+        first = false;
     }
     __host__ __device__ __forceinline__ uint32_t next() {
         const int i = pos;
@@ -96,9 +67,20 @@ struct MTScene {
         y ^= (y >> 11); y ^= (y << 7) & 0x9d2c5680u; y ^= (y << 15) & 0xefc60000u; y ^= (y >> 18);
         return y;
     }
-    __host__ __device__ __forceinline__ double next_double() { // genrand_res53, as MT::next_double
+    __host__ __device__ __forceinline__ double next_double() { // genrand_res53
         const uint32_t a_ = next() >> 5, b_ = next() >> 6;
         return (a_ * 67108864.0 + b_) / 9007199254740992.0;
+    }
+    // RandomState.choice(A) for 1 <= A <= 2^31: legacy randint(0, A) by masked rejection, one 32-bit word per try, with
+    // the smallest mask 2^k - 1 >= A - 1; A == 1 draws no word.
+    __host__ __device__ __forceinline__ int next_index(uint32_t A) {
+        const uint32_t rng = A - 1u;
+        if (rng == 0u) return 0;
+        uint32_t mask = rng;
+        mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
+        uint32_t v;
+        do { v = next() & mask; } while (v > rng);
+        return (int)v;
     }
 };
 
@@ -216,19 +198,6 @@ __host__ __device__ __forceinline__ void generate_scene(RNG &rng, const crowdsim
 __device__ __forceinline__ uint32_t queue_seed(const crowdsim_reset_args &a, int c)
 {
     return a.seed_base + (a.case_wrap > 0 ? (uint32_t)(((long long)a.case_first + c) % a.case_wrap) : (uint32_t)c);
-}
-
-constexpr int kSlotsPerBlock = 128;   // env slots scanned per block of the draws kernel
-constexpr int kGen = 32;              // streams regenerated concurrently per draws block (624 * kGen * 4 B = 78 KB shared memory)
-
-// Compact the slots of this block that need a scene; returns the count (block-uniform). s_list[0..count) = env ids.
-__device__ __forceinline__ int compact_block(bool need, int e, int *s_list, int *s_count)
-{
-    if (threadIdx.x == 0) *s_count = 0;
-    __syncthreads();
-    if (need) s_list[atomicAdd(s_count, 1)] = e;
-    __syncthreads();
-    return *s_count;
 }
 
 }  // namespace cs

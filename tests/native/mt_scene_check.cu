@@ -1,12 +1,15 @@
-// mt_scene_check.cu -- CPU check (test infrastructure): scene.cuh's MT19937s and scene generator compiled FOR THE HOST
-// (MT, MTScene and generate_scene are __host__ __device__) against the CPU oracle (oracle/crowdsim_oracle.c, exported by
+// mt_scene_check.cu -- CPU check (test infrastructure): scene.cuh's MT19937 and scene generator compiled FOR THE HOST
+// (MT and generate_scene are __host__ __device__) against the CPU oracle (oracle/crowdsim_oracle.c, exported by
 // tests/native/stream_oracle.c), word for word and bit for bit:
-//   W  MTScene and MT against the oracle's mt_next over the first 4 x 624 + 8 words of many seeds. MTScene runs on one
-//      scratch column that every seed reuses, prefilled with junk, as a scene_kernel lane does.
-//   S  generate_scene driven by MTScene (scene_kernel) and by MT (draws kernel): the scene, and the next 2 x 624 + 4 words
-//      of its stream, for the long scenes of tests/golden/reset_scenes_long (square N = 40 and 63 at both profiles, square
-//      N = 32 with random attributes, circle N = 15). After every long scene the same column generates a short one
-//      (N = 5) and its stream. Circle scenes take glibc's cos / sin here, like the oracle, so they too match bit for bit.
+//   W  MT against the oracle's mt_next over the first 4 x 624 + 8 words of many seeds, on one scratch column that every
+//      seed reuses, prefilled with junk, as a scene_kernel lane does. Hand-over: after k words (k on and beside the
+//      first-block edges 227, 397, 624 and 1248), store_seeded() on a junk-prefilled column, and a fresh generator resumed
+//      at pos continues with the oracle's next 624 + 8 words.
+//   S  generate_scene and the next 2 x 624 + 4 words of its stream, as scene_kernel runs it (scene, then continue) and as
+//      the draws kernel leaves it (scene, store_seeded(), resume on the same column), for the long scenes of
+//      tests/golden/reset_scenes_long (square N = 40 and 63 at both profiles, square N = 32 with random attributes, circle
+//      N = 15). After every long scene the same column generates a short one (N = 5) and its stream. Circle scenes take
+//      glibc's cos / sin here, like the oracle, so they too match bit for bit.
 // Build (tests/test_native_cpu.py): gcc -c stream_oracle.c with the oracle's flags, then
 //   nvcc -O2 --fmad=false -Xcompiler -ffp-contract=off -std=c++17 mt_scene_check.cu stream_oracle.o -lgomp
 // Usage: mt_scene_check <seeds per config>; stdin: extra "<config> <seed>" lines (the fixture's seeds). Prints coverage
@@ -30,7 +33,9 @@ namespace {
 
 constexpr int kWords = 4 * 624 + 8;      // part W
 constexpr int kAfter = 2 * 624 + 4;      // part S: words drawn after a scene
+constexpr int kResume = 624 + 8;         // part W: words after a hand-over
 constexpr int kStride = 3;               // columns of the scratch array; the generators use column 1
+const int kHandover[] = {0, 1, 226, 227, 228, 396, 397, 398, 623, 624, 625, 1247, 1248, 1249};
 
 struct Config { const char *name; int rule, N, randomize; bool env_config; };
 const Config kConfigs[] = {
@@ -57,35 +62,47 @@ crowdsim_reset_args make_args(int rule, int randomize, bool env_config)
     return a;
 }
 
-std::vector<uint32_t> g_col(624 * kStride);     // the scratch column MTScene keeps for every seed and scene
+std::vector<uint32_t> g_col(624 * kStride);     // the scratch column scene_kernel's generator keeps for every seed and scene
 
 void fill_junk(std::vector<uint32_t> &v, uint32_t x)
 {
     for (auto &w : v) { x ^= x << 13; x ^= x >> 17; x ^= x << 5; w = x; }
 }
 
-// Part W: seeding and the raw stream across three block edges.
-bool check_words(uint32_t seed, long *words)
+// Part W: seeding and the raw stream across three block edges, and the stored state after k words.
+bool check_words(uint32_t seed, long *words, long *handovers)
 {
     std::vector<uint32_t> want(kWords);
     so_mt_words(seed, kWords, want.data());
-    std::vector<uint32_t> own(624);
-    cs::MT mt; mt.mt = own.data(); mt.stride = 1; mt.seed(seed);
-    cs::MTScene ms; ms.mt = g_col.data() + 1; ms.stride = kStride; ms.seed(seed);
+    cs::MT mt; mt.mt = g_col.data() + 1; mt.stride = kStride; mt.seed(seed);
     for (int i = 0; i < kWords; ++i) {
-        const uint32_t a = ms.next(), b = mt.next();
-        if (a != want[i] || b != want[i]) {
-            printf("W seed %u word %d: MTScene %08x MT %08x oracle %08x\n", seed, i, a, b, want[i]);
-            return false;
-        }
+        const uint32_t w = mt.next();
+        if (w != want[i]) { printf("W seed %u word %d: MT %08x oracle %08x\n", seed, i, w, want[i]); return false; }
     }
-    *words += 2 * kWords;
+    *words += kWords;
+    for (int k : kHandover) {
+        std::vector<uint32_t> col(624 * kStride);
+        fill_junk(col, seed ^ (uint32_t)k ^ 0x85ebca6bu);
+        cs::MT src; src.mt = col.data() + 1; src.stride = kStride; src.seed(seed);
+        for (int i = 0; i < k; ++i) src.next();
+        src.store_seeded();
+        cs::MT dst; dst.mt = col.data() + 1; dst.stride = kStride; dst.resume(src.pos);
+        for (int i = 0; i < kResume; ++i) {
+            const uint32_t w = dst.next();
+            if (w != want[k + i]) {
+                printf("W seed %u: resumed after %d words, word %d: MT %08x oracle %08x\n", seed, k, i, w, want[k + i]);
+                return false;
+            }
+        }
+        ++*handovers;
+    }
     return true;
 }
 
-template <class RNG>
-bool same_scene(RNG &rng, const crowdsim_reset_args &a, int N, uint32_t seed, const char *what, const double *ohp,
-                const double *ohg, const double *oha, const uint32_t *oafter)
+// One scene from `seed` on the generator's column, then kAfter words: straight on (scene_kernel), or after store_seeded()
+// and a fresh generator resumed on the same column (the draws kernel).
+bool same_scene(cs::MT &rng, bool hand_over, const crowdsim_reset_args &a, int N, uint32_t seed, const char *what,
+                const double *ohp, const double *ohg, const double *oha, const uint32_t *oafter)
 {
     double hp[2 * CROWDSIM_MAX_HUMANS], hg[2 * CROWDSIM_MAX_HUMANS], ha[2 * CROWDSIM_MAX_HUMANS];
     rng.seed(seed);
@@ -95,24 +112,28 @@ bool same_scene(RNG &rng, const crowdsim_reset_args &a, int N, uint32_t seed, co
         printf("S %s N=%d seed %u: scene differs\n", what, N, seed);
         return false;
     }
+    cs::MT fresh; fresh.mt = rng.mt; fresh.stride = rng.stride;
+    if (hand_over) { rng.store_seeded(); fresh.resume(rng.pos); }
+    cs::MT &g = hand_over ? fresh : rng;
     for (int i = 0; i < kAfter; ++i) {
-        const uint32_t w = rng.next();
+        const uint32_t w = g.next();
         if (w != oafter[i]) { printf("S %s N=%d seed %u: word %d after the scene %08x vs %08x\n", what, N, seed, i, w, oafter[i]); return false; }
     }
     return true;
 }
 
-// Part S: one scene through both generators against the oracle's.
+// Part S: one scene through both kernels' paths against the oracle's.
 bool check_scene(const crowdsim_reset_args &a, int N, uint32_t seed, const char *what)
 {
     double hp[2 * CROWDSIM_MAX_HUMANS], hg[2 * CROWDSIM_MAX_HUMANS], ha[2 * CROWDSIM_MAX_HUMANS];
     std::vector<uint32_t> after(kAfter);
     so_scene_stream(&a, N, seed, hp, hg, ha, kAfter, after.data());
-    cs::MTScene ms; ms.mt = g_col.data() + 1; ms.stride = kStride;
+    cs::MT scene; scene.mt = g_col.data() + 1; scene.stride = kStride;
     std::vector<uint32_t> own(624);
     fill_junk(own, seed | 1u);
-    cs::MT mt; mt.mt = own.data(); mt.stride = 1;
-    return same_scene(ms, a, N, seed, what, hp, hg, ha, after.data()) && same_scene(mt, a, N, seed, what, hp, hg, ha, after.data());
+    cs::MT draws; draws.mt = own.data(); draws.stride = 1;
+    return same_scene(scene, false, a, N, seed, what, hp, hg, ha, after.data()) &&
+           same_scene(draws, true, a, N, seed, what, hp, hg, ha, after.data());
 }
 
 }  // namespace
@@ -125,9 +146,9 @@ int main(int argc, char **argv)
     std::vector<uint32_t> seeds = {0u, 1u, 2u, 5489u, 2000u, 4294967294u, 4294967295u, 2147483648u};
     uint32_t x = 0x9e3779b9u;
     for (int i = 0; i < 200; ++i) { x ^= x << 13; x ^= x >> 17; x ^= x << 5; seeds.push_back(x); }
-    long words = 0;
+    long words = 0, handovers = 0;
     for (uint32_t s : seeds)
-        if (!check_words(s, &words)) return 1;
+        if (!check_words(s, &words, &handovers)) return 1;
     // ---- S ----
     std::vector<std::vector<uint32_t>> scene_seeds(sizeof(kConfigs) / sizeof(kConfigs[0]));
     for (auto &v : scene_seeds) {
@@ -156,7 +177,8 @@ int main(int argc, char **argv)
             }
         }
     }
-    printf("ok words=%ld seeds=%zu scenes=%ld above624=%ld above1248=%ld edge624=%ld edge1248=%ld short_after_long=%ld\n",
-           words, seeds.size(), scenes, above624, above1248, edge624, edge1248, short_after_long);
+    printf("ok words=%ld handovers=%ld seeds=%zu scenes=%ld above624=%ld above1248=%ld edge624=%ld edge1248=%ld "
+           "short_after_long=%ld\n", words, handovers, seeds.size(), scenes, above624, above1248, edge624, edge1248,
+           short_after_long);
     return 0;
 }

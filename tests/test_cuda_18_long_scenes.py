@@ -1,10 +1,10 @@
 """GPU tests of scenes that draw past the first MT19937 block (624 words) and of the exploration streams after them: square
-crossing at N = 40 and 63 and circle crossing at N = 15. scene_kernel's generator (MTScene) leaves its register-held
-first block at word 623 and continues as MT's lazy twist over the slot's scratch column; the draws kernel regenerates
-such scenes with MT and draws from the global column across word 624. Both refill paths, the device reset against the
-reference's scenes (tests/golden/reset_scenes_long), crowdsim_mt_streams and crowdsim_policy_draws are compared with the
-CPU oracle and numpy word for word, and every test counts, with the oracle's word counter, the scenes and draws that
-reached the second block, so that it fails if it stops reaching it."""
+crossing at N = 40 and 63 and circle crossing at N = 15. scene.cuh's generator leaves its register-held first block at
+word 623 and continues as the lazy twist over the slot's scratch column; the draws kernel regenerates such scenes on the
+env's global column and draws from it across word 624. Both refill paths, the device reset against the reference's scenes
+(tests/golden/reset_scenes_long), crowdsim_mt_streams and crowdsim_policy_draws are compared with the CPU oracle and numpy
+word for word, and every test counts, with the oracle's word counter, the scenes and draws that reached the second block,
+so that it fails if it stops reaching it."""
 import numpy as np
 import pytest
 import torch
@@ -203,7 +203,7 @@ def test_device_reset_equals_reference_long_scenes(name):
 
 @pytest.mark.parametrize('rule,N', LONG)
 def test_mt_streams_of_long_scenes_equal_oracle(rule, N):
-    """crowdsim_mt_streams (the draws kernel's regeneration, N = 63 takes 175 KB of dynamic shared memory) against the
+    """crowdsim_mt_streams (the draws kernel's regeneration, N = 63 takes 96.8 KB of dynamic shared memory) against the
     oracle's post-generation state word for word, for 1024 seeds with the block-edge seeds in the first block; envs at
     device pos 0 (a scene that ended on a block edge) included."""
     from crowdnav_b200.batched import numpy_state

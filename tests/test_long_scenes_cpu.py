@@ -1,7 +1,7 @@
 """CPU checks of scenes that draw more than one MT19937 block (624 words): square crossing at N = 40 and 63, N = 32 with
 random attributes, circle crossing at N = 15. The CPU oracle's reset, prefetch and post-generation stream against the
 reference's own scenes and numpy states (tests/golden/reset_scenes_long, oracle/gen_golden.py --only resets_long), the
-oracle's word counter against numpy, and scene.cuh's generators compiled for the host against the oracle word for word
+oracle's word counter against numpy, and scene.cuh's generator compiled for the host against the oracle word for word
 (tests/native/mt_scene_check.cu)."""
 import os
 import subprocess
@@ -104,16 +104,18 @@ def scene_check(tmp_path_factory):
     return exe
 
 
-def test_host_compiled_scene_generator_matches_oracle(scene_check):
-    """MTScene (scene_kernel's generator) and MT (the draws kernel's) against the oracle's mt_next over 4 x 624 + 8 words
-    of 208 seeds; generate_scene through both, and 1252 words after it, for 40 plain seeds per configuration, 0, 2^32 - 1
-    and every fixture seed; each long scene's scratch column then generates a short scene."""
+def test_host_compiled_generator_and_hand_over_match_oracle(scene_check):
+    """scene.cuh's MT against the oracle's mt_next over 4 x 624 + 8 words of 208 seeds, and its stored state after 14
+    word counts around the first block's edges continued by a resumed generator over 624 + 8 words; generate_scene, and
+    1252 words after it, as scene_kernel continues and as the draws kernel stores and resumes, for 40 plain seeds per
+    configuration, 0, 2^32 - 1 and every fixture seed; each long scene's scratch column then generates a short scene."""
     stdin = ''.join('%s %d\n' % (name, r['seed']) for name, _, _, _, _, rows in long_blocks() for r in rows)
     out = subprocess.run([scene_check, '40'], input=stdin, capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stdout[-500:]
     print(out.stdout.strip())
     fields = dict(kv.split('=') for kv in out.stdout.strip().split()[1:])
-    assert int(fields['seeds']) >= 200 and int(fields['words']) == 2 * int(fields['seeds']) * (4 * 624 + 8)
+    assert int(fields['seeds']) >= 200 and int(fields['words']) == int(fields['seeds']) * (4 * 624 + 8)
+    assert int(fields['handovers']) == int(fields['seeds']) * 14
     assert int(fields['scenes']) >= 300
     assert int(fields['above624']) >= 200 and int(fields['above1248']) >= 50
     assert int(fields['edge624']) >= 10 and int(fields['edge1248']) >= 3
