@@ -34,6 +34,15 @@ def _struct(buffers):
     return None if buffers is None else buffers.struct()
 
 
+def call(lib, device, name, *args):
+    """crowdsim_<name>(*args, stream) on `device` with its current stream; a non-zero return raises (_abi.check) with the
+    name of the entry point called."""
+    fn = 'crowdsim_' + name
+    with torch.cuda.device(device):
+        rc = getattr(lib, fn)(*args, C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+    _abi.check(rc, fn)
+
+
 def max_episode_steps(time_limit, time_step):
     """Steps an episode can last: the timeout fires on the first step with global_time >= time_limit - 1
     (crowd_sim.py:368; 97 with the default 25 s / 0.25 s). +2 of slack."""
@@ -101,7 +110,9 @@ class DeviceState(object):
         self.active = torch.ones(B, dtype=torch.uint8, device=device)
 
     def struct(self, with_active=True):
-        return _abi.State(*[_ptr(getattr(self, f)) for f in self.FIELDS], _ptr(self.active) if with_active else None)
+        return _abi.State(h_pos=_ptr(self.h_pos), h_vel=_ptr(self.h_vel), h_goal=_ptr(self.h_goal), h_attr=_ptr(self.h_attr),
+                          r_pos=_ptr(self.r_pos), r_vel=_ptr(self.r_vel), r_goal=_ptr(self.r_goal), r_attr=_ptr(self.r_attr),
+                          r_theta=_ptr(self.r_theta), g_time=_ptr(self.g_time), active=_ptr(self.active) if with_active else None)
 
     def load_host(self, host):
         """Copy from an object with the same numpy fields (e.g. oracle.pyoracle.HostState in tests)."""
@@ -132,10 +143,12 @@ class EpisodeBuffers(object):
         self.res_final_rpos = f64(k, 2)
 
     def struct(self):
-        return _abi.Episodes(_ptr(self.ep_case), _ptr(self.ep_steps), _ptr(self.ep_return), _ptr(self.ep_too_close),
-                             _ptr(self.ep_min_dist_sum), _ptr(self.discount), self.discount.numel(),
-                             _ptr(self.res_info), _ptr(self.res_steps), _ptr(self.res_time), _ptr(self.res_return),
-                             _ptr(self.res_too_close), _ptr(self.res_min_dist_sum), _ptr(self.res_final_rpos))
+        return _abi.Episodes(ep_case=_ptr(self.ep_case), ep_steps=_ptr(self.ep_steps), ep_return=_ptr(self.ep_return),
+                             ep_too_close=_ptr(self.ep_too_close), ep_min_dist_sum=_ptr(self.ep_min_dist_sum),
+                             discount=_ptr(self.discount), discount_len=self.discount.numel(),
+                             res_info=_ptr(self.res_info), res_steps=_ptr(self.res_steps), res_time=_ptr(self.res_time),
+                             res_return=_ptr(self.res_return), res_too_close=_ptr(self.res_too_close),
+                             res_min_dist_sum=_ptr(self.res_min_dist_sum), res_final_rpos=_ptr(self.res_final_rpos))
 
 
 class AutoResetBuffers(object):
@@ -152,8 +165,9 @@ class AutoResetBuffers(object):
     FIELDS = ('n_h_pos', 'n_h_goal', 'n_h_attr', 'n_case', 'n_state', 'want')
 
     def struct(self):
-        return _abi.AutoReset(_ptr(self.n_h_pos), _ptr(self.n_h_goal), _ptr(self.n_h_attr), _ptr(self.n_case),
-                              _ptr(self.n_state), _ptr(self.want), self.circle_radius, self.robot_radius, self.robot_v_pref)
+        return _abi.AutoReset(n_h_pos=_ptr(self.n_h_pos), n_h_goal=_ptr(self.n_h_goal), n_h_attr=_ptr(self.n_h_attr),
+                              n_case=_ptr(self.n_case), n_state=_ptr(self.n_state), want=_ptr(self.want),
+                              circle_radius=self.circle_radius, robot_radius=self.robot_radius, robot_v_pref=self.robot_v_pref)
 
     def load_host(self, host):
         for f in self.FIELDS:
@@ -179,8 +193,9 @@ class ArrivalBuffers(object):
             self.snap_r_vel = self.snap_h_pos = self.snap_h_vel = self.snap_h_goal = self.snap_h_attr = self.snap_arrival = None
 
     def struct(self):
-        return _abi.Arrivals(*[_ptr(getattr(self, f)) for f in ('h_arrival', 'snap_r_vel', 'snap_h_pos', 'snap_h_vel',
-                                                                  'snap_h_goal', 'snap_h_attr', 'snap_arrival')])
+        return _abi.Arrivals(h_arrival=_ptr(self.h_arrival), snap_r_vel=_ptr(self.snap_r_vel), snap_h_pos=_ptr(self.snap_h_pos),
+                             snap_h_vel=_ptr(self.snap_h_vel), snap_h_goal=_ptr(self.snap_h_goal),
+                             snap_h_attr=_ptr(self.snap_h_attr), snap_arrival=_ptr(self.snap_arrival))
 
 
 class BatchedCrowdSim(object):
@@ -266,13 +281,19 @@ class BatchedCrowdSim(object):
                              'external_rot': _abi.ROBOT_EXTERNAL_ROT, 'unicycle': _abi.ROBOT_EXTERNAL_ROT}[kind]
 
     def params(self):
-        return _abi.Params(self.time_step, float(self.time_limit), self.success_reward, self.collision_penalty,
-                           self.discomfort_dist, self.discomfort_penalty_factor, self.neighbor_dist, self.time_horizon,
-                           self.max_neighbors, self.human_safety_space, self.robot_safety_space,
-                           int(bool(self.robot_visible)), self.robot_policy)
+        return _abi.Params(time_step=self.time_step, time_limit=float(self.time_limit), success_reward=self.success_reward,
+                           collision_penalty=self.collision_penalty, discomfort_dist=self.discomfort_dist,
+                           discomfort_penalty_factor=self.discomfort_penalty_factor, neighbor_dist=self.neighbor_dist,
+                           time_horizon=self.time_horizon, max_neighbors=self.max_neighbors,
+                           human_safety_space=self.human_safety_space, robot_safety_space=self.robot_safety_space,
+                           robot_visible=int(bool(self.robot_visible)), robot_policy=self.robot_policy)
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _call(self, name, *args):
+        """crowdsim_<name>(*args, stream) on this batch's device and current stream (call())."""
+        call(self.lib, self.device, name, *args)
 
     # ---- episodes ------------------------------------------------------------------------------------------------
     def track_episodes(self, k, gamma=0.9):
@@ -321,15 +342,15 @@ class BatchedCrowdSim(object):
         if k == 0:
             return ht, gt, fp
         f64 = lambda vals: torch.tensor(vals, dtype=torch.float64, device=self.device).expand(k, len(vals)).contiguous()  # noqa: E731
-        snap = [arr.snap_h_pos[idx].contiguous(), arr.snap_h_vel[idx].contiguous(), arr.snap_h_goal[idx].contiguous(),
-                arr.snap_h_attr[idx].contiguous(), ep.res_final_rpos[idx].contiguous(), arr.snap_r_vel[idx].contiguous(),
-                f64([0.0, self.circle_radius]), f64([self.robot_radius, self.robot_v_pref]),
-                torch.full((k,), np.pi / 2, dtype=torch.float64, device=self.device), ep.res_time[idx].contiguous()]
-        st = _abi.State(*[_ptr(t) for t in snap], None)
+        snap = dict(h_pos=arr.snap_h_pos[idx].contiguous(), h_vel=arr.snap_h_vel[idx].contiguous(),
+                    h_goal=arr.snap_h_goal[idx].contiguous(), h_attr=arr.snap_h_attr[idx].contiguous(),
+                    r_pos=ep.res_final_rpos[idx].contiguous(), r_vel=arr.snap_r_vel[idx].contiguous(),
+                    r_goal=f64([0.0, self.circle_radius]), r_attr=f64([self.robot_radius, self.robot_v_pref]),
+                    r_theta=torch.full((k,), np.pi / 2, dtype=torch.float64, device=self.device),
+                    g_time=ep.res_time[idx].contiguous())
+        st = _abi.State(**{f: _ptr(t) for f, t in snap.items()})
         prm = self.params()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_human_times(C.byref(prm), k, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps), self._stream())
-        _abi.check(rc, 'crowdsim_human_times')
+        self._call('human_times', C.byref(prm), k, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps))
         return ht, gt, fp
 
     # ---- reset ---------------------------------------------------------------------------------------------------
@@ -354,11 +375,14 @@ class BatchedCrowdSim(object):
 
     def _reset_args(self, mask, rule, seed_stride, use_queue):
         q = use_queue and self._case_counter is not None
-        return _abi.ResetArgs(_ptr(mask), _ptr(self._seed32), int(seed_stride) % 2 ** 32, _abi.RULES[rule], self.circle_radius,
-                              self.square_width, self.human_radius, self.human_v_pref, self.robot_radius, self.robot_v_pref,
-                              self.discomfort_dist, int(bool(self.randomize_attributes)),
-                              _ptr(self._case_counter) if q else None, self._case_total if q else 0, self._seed_base if q else 0,
-                              self._case_first if q else 0, self._case_wrap if q else 0, _ptr(self._scene_mt))
+        return _abi.ResetArgs(mask=_ptr(mask), seed=_ptr(self._seed32), seed_stride=int(seed_stride) % 2 ** 32,
+                              rule=_abi.RULES[rule], circle_radius=self.circle_radius, square_width=self.square_width,
+                              human_radius=self.human_radius, human_v_pref=self.human_v_pref, robot_radius=self.robot_radius,
+                              robot_v_pref=self.robot_v_pref, discomfort_dist=self.discomfort_dist,
+                              randomize_attributes=int(bool(self.randomize_attributes)),
+                              case_counter=_ptr(self._case_counter) if q else None, case_total=self._case_total if q else 0,
+                              seed_base=self._seed_base if q else 0, case_first=self._case_first if q else 0,
+                              case_wrap=self._case_wrap if q else 0, scene_mt=_ptr(self._scene_mt))
 
     def reset_seeds(self, seeds=None, mask=None, rule='circle_crossing', seed_stride=0, use_queue=False):
         """crowdsim_reset for the envs selected by `mask` (uint8 device tensor, None = all) from the per-slot seeds.
@@ -378,9 +402,7 @@ class BatchedCrowdSim(object):
             else:
                 self._scene_seed32.copy_(torch.where(mask != 0, self._seed32, self._scene_seed32))
         st, ep = self.state.struct(), _struct(self.episodes)
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_reset(C.byref(a), self.B, self.human_num, C.byref(st), _ref(ep), self._stream())
-        _abi.check(rc, 'crowdsim_reset')
+        self._call('reset', C.byref(a), self.B, self.human_num, C.byref(st), _ref(ep))
         self._keep = (mask, a)
         if self.arrivals is not None:                   # crowd_sim.py:263-265
             if mask is None:
@@ -414,9 +436,7 @@ class BatchedCrowdSim(object):
     def prefetch(self):
         a = self._reset_args(None, self._ar_rule, self._ar_seed_stride, True)
         ar = self.autoreset.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_prefetch_scenes(C.byref(a), self.B, self.human_num, C.byref(ar), self._stream())
-        _abi.check(rc, 'crowdsim_prefetch_scenes')
+        self._call('prefetch_scenes', C.byref(a), self.B, self.human_num, C.byref(ar))
 
     # ---- exploration draws from numpy's stream ---------------------------------------------------------------------
     def _stream_bufs(self):
@@ -450,13 +470,10 @@ class BatchedCrowdSim(object):
         if not use_queue:
             a.seed = _ptr(self._scene_seed32)
         st, ep = self.state.struct(), self.episodes.struct()
-        ms = _abi.MTStream(_ptr(b['mt']), _ptr(b['pos']))
-        d = _abi.PolicyDraw(float(epsilon), int(A), int(bool(train)), _ptr(b['u']), _ptr(b['explored']), _ptr(b['index']),
-                            _ptr(b['reached']))
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_policy_draws(C.byref(a), self.B, self.human_num, C.byref(st), C.byref(ep), C.byref(ms),
-                                                C.byref(d), self._stream())
-        _abi.check(rc, 'crowdsim_policy_draws')
+        ms = _abi.MTStream(mt=_ptr(b['mt']), pos=_ptr(b['pos']))
+        d = _abi.PolicyDraw(epsilon=float(epsilon), A=int(A), train=int(bool(train)), u=_ptr(b['u']), explored=_ptr(b['explored']),
+                            index=_ptr(b['index']), reached=_ptr(b['reached']))
+        self._call('policy_draws', C.byref(a), self.B, self.human_num, C.byref(st), C.byref(ep), C.byref(ms), C.byref(d))
         return b['u'], b['explored'].bool(), b['index'].long(), b['reached'].bool()
 
     def mt_streams(self, seeds=None, rule='circle_crossing'):
@@ -472,10 +489,8 @@ class BatchedCrowdSim(object):
         pos = torch.empty((self.B,), dtype=torch.int32, device=self.device)
         a = self._reset_args(None, rule, 0, False)
         a.seed = _ptr(seed32)
-        ms = _abi.MTStream(_ptr(words), _ptr(pos))
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_mt_streams(C.byref(a), self.B, self.human_num, C.byref(ms), self._stream())
-        _abi.check(rc, 'crowdsim_mt_streams')
+        ms = _abi.MTStream(mt=_ptr(words), pos=_ptr(pos))
+        self._call('mt_streams', C.byref(a), self.B, self.human_num, C.byref(ms))
         return words, pos
 
     # ---- step ----------------------------------------------------------------------------------------------------
@@ -506,9 +521,7 @@ class BatchedCrowdSim(object):
                 raise ValueError('a recorded rollout runs the ORCA robot on device: no actions')
             rec, maps = record.struct(), record.maps_struct()
             self._step_record_orca(int(n_steps), rec, maps, getattr(record, 'unicycle', False))
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_record_flush_ex(self.B, self.human_num, C.byref(rec), _ref(maps), int(n_steps), self._stream())
-            _abi.check(rc, 'crowdsim_record_flush_ex')
+            self._call('record_flush_ex', self.B, self.human_num, C.byref(rec), _ref(maps), int(n_steps))
             return self.observation(), self.reward, self.done, self.info
         if self.robot_policy != _abi.ROBOT_ORCA:
             if actions is None:
@@ -518,30 +531,25 @@ class BatchedCrowdSim(object):
         prm, st, io = self.params(), self.state.struct(), self._io()
         head = (C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(_struct(self.episodes)),
                 _ref(_struct(self.autoreset)), int(n_steps))
-        with torch.cuda.device(self.device):
-            if self.arrivals is not None:
-                arr = self.arrivals.struct()
-                rc = self.lib.crowdsim_step_n_arrivals(*head, C.byref(arr), self._stream())
-            else:
-                rc = self.lib.crowdsim_step_n(*head, self._stream())
-        _abi.check(rc, 'crowdsim_step')
+        if self.arrivals is not None:
+            self._call('step_n_arrivals', *head, C.byref(self.arrivals.struct()))
+        else:
+            self._call('step_n', *head)
         return self.observation(), self.reward, self.done, self.info
 
     def _io(self, obs32=True):
         """crowdsim_step_io on this env's buffers, with the float32 observation when write_obs32 is set and obs32 allows it."""
-        return _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin), _ptr(self.done),
-                           _ptr(self.info), _ptr(self.obs32) if obs32 and self.write_obs32 else None)
+        return _abi.StepIO(action=_ptr(self.action), action_out=_ptr(self.action_out), reward=_ptr(self.reward),
+                           dmin=_ptr(self.dmin), done=_ptr(self.done), info=_ptr(self.info),
+                           obs32=_ptr(self.obs32) if obs32 and self.write_obs32 else None)
 
     def _step_record_orca(self, n_steps, rec, maps, unicycle):
         """n_steps closed-loop steps of the ORCA robot, staged at `rec` / `maps` for a recorder: crowdsim_step_n_record_ex,
         or crowdsim_step_n_record_rot for a unicycle target's rows."""
-        name = 'crowdsim_step_n_record_rot' if unicycle else 'crowdsim_step_n_record_ex'
         prm, st, io = self.params(), self.state.struct(), self._io()
         ep, ar = _struct(self.episodes), _struct(self.autoreset)
-        with torch.cuda.device(self.device):
-            rc = getattr(self.lib, name)(C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(ep), _ref(ar),
-                                         n_steps, C.byref(rec), _ref(maps), self._stream())
-        _abi.check(rc, name)
+        self._call('step_n_record_rot' if unicycle else 'step_n_record_ex', C.byref(prm), self.B, self.human_num, C.byref(st),
+                   C.byref(io), _ref(ep), _ref(ar), n_steps, C.byref(rec), _ref(maps))
 
     def _step_record_rl(self, actions, n_steps, record):
         """step(actions, n_steps, record=DeviceRLRecorder): stage the steps at the recorder's next free staging slots."""
@@ -567,10 +575,7 @@ class BatchedCrowdSim(object):
         s = record.s
         rec, maps = record.struct(), record.maps_struct()
         st, io, ep = self.state.struct(), self._io(), self.episodes.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec),
-                                               _ref(maps), -1, s, self._stream())
-        _abi.check(rc, 'crowdsim_record_book')
+        self._call('record_book', self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), _ref(maps), -1, s)
         if getattr(record, 'sort_humans', False):
             # LSTM-RL's rows, and the sorted human state over the env-order state the booking staged for the maps
             self.pack_joint(unicycle=record.unicycle, out=record.rows[s], order_by_distance=True,
@@ -578,10 +583,7 @@ class BatchedCrowdSim(object):
         else:
             self.pack_joint(unicycle=record.unicycle, out=record.rows[s])   # TrajectoryRecorder.before_step's rows
         self.step(actions)
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_record_book(self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec),
-                                               _ref(maps), s, -1, self._stream())
-        _abi.check(rc, 'crowdsim_record_book')
+        self._call('record_book', self.B, self.human_num, C.byref(st), C.byref(io), C.byref(ep), C.byref(rec), _ref(maps), s, -1)
         record.staged(1)
         return self.observation(), self.reward, self.done, self.info
 
@@ -592,9 +594,7 @@ class BatchedCrowdSim(object):
     def orca_act(self, out=None):
         out = self.action_out if out is None else out
         prm = self.params(); st = self.state.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_orca_act(C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(out), self._stream())
-        _abi.check(rc, 'crowdsim_orca_act')
+        self._call('orca_act', C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(out))
         return out
 
     def observation(self):
@@ -616,19 +616,14 @@ class BatchedCrowdSim(object):
             out = torch.empty((B, N, 13), dtype=torch.float32, device=self.device)
         st = self.state.struct()
         if not order_by_distance:
-            with torch.cuda.device(self.device):
-                rc = self.lib.crowdsim_pack_joint(B, N, C.byref(st), int(unicycle), _ptr(out), self._stream())
-            _abi.check(rc, 'crowdsim_pack_joint')
+            self._call('pack_joint', B, N, C.byref(st), int(unicycle), _ptr(out))
             return out
         if return_state:
             f = lambda t, shape, dtype: torch.empty(shape, dtype=dtype, device=self.device) if t is None else t  # noqa: E731
             out_order = f(out_order, (B, N), torch.int32)
             out_pos = f(out_pos, (B, N, 2), torch.float64)
             out_vel = f(out_vel, (B, N, 2), torch.float64)
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_pack_joint_sorted(B, N, C.byref(st), int(unicycle), _ptr(out), _ptr(out_order),
-                                                     _ptr(out_pos), _ptr(out_vel), self._stream())
-        _abi.check(rc, 'crowdsim_pack_joint_sorted')
+        self._call('pack_joint_sorted', B, N, C.byref(st), int(unicycle), _ptr(out), _ptr(out_order), _ptr(out_pos), _ptr(out_vel))
         return (out, out_order, out_pos, out_vel) if return_state else out
 
     def lookahead_pack(self, actions, unicycle=False, out_states=None, out_reward=None):
@@ -639,10 +634,8 @@ class BatchedCrowdSim(object):
         if out_reward is None:
             out_reward = torch.empty((self.B, A), dtype=torch.float64, device=self.device)
         prm = self.params(); st = self.state.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_lookahead_pack(C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(actions), A,
-                                                  int(unicycle), _ptr(out_states), _ptr(out_reward), self._stream())
-        _abi.check(rc, 'crowdsim_lookahead_pack')
+        self._call('lookahead_pack', C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(actions), A, int(unicycle),
+                   _ptr(out_states), _ptr(out_reward))
         return out_states, out_reward
 
     def propagate_pack(self, actions, unicycle=False, order_by_distance=False, out_states=None, out_reward=None, out_pos=None,
@@ -659,11 +652,8 @@ class BatchedCrowdSim(object):
         out_vel = f(out_vel, (B, N, 2), torch.float64)
         out_order = f(out_order, (B, N), torch.int32)
         prm = self.params(); st = self.state.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_propagate_pack(C.byref(prm), B, N, C.byref(st), _ptr(actions), A, int(unicycle),
-                                                  int(order_by_distance), _ptr(out_states), _ptr(out_reward), _ptr(out_pos),
-                                                  _ptr(out_vel), _ptr(out_order), self._stream())
-        _abi.check(rc, 'crowdsim_propagate_pack')
+        self._call('propagate_pack', C.byref(prm), B, N, C.byref(st), _ptr(actions), A, int(unicycle), int(order_by_distance),
+                   _ptr(out_states), _ptr(out_reward), _ptr(out_pos), _ptr(out_vel), _ptr(out_order))
         return out_states, out_reward, out_pos, out_vel, out_order
 
 
@@ -680,10 +670,7 @@ class BatchedCrowdSim(object):
         if out_vel is None:
             out_vel = torch.empty((self.B, self.human_num, 2), dtype=torch.float64, device=self.device)
         prm = self.params(); st = self.state.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_lookahead_humans(C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(out_pos), _ptr(out_vel),
-                                                    self._stream())
-        _abi.check(rc, 'crowdsim_lookahead_humans')
+        self._call('lookahead_humans', C.byref(prm), self.B, self.human_num, C.byref(st), _ptr(out_pos), _ptr(out_vel))
         return out_pos, out_vel
 
     def onestep_lookahead(self, actions, out_pos=None, out_vel=None):
@@ -695,9 +682,7 @@ class BatchedCrowdSim(object):
         if actions.data_ptr() != self.action.data_ptr():
             self.action.copy_(actions, non_blocking=True)
         prm, st, io = self.params(), self.state.struct(), self._io(obs32=False)
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_onestep_lookahead(C.byref(prm), B, N, C.byref(st), C.byref(io), _ptr(out_pos), _ptr(out_vel), self._stream())
-        _abi.check(rc, 'crowdsim_onestep_lookahead')
+        self._call('onestep_lookahead', C.byref(prm), B, N, C.byref(st), C.byref(io), _ptr(out_pos), _ptr(out_vel))
         return (out_pos, out_vel, self.state.h_attr[..., 0]), self.reward, self.done, self.info
 
     def human_times(self, human_times=None, max_steps=4000):
@@ -714,9 +699,7 @@ class BatchedCrowdSim(object):
         gt = torch.empty((B,), dtype=torch.float64, device=self.device)
         fp = torch.empty((B, N + 1, 2), dtype=torch.float64, device=self.device)
         prm = self.params(); st = self.state.struct()
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_human_times(C.byref(prm), B, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps), self._stream())
-        _abi.check(rc, 'crowdsim_human_times')
+        self._call('human_times', C.byref(prm), B, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps))
         return ht, gt, fp
 
     def occupancy_maps(self, h_pos=None, h_vel=None, cell_num=4, cell_size=1.0, om_channel_size=3, out=None):
@@ -728,10 +711,8 @@ class BatchedCrowdSim(object):
         h_vel = self.state.h_vel if h_vel is None else h_vel
         if out is None:
             out = torch.empty((self.B, self.human_num, cell_num * cell_num * om_channel_size), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self.lib.crowdsim_occupancy_maps(self.B, self.human_num, _ptr(h_pos), _ptr(h_vel), int(cell_num), float(cell_size),
-                                                  int(om_channel_size), _ptr(out), self._stream())
-        _abi.check(rc, 'crowdsim_occupancy_maps')
+        self._call('occupancy_maps', self.B, self.human_num, _ptr(h_pos), _ptr(h_vel), int(cell_num), float(cell_size),
+                   int(om_channel_size), _ptr(out))
         return out
 
 

@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from .. import _abi
+from ..batched import call
 from .statetypes import ActionXY
 
 
@@ -90,16 +91,15 @@ class ORCA(Policy):
         flat = [c for o in others for c in (o.px, o.py)] + [c for o in others for c in (o.vx, o.vy)] + [0.0] * (2 * m) + \
                [c for o in others for c in (o.radius, 1.0)] + [me.px, me.py, me.vx, me.vy, me.gx, me.gy, me.radius, me.v_pref, 0.0, 0.0, 0.0, 0.0]
         host.copy_(torch.tensor(flat, dtype=torch.float64))
-        prm = _abi.Params(float(self.time_step), 25.0, 1.0, -0.25, 0.2, 0.5, float(self.neighbor_dist), float(self.time_horizon),
-                          int(self.max_neighbors), 0.0, float(self.safety_space), 0, _abi.ROBOT_ORCA)
-        st = _abi.State(*[d[f].data_ptr() for f in ('h_pos', 'h_vel', 'h_goal', 'h_attr', 'r_pos', 'r_vel', 'r_goal', 'r_attr',
-                                                      'r_theta', 'g_time')], None)
-        with torch.cuda.device(dev):
-            slab.copy_(host, non_blocking=True)
-            rc = lib.crowdsim_orca_act(C.byref(prm), 1, m, C.byref(st), d['out'].data_ptr(),
-                                       C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-            _abi.check(rc, 'crowdsim_orca_act')
-            vx, vy = d['out'].tolist()
+        prm = _abi.Params(time_step=float(self.time_step), time_limit=25.0, success_reward=1.0, collision_penalty=-0.25,
+                          discomfort_dist=0.2, discomfort_penalty_factor=0.5, neighbor_dist=float(self.neighbor_dist),
+                          time_horizon=float(self.time_horizon), max_neighbors=int(self.max_neighbors), human_safety_space=0.0,
+                          robot_safety_space=float(self.safety_space), robot_visible=0, robot_policy=_abi.ROBOT_ORCA)
+        st = _abi.State(**{f: d[f].data_ptr() for f in ('h_pos', 'h_vel', 'h_goal', 'h_attr', 'r_pos', 'r_vel', 'r_goal', 'r_attr',
+                                                          'r_theta', 'g_time')})
+        slab.copy_(host, non_blocking=True)                 # on dev's current stream, the one call() passes
+        call(lib, dev, 'orca_act', C.byref(prm), 1, m, C.byref(st), d['out'].data_ptr())
+        vx, vy = d['out'].tolist()
         self.last_state = state
         return ActionXY(vx, vy)
 

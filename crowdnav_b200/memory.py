@@ -193,17 +193,18 @@ class _DeviceRecorder(object):
         """crowdsim_record with its staging starting at step s of the window."""
         m = self.memory
         p = lambda t: t.data_ptr()  # noqa: E731
-        return _abi.Record(p(self.rows[s]), p(self.reward[s]), p(self.t[s]), p(self.code[s]), self.n_max - s,
-                           p(self.traj_rows), p(self.traj_reward), self.T, None if self.g is None else p(self.g), p(m.states),
-                           p(m.values), m.capacity, self.position0, p(self.pushed), p(self.scan))
+        return _abi.Record(rows=p(self.rows[s]), reward=p(self.reward[s]), t=p(self.t[s]), code=p(self.code[s]),
+                           n_max=self.n_max - s, traj_rows=p(self.traj_rows), traj_reward=p(self.traj_reward), T=self.T,
+                           g=None if self.g is None else p(self.g), mem_states=p(m.states), mem_values=p(m.values),
+                           capacity=m.capacity, position0=self.position0, pushed=p(self.pushed), scan=p(self.scan))
 
     def maps_struct(self, s=0):
         """crowdsim_record_maps with its staging starting at step s, or None without maps."""
         if not self.om:
             return None
         cell_num, cell_size, channels = self.om
-        return _abi.RecordMaps(self.h_pos[s].data_ptr(), self.h_vel[s].data_ptr(), self.maps[s].data_ptr(), int(cell_num),
-                               int(channels), float(cell_size))
+        return _abi.RecordMaps(h_pos=self.h_pos[s].data_ptr(), h_vel=self.h_vel[s].data_ptr(), maps=self.maps[s].data_ptr(),
+                               cell_num=int(cell_num), channels=int(channels), cell_size=float(cell_size))
 
 
 class DeviceILRecorder(_DeviceRecorder):
@@ -266,7 +267,7 @@ class DeviceRLRecorder(_DeviceRecorder):
         return super().finish()
 
     def rl_struct(self):
-        return _abi.RecordRL(self.boot.data_ptr(), self.traj_boot.data_ptr(), float(self.gamma_bar))
+        return _abi.RecordRL(boot=self.boot.data_ptr(), traj_boot=self.traj_boot.data_ptr(), gamma_bar=float(self.gamma_bar))
 
     def staged(self, n):
         """env.step staged n more steps; a full staging is flushed."""
@@ -284,14 +285,12 @@ class DeviceRLRecorder(_DeviceRecorder):
         import ctypes as C
         rec, maps, rl = self.struct(), self.maps_struct(), self.rl_struct()
         mp = C.byref(maps) if maps is not None else None
+        if maps is not None:
+            env._call('record_flush_maps', B, N, C.byref(rec), mp, n)
         with torch.cuda.device(env.device):
-            if maps is not None:
-                _abi.check(env.lib.crowdsim_record_flush_maps(B, N, C.byref(rec), mp, n, env._stream()),
-                           'crowdsim_record_flush_maps')
             x = self.rows[:n].view(n * B, N, 13)
             if maps is not None:
                 x = torch.cat([x, self.maps[:n].view(n * B, N, -1)], dim=2)
             with torch.no_grad():
                 self.boot[:n].copy_(self.target_model(x).view(n, B))
-            _abi.check(env.lib.crowdsim_record_flush_rl(B, N, C.byref(rec), mp, C.byref(rl), n, env._stream()),
-                       'crowdsim_record_flush_rl')
+        env._call('record_flush_rl', B, N, C.byref(rec), mp, C.byref(rl), n)

@@ -64,7 +64,7 @@ class HostState(object):
     FIELDS = ('h_pos', 'h_vel', 'h_goal', 'h_attr', 'r_pos', 'r_vel', 'r_goal', 'r_attr', 'r_theta', 'g_time')
 
     def struct(self):
-        return _abi.State(*[_ptr(getattr(self, f)) for f in self.FIELDS], _ptr(self.active))
+        return _abi.State(active=_ptr(self.active), **{f: _ptr(getattr(self, f)) for f in self.FIELDS})
 
     def copy(self):
         o = HostState(self.B, self.N, self.active is not None)
@@ -95,8 +95,8 @@ class HostStepIO(object):
         self.done = np.zeros(B, dtype=np.uint8); self.info = np.zeros(B, dtype=np.uint8)
 
     def struct(self):
-        return _abi.StepIO(_ptr(self.action), _ptr(self.action_out), _ptr(self.reward), _ptr(self.dmin),
-                           _ptr(self.done), _ptr(self.info))
+        return _abi.StepIO(action=_ptr(self.action), action_out=_ptr(self.action_out), reward=_ptr(self.reward),
+                           dmin=_ptr(self.dmin), done=_ptr(self.done), info=_ptr(self.info))
 
 
 def discount_table(gamma, time_step, v_pref, n=128):
@@ -122,10 +122,8 @@ class HostEpisodes(object):
         self.res_final_rpos = np.zeros((k, 2))
 
     def struct(self):
-        return _abi.Episodes(_ptr(self.ep_case), _ptr(self.ep_steps), _ptr(self.ep_return), _ptr(self.ep_too_close),
-                             _ptr(self.ep_min_dist_sum), _ptr(self.discount), len(self.discount),
-                             _ptr(self.res_info), _ptr(self.res_steps), _ptr(self.res_time), _ptr(self.res_return),
-                             _ptr(self.res_too_close), _ptr(self.res_min_dist_sum), _ptr(self.res_final_rpos))
+        return _abi.Episodes(discount_len=len(self.discount),
+                             **{f: _ptr(getattr(self, f)) for f, _ in _abi.Episodes._fields_ if f != 'discount_len'})
 
 
 class HostAutoReset(object):
@@ -138,15 +136,19 @@ class HostAutoReset(object):
         self.circle_radius, self.robot_radius, self.robot_v_pref = circle_radius, robot_radius, robot_v_pref
 
     def struct(self):
-        return _abi.AutoReset(_ptr(self.n_h_pos), _ptr(self.n_h_goal), _ptr(self.n_h_attr), _ptr(self.n_case),
-                              _ptr(self.n_state), _ptr(self.want), self.circle_radius, self.robot_radius, self.robot_v_pref)
+        return _abi.AutoReset(n_h_pos=_ptr(self.n_h_pos), n_h_goal=_ptr(self.n_h_goal), n_h_attr=_ptr(self.n_h_attr),
+                              n_case=_ptr(self.n_case), n_state=_ptr(self.n_state), want=_ptr(self.want),
+                              circle_radius=self.circle_radius, robot_radius=self.robot_radius, robot_v_pref=self.robot_v_pref)
 
 
 def _reset_args(seeds, rule, mask, circle_radius, square_width, human_radius, human_v_pref, robot_radius, robot_v_pref,
                 discomfort_dist, randomize_attributes, seed_stride, case_counter, case_total, seed_base, case_first=0, case_wrap=0):
-    return _abi.ResetArgs(_ptr(mask), _ptr(seeds), int(seed_stride), _abi.RULES[rule], circle_radius, square_width,
-                          human_radius, human_v_pref, robot_radius, robot_v_pref, discomfort_dist,
-                          int(randomize_attributes), _ptr(case_counter), int(case_total), int(seed_base), int(case_first), int(case_wrap))
+    return _abi.ResetArgs(mask=_ptr(mask), seed=_ptr(seeds), seed_stride=int(seed_stride), rule=_abi.RULES[rule],
+                          circle_radius=circle_radius, square_width=square_width, human_radius=human_radius,
+                          human_v_pref=human_v_pref, robot_radius=robot_radius, robot_v_pref=robot_v_pref,
+                          discomfort_dist=discomfort_dist, randomize_attributes=int(randomize_attributes),
+                          case_counter=_ptr(case_counter), case_total=int(case_total), seed_base=int(seed_base),
+                          case_first=int(case_first), case_wrap=int(case_wrap))
 
 
 def prefetch(ar, B, N, seeds=None, rule='circle_crossing', circle_radius=4.0, square_width=10.0, human_radius=0.3,

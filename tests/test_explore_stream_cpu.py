@@ -1,10 +1,8 @@
-"""CPU checks of the exploration draws from numpy's stream (crowdsim_policy_draws / crowdsim_mt_streams): the exports and
-struct layout, every argument rule (decided before any CUDA call, so the launch counter does not move), the draw semantics
+"""CPU checks of the exploration draws from numpy's stream (crowdsim_policy_draws / crowdsim_mt_streams): every
+argument rule (decided before any CUDA call, so the launch counter does not move), the draw semantics
 pinned to numpy's own RandomState, the device stream's conversion to numpy's state, the CPU oracle's post-generation states
 against the reference's fixture, and BatchedValuePolicy's routing of the draws."""
 import ctypes as C
-import os
-import subprocess
 import types
 
 import numpy as np
@@ -12,44 +10,12 @@ import pytest
 
 import explore_oracle as eo
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, 'include', 'crowdsim_b200.h')
-NEW = ('crowdsim_policy_draws', 'crowdsim_mt_streams')
-
 
 @pytest.fixture(scope='module')
 def lib():
     from crowdnav_b200 import build, _abi
     build.build()
     return _abi.load()
-
-
-def test_draw_exports(lib):
-    from crowdnav_b200 import _abi
-    src = open(HEADER).read()
-    for name in NEW:
-        assert name in _abi.EXPORTS and hasattr(lib, name)
-        assert 'int %s(' % name in src
-
-
-def test_draw_struct_layout_matches_header(tmp_path):
-    from crowdnav_b200 import _abi
-    pairs = (('crowdsim_mt_stream', _abi.MTStream), ('crowdsim_policy_draw', _abi.PolicyDraw))
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "%s"' % HEADER, 'int main(void){']
-    for name, ct in pairs:
-        lines.append('printf("%%zu", sizeof(%s));' % name)
-        lines += ['printf(" %%zu", offsetof(%s, %s));' % (name, f) for f, _ in ct._fields_]
-        lines.append('printf("\\n");')
-    lines.append('return 0;}')
-    c = tmp_path / 'draws.c'
-    c.write_text('\n'.join(lines))
-    exe = tmp_path / 'draws'
-    subprocess.check_call(['gcc', str(c), '-o', str(exe)])
-    out = subprocess.check_output([str(exe)]).decode().strip().splitlines()
-    for line, (_, ct) in zip(out, pairs):
-        parts = [int(x) for x in line.split()]
-        assert parts[0] == C.sizeof(ct)
-        assert parts[1:] == [getattr(ct, f).offset for f, _ in ct._fields_]
 
 
 def _args():

@@ -1,17 +1,11 @@
 """CPU checks of reinforcement-learning recording on device (crowdsim_record_book / crowdsim_record_flush_maps /
-crowdsim_record_flush_rl): the exports, the ctypes layout of crowdsim_record_rl, every argument rule (decided before any
+crowdsim_record_flush_rl): every argument rule (decided before any
 CUDA call, so the launch counter does not move), and DeviceRLRecorder's discount and row checks."""
 import ctypes as C
-import os
 import struct
-import subprocess
 import types
 
 import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, 'include', 'crowdsim_b200.h')
-NEW = ('crowdsim_record_book', 'crowdsim_record_flush_maps', 'crowdsim_record_flush_rl')
 
 
 @pytest.fixture(scope='module')
@@ -19,34 +13,6 @@ def lib():
     from crowdnav_b200 import build, _abi
     build.build()
     return _abi.load()
-
-
-def test_rl_exports(lib):
-    from crowdnav_b200 import _abi
-    src = open(HEADER).read()
-    for name in NEW:
-        assert name in _abi.EXPORTS and hasattr(lib, name)
-        assert 'int %s(' % name in src
-
-
-def test_record_rl_struct_layout_matches_header(tmp_path):
-    from crowdnav_b200 import _abi
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "%s"' % HEADER, 'int main(void){']
-    for name, ct in (('crowdsim_record_rl', _abi.RecordRL), ('crowdsim_record', _abi.Record),
-                     ('crowdsim_record_maps', _abi.RecordMaps)):
-        lines.append('printf("%%zu", sizeof(%s));' % name)
-        lines += ['printf(" %%zu", offsetof(%s, %s));' % (name, f) for f, _ in ct._fields_]
-        lines.append('printf("\\n");')
-    lines.append('return 0;}')
-    c = tmp_path / 'rl.c'
-    c.write_text('\n'.join(lines))
-    exe = tmp_path / 'rl'
-    subprocess.check_call(['gcc', str(c), '-o', str(exe)])
-    out = subprocess.check_output([str(exe)]).decode().strip().splitlines()
-    for line, ct in zip(out, (_abi.RecordRL, _abi.Record, _abi.RecordMaps)):
-        parts = [int(x) for x in line.split()]
-        assert parts[0] == C.sizeof(ct)
-        assert parts[1:] == [getattr(ct, f).offset for f, _ in ct._fields_]
 
 
 def _args(N):
