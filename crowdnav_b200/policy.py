@@ -10,6 +10,7 @@ Module / parameter names of the networks equal the reference's (sarl.py:9-65, ca
 checkpoints (rl_model.pth / il_model.pth state_dicts) load unchanged with load_state_dict().
 """
 import itertools
+import logging
 
 import numpy as np
 import torch
@@ -200,7 +201,8 @@ class BatchedValuePolicy(object):
             self.set_device(env.device)
         A = self.actions.shape[0]
         B, N = env.B, env.human_num
-        if self._buf_states is None or self._buf_states.shape[0] != B:
+        # sized per env: one policy may act in envs of different sizes (CADRL trains on one human and tests on N)
+        if self._buf_states is None or tuple(self._buf_states.shape[:3]) != (B, A, N):
             self._buf_states = torch.empty((B, A, N, 13), dtype=torch.float32, device=self.device)
             self._buf_reward = torch.empty((B, A), dtype=torch.float64, device=self.device)
         unicycle = self.kinematics == 'unicycle'
@@ -208,7 +210,7 @@ class BatchedValuePolicy(object):
             uni = {'unicycle': True} if unicycle else {}              # holonomic: lookahead_pack's default, the call as before
             states, reward = env.lookahead_pack(self.actions, out_states=self._buf_states, out_reward=self._buf_reward, **uni)
         else:
-            if self._buf_next is None or self._buf_next[0].shape[0] != B:
+            if self._buf_next is None or tuple(self._buf_next[0].shape[:2]) != (B, N):
                 self._buf_next = (torch.empty((B, N, 2), dtype=torch.float64, device=self.device),
                                   torch.empty((B, N, 2), dtype=torch.float64, device=self.device),
                                   torch.empty((B, N), dtype=torch.int32, device=self.device))
@@ -255,46 +257,144 @@ class BatchedValuePolicy(object):
 
 
 def make_sarl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_om=False, cell_num=4, cell_size=1.0,
-              om_channel_size=3, query_env=True, kinematics='holonomic', exploration='torch', **net_kw):
+              om_channel_size=3, query_env=True, kinematics='holonomic', exploration='torch', speed_samples=5,
+              rotation_samples=16, **net_kw):
     """SARL with the reference's default architecture (crowd_nav/configs/policy.config:43-50); random-init weights when
     no checkpoint is loaded (there are no checkpoints in the reference repo). with_om=True gives OM-SARL: input_dim grows
-    by cell_num^2 * om_channel_size (multi_human_rl.py:106-107)."""
+    by cell_num^2 * om_channel_size (multi_human_rl.py:106-107). net_kw: SARLValueNetwork's layer sizes and
+    with_global_state."""
     if seed is not None:
         torch.manual_seed(seed)
     if with_om:
         net_kw.setdefault('input_dim', 13 + cell_num * cell_num * om_channel_size)
     p = BatchedValuePolicy(SARLValueNetwork(**net_kw), gamma, v_pref, time_step, joint=True, with_om=with_om,
                            cell_num=cell_num, cell_size=cell_size, om_channel_size=om_channel_size, query_env=query_env,
-                           kinematics=kinematics, exploration=exploration)
+                           kinematics=kinematics, exploration=exploration, speed_samples=speed_samples,
+                           rotation_samples=rotation_samples)
     p.name = 'OM-SARL' if with_om else 'SARL'
     return p
 
 
-def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='holonomic', exploration='torch'):
+def make_cadrl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, kinematics='holonomic', exploration='torch',
+               speed_samples=5, rotation_samples=16, mlp_dims=(150, 100, 100, 1)):
     """CADRL queries the env whatever policy.config's query_env says (cadrl.py:156-170), so there is no query_env here."""
     if seed is not None:
         torch.manual_seed(seed)
-    p = BatchedValuePolicy(CADRLValueNetwork(), gamma, v_pref, time_step, joint=False, kinematics=kinematics,
-                           exploration=exploration)
+    p = BatchedValuePolicy(CADRLValueNetwork(mlp_dims=mlp_dims), gamma, v_pref, time_step, joint=False,
+                           kinematics=kinematics, exploration=exploration, speed_samples=speed_samples,
+                           rotation_samples=rotation_samples)
     p.name = 'CADRL'
     p.multiagent_training = False
     return p
 
 
 def make_lstm_rl(gamma=0.9, v_pref=1.0, time_step=0.25, seed=None, with_interaction_module=False, query_env=True,
-                 kinematics='holonomic', exploration='torch', with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3):
+                 kinematics='holonomic', exploration='torch', with_om=False, cell_num=4, cell_size=1.0, om_channel_size=3,
+                 speed_samples=5, rotation_samples=16, mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
+                 mlp1_dims=(150, 100, 100, 50)):
     """LSTM-RL with the reference's default sizes (crowd_nav/configs/policy.config:24-31). With query_env=False its rows
     follow the reference's sort of the humans by decreasing distance to the robot (lstm_rl.py:99-103); its last_state,
     the rows of its replay pairs, always does (sort_last_state). with_om=True gives OM-LSTM-RL ([lstm_rl] with_om,
     lstm_rl.py:79-88): input_dim grows by cell_num^2 * om_channel_size (multi_human_rl.py:106-107), the LSTM's input or,
-    with the interaction module, mlp1's."""
+    with the interaction module, mlp1's. mlp_dims, lstm_hidden_dim and mlp1_dims are policy.config's [lstm_rl] mlp2_dims,
+    global_state_dim and mlp1_dims (lstm_rl.py:77-85)."""
     if seed is not None:
         torch.manual_seed(seed)
     net = LSTMRLValueNetwork(input_dim=13 + (cell_num * cell_num * om_channel_size if with_om else 0),
-                             mlp_dims=(150, 100, 100, 1), lstm_hidden_dim=50,
-                             mlp1_dims=(150, 100, 100, 50) if with_interaction_module else None)
+                             mlp_dims=mlp_dims, lstm_hidden_dim=lstm_hidden_dim,
+                             mlp1_dims=mlp1_dims if with_interaction_module else None)
     p = BatchedValuePolicy(net, gamma, v_pref, time_step, joint=True, with_om=with_om, cell_num=cell_num,
                            cell_size=cell_size, om_channel_size=om_channel_size, query_env=query_env, kinematics=kinematics,
-                           order_by_distance=not query_env, exploration=exploration, sort_last_state=True)
+                           order_by_distance=not query_env, exploration=exploration, sort_last_state=True,
+                           speed_samples=speed_samples, rotation_samples=rotation_samples)
     p.name = 'OM-LSTM-RL' if with_om else 'LSTM-RL'
     return p
+
+
+def _dims(config, section, key):
+    """A layer-size list of policy.config, parsed as the reference parses it (cadrl.py:59)."""
+    return [int(x) for x in config.get(section, key).split(', ')]
+
+
+def _common_parameters(config):
+    """CADRL.set_common_parameters (cadrl.py:64-73) as keyword arguments of the make_* builders. [action_space] sampling is
+    read and unused, as in the reference (build_action_space always samples speeds exponentially, cadrl.py:82-102)."""
+    config.get('action_space', 'sampling')
+    return dict(gamma=config.getfloat('rl', 'gamma'), kinematics=config.get('action_space', 'kinematics'),
+                speed_samples=config.getint('action_space', 'speed_samples'),
+                rotation_samples=config.getint('action_space', 'rotation_samples'),
+                query_env=config.getboolean('action_space', 'query_env'), cell_num=config.getint('om', 'cell_num'),
+                cell_size=config.getfloat('om', 'cell_size'), om_channel_size=config.getint('om', 'om_channel_size'))
+
+
+class ConfiguredPolicy(BatchedValuePolicy):
+    """A policy_factory entry: built empty, then configure(policy_config) reads the keys the reference's
+    policy.configure(config) reads and builds the network and the action space (sarl.py:73-86, lstm_rl.py:75-88,
+    cadrl.py:57-72). The configured policy is the one its make_* builder returns for the same values; `exploration`
+    ('torch' or 'numpy') is passed on to it."""
+
+    def __init__(self, exploration='torch'):
+        self.exploration = exploration
+        self.model = None
+
+    def configure(self, config):
+        common = _common_parameters(config)
+        policy = self.build(config, common)
+        self.__dict__.update(policy.__dict__)
+        self.speed_samples, self.rotation_samples = common['speed_samples'], common['rotation_samples']
+
+    def build(self, config, common):
+        raise NotImplementedError
+
+
+class CADRL(ConfiguredPolicy):
+    """cadrl.py:57-62. CADRL always queries the env, so its query_env is True whatever the config says."""
+    name = 'CADRL'
+
+    def build(self, config, common):
+        policy = make_cadrl(gamma=common['gamma'], kinematics=common['kinematics'], exploration=self.exploration,
+                            speed_samples=common['speed_samples'], rotation_samples=common['rotation_samples'],
+                            mlp_dims=_dims(config, 'cadrl', 'mlp_dims'))
+        policy.multiagent_training = config.getboolean('cadrl', 'multiagent_training')
+        logging.info('Policy: CADRL without occupancy map')
+        return policy
+
+
+class LstmRL(ConfiguredPolicy):
+    """lstm_rl.py:75-88: [lstm_rl] mlp2_dims is the value MLP, global_state_dim the LSTM's hidden size, mlp1_dims the
+    interaction module's MLP (read only with with_interaction_module). With with_om the name is OM-LSTM-RL, as make_lstm_rl
+    names it; the reference keeps 'LSTM-RL' as the attribute and writes 'OM-' only in its log line."""
+    name = 'LSTM-RL'
+
+    def build(self, config, common):
+        with_interaction_module = config.getboolean('lstm_rl', 'with_interaction_module')
+        kw = dict(common, mlp_dims=_dims(config, 'lstm_rl', 'mlp2_dims'),
+                  lstm_hidden_dim=config.getint('lstm_rl', 'global_state_dim'),
+                  with_om=config.getboolean('lstm_rl', 'with_om'), with_interaction_module=with_interaction_module)
+        if with_interaction_module:
+            kw['mlp1_dims'] = _dims(config, 'lstm_rl', 'mlp1_dims')
+        policy = make_lstm_rl(exploration=self.exploration, **kw)
+        policy.multiagent_training = config.getboolean('lstm_rl', 'multiagent_training')
+        logging.info('Policy: {}LSTM-RL {} pairwise interaction module'.format(
+            'OM-' if kw['with_om'] else '', 'w/' if with_interaction_module else 'w/o'))
+        return policy
+
+
+class SARL(ConfiguredPolicy):
+    """sarl.py:73-86"""
+    name = 'SARL'
+
+    def build(self, config, common):
+        with_om = config.getboolean('sarl', 'with_om')
+        with_global_state = config.getboolean('sarl', 'with_global_state')
+        kw = dict(common, with_om=with_om, with_global_state=with_global_state,
+                  mlp1_dims=_dims(config, 'sarl', 'mlp1_dims'), mlp2_dims=_dims(config, 'sarl', 'mlp2_dims'),
+                  mlp3_dims=_dims(config, 'sarl', 'mlp3_dims'), attention_dims=_dims(config, 'sarl', 'attention_dims'))
+        policy = make_sarl(exploration=self.exploration, **kw)
+        policy.multiagent_training = config.getboolean('sarl', 'multiagent_training')
+        logging.info('Policy: {} {} global state'.format(policy.name, 'w/' if with_global_state else 'w/o'))
+        return policy
+
+
+# crowd_nav/policy/policy_factory.py: the trainable policies by the names train.py / test.py take with --policy
+policy_factory = {'cadrl': CADRL, 'lstm_rl': LstmRL, 'sarl': SARL}
