@@ -17,9 +17,10 @@
 // one common instruction stream with M(M-1)/2 independent divisions in flight instead of the union of 32 divergent
 // control paths.
 // linearProgram3 has a similar structure one level up (its per-line sub-problems do not depend on the running result);
-// step_flat.cuh exploits that by running the sub-problems of a queued solve on parallel lanes, each with the sequential
-// code of orca_device.cuh. A finer split, the (i, j) projections on lanes of their own and every sub-problem speculative
-// in registers (lp1_all + lp2_scan over the projected lines), was bit-identical and slower, and was not kept.
+// the step kernels exploit that by queueing the solves that need it (Lp3Queue below) and running the sub-problems of a
+// queued solve on parallel lanes, each with the sequential code of orca_device.cuh. A finer split, the (i, j) projections
+// on lanes of their own and every sub-problem speculative in registers (lp1_all + lp2_scan over the projected lines), was
+// bit-identical and slower, and was not kept.
 #pragma once
 #include "orca_device.cuh"
 
@@ -168,6 +169,56 @@ ORCA_HD __forceinline__ V2 lp2_init(V2 opt, float radius)
     if (abssq(opt) > sqr(radius)) { const V2 nv = normalize(opt); return mk(nv.x * radius, nv.y * radius); }
     return opt;
 }
+
+// Bit casts of the integer fields of a queued item (__int_as_float / __float_as_int have no host version).
+ORCA_HD __forceinline__ float int_bits(int i) { float f; __builtin_memcpy(&f, &i, sizeof f); return f; }
+ORCA_HD __forceinline__ int bits_int(float f) { int i; __builtin_memcpy(&i, &f, sizeof i); return i; }
+
+// The linearProgram3 queue of the step kernels (step_flat.cuh, step_multi.cuh, step_mid.cuh): a solve that needs
+// linearProgram3 is put in one column of a [rows][stride] float array in shared memory, its M lines first (line k in rows
+// 4k .. 4k+3, the layout of orca::Lines), then its line count, the position where linearProgram2 failed (both as int
+// bits) and the radius: kRows rows in all. Rows from kRows on belong to the kernel (its start point, or the owner thread).
+template <int M>
+struct Lp3Queue {
+    static constexpr int kLines = M, kRows = 4 * M + 3;
+    float *base;   // row 0, column 0
+    int stride;    // columns
+    ORCA_HD __forceinline__ Lines lines(int col) const { return { base + col, stride }; }
+    ORCA_HD __forceinline__ int n(int col) const { return bits_int(base[(4 * M + 0) * stride + col]); }
+    ORCA_HD __forceinline__ int fail(int col) const { return bits_int(base[(4 * M + 1) * stride + col]); }
+    ORCA_HD __forceinline__ float radius(int col) const { return base[(4 * M + 2) * stride + col]; }
+    ORCA_HD __forceinline__ void put(int col, const RegLines<M> &R, int nl, int fail, float radius) const
+    {
+        #pragma unroll
+        for (int kk = 0; kk < M; ++kk) lines(col).set(kk, R.p[kk], R.d[kk]);
+        base[(4 * M + 0) * stride + col] = int_bits(nl); base[(4 * M + 1) * stride + col] = int_bits(fail);
+        base[(4 * M + 2) * stride + col] = radius;
+    }
+};
+
+// The two lanes of a queued item Q[col], on a result array R2 of [3][RS] floats (x, y, ok). Macros rather than member
+// functions: nvcc optimises a function on its own before inlining it, and the lanes compiled that way changed the code of
+// every kernel with a queue (the single-step kernel spilled more); expanded in place they compile as the kernels' own code.
+// Sub-problem I of the item on the lane whose projected-line scratch is P, result to column C. No lp3_subproblem is
+// compiled for one-line items.
+#define ORCA_LP3_SUBPROBLEM_LANE(Q, COL, I, P, R2, RS, C) do {                                                         \
+        const orca::Lines lq_ = (Q).lines(COL);                                                                          \
+        const int qn_ = (Q).n(COL);                                                                                      \
+        bool ok_ = false; orca::V2 r_ = orca::mk(0.f, 0.f);                                                             \
+        if ((Q).kLines > 1 && (I) < qn_) ok_ = orca::lp3_subproblem(lq_, (I), (Q).radius(COL), (P), r_);                \
+        (R2)[C] = r_.x; (R2)[(RS) + (C)] = r_.y; (R2)[2 * (RS) + (C)] = ok_ ? 1.0f : 0.0f;                             \
+    } while (0)
+// linearProgram3's outer scan of the item from RES (its linearProgram2 result), on the lane of its first sub-problem:
+// sub-problem ii is read from column C + ii - 1 (the item's sub-problem lanes are consecutive).
+#define ORCA_LP3_SCAN_LANE(Q, COL, RES, R2, RS, C) do {                                                                \
+        const int qn_ = (Q).n(COL), qf_ = (Q).fail(COL);                                                                 \
+        const float qr_ = (Q).radius(COL);                                                                               \
+        orca::lp3_outer_scan((Q).lines(COL), qn_, qf_, qr_, (RES), [&](int ii_, orca::V2 &r_) {                         \
+            const int src_ = (C) + (ii_ - 1);                                                                            \
+            r_ = orca::mk((R2)[src_], (R2)[(RS) + src_]);                                                                \
+            return (R2)[2 * (RS) + src_] != 0.0f;                                                                        \
+        });                                                                                                              \
+    } while (0)
 
 // Sorted-list form of RVO2's insertAgentNeighbor for the crowd kernel (step_mid.cuh): (td, tj) = the <= M nearest
 // candidates seen so far, ascending; a candidate is inserted with an unrolled compare-and-shift network (static register

@@ -10,7 +10,8 @@
 // across the independent (i, j) line pairs (speculative lp1 candidates + lp2 as a scan, orca_spec.cuh).
 //
 // linearProgram3 (needed by ~4.6 % of the solves, i.e. by some lane of ~3 of 4 warps) is NOT run in place: the
-// solves that need it are compacted into a shared-memory queue. Inside linearProgram3 the sub-problem of each line i
+// solves that need it are compacted into a shared-memory queue (orca::Lp3Queue and its lanes, orca_spec.cuh;
+// this kernel adds the start point). Inside linearProgram3 the sub-problem of each line i
 // (linearProgram2 over the lines projected onto i, started from optVelocity * radius) depends only on the lines, not
 // on the running result, so the <= N-1 sub-problems of a queued solve run on N-1 LANES IN PARALLEL (the sequential
 // shared-memory LP code of orca_device.cuh), followed by a 4-step scan.
@@ -25,7 +26,7 @@
 // form executes more instructions than early-exit code; at 1-2 warps per scheduler a warp's time is its instruction count.
 //
 // The single-step kernel stores as it goes. crowdsim_step_n (n steps per launch) has a kernel of its own, with the robots on
-// a warp of their own (step_multi.cuh); it shares this file's lp3 queue layout and the solver headers.
+// a warp of their own (step_multi.cuh); it shares the lp3 queue item (orca::Lp3Queue) and the solver headers.
 #pragma once
 #include "crowdsim_common.cuh"
 #include "orca_spec.cuh"
@@ -70,12 +71,13 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     constexpr int L = N + 1, M = N, EPW = 32 / L, WPB = CS_FLAT_WPB;
     constexpr int T = 32 * WPB;
     constexpr int SUB = (M > 1) ? M - 1 : 1;                // lanes per queued lp3 item (sub-problems i = 1 .. M-1)
-    constexpr int QF = 4 * M + 5;                           // floats per queued lp3 work item
-    __shared__ float s_q[QF][T];                            // [field][slot]: lines of an item = orca::Lines(base = &s_q[0][slot], stride = T)
+    constexpr int QF = Lp3Queue<M>::kRows + 2;              // floats per queued lp3 item: orca::Lp3Queue's, then its start point
+    __shared__ float s_q[QF][T];                            // [field][slot]
     __shared__ float s_p[4 * SUB][T];                       // per-thread projected lines of the sub-problem
     __shared__ float s_r2[3][T];                            // per-thread sub-problem result (x, y, ok)
     __shared__ float s_res[2][T];
     __shared__ int s_qcount;
+    const Lp3Queue<M> Q = { &s_q[0][0], T };
 
     const KParams &k = A.k;
     const int tid = threadIdx.x, lane = tid & 31, wib = tid >> 5;
@@ -177,9 +179,9 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         return;
     }
 
-    // ---- linearProgram3: the solves that need it are compacted into a shared-memory queue; the sub-problems of an item
-    // run on SUB lanes in parallel (sequential shared-memory LP code of orca_device.cuh), one lane finishes with
-    // linearProgram3's outer scan ----
+    // ---- linearProgram3: the solves that need it are compacted into a shared-memory queue (orca::Lp3Queue plus the start
+    // point in rows QF - 2, QF - 1); the sub-problems of an item run on SUB lanes in parallel (sequential shared-memory LP
+    // code of orca_device.cuh), one lane finishes with linearProgram3's outer scan ----
     const bool need3 = solves && fail < nl;
     if constexpr (WARPQ) {
         // warp-level queue: no block barrier; every warp runs the sub-problems of its own solves
@@ -188,41 +190,17 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             const int wbase = wib * 32;
             const int cnt = __popc(m3);
             const int slot = wbase + __popc(m3 & ((1u << lane) - 1u));
-            if (need3) {
-                #pragma unroll
-                for (int kk = 0; kk < M; ++kk) {
-                    s_q[4 * kk + 0][slot] = R.p[kk].x; s_q[4 * kk + 1][slot] = R.p[kk].y;
-                    s_q[4 * kk + 2][slot] = R.d[kk].x; s_q[4 * kk + 3][slot] = R.d[kk].y;
-                }
-                s_q[4 * M + 0][slot] = __int_as_float(nl); s_q[4 * M + 1][slot] = __int_as_float(fail);
-                s_q[4 * M + 2][slot] = max_speed; s_q[4 * M + 3][slot] = nv.x; s_q[4 * M + 4][slot] = nv.y;
-            }
+            if (need3) { Q.put(slot, R, nl, fail, max_speed); s_q[QF - 2][slot] = nv.x; s_q[QF - 1][slot] = nv.y; }
             __syncwarp();
             constexpr int IPP = 32 / SUB;                        // items per pass
             for (int base = 0; base < cnt; base += IPP) {
                 const int item = wbase + base + lane / SUB, i = lane % SUB + 1;
                 const bool mine = (lane < IPP * SUB) && (base + lane / SUB) < cnt;
-                if (mine) {
-                    const Lines Lq = { &s_q[0][item], T };
-                    const int qn = __float_as_int(s_q[4 * M + 0][item]);
-                    bool ok = false; V2 r2 = mk(0.f, 0.f);
-                    if (M > 1 && i < qn) {
-                        const Lines Pq = { &s_p[0][tid], T };
-                        ok = lp3_subproblem(Lq, i, s_q[4 * M + 2][item], Pq, r2);
-                    }
-                    s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
-                }
+                if (mine) { const Lines Pq = { &s_p[0][tid], T }; ORCA_LP3_SUBPROBLEM_LANE(Q, item, i, Pq, &s_r2[0][0], T, tid); }
                 __syncwarp();
                 if (mine && i == 1) {
-                    const Lines Lq = { &s_q[0][item], T };
-                    const int qn = __float_as_int(s_q[4 * M + 0][item]), qf = __float_as_int(s_q[4 * M + 1][item]);
-                    const float qr = s_q[4 * M + 2][item];
-                    V2 res = mk(s_q[4 * M + 3][item], s_q[4 * M + 4][item]);
-                    lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
-                        const int src_ = tid + (ii - 1);
-                        r2 = mk(s_r2[0][src_], s_r2[1][src_]);
-                        return s_r2[2][src_] != 0.0f;
-                    });
+                    V2 res = mk(s_q[QF - 2][item], s_q[QF - 1][item]);
+                    ORCA_LP3_SCAN_LANE(Q, item, res, &s_r2[0][0], T, tid);
                     s_res[0][item] = res.x; s_res[1][item] = res.y;
                 }
                 __syncwarp();
@@ -235,13 +213,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         int slot = -1;
         if (need3) {
             slot = atomicAdd(&s_qcount, 1);
-            #pragma unroll
-            for (int kk = 0; kk < M; ++kk) {
-                s_q[4 * kk + 0][slot] = R.p[kk].x; s_q[4 * kk + 1][slot] = R.p[kk].y;
-                s_q[4 * kk + 2][slot] = R.d[kk].x; s_q[4 * kk + 3][slot] = R.d[kk].y;
-            }
-            s_q[4 * M + 0][slot] = __int_as_float(nl); s_q[4 * M + 1][slot] = __int_as_float(fail);
-            s_q[4 * M + 2][slot] = max_speed; s_q[4 * M + 3][slot] = nv.x; s_q[4 * M + 4][slot] = nv.y;
+            Q.put(slot, R, nl, fail, max_speed); s_q[QF - 2][slot] = nv.x; s_q[QF - 1][slot] = nv.y;
         }
         if (__syncthreads_or(need3 ? 1 : 0)) {
             const int cnt = s_qcount;
@@ -249,29 +221,13 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             for (int base = 0; base < cnt; base += IPP) {
                 const int item = base + tid / SUB, i = tid % SUB + 1;
                 const bool mine = (tid < IPP * SUB) && item < cnt;
-                if (mine) {
-                    const Lines Lq = { &s_q[0][item], T };
-                    const int qn = __float_as_int(s_q[4 * M + 0][item]);
-                    bool ok = false; V2 r2 = mk(0.f, 0.f);
-                    if (M > 1 && i < qn) {
-                        // sequential shared-memory LP code with early exits: faster here than every finer or
-                        // speculative split tried (header)
-                        const Lines Pq = { &s_p[0][tid], T };
-                        ok = lp3_subproblem(Lq, i, s_q[4 * M + 2][item], Pq, r2);
-                    }
-                    s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
-                }
+                // sequential shared-memory LP code with early exits: faster here than every finer or speculative split
+                // tried (header)
+                if (mine) { const Lines Pq = { &s_p[0][tid], T }; ORCA_LP3_SUBPROBLEM_LANE(Q, item, i, Pq, &s_r2[0][0], T, tid); }
                 __syncthreads();
                 if (mine && i == 1) {                            // the item's first lane runs linearProgram3's outer scan
-                    const Lines Lq = { &s_q[0][item], T };
-                    const int qn = __float_as_int(s_q[4 * M + 0][item]), qf = __float_as_int(s_q[4 * M + 1][item]);
-                    const float qr = s_q[4 * M + 2][item];
-                    V2 res = mk(s_q[4 * M + 3][item], s_q[4 * M + 4][item]);
-                    lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
-                        const int src_ = tid + (ii - 1);              // lane of sub-problem ii of this item
-                        r2 = mk(s_r2[0][src_], s_r2[1][src_]);
-                        return s_r2[2][src_] != 0.0f;
-                    });
+                    V2 res = mk(s_q[QF - 2][item], s_q[QF - 1][item]);
+                    ORCA_LP3_SCAN_LANE(Q, item, res, &s_r2[0][0], T, tid);
                     s_res[0][item] = res.x; s_res[1][item] = res.y;
                 }
                 __syncthreads();

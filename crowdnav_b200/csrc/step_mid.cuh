@@ -13,8 +13,8 @@
 //     orca_spec.cuh (lp1_all<10> = 45 independent pair intersections, lp2 as a scan): one common instruction stream for the
 //     32 solves of a warp instead of the union of 32 divergent paths, no shared-memory traffic in the solver;
 //   * the solves that need linearProgram3 (5.8 % at N = 20) are compacted per BLOCK into a shared-memory queue and their
-//     M - 1 sub-problems run on M - 1 lanes in parallel (the sequential shared-memory code of orca_device.cuh), like the
-//     small-crowd kernel does.
+//     M - 1 sub-problems run on M - 1 lanes in parallel (the sequential shared-memory code of orca_device.cuh), with the
+//     small-crowd kernels' queue item (orca::Lp3Queue, orca_spec.cuh) plus the start point.
 // Results are bit-identical to the generic kernel and the oracle (same operations per candidate, same order).
 #pragma once
 #include "crowdsim_common.cuh"
@@ -26,7 +26,7 @@ constexpr int kMidM = CROWDSIM_MAX_NEIGHBORS;                 // lines per solve
 constexpr int kMidQC = 48;                                    // linearProgram3 items queued per round (a 126-thread block has ~7)
 constexpr int kMidIPP = 14;                                   // items solved per pass: kMidIPP x (M - 1) = 126 lanes (one pass serves a block's ~7 items; a pass is a ~2 k-instruction chain)
 // shared memory of the linearProgram3 pass, in floats (independent of the block size)
-__host__ __device__ constexpr int mid_lp3_floats() { return (4 * kMidM + 5) * kMidQC + (4 * (kMidM - 1) + 3) * kMidIPP * (kMidM - 1) + 2 * kMidQC; }
+__host__ __device__ constexpr int mid_lp3_floats() { return (orca::Lp3Queue<kMidM>::kRows + 2) * kMidQC + (4 * (kMidM - 1) + 3) * kMidIPP * (kMidM - 1) + 2 * kMidQC; }
 
 // Block-collective: every thread of the block calls it (threads without a solve pass solve = false).
 // s_f = mid_lp3_floats() floats of shared memory, s_qcount = a shared counter zeroed before the last barrier.
@@ -35,11 +35,12 @@ __device__ __forceinline__ orca::V2 mid_solve(const Stage &s, const KParams &k, 
                                               double2 pos, double2 goal, double v_pref, int tid, int T, float *s_f, int *s_qcount)
 {
     using namespace orca;
-    constexpr int SUB = M - 1, QF = 4 * M + 5, QC = kMidQC, PL = kMidIPP * SUB;   // PL = lanes of a pass
-    float *s_q = s_f;                                        // [QF][QC]    queued item: lines, count, fail, radius, result
+    constexpr int SUB = M - 1, QF = Lp3Queue<M>::kRows + 2, QC = kMidQC, PL = kMidIPP * SUB;   // PL = lanes of a pass
+    float *s_q = s_f;                                        // [QF][QC]    queued item: orca::Lp3Queue's, then its start point
     float *s_p = s_q + QF * QC;                              // [4 SUB][PL] per-lane projected lines of a sub-problem
     float *s_r2 = s_p + 4 * SUB * PL;                        // [3][PL]     per-lane sub-problem result
     float *s_res = s_r2 + 3 * PL;                            // [2][QC]     per-item result
+    const Lp3Queue<M> Q = { s_q, QC };
 
     V2 nv = mk(0.f, 0.f);
     int nl = 0, fail = 0; float max_speed = 0.f;
@@ -101,13 +102,7 @@ __device__ __forceinline__ orca::V2 mid_solve(const Stage &s, const KParams &k, 
         if (pending) {
             slot = atomicAdd(s_qcount, 1);
             if (slot < QC) {
-                #pragma unroll
-                for (int kk = 0; kk < M; ++kk) {
-                    s_q[(4 * kk + 0) * QC + slot] = R.p[kk].x; s_q[(4 * kk + 1) * QC + slot] = R.p[kk].y;
-                    s_q[(4 * kk + 2) * QC + slot] = R.d[kk].x; s_q[(4 * kk + 3) * QC + slot] = R.d[kk].y;
-                }
-                s_q[(4 * M + 0) * QC + slot] = __int_as_float(nl); s_q[(4 * M + 1) * QC + slot] = __int_as_float(fail);
-                s_q[(4 * M + 2) * QC + slot] = max_speed; s_q[(4 * M + 3) * QC + slot] = nv.x; s_q[(4 * M + 4) * QC + slot] = nv.y;
+                Q.put(slot, R, nl, fail, max_speed); s_q[(QF - 2) * QC + slot] = nv.x; s_q[(QF - 1) * QC + slot] = nv.y;
             } else slot = -1;                                    // queue full: next round
         }
         __syncthreads();
@@ -116,27 +111,11 @@ __device__ __forceinline__ orca::V2 mid_solve(const Stage &s, const KParams &k, 
         for (int base = 0; base < cnt; base += ipp) {
             const int item = base + tid / SUB, i = tid % SUB + 1;
             const bool mine = (tid < ipp * SUB) && item < cnt;
-            if (mine) {
-                const Lines Lq = { s_q + item, QC };
-                const int qn = __float_as_int(s_q[(4 * M + 0) * QC + item]);
-                bool ok = false; V2 r2 = mk(0.f, 0.f);
-                if (i < qn) {
-                    const Lines Pq = { s_p + tid, PL };
-                    ok = lp3_subproblem(Lq, i, s_q[(4 * M + 2) * QC + item], Pq, r2);
-                }
-                s_r2[0 * PL + tid] = r2.x; s_r2[1 * PL + tid] = r2.y; s_r2[2 * PL + tid] = ok ? 1.0f : 0.0f;
-            }
+            if (mine) { const Lines Pq = { s_p + tid, PL }; ORCA_LP3_SUBPROBLEM_LANE(Q, item, i, Pq, s_r2, PL, tid); }
             __syncthreads();
             if (mine && i == 1) {                                // the item's first lane runs linearProgram3's outer scan
-                const Lines Lq = { s_q + item, QC };
-                const int qn = __float_as_int(s_q[(4 * M + 0) * QC + item]), qf = __float_as_int(s_q[(4 * M + 1) * QC + item]);
-                const float qr = s_q[(4 * M + 2) * QC + item];
-                V2 res = mk(s_q[(4 * M + 3) * QC + item], s_q[(4 * M + 4) * QC + item]);
-                lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
-                    const int src_ = tid + (ii - 1);                  // lane of sub-problem ii of this item
-                    r2 = mk(s_r2[0 * PL + src_], s_r2[1 * PL + src_]);
-                    return s_r2[2 * PL + src_] != 0.0f;
-                });
+                V2 res = mk(s_q[(QF - 2) * QC + item], s_q[(QF - 1) * QC + item]);
+                ORCA_LP3_SCAN_LANE(Q, item, res, s_r2, PL, tid);
                 s_res[0 * QC + item] = res.x; s_res[1 * QC + item] = res.y;
             }
             __syncthreads();

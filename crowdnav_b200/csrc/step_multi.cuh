@@ -24,9 +24,9 @@
 //      (__syncthreads_or) makes them visible.
 //   2. every human builds the robot's line against itself and arrives at named barrier 1; every thread solves (flat solver
 //      of orca_spec.cuh, lines in registers; the robot waits on barrier 1 and reads its lines instead of building them)
-//      and publishes its lp2 result; the solves that need linearProgram3 go to a block queue of T / (N - 1) items (one
-//      item layout, sized for N lines), one pass. The pass writes each result over its owner's lp2 result, so that after
-//      it the humans read their robot's velocity without a barrier.
+//      and publishes its lp2 result; the solves that need linearProgram3 go to a block queue of T / (N - 1) items (the
+//      step kernels' orca::Lp3Queue item, sized for N lines, plus the owner thread), one pass. The pass writes each result
+//      over its owner's lp2 result, so that after it the humans read their robot's velocity without a barrier.
 //   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; meanwhile the robot
 //      publishes the rest of what the env's ending depends on (timeout, goal reached, its slot's state, read after its
 //      solve, and whether it is parked); a barrier.
@@ -194,7 +194,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     constexpr int SUB = N - 1;                              // lanes per queued lp3 item (sub-problems i = 1 .. N-1)
     constexpr int IPW = 32 / SUB;                           // lp3 items per warp: an item never straddles two warps
     constexpr int QC = IPW * L;                             // lp3 items queued per step = one pass (N = 5: 48 of 192 solves)
-    constexpr int QF = 4 * N + 4;                           // floats per queued lp3 item: lines, count, fail, radius, owner
+    constexpr int QF = Lp3Queue<N>::kRows + 1;              // floats per queued lp3 item: orca::Lp3Queue's, then the owner thread
     constexpr int PV = (4 * SUB > 10) ? 4 * SUB : 10;
     __shared__ float s_q[QF][QC];
     // the float32 views (rows 0-3: position and velocity of slot le * L + a as a float4; rows 4, 5: radius as seen by a
@@ -217,6 +217,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     constexpr unsigned PRE_TIMEOUT = 1, PRE_GOAL = 2, PRE_READY = 4, PRE_WANT = 8;   // timeout, goal reached, slot READY, parked
     float4 *const s_view = reinterpret_cast<float4 *>(&s_pv[0][0]);
     float *const s_radh = s_pv[4], *const s_radr = s_pv[5];
+    const Lp3Queue<N> Q = { &s_q[0][0], QC };
 
     const KParams &k = A.k;
     const int tid = threadIdx.x;
@@ -311,7 +312,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
 
     // ---- linearProgram3 of the solves that need it: a block queue of QC items, one pass. The sub-problems of an item run
     // on SUB lanes of one warp in parallel (sequential shared-memory LP code of orca_device.cuh), the item's first lane finishes
-    // with the outer scan (step_flat.cuh) and writes the result over its owner's lp2 result in s_nv, where the humans also
+    // with the outer scan (orca_spec.cuh) and writes the result over its owner's lp2 result in s_nv, where the humans also
     // read their robot's. A solve that finds the queue full (more than QC in one block step: scenes where most agents
     // overlap) runs RVO2's sequential linearProgram3 alone (out of line, on lines in local memory; tests/native/lp_fuzz.cu
     // checks both forms against the oracle bit for bit) before the pass, so that no solve's lines stay live across it ----
@@ -325,12 +326,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
         lp3(Lq, nl, fail, max_speed, Pq, nv);
         slot = -1;
     } else if (slot >= 0) {
-        #pragma unroll
-        for (int kk = 0; kk < N; ++kk) {
-            s_q[4 * kk + 0][slot] = R.p[kk].x; s_q[4 * kk + 1][slot] = R.p[kk].y; s_q[4 * kk + 2][slot] = R.d[kk].x; s_q[4 * kk + 3][slot] = R.d[kk].y;
-        }
-        s_q[4 * N + 0][slot] = __int_as_float(nl); s_q[4 * N + 1][slot] = __int_as_float(fail);
-        s_q[4 * N + 2][slot] = max_speed; s_q[4 * N + 3][slot] = __int_as_float(tid);
+        Q.put(slot, R, nl, fail, max_speed); s_q[QF - 1][slot] = __int_as_float(tid);
     }
     s_nv[tid] = make_float2(nv.x, nv.y);
     // the state of the env's next-scene slot, for the ending of this step: read before the queue barrier, so that the L2
@@ -354,29 +350,13 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
         if (tid == 0) s_qcount = 0;                          // every slot of the step is taken; the next step's come after more barriers
         const int lane = tid & 31, item = (tid >> 5) * IPW + lane / SUB, i = lane % SUB + 1;
         const bool mine = lane < IPW * SUB && item < cnt;
-        if (mine) {
-            const Lines Lq = { &s_q[0][item], QC };
-            const int qn = __float_as_int(s_q[4 * N + 0][item]);
-            bool ok = false; V2 r2 = mk(0.f, 0.f);
-            if (i < qn) {
-                const Lines Pq = { &s_pv[0][tid], T };
-                ok = lp3_subproblem(Lq, i, s_q[4 * N + 2][item], Pq, r2);
-            }
-            s_r2[0][tid] = r2.x; s_r2[1][tid] = r2.y; s_r2[2][tid] = ok ? 1.0f : 0.0f;
-        }
+        if (mine) { const Lines Pq = { &s_pv[0][tid], T }; ORCA_LP3_SUBPROBLEM_LANE(Q, item, i, Pq, &s_r2[0][0], T, tid); }
         __syncwarp();                                        // an item's sub-problem results are read by its first lane, in the same warp
         if (mine && i == 1) {
-            const Lines Lq = { &s_q[0][item], QC };
-            const int qn = __float_as_int(s_q[4 * N + 0][item]), qf = __float_as_int(s_q[4 * N + 1][item]);
-            const float qr = s_q[4 * N + 2][item];
-            const int owner = __float_as_int(s_q[4 * N + 3][item]);
+            const int owner = __float_as_int(s_q[QF - 1][item]);
             const float2 r0 = s_nv[owner];
             V2 res = mk(r0.x, r0.y);
-            lp3_outer_scan(Lq, qn, qf, qr, res, [&](int ii, V2 &r2) {
-                const int src_ = tid + (ii - 1);              // thread of sub-problem ii of this item
-                r2 = mk(s_r2[0][src_], s_r2[1][src_]);
-                return s_r2[2][src_] != 0.0f;
-            });
+            ORCA_LP3_SCAN_LANE(Q, item, res, &s_r2[0][0], T, tid);
             s_nv[owner] = make_float2(res.x, res.y);
         }
         __syncthreads();

@@ -5,6 +5,8 @@
 //   B  sequential lp2 + lp3 (shared-memory-column code path of the generic kernel, n <= 10)   vs  orc_lp2 / orc_lp3
 //   C  speculative lp1_all + lp2_scan (register path of the small-crowd kernel, n <= 5)        vs  orc_lp2
 //   D  lp3 as independent per-line sub-problems + lp3_outer_scan (the lane-parallel pass)      vs  orc_lp3
+//   Q  the same solve through the step kernels' queue item and lanes (orca::Lp3Queue, ORCA_LP3_*_LANE, widths 1-5, 10)
+//                                                                                               vs  orc_lp3
 //   H  insert_sorted<10> (sorted register list of the crowd kernel, 20-60 candidates incl. ties) vs  orc_insert_neighbor
 //   E  neighbour_order (pair-wise ranks + packed indices of the small-crowd kernel)            vs  orc_insert_neighbor
 // Build (tests/test_native_cpu.py): nvcc -O2 --fmad=false -Xcompiler -ffp-contract=off -std=c++17 lp_fuzz.cu
@@ -59,6 +61,43 @@ static bool check_case(int n, const orc_line *ol, float radius, orc_v2 opt, long
         cov[1]++;
     }
     return true;
+}
+
+// ---- Q: a solve that needs lp3 as a queued item of width W >= n, in column col of a queue with QS columns: put, the
+// sub-problem lanes i = 1 .. max(W - 1, 1) into consecutive columns from c of the result array, then the outer-scan lane
+// from the lp2 result. Every other column holds NaN, so a lane that reads the wrong one changes the result. ----
+template <int W>
+static bool check_queued(int n, const orc_line *ol, int fail, float radius, orc_v2 start, orc_v2 want, long *cov)
+{
+    using namespace orca;
+    if (n > W) return true;
+    constexpr int SUB = W > 1 ? W - 1 : 1, QS = 3, RS = SUB + 2;
+    const int col = (n + fail) % QS, c = fail % 3;
+    float q[Lp3Queue<W>::kRows * QS], r2[3 * RS], pbuf[4 * 16];
+    for (float &x : q) x = __builtin_nanf("");
+    for (float &x : r2) x = __builtin_nanf("");
+    RegLines<W> R;
+    for (int k = 0; k < W; ++k) { R.p[k] = k < n ? mk(ol[k].point.x, ol[k].point.y) : mk(0, 0); R.d[k] = k < n ? mk(ol[k].dir.x, ol[k].dir.y) : mk(0, 0); }
+    const Lp3Queue<W> Q = { q, QS };
+    Q.put(col, R, n, fail, radius);
+    if (Q.n(col) != n || Q.fail(col) != fail || !same(Q.radius(col), radius)) { printf("Q item fields mismatch W=%d\n", W); return false; }
+    const Lines P = { pbuf, 1 };
+    for (int i = 1; i <= SUB; ++i) ORCA_LP3_SUBPROBLEM_LANE(Q, col, i, P, r2, RS, c + i - 1);
+    V2 res = mk(start.x, start.y);
+    ORCA_LP3_SCAN_LANE(Q, col, res, r2, RS, c);
+    if (!same(res.x, want.x) || !same(res.y, want.y)) { printf("Q queued lp3 mismatch W=%d n=%d fail=%d\n", W, n, fail); return false; }
+    cov[7]++;
+    return true;
+}
+
+static bool check_queued_widths(int n, const orc_line *ol, float radius, orc_v2 opt, long *cov)
+{
+    orc_v2 r; const int fail = orc_lp2(ol, n, radius, opt, 0, &r);
+    if (fail == n) return true;
+    orc_v2 want = r; orc_lp3(ol, n, fail, radius, &want);
+    return check_queued<1>(n, ol, fail, radius, r, want, cov) && check_queued<2>(n, ol, fail, radius, r, want, cov) &&
+           check_queued<3>(n, ol, fail, radius, r, want, cov) && check_queued<4>(n, ol, fail, radius, r, want, cov) &&
+           check_queued<5>(n, ol, fail, radius, r, want, cov) && check_queued<10>(n, ol, fail, radius, r, want, cov);
 }
 
 // ---- E: M candidates in scan order, some out of range, many exact ties: order and count must equal RVO2's insertion sort
@@ -117,7 +156,7 @@ int main(int argc, char **argv)
 {
     const long cases = argc > 1 ? atol(argv[1]) : 200000;
     rng_state = argc > 2 ? strtoull(argv[2], nullptr, 10) * 2654435761ull + 88172645463325252ull : 88172645463325252ull;
-    long cov[7] = {0, 0, 0, 0, 0, 0, 0};
+    long cov[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     using namespace orca;
     for (long c = 0; c < cases; ++c) {
         const int kind = rnd() % 4;
@@ -154,9 +193,10 @@ int main(int argc, char **argv)
         }
         if (!check_case<5>(n, ol, radius, opt, cov)) { printf("case %ld kind %d\n", c, kind); return 1; }
         if (n > 5) { long dummy[7] = {0}; if (!check_case<10>(n, ol, radius, opt, dummy)) { printf("case %ld kind %d (M = 10)\n", c, kind); return 1; } cov[1] += dummy[1]; }
+        if (!check_queued_widths(n, ol, radius, opt, cov)) { printf("case %ld kind %d\n", c, kind); return 1; }
         if (!check_sorted_insert(cov)) { printf("case %ld\n", c); return 1; }
         if (!(check_order<5>(cov) && check_order<4>(cov) && check_order<2>(cov) && check_order<1>(cov))) { printf("case %ld\n", c); return 1; }
     }
-    printf("ok cases=%ld lp3_needed=%ld speculative_checked=%ld overlapping_pairs=%ld forced_parallel_lines=%ld neighbour_orders=%ld neighbour_ties=%ld sorted_lists=%ld\n", cases, cov[0], cov[1], cov[2], cov[3], cov[4], cov[5], cov[6]);
+    printf("ok cases=%ld lp3_needed=%ld speculative_checked=%ld overlapping_pairs=%ld forced_parallel_lines=%ld neighbour_orders=%ld neighbour_ties=%ld sorted_lists=%ld queued_items=%ld\n", cases, cov[0], cov[1], cov[2], cov[3], cov[4], cov[5], cov[6], cov[7]);
     return 0;
 }

@@ -1,7 +1,8 @@
 """CPU fuzz of the CUDA solver's arithmetic: orca_device.cuh / orca_spec.cuh are __host__ __device__, so the exact code the
 kernels run is compiled for the host (nvcc, --fmad=false, -ffp-contract=off) and compared bit for bit with the C oracle on
-millions of random ORCA problems -- line construction, sequential lp2/lp3, the speculative lp1_all + lp2_scan path and the
-lane-parallel formulation of lp3 (independent per-line sub-problems + outer scan). See tests/native/lp_fuzz.cu."""
+millions of random ORCA problems -- line construction, sequential lp2/lp3, the speculative lp1_all + lp2_scan path, the
+lane-parallel formulation of lp3 (independent per-line sub-problems + outer scan) and the step kernels' queued lp3 item
+with the two lanes that run it (orca::Lp3Queue, ORCA_LP3_SUBPROBLEM_LANE, ORCA_LP3_SCAN_LANE). See tests/native/lp_fuzz.cu."""
 import os
 import subprocess
 
@@ -31,3 +32,4 @@ def test_host_compiled_kernel_solver_matches_oracle_bitwise(fuzz_binary, seed):
     assert int(fields['overlapping_pairs']) > 100000 and int(fields['forced_parallel_lines']) > 100000
     assert int(fields['sorted_lists']) == 1000000                                                    # part H
     assert int(fields['neighbour_orders']) == 4000000 and int(fields['neighbour_ties']) > 1000000    # part E, M = 5, 4, 2, 1
+    assert int(fields['queued_items']) > 500000                                                      # part Q, widths 1-5, 10
