@@ -5,6 +5,11 @@
 
 namespace cs {
 
+// torch.norm(torch.cat([x, y], 1), 2, dim=1) of one float32 pair as torch CPU evaluates it: x * x rounded, y * y fused into
+// the sum. The plain sqrtf(x * x + y * y) is 1 ulp off on about one pair in twelve. fmaf is an explicit FMA, which
+// --fmad=false leaves alone.
+__device__ __forceinline__ float norm2f(float x, float y) { return sqrtf(fmaf(y, y, x * x)); }
+
 // cadrl.py:187-222 on one 14-tuple already cast to float32.
 __device__ __forceinline__ void rotate_self(float px, float py, float vx, float vy, float gx, float gy,
                                             float &rot_c, float &rot_s, float &rot, float &dg, float &rvx, float &rvy)
@@ -12,7 +17,7 @@ __device__ __forceinline__ void rotate_self(float px, float py, float vx, float 
     const float dx = gx - px, dy = gy - py;
     rot = atan2f(dy, dx);
     rot_c = cosf(rot); rot_s = sinf(rot);
-    dg = sqrtf(dx * dx + dy * dy);
+    dg = norm2f(dx, dy);
     rvx = vx * rot_c + vy * rot_s;
     rvy = vy * rot_c - vx * rot_s;
 }
@@ -27,7 +32,7 @@ __device__ __forceinline__ void rotate_row(float *out, float px, float py, float
     out[8] = hvx * c + hvy * s;
     out[9] = hvy * c - hvx * s;
     out[10] = hr;
-    { const float ax = px - hx, ay = py - hy; out[11] = sqrtf(ax * ax + ay * ay); }
+    out[11] = norm2f(px - hx, py - hy);
     out[12] = radius + hr;
 }
 

@@ -475,14 +475,18 @@ int oracle_crowdsim_orca_act(const crowdsim_params *prm, int B, int N, const cro
 }
 
 /* ---------------- state packing: state.py:17-18,36-37 + cadrl.py:187-222 (float32 torch ops) ---------------- */
-/* torch CPU float32 semantics: every op rounds to float32; atan2f/cosf/sinf/sqrtf of libm. The CUDA side is
- * compared with a tolerance (1e-5), since torch's own CPU/GPU kernels differ from each other at that level. */
+/* torch CPU float32 semantics: every op rounds to float32; atan2f/cosf/sinf/sqrtf of libm. torch.norm(cat([x, y]), 2)
+ * of a float32 pair is sqrtf(fmaf(y, y, x * x)) on torch CPU: x * x rounded, y * y fused into the sum (pinned by
+ * tests/test_rotated_rows_cpu.py). dg, v_pref, radius, radius1, da, radius_sum (and theta when holonomic) use no
+ * atan2 / cos / sin and equal the reference's bit for bit; the turned columns are held to tests/util.py:rotate_model. */
+static inline float norm2f(float x, float y) { return sqrtf(fmaf(y, y, x * x)); }
+
 static void rotate_row(const float s[14], int unicycle, float out[13])
 {
     const float dx = s[5] - s[0], dy = s[6] - s[1];
     const float rot = atan2f(dy, dx);
     const float c = cosf(rot), sn = sinf(rot);
-    out[0] = sqrtf(dx * dx + dy * dy);                 /* dg */
+    out[0] = norm2f(dx, dy);                            /* dg */
     out[1] = s[7];                                      /* v_pref */
     out[2] = unicycle ? (s[8] - rot) : 0.0f;            /* theta */
     out[3] = s[4];                                      /* radius */
@@ -493,8 +497,16 @@ static void rotate_row(const float s[14], int unicycle, float out[13])
     out[8] = s[11] * c + s[12] * sn;                    /* vx1 */
     out[9] = s[12] * c - s[11] * sn;                    /* vy1 */
     out[10] = s[13];                                    /* radius1 */
-    { const float ax = s[0] - s[9], ay = s[1] - s[10]; out[11] = sqrtf(ax * ax + ay * ay); }  /* da */
+    out[11] = norm2f(s[0] - s[9], s[1] - s[10]);        /* da */
     out[12] = s[4] + s[13];                             /* radius sum */
+}
+
+/* rotate on n float32 14-tuples as given: the float32 restatement tests/util.py holds every producer's exact columns to. */
+int oracle_rotate_rows(int n, const float *s, int unicycle, float *out)
+{
+    if (n < 0 || (n > 0 && (!s || !out))) return CROWDSIM_EINVAL;
+    for (int i = 0; i < n; ++i) rotate_row(s + (size_t)i * 14, unicycle, out + (size_t)i * 13);
+    return 0;
 }
 
 int oracle_crowdsim_pack_joint(int B, int N, const crowdsim_state *st, int unicycle, float *out)

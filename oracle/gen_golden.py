@@ -18,6 +18,7 @@ What is recorded (floats as repr() strings, exact round trip):
   network_ports.json  the reference's value-network modules run with the weights of crowdnav_b200.policy's seeded ports
   boundary_steps.json  one reference step on every constructed boundary scene (tests/boundary_scenes.py) and
                  get_human_times on the arrival-edge scenes
+  rotate_edges.json  CADRL.rotate, holonomic and unicycle, on constructed edge scenes (--only rotate_edges)
 
 usage: python oracle/gen_golden.py [--quick]
        python oracle/gen_golden.py --only NAME     one generator of ONLY (the non-default parameter profiles, boundary)
@@ -425,6 +426,191 @@ def run_rotate_unicycle():
         json.dump({'seed': 0, 'blocks': blocks}, f, separators=(',', ':'))
 
 
+def _norms32(dx, dy):
+    """(fused, plain) float32 2-norms of float32 pairs: sqrtf(fmaf(dy, dy, dx * dx)) as torch CPU's torch.norm evaluates it
+    (through the oracle's rotate_row and libm's fmaf), and sqrtf(dx * dx + dy * dy)."""
+    import pyoracle
+    dx = np.asarray(dx, dtype=np.float32); dy = np.asarray(dy, dtype=np.float32)
+    s = np.zeros(dx.shape + (14,), dtype=np.float32)
+    s[..., 5], s[..., 6] = dx, dy
+    return pyoracle.rotate_rows(s)[..., 0], np.sqrt(dx * dx + dy * dy)
+
+
+def _edge_scene(robot, humans):
+    """A scene dict of float32 values (robot px, py, vx, vy, gx, gy, radius, v_pref, theta; humans px, py, vx, vy, radius):
+    float64 state whose cast to float32 is exact. Human goals sit on the humans, v_pref 1."""
+    f = lambda x: float(np.float32(x))  # noqa: E731
+    r = [f(x) for x in robot]
+    return {'robot': [R(x) for x in r],
+            'humans': [[R(f(h[0])), R(f(h[1])), R(f(h[2])), R(f(h[3])), R(f(h[0])), R(f(h[1])), R(f(h[4])), R(1.0)]
+                       for h in humans]}
+
+
+def _edge_tuples(sc):
+    """The 14-tuples of a scene, (robot FullState + human ObservableState) as MultiHumanRL.transform joins them."""
+    from crowd_sim.envs.utils.state import FullState, ObservableState
+    r = [float(x) for x in sc['robot']]
+    self_state = FullState(r[0], r[1], r[2], r[3], r[6], r[4], r[5], r[7], r[8])
+    return [self_state + ObservableState(*[float(h[i]) for i in (0, 1, 2, 3, 6)]) for h in sc['humans']]
+
+
+def run_rotate_edges(N=5):
+    """CADRL.rotate (cadrl.py:187-222), the reference's own method on a CADRL policy set to holonomic and to unicycle
+    kinematics, on constructed scenes of N humans. Every builder asserts the edge it makes:
+      norm near      dg and da values 0.05 to 20 m whose fused and plain float32 norms differ
+      norm parked    the same at the `mixed` rule's parked humans (x = PARKED_X + 100 i, y = PARKED_X: about 1e6 m)
+      on goal        the robot on its goal: dx = dy = 0, rot = atan2(0, 0) = 0, dg = 0
+      on human       a human on the robot: da = 0
+      goal behind    rot = +pi (dy = +0) and -pi (dy = -0: the robot at y = +0, its goal at y = -0)
+      goal beside    rot = +pi / 2 and -pi / 2
+      zero velocity  the robot's and the humans' velocities +0 and -0
+      heading wraps  theta - rot outside (-pi, pi]
+    Written: per case and kinematics the scenes, their tuples and the reference's rows (float32 shortest strings)."""
+    rng = np.random.RandomState(2025)
+    f32 = np.float32
+    u = lambda lo, hi, n=None: f32(rng.uniform(lo, hi)) if n is None else rng.uniform(lo, hi, n).astype(f32)  # noqa: E731
+    uvel = lambda: list(u(-1, 1, 2))  # noqa: E731
+
+    def tells(robot, humans):
+        """(dg differs, [da differs per human]) between the fused and the plain norm, on the float32 values."""
+        px, py, gx, gy = (f32(robot[i]) for i in (0, 1, 4, 5))
+        fd, pd = _norms32(gx - px, gy - py)
+        fa, pa = _norms32(np.array([px - f32(h[0]) for h in humans]), np.array([py - f32(h[1]) for h in humans]))
+        return bool(fd != pd), list(fa != pa)
+
+    def human_near(px, py):
+        d, a = u(0.05, 20), u(-np.pi, np.pi)
+        return [px + d * np.cos(a), py + d * np.sin(a)] + uvel() + [u(0.2, 0.5)]
+
+    def robot(px, py, gx, gy, theta=0.0, vel=None):
+        return [px, py] + (uvel() if vel is None else vel) + [gx, gy, u(0.2, 0.5), u(0.5, 1.5), theta]
+
+    def norm_near():
+        scenes = []
+        while len(scenes) < 8:
+            px, py = u(-5, 5), u(-5, 5)
+            d, a = u(0.05, 20), u(-np.pi, np.pi)
+            r = robot(px, py, px + d * np.cos(a), py + d * np.sin(a))
+            hs = [human_near(px, py) for _ in range(N)]
+            dg, da = tells(r, hs)
+            if dg and any(da):
+                scenes.append((r, hs))
+        return scenes
+
+    def norm_parked():
+        scenes = []
+        while len(scenes) < 8:
+            px, py = u(-5, 5), u(-5, 5)
+            d, a = u(0.05, 20), u(-np.pi, np.pi)
+            r = robot(px, py, px + d * np.cos(a), py + d * np.sin(a))
+            k = 1 + len(scenes) % N
+            hs = [human_near(px, py) for _ in range(k - 1)] + [[test_util.PARKED_X + 100.0 * i, test_util.PARKED_X, 0.0, 0.0, 0.3]
+                                                                for i in range(k - 1, N)]
+            dg, da = tells(r, hs)
+            if dg and any(da[k - 1:]):
+                scenes.append((r, hs))
+        return scenes
+
+    def on_goal():
+        out = []
+        for _ in range(4):
+            px, py = u(-5, 5), u(-5, 5)
+            out.append((robot(px, py, px, py, theta=u(-np.pi, np.pi)), [human_near(px, py) for _ in range(N)]))
+        return out
+
+    def on_human():
+        out = []
+        for _ in range(4):
+            px, py = u(-5, 5), u(-5, 5)
+            hs = [human_near(px, py) for _ in range(N)]
+            hs[len(out) % N][0:2] = [px, py]
+            out.append((robot(px, py, u(-5, 5), u(-5, 5)), hs))
+        return out
+
+    def goal_behind():
+        out = []
+        for sign_y in (0.0, -0.0, 0.0, -0.0):
+            px = u(-5, 5)
+            out.append((robot(px, 0.0, px - u(0.5, 10), sign_y, theta=u(-np.pi, np.pi)), [human_near(px, 0.0) for _ in range(N)]))
+        return out
+
+    def goal_beside():
+        out = []
+        for side in (1, -1, 1, -1):
+            px, py = u(-5, 5), u(-5, 5)
+            out.append((robot(px, py, px, py + side * u(0.5, 10)), [human_near(px, py) for _ in range(N)]))
+        return out
+
+    def zero_velocity():
+        out = []
+        for z in ([0.0, 0.0], [-0.0, 0.0], [0.0, -0.0], [-0.0, -0.0]):
+            px, py = u(-5, 5), u(-5, 5)
+            hs = [human_near(px, py)[:2] + list(z) + [u(0.2, 0.5)] for _ in range(N)]
+            out.append((robot(px, py, u(-5, 5), u(-5, 5), vel=list(z)), hs))
+        return out
+
+    def heading_wraps():
+        out = []
+        while len(out) < 8:
+            px, py = u(-5, 5), u(-5, 5)
+            th = u(-np.pi, np.pi) if len(out) % 2 else u(np.pi, 2 * np.pi)
+            r = robot(px, py, u(-5, 5), u(-5, 5), theta=th)
+            rot = np.arctan2(f32(r[5]) - f32(py), f32(r[4]) - f32(px))
+            if not -np.pi < f32(th) - f32(rot) <= np.pi:
+                out.append((r, [human_near(px, py) for _ in range(N)]))
+        return out
+
+    builders = (('norm near', norm_near), ('norm parked', norm_parked), ('on goal', on_goal), ('on human', on_human),
+                ('goal behind', goal_behind), ('goal beside', goal_beside), ('zero velocity', zero_velocity),
+                ('heading wraps', heading_wraps))
+    pcfg = configparser.RawConfigParser()
+    pcfg.read(os.path.join(REF, 'crowd_nav', 'configs', 'policy.config'))
+    policy = policy_factory['cadrl']()
+    policy.configure(pcfg)
+    cases = []
+    for tag, build in builders:
+        scenes = [_edge_scene(r, hs) for r, hs in build()]
+        tuples = [t for sc in scenes for t in _edge_tuples(sc)]
+        s = torch.Tensor(tuples)
+        sf = s.numpy()
+        if tag == 'on goal':
+            assert (sf[:, 5] == sf[:, 0]).all() and (sf[:, 6] == sf[:, 1]).all()
+        if tag == 'on human':
+            assert sum(int((sf[i, 9:11] == sf[i, 0:2]).all()) for i in range(len(sf))) >= len(scenes)
+        for kin in ('holonomic', 'unicycle'):
+            policy.kinematics = kin
+            rows = policy.rotate(s).numpy()
+            rot = torch.atan2(s[:, 6] - s[:, 1], s[:, 5] - s[:, 0]).numpy()          # float32, as rotate's
+            if tag == 'on goal':
+                assert (rows[:, 0] == 0).all() and (rot == 0).all()
+            if tag == 'on human':
+                assert (rows[:, 11] == 0).sum() >= len(scenes)
+            if tag == 'goal behind':
+                assert (np.abs(rot) == np.pi).all() and (rot > 0).any() and (rot < 0).any()
+            if tag == 'goal beside':
+                assert (np.abs(rot) == np.pi / 2).all() and (rot > 0).any() and (rot < 0).any()
+            if tag == 'zero velocity':
+                assert (sf[:, [2, 3, 11, 12]] == 0).all() and np.signbit(sf[:, [2, 3, 11, 12]]).any()
+            if tag == 'heading wraps':
+                th = sf[:, 8] - rot
+                assert ((th <= -np.pi) | (th > np.pi)).any()
+                if kin == 'unicycle':
+                    assert ((rows[:, 2] <= -np.pi) | (rows[:, 2] > np.pi)).any()
+            if tag.startswith('norm'):
+                fd, pd = _norms32(sf[:, 5] - sf[:, 0], sf[:, 6] - sf[:, 1])
+                fa, pa = _norms32(sf[:, 0] - sf[:, 9], sf[:, 1] - sf[:, 10])
+                assert (rows[:, 0] == fd).all() and (rows[:, 11] == fa).all()
+                assert (fd != pd).any() and (fa != pa).any()
+                if tag == 'norm parked':
+                    assert (fa[sf[:, 9] >= test_util.PARKED_X] != pa[sf[:, 9] >= test_util.PARKED_X]).any()
+            cases.append({'tag': tag, 'unicycle': int(kin == 'unicycle'), 'N': N, 'scenes': scenes,
+                          'tuples': [[R32(v) for v in t] for t in sf.tolist()],
+                          'rows': [[R32(v) for v in r] for r in rows.tolist()]})
+        print(tag, len(scenes), 'scenes')
+    with gzip.open(os.path.join(OUT, 'rotate_edges.json.gz'), 'wt') as f:
+        json.dump({'seed': 2025, 'cases': cases}, f, separators=(',', ':'))
+
+
 def run_om():
     """MultiHumanRL.build_occupancy_maps (multi_human_rl.py:109-163), reference code only: (a) on the humans of real
     scenes a few steps into test episodes and on the next human states env.onestep_lookahead returns, (b) on random
@@ -745,6 +931,7 @@ ONLY = {
     'human_times_envcfg': lambda: run_human_times('human_times_envcfg', HUMAN_TIMES_ENVCFG),
     'rotate_envcfg': lambda: run_rotate('rotate_lookahead_envcfg', 'env_config', cases=(0, 3, 11), steps=16, every=4),
     'rotate_unicycle': run_rotate_unicycle,
+    'rotate_edges': run_rotate_edges,
 }
 
 

@@ -31,6 +31,7 @@ def lib():
         _abi.declare(l, prefix='oracle_crowdsim_', with_stream=False)
         l.oracle_mt19937_doubles.argtypes = [C.c_uint32, C.c_int, C.c_void_p]
         l.oracle_get_stats.argtypes = [C.c_void_p]
+        l.oracle_rotate_rows.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         l.oracle_crowdsim_run_passes.restype = C.c_int
         l.oracle_crowdsim_run_passes.argtypes = [C.POINTER(_abi.Params), C.c_int, C.c_int, C.POINTER(_abi.State),
                                                  C.POINTER(_abi.StepIO), C.POINTER(_abi.ResetArgs), C.c_int]
@@ -206,6 +207,16 @@ def orca_act(prm, st):
 def pack_joint(st, unicycle=False):
     out = np.zeros((st.B, st.N, 13), dtype=np.float32); s = st.struct()
     rc = lib().oracle_crowdsim_pack_joint(st.B, st.N, C.byref(s), int(unicycle), _ptr(out))
+    assert rc == 0, rc
+    return out
+
+
+def rotate_rows(s, unicycle=False):
+    """CADRL.rotate (cadrl.py:187-222) of float32 14-tuples s [..., 14] -> float32 rows [..., 13], torch CPU's op order."""
+    s = np.ascontiguousarray(s, dtype=np.float32)
+    assert s.shape[-1] == 14, s.shape
+    out = np.zeros(s.shape[:-1] + (13,), dtype=np.float32)
+    rc = lib().oracle_rotate_rows(int(s.size // 14), _ptr(s), int(unicycle), _ptr(out))
     assert rc == 0, rc
     return out
 

@@ -8,7 +8,8 @@ import pytest
 import torch
 
 from util import (SUITES, NON_DEFAULT, ORCA_TIGHT, PROFILE_SUITES, load_golden, scene_arrays, fill_host_state, pre_step_times,
-                  profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits, assert_unicycle_step_within_bounds)
+                  profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits, assert_unicycle_step_within_bounds,
+                  assert_rotate_within_model, assert_rows_match, pack_inputs, lookahead_inputs)
 
 pytestmark = pytest.mark.gpu
 
@@ -290,14 +291,21 @@ def test_pack_and_lookahead_match_oracle_and_reference(cuda_env, oracle):
     o_packed = oracle.pack_joint(host)
     o_states, o_reward = oracle.lookahead_pack(oracle.default_params(robot_policy=0), host, actions)
     assert same_bits(reward, o_reward)
-    assert np.abs(packed - o_packed).max() < 1e-5 and np.abs(states - o_states).max() < 1e-5
+    npos, nvel = oracle.lookahead_humans(oracle.default_params(robot_policy=0), host)
+    s_cur, s_next = pack_inputs(host), lookahead_inputs(host, actions, npos, nvel, 0.25, False)
+    assert_rotate_within_model(packed, s_cur, False, what='pack_joint')
+    assert_rotate_within_model(states, s_next, False, what='lookahead_pack')
+    assert_rotate_within_model(o_packed, s_cur, False, what='oracle pack_joint')
+    assert_rotate_within_model(o_states, s_next, False, what='oracle lookahead_pack')
     for e, r in enumerate(rows):      # the reference's own torch rotate / onestep_lookahead outputs
         ref_cur = np.array([[float(v) for v in row] for row in r['rotated_current']], dtype=np.float32)
-        assert np.abs(packed[e] - ref_cur).max() < 1e-5
+        assert_rotate_within_model(ref_cur, s_cur[e], False, what='reference rotate(current) %d' % e)
+        assert_rows_match(packed[e], ref_cur, False, turned_atol=1e-5, what='pack_joint vs reference %d' % e)
         for k, la in enumerate(r['lookahead']):
             assert reward[e, k] == float(la['reward'])
             ref = np.array([[float(v) for v in row] for row in la['rotated']], dtype=np.float32)
-            assert np.abs(states[e, k] - ref).max() < 2e-5, (e, k)
+            assert_rotate_within_model(ref, s_next[e, k], False, what='reference rotate(lookahead) %d %d' % (e, k))
+            assert_rows_match(states[e, k], ref, False, turned_atol=2e-5, what='lookahead_pack vs reference %d %d' % (e, k))
     # bigger random batch, N = 20 (tile path with many rows)
     host = _random_host_state(oracle, 257, 20, seed=9)
     env = cuda_env(257, 20, robot_visible=True, robot_policy='external_xy')
@@ -305,7 +313,9 @@ def test_pack_and_lookahead_match_oracle_and_reference(cuda_env, oracle):
     states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
     o_states, o_reward = oracle.lookahead_pack(oracle.default_params(robot_visible=1, robot_policy=0), host, actions)
     assert same_bits(reward.cpu().numpy(), o_reward)
-    assert np.abs(states.cpu().numpy() - o_states).max() < 1e-4
+    npos, nvel = oracle.lookahead_humans(oracle.default_params(robot_visible=1, robot_policy=0), host)
+    assert_rotate_within_model(states.cpu().numpy(), lookahead_inputs(host, actions, npos, nvel, 0.25, False), False,
+                               what='lookahead_pack N=20')
 
 
 def test_large_batch_linearity(cuda_env, oracle):
@@ -843,13 +853,15 @@ def test_profile_orca_act_and_lookahead_kernels(cuda_env, oracle, prof):
         states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
         o_states, o_reward = oracle.lookahead_pack(prm, host, actions)
         assert same_bits(reward.cpu().numpy(), o_reward), (prof, N)
-        assert np.abs(states.cpu().numpy() - o_states).max() < 1e-5
+        assert_rotate_within_model(states.cpu().numpy(), lookahead_inputs(host, actions, o_pos, o_vel, prm.time_step, False),
+                                   False, what='%s N=%d lookahead_pack' % (prof, N))
         _assert_state_equal(env, host, what='%s N=%d: the lookahead kernels leave the state alone' % (prof, N))
 
 
 def test_profile_lookahead_pack_matches_reference(cuda_env, oracle):
     """lookahead_pack at env_config (dt 0.1, robot v_pref 0.8 action space, radii, rewards) against the reference's own
-    onestep_lookahead rewards (bit-exact) and CADRL.rotate rows (1e-5 abs) -- tests/golden/rotate_lookahead_envcfg."""
+    onestep_lookahead rewards (bit-exact) and CADRL.rotate rows (tests/util.py's row contract: exact columns bit for bit)
+    -- tests/golden/rotate_lookahead_envcfg."""
     d = load_golden('rotate_lookahead_envcfg')
     prof = d['profile']
     actions = np.array([[float(x) for x in a] for a in d['action_space']])
@@ -861,14 +873,18 @@ def test_profile_lookahead_pack_matches_reference(cuda_env, oracle):
     env.state.load_host(host)
     states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
     states = states.cpu().numpy(); reward = reward.cpu().numpy()
-    o_states, o_reward = oracle.lookahead_pack(profile_params(oracle, prof, robot_policy=0), host, actions)
+    prm = profile_params(oracle, prof, robot_policy=0)
+    o_states, o_reward = oracle.lookahead_pack(prm, host, actions)
     assert same_bits(reward, o_reward)
-    assert np.abs(states - o_states).max() < 1e-5
+    npos, nvel = oracle.lookahead_humans(prm, host)
+    s_next = lookahead_inputs(host, actions, npos, nvel, prm.time_step, False)
+    assert_rotate_within_model(states, s_next, False, what='envcfg lookahead_pack')
     for e, r in enumerate(rows):
         for k, la in enumerate(r['lookahead']):
             assert reward[e, k] == float(la['reward']), (e, k)
             ref = np.array([[float(v) for v in row] for row in la['rotated']], dtype=np.float32)
-            assert np.abs(states[e, k] - ref).max() < 2e-5, (e, k)
+            assert_rotate_within_model(ref, s_next[e, k], False, what='envcfg reference rows %d %d' % (e, k))
+            assert_rows_match(states[e, k], ref, False, turned_atol=2e-5, what='envcfg lookahead_pack vs reference %d %d' % (e, k))
 
 
 def test_profile_reset_and_prefetch_match_oracle_and_reference(cuda_env, oracle):

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from crowdnav_b200 import _abi
-from util import assert_same_bits, profile_env
+from util import assert_rows_match, assert_same_bits, profile_env
 from test_cuda_9_il_record import (AR_FIELDS, EP_FIELDS, GAMMA, STATE_FIELDS, _expected_ring, _idle, _make, _pair_multiset,
                                    _refill)
 
@@ -262,7 +262,7 @@ def _assert_matches_reference(mem, ref_mem):
     assert len(mem) == len(ref_mem) > 50
     ref_states = torch.stack([s for s, _ in ref_mem]); ref_values = torch.cat([v for _, v in ref_mem])
     assert torch.equal(mem.values[:len(mem), 0].cpu(), ref_values)
-    assert (mem.states[:len(mem)].cpu() - ref_states).abs().max() < 2e-5
+    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, what='IL memory rows')
 
 
 def test_cadrl_il_matches_single_env_explorer(cuda_env):

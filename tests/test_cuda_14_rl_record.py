@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from crowdnav_b200 import _abi
-from util import assert_same_bits, load_golden, profile_env
+from util import assert_rows_match, assert_same_bits, load_golden, profile_env
 from test_cuda_9_il_record import GAMMA, _expected_ring, _idle, _make, _pair_multiset, _refill
 from test_cuda_10_il_record_ex import _F, _same_state
 
@@ -195,7 +195,7 @@ def test_rl_update_memory_reference_fixture_through_device_recorder(cuda_env, mo
     assert len(mem) == d['pairs'] == sum(e['stored'] for e in d['episodes'])
     ref_values = torch.tensor([float(v) for v in d['values']], dtype=torch.float32)
     ref_states = torch.tensor([[[float(x) for x in row] for row in st] for st in d['states']], dtype=torch.float32)
-    assert (mem.states[:len(mem)].cpu() - ref_states).abs().max() < 2e-5
+    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, what='RL memory rows')
     assert (mem.values[:len(mem), 0].cpu() - ref_values).abs().max() < 1e-5
     ends = torch.tensor([e['stored'] for e in d['episodes']]).cumsum(0) - 1
     assert [float(v) for v in mem.values[ends.to(mem.values.device), 0].cpu()] == [1.0 if e['info'] == 2 else -0.25 for e in d['episodes']]

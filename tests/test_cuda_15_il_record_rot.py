@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from crowdnav_b200 import _abi
-from util import assert_rotate_within_model, assert_same_bits, load_golden, pack_inputs, profile_env
+from util import assert_rotate_within_model, assert_same_bits, exact_columns, load_golden, pack_inputs, profile_env
 from test_cuda_9_il_record import GAMMA, _expected_ring, _idle, _make, _refill
 from test_cuda_10_il_record_ex import _F, _same_state
 
@@ -162,13 +162,13 @@ def _f32(s, shape):
 
 
 @pytest.mark.parametrize('tag', ['sarl5_unicycle', 'cadrl1_unicycle'])
-def test_reference_fixture_through_explorer(cuda_env, monkeypatch, tag):
+def test_reference_fixture_rows_through_explorer(cuda_env, monkeypatch, tag):
     """tests/golden/il_unicycle_rows (scripts/gen_il_unicycle_golden.py): the reference's Explorer.run_k_episodes(
     imitation_learning=True) with an invisible ORCA robot (safety space 0.15) and a unicycle target, SARL at N = 5 and
     CADRL at N = 1. BatchedExplorer (B = 1, device recorder; the per-step recorder refuses here) stores the same pairs in the
-    same order with the same float32 values. Row columns without trigonometry are the reference's bits (dg and da, which
-    torch.norm rounds its own way, are the float32 expression of the reference's inputs); every column is within
-    rotate_model's bound of the reference's float32 inputs."""
+    same order with the same float32 values. Row columns without trigonometry (tests/util.py:exact_columns, dg and da
+    included: torch.norm's sqrtf(fmaf(dy, dy, dx * dx))) are the reference's bits; every column is within rotate_model's
+    bound of the reference's float32 inputs."""
     import crowdnav_b200.memory as memory
     from crowdnav_b200.explorer import BatchedExplorer
     from crowdnav_b200.memory import DeviceReplayMemory
@@ -190,12 +190,11 @@ def test_reference_fixture_through_explorer(cuda_env, monkeypatch, tag):
     values = np.array([float(v) for v in b['values']], dtype=np.float32)
     assert_same_bits(mem.values[:P, 0].cpu().numpy(), values, 'IL values')
     rows = mem.states[:P].cpu().numpy()
-    for c in (1, 3, 10, 12):
+    for c in exact_columns(True):
         assert_same_bits(rows[..., c], rows_ref[..., c], 'column %d' % c)
-    dx, dy = tup[..., 5] - tup[..., 0], tup[..., 6] - tup[..., 1]
-    ax, ay = tup[..., 0] - tup[..., 9], tup[..., 1] - tup[..., 10]
-    assert_same_bits(rows[..., 0], np.sqrt(dx * dx + dy * dy), 'dg')
-    assert_same_bits(rows[..., 11], np.sqrt(ax * ax + ay * ay), 'da')
+    plain = lambda x, y: np.sqrt(x * x + y * y)  # noqa: E731  (the fixture tells it from the reference's norm)
+    assert (plain(tup[..., 5] - tup[..., 0], tup[..., 6] - tup[..., 1]) != rows_ref[..., 0]).any()
+    assert (plain(tup[..., 0] - tup[..., 9], tup[..., 1] - tup[..., 10]) != rows_ref[..., 11]).any()
     assert (tup[..., 8] == np.float32(np.pi / 2)).all()
     assert_rotate_within_model(rows, tup, True, what=tag + ' device rows')
     assert_rotate_within_model(rows_ref, tup, True, what=tag + ' reference rows')

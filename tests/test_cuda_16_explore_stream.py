@@ -327,9 +327,10 @@ def test_compat_numpy_stream():
         compat.install()
 
 
-def test_explorer_replay_pairs_match_reference():
+def test_explorer_replay_pairs_match_reference(oracle):
     """With a target model, DeviceRLRecorder stores the reference's pairs (Explorer.update_memory, explorer.py:107-113) of
-    the epsilon = 1 episodes: the same count and order, rows within 2e-5 (float32 rotate), values within 1e-5."""
+    the epsilon = 1 episodes: the same count and order, values within 1e-5, rows within 2e-5 (float32 rotate) and, where
+    every scene is the reference's bit for bit, their exact columns (tests/util.py:exact_columns) bit for bit."""
     from crowdnav_b200.explorer import BatchedExplorer
     from crowdnav_b200.memory import DeviceReplayMemory
     from crowdnav_b200.policy import make_sarl
@@ -347,6 +348,12 @@ def test_explorer_replay_pairs_match_reference():
     rows = np.frombuffer(base64.b64decode(d['rows']), dtype='<f4').reshape(d['shape'])
     assert len(mem) == d['count']
     assert np.abs(mem.states[:len(mem)].cpu().numpy() - rows).max() < 2e-5
+    gen, rule = _block_env(block, block['k'])
+    gen.reset('train', cases=list(range(block['k'])), rule=rule)
+    if all(_device_scenes_match(gen, _reference_scenes(block, oracle))):
+        uni = block['kinematics'] == 'unicycle'
+        util.assert_rows_match(mem.states[:len(mem)].cpu().numpy(), rows, uni, robot_ulps=int(uni), turned_atol=2e-5,
+                               what='replay rows')
     values = np.array([float(v) for v in d['values']], dtype=np.float32)
     assert np.abs(mem.values[:len(mem), 0].cpu().numpy() - values).max() < 1e-5
 

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import assert_same_bits, load_golden
+from util import assert_rows_match, assert_same_bits, load_golden
 from test_cuda_9_il_record import GAMMA, _idle, _make, _refill
 from test_cuda_14_rl_record import BatchInvariant, RandomActions, _check
 from test_cuda_10_il_record_ex import _F
@@ -316,6 +316,10 @@ def test_explorer_reproduces_reference_lstm_rl(cuda_env, oracle, tag):
             continue
         (a, n), (b, m) = ours[e], theirs[e]
         assert n == m, (tag, e)
+        if same[e]:                       # the reference's scene: exact columns bit for bit (a unicycle's dg, da turned)
+            uni = block['kinematics'] == 'unicycle'
+            assert_rows_match(states[a:a + n], ref_rows[b:b + n], uni, robot_ulps=int(uni), turned_atol=2e-5,
+                              what='%s episode %d rows' % (tag, e))
         assert np.abs(states[a:a + n] - ref_rows[b:b + n]).max(initial=0.0) < 2e-5, (tag, e)
         assert np.abs(values[a:a + n] - ref_values[b:b + n]).max(initial=0.0) < 1e-5, (tag, e)
         compared += n

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import SUITES, PROFILE_SUITES, load_golden, fill_host_state, profile_env, same_bits
+from util import SUITES, PROFILE_SUITES, load_golden, fill_host_state, profile_env, same_bits, assert_rows_match
 
 pytestmark = pytest.mark.gpu
 
@@ -124,15 +124,16 @@ def test_sarl_rollout_terminates_and_classifies(cuda_env):
 
 
 def _torch_rotate(rows14):
-    """cadrl.py:187-222 in float32 torch ops (test-side restatement, holonomic)."""
+    """cadrl.py:187-222 in float32 torch ops (test-side restatement, holonomic); dg and da with the reference's torch.norm."""
     s = rows14
     dx, dy = s[:, 5] - s[:, 0], s[:, 6] - s[:, 1]
     rot = torch.atan2(dy, dx); c, sn = torch.cos(rot), torch.sin(rot)
-    dg = torch.sqrt(dx * dx + dy * dy)
+    norm = lambda x, y: torch.norm(torch.stack([x, y], dim=1), 2, dim=1)  # noqa: E731
+    dg = norm(dx, dy)
     cols = [dg, s[:, 7], torch.zeros_like(dg), s[:, 4], s[:, 2] * c + s[:, 3] * sn, s[:, 3] * c - s[:, 2] * sn,
             (s[:, 9] - s[:, 0]) * c + (s[:, 10] - s[:, 1]) * sn, (s[:, 10] - s[:, 1]) * c - (s[:, 9] - s[:, 0]) * sn,
             s[:, 11] * c + s[:, 12] * sn, s[:, 12] * c - s[:, 11] * sn, s[:, 13],
-            torch.sqrt((s[:, 0] - s[:, 9]) ** 2 + (s[:, 1] - s[:, 10]) ** 2), s[:, 4] + s[:, 13]]
+            norm(s[:, 0] - s[:, 9], s[:, 1] - s[:, 10]), s[:, 4] + s[:, 13]]
     return torch.stack(cols, dim=1)
 
 
@@ -173,7 +174,7 @@ def test_update_memory_matches_single_env_explorer(cuda_env):
     assert len(mem) == len(ref_mem) > 100
     ref_states = torch.stack([s for s, _ in ref_mem]); ref_values = torch.cat([v for _, v in ref_mem])
     assert torch.equal(mem.values[:len(mem), 0].cpu(), ref_values)
-    assert (mem.states[:len(mem)].cpu() - ref_states).abs().max() < 2e-5
+    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, what='IL memory rows')
 
 
 def test_rl_update_memory_matches_reference_fixture(cuda_env):
@@ -195,7 +196,7 @@ def test_rl_update_memory_matches_reference_fixture(cuda_env):
     assert len(mem) == d['pairs'] == sum(e['stored'] for e in d['episodes'])
     ref_values = torch.tensor([float(v) for v in d['values']], dtype=torch.float32)
     ref_states = torch.tensor([[[float(x) for x in row] for row in st] for st in d['states']], dtype=torch.float32)
-    assert (mem.states[:len(mem)].cpu() - ref_states).abs().max() < 2e-5
+    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, what='RL memory rows')
     assert (mem.values[:len(mem), 0].cpu() - ref_values).abs().max() < 1e-5
     # terminal steps carry the bare reward: 1 for ReachGoal, -0.25 for Collision
     ends = torch.tensor([e['stored'] for e in d['episodes']]).cumsum(0) - 1

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import crowd_lp3 as c3
-from util import assert_same_bits, profile_env, profile_params
+from util import assert_rotate_within_model, assert_same_bits, lookahead_inputs, profile_env, profile_params
 
 pytestmark = pytest.mark.gpu
 
@@ -195,7 +195,9 @@ def test_lookahead_kernels_on_piled_scenes(cuda_env, oracle, count, N):
         states, reward = env.lookahead_pack(torch.from_numpy(actions).to(env.device))
         o_states, o_reward = oracle.lookahead_pack(prm, scene, actions)
         assert_same_bits(reward.cpu().numpy(), o_reward, 'N=%d lookahead_pack reward' % N)
-        assert np.abs(states.cpu().numpy() - o_states).max() < 1e-5
+        s = lookahead_inputs(scene, actions, o_pos, o_vel, prm.time_step, False)
+        assert_rotate_within_model(states.cpu().numpy(), s, False, what='N=%d lookahead_pack rows' % N)
+        assert_rotate_within_model(o_states, s, False, what='N=%d oracle lookahead_pack rows' % N)
     dev = env.state.to_host()
     for f in STATE_FIELDS:
         assert_same_bits(dev[f], getattr(scene, f), 'N=%d lookahead kernels leave %s alone' % (N, f))

@@ -186,6 +186,30 @@ def ulp64(x):
     return np.spacing(np.abs(np.asarray(x, dtype=np.float64)))
 
 
+# The rotated-row contract (cadrl.py:187-222, 13 float32 columns). EXACT columns use no atan2 / cos / sin: dg (0), v_pref
+# (1), theta (2, holonomic: zero), radius (3), radius1 (10), da (11), radius_sum (12). Every producer's exact columns equal
+# the reference's bit for bit: a float32 subtraction, torch's 2-norm sqrtf(fmaf(dy, dy, dx * dx)) (x first, as
+# torch.norm(torch.cat([dx, dy], 1)) evaluates it on CPU) and a float32 sum. dg and da read the robot's position, so they
+# are exact only where that position is the same float32 input on both sides (robot_ulps == 0). TURNED columns (4 to 9;
+# theta for a unicycle; dg and da when robot_ulps > 0) go through atan2 / cos / sin and are held to rotate_model's bound.
+def exact_columns(unicycle, robot_ulps=0):
+    """Indices of the rotated row's exact columns (see above)."""
+    cols = [1, 3, 10, 12] + ([] if unicycle else [2]) + ([0, 11] if robot_ulps == 0 else [])
+    return sorted(cols)
+
+
+def turned_columns(unicycle, robot_ulps=0):
+    exact = exact_columns(unicycle, robot_ulps)
+    return [c for c in range(13) if c not in exact]
+
+
+def rotate_exact(s, unicycle):
+    """The float32 restatement of CADRL.rotate on 14-tuples s [..., 14] (the oracle's rotate_row: libm's correctly rounded
+    fmaf and sqrtf, every other operation rounded to float32 on its own). Only its exact columns are a contract."""
+    import pyoracle
+    return pyoracle.rotate_rows(s, unicycle)
+
+
 def rotate_model(s, unicycle, robot_ulps=0):
     """CADRL.rotate (cadrl.py:187-222) evaluated in float64 on float32 14-tuples s [..., 14], and a bound on how far any
     float32 implementation of it can be from that value: (model [..., 13], bound [..., 13]).
@@ -193,8 +217,9 @@ def rotate_model(s, unicycle, robot_ulps=0):
     Derivation, u = 2^-24: dx = gx - px is rounded once (|err| <= u |dx|). atan2 moves by at most (|dx| e_y + |dy| e_x) / r^2
     for input errors e_x, e_y, and atan2f adds ULP_ATAN2F ulps of its result: drot. cos(rot + drot) is within |sin| drot
     of cos(rot), and cosf adds ULP_COSF ulps: dc (ds likewise). A product a * c rounds once, a sum of two products once more,
-    a coordinate difference once more (px1: 3 roundings of |dx c| + |dy s|). A norm sqrtf(x*x + y*y) carries 3u
-    relative (2u from the squares' and the sum's rounding, halved by the square root, plus sqrtf's own rounding).
+    a coordinate difference once more (px1: 3 roundings of |dx c| + |dy s|). The norm sqrtf(fmaf(y, y, x * x)) carries 3u
+    relative: the difference's rounding (u), x * x's and the fma's rounding (u x^2 + u r^2 <= 2u r^2, halved by the square
+    root) and sqrtf's own rounding (u).
     robot_ulps: the robot's px, py, vx, vy (and theta) may differ by that many float32 ulps between two implementations
     (they come from double cos / sin, rounded to float32 once: 1 when one rounding may go either way); their effect is
     propagated through the same terms. The bound is widened by 1 % for the second-order terms (products of two errors,
@@ -231,7 +256,12 @@ def rotate_model(s, unicycle, robot_ulps=0):
 
 
 def assert_rotate_within_model(rows, s, unicycle, robot_ulps=0, what=''):
-    """Every float32 row element within rotate_model's bound of the float64 value; returns the largest |error| / bound."""
+    """The rotated-row contract on rows [..., 13] rotated from the float32 tuples s [..., 14]: the exact columns equal
+    rotate_exact's bit for bit, and every element is within rotate_model's bound of the float64 value. Returns the largest
+    |error| / bound."""
+    cols = exact_columns(unicycle, robot_ulps)
+    assert_same_bits(np.asarray(rows, dtype=np.float32)[..., cols], rotate_exact(s, unicycle)[..., cols],
+                     '%s: exact columns %s' % (what, cols))
     model, bound = rotate_model(s, unicycle, robot_ulps)
     err = np.abs(np.asarray(rows, dtype=np.float64) - model)
     bad = err > bound
@@ -241,6 +271,17 @@ def assert_rotate_within_model(rows, s, unicycle, robot_ulps=0, what=''):
             what, int(bad.sum()), i, float(np.asarray(rows)[i]), float(model[i]), float(bound[i])))
     with np.errstate(divide='ignore', invalid='ignore'):
         return float(np.nanmax(np.where(bound > 0, err / bound, 0.0)))
+
+
+def assert_rows_match(rows, ref, unicycle, robot_ulps=0, turned_atol=0.0, what=''):
+    """Rows [..., 13] against another implementation's rows of the same float32 inputs where the inputs are not at hand:
+    the exact columns bit for bit, the turned columns within turned_atol."""
+    rows = np.asarray(rows, dtype=np.float32); ref = np.asarray(ref, dtype=np.float32)
+    cols = exact_columns(unicycle, robot_ulps)
+    assert_same_bits(rows[..., cols], ref[..., cols], '%s: exact columns %s' % (what, cols))
+    turned = turned_columns(unicycle, robot_ulps)
+    err = np.abs(rows[..., turned].astype(np.float64) - ref[..., turned])
+    assert not (err > turned_atol).any(), '%s: turned columns %s differ by %r > %r' % (what, turned, float(err.max()), turned_atol)
 
 
 def _tuples(rp, rv, ra, rg, th, hp, hv, hr):
