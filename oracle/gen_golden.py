@@ -19,6 +19,7 @@ What is recorded (floats as repr() strings, exact round trip):
   boundary_steps.json  one reference step on every constructed boundary scene (tests/boundary_scenes.py) and
                  get_human_times on the arrival-edge scenes
   rotate_edges.json  CADRL.rotate, holonomic and unicycle, on constructed edge scenes (--only rotate_edges)
+  om_edges.json  MultiHumanRL.build_occupancy_maps on constructed cell-edge, signed-zero and fold scenes (--only om_edges)
 
 usage: python oracle/gen_golden.py [--quick]
        python oracle/gen_golden.py --only NAME     one generator of ONLY (the non-default parameter profiles, boundary)
@@ -28,6 +29,7 @@ import gzip
 import io
 import json
 import logging
+import math
 import os
 import sys
 
@@ -685,6 +687,157 @@ def run_om():
     print('occupancy map rows', len(rows))
 
 
+OM_CONFIGS = [(cell_num, cell_size) for cell_num in range(1, 9) for cell_size in (1.0, 0.5, 0.75, 0.3)]
+
+
+def _om_x(r, cell_num, cell_size):
+    """floor(r / cs + cell_num / 2) in float64, the cell index of a rotated coordinate r (multi_human_rl.py:130-131)."""
+    return math.floor(r / cell_size + cell_num / 2)
+
+
+def _om_edge(k, cell_num, cell_size):
+    """The smallest double r with _om_x(r) >= k: the edge below cell k (k = 0 and k = cell_num are the grid's outer edges)."""
+    r = (k - cell_num / 2) * cell_size
+    while _om_x(r, cell_num, cell_size) >= k:
+        r = np.nextafter(r, -np.inf)
+    while _om_x(r, cell_num, cell_size) < k:
+        r = np.nextafter(r, np.inf)
+    return float(r)
+
+
+def _om_in_cell(m, n, cell_num, cell_size):
+    """The m-th of n positions r > 0 inside the cell that holds r = 0+ (cell_num / 2 rounded down)."""
+    return cell_size * (math.floor(cell_num / 2) - cell_num / 2 + 0.55 + 0.4 * (m + 0.5) / n)
+
+
+def run_om_edges():
+    """MultiHumanRL.build_occupancy_maps (multi_human_rl.py:109-163), the reference's own method, on constructed scenes at
+    cell_num 1..8 x cell_size 1.0, 0.5, 0.75, 0.3 (where r / cs rounds) x channels 1, 2, 3. Every builder asserts its edge
+    in float64. The centre human sits at the origin; occupants lie on the axes, so every atan2 argument is +-0 except where
+    a builder says otherwise, and the trig values that reach each output cell are one of (tests/util.py om_map_model):
+    0 every angle is +-0 (bit for bit on every side), 1 they are 0, +-pi/2, +-pi, 2 other (float64 model only).
+      x edge / y edge  an occupant at every cell edge r_k (the grid's outer edges included) and one ulp either side, in
+                       front of and behind the centre (x; behind: rot = pi) and beside it (y: rot = +-pi/2); one scene per
+                       variant and parity of k, so a move by one cell lands in an empty cell
+      centre line      the centre moving along -x (rot = -+pi): ry = sin(-+pi) dist is about -+1e-16 and ry / cs + half
+                       rounds to half for either sign
+      standing         the centre with velocity (+-0, +-0), and moving along -x with vy = +-0 (angle 0, -0, pi, -pi):
+                       occupants on both axes, standing occupants with velocities +-0, one off the axes at (1.5, 0.2)
+      same position    two humans at one position (dist = 0)
+      fold             3 to 5 occupants of one cell whose plain left fold and compensated sum round the cell's mean to
+                       different float32 values, or whose forward and reverse folds do; in front, mirrored behind, and
+                       along y (vy); 62 occupants of one cell at N = 63
+      lattice          cell_num 8: 62 occupants on the cell centres off the axes (model only)
+    Written: per scene tag, cell_num, cell_size, channels, the humans (px, py, vx, vy as repr strings), the reference's
+    maps (float32 shortest strings) and, per row, each cell's trig class as a digit string."""
+    from crowd_sim.envs.utils.state import ObservableState
+    pcfg = configparser.RawConfigParser()
+    pcfg.read(os.path.join(REF, 'crowd_nav', 'configs', 'policy.config'))
+    policy = policy_factory['sarl']()
+    policy.configure(pcfg)
+    scenes = []              # (tag, cell_num, cell_size, [[px, py, vx, vy], ...])
+
+    def edges(cn, cs):
+        half = cn / 2
+        for axis in ('x', 'y'):
+            centre = [0.0, 0.0, 0.8, 0.0] if axis == 'x' else [0.0, 0.0, 0.0, 0.8]
+            for variant in (-1, 0, 1):
+                for parity in (0, 1):
+                    hs = [centre]
+                    for k in range(parity, cn + 1, 2):
+                        if k == half:
+                            continue                        # r = 0: the same-position scenes
+                        e = _om_edge(k, cn, cs)
+                        r = {-1: np.nextafter(e, -np.inf), 0: e, 1: np.nextafter(e, np.inf)}[variant]
+                        assert _om_x(r, cn, cs) == (k - 1 if variant < 0 else k) and r != 0
+                        # x: the occupant at (r, +0) (rot = 0 in front, pi behind); y: at (-r, +0) with the centre moving
+                        # along +y (rot = -+pi/2): the rotated coordinate is r itself
+                        assert math.sqrt(r * r) == abs(r)
+                        hs.append([r if axis == 'x' else -r, 0.0, 0.5 + 0.125 * len(hs), 0.0])
+                    if len(hs) > 1:
+                        scenes.append(('%s edge %+d parity %d' % (axis, variant, parity), cn, cs, hs))
+
+    def centre_line(cn, cs):
+        half = cn / 2
+        for d in (0.45 * cs, 0.2 * cs, 0.05 * cs, 0.01 * cs):
+            ry = math.sin(math.pi) * d
+            if (-d / cs + half >= 0 and ry / cs + half == half and -ry / cs + half == half):
+                break
+        else:
+            raise AssertionError('no centre-line distance at %d %r' % (cn, cs))
+        for vy in (0.0, -0.0):
+            scenes.append(('centre line vy=%r' % vy, cn, cs, [[0.0, 0.0, -0.9, vy], [d, 0.0, 0.3, 0.0], [0.5 * d, -0.0, 0.6, -0.0]]))
+
+    def standing(cn, cs):
+        others = [[1.5, 0.2, 0.3, 0.1], [0.5 * cs, 0.0, 0.3, 0.0], [-0.7 * cs, 0.0, -0.4, 0.0], [0.0, 0.9 * cs, 0.0, 0.0],
+                  [0.25 * cs, 0.0, -0.0, -0.0]]
+        for v in ([0.0, 0.0], [-0.0, 0.0], [-0.0, -0.0], [0.0, -0.0], [-0.8, 0.0], [-0.8, -0.0]):
+            scenes.append(('centre velocity (%r, %r)' % tuple(v), cn, cs, [[0.0, 0.0] + v] + others))
+
+    def same_position(cn, cs):
+        scenes.append(('same position on axis', cn, cs, [[0.25, -0.5, 0.6, 0.0], [0.25, -0.5, 0.4, 0.0], [0.25 + 0.3 * cs, -0.5, 0.2, 0.0]]))
+        scenes.append(('same position', cn, cs, [[0.25, -0.5, 0.3, 0.4], [0.25, -0.5, -0.2, 0.1]]))
+
+    def fold(cn, cs):
+        cases = {'compensated 3': [3 + 3 * 2.0 ** -24] + [2.0 ** -52] * 2,
+                 'compensated 4': [4 + 2.0 ** -22] + [2.0 ** -52] * 3,
+                 'compensated 5': [5 + 5 * 2.0 ** -24] + [2.0 ** -52] * 4,
+                 'reverse 4': [2.0 ** -52] * 3 + [4 + 2.0 ** -22]}
+        for name, vs in cases.items():
+            plain, rev = 0.0, 0.0
+            for v, w in zip(vs, reversed(vs)):
+                plain, rev = plain + v, rev + w
+            n = len(vs)
+            fwd, comp, rev = np.float32(plain / n), np.float32(math.fsum(vs) / n), np.float32(rev / n)
+            assert fwd != rev if name.startswith('reverse') else (fwd != comp and fwd != rev), name
+            xs = [_om_in_cell(m, n, cn, cs) for m in range(n)]
+            assert len({_om_x(x, cn, cs) for x in xs}) == 1 and 0 <= _om_x(xs[0], cn, cs) < cn and min(xs) > 0
+            scenes.append(('fold %s' % name, cn, cs, [[0.0, 0.0, 1.0, 0.0]] + [[x, 0.0, v, 0.0] for x, v in zip(xs, vs)]))
+            scenes.append(('fold %s mirrored' % name, cn, cs, [[0.0, 0.0, -1.0, 0.0]] + [[-x, 0.0, -v, 0.0] for x, v in zip(xs, vs)]))
+            scenes.append(('fold %s along y' % name, cn, cs, [[0.0, 0.0, 0.0, 1.0]] + [[0.0, x, 0.0, v] for x, v in zip(xs, vs)]))
+
+    def crowd_cell(cn, cs, rng):
+        xs = [_om_in_cell(m, 62, cn, cs) for m in range(62)]
+        assert len({_om_x(x, cn, cs) for x in xs}) == 1 and min(xs) > 0
+        scenes.append(('62 in one cell', cn, cs, [[0.0, 0.0, 0.7, 0.0]] + [[x, 0.0, float(rng.uniform(0.1, 2.0)), 0.0] for x in xs]))
+
+    def lattice(cs, rng):
+        pts = [((ix + 0.5 - 4) * cs, (iy + 0.5 - 4) * cs) for iy in range(8) for ix in range(8)]
+        pts = [p for p in pts if p != (0.5 * cs, 0.5 * cs) and p != (-0.5 * cs, -0.5 * cs)]
+        scenes.append(('lattice', 8, cs, [[0.0, 0.0, 0.7, 0.0]] + [[x, y] + list(rng.uniform(-1, 1, 2)) for x, y in pts]))
+
+    rng = np.random.RandomState(2026)
+    for cn, cs in OM_CONFIGS:
+        edges(cn, cs)
+        centre_line(cn, cs)
+        standing(cn, cs)
+        same_position(cn, cs)
+        fold(cn, cs)
+        if cn in (1, 4, 7, 8):
+            crowd_cell(cn, cs, rng)
+        if cn == 8:
+            lattice(cs, rng)
+    rows = []
+    for tag, cn, cs, hs in scenes:
+        states = [ObservableState(px, py, vx, vy, 0.3) for px, py, vx, vy in hs]
+        h = np.array(hs, dtype=np.float64)[None]
+        for ch in (1, 2, 3):
+            policy.cell_num, policy.cell_size, policy.om_channel_size = cn, cs, ch
+            om = policy.build_occupancy_maps(states).numpy().reshape(len(states), -1)
+            trig = test_util.om_map_model(h[..., 0:2], h[..., 2:4], cn, cs, ch)['trig'][0]
+            rows.append({'tag': tag, 'cell_num': cn, 'cell_size': cs, 'channels': ch, 'humans': [[R(v) for v in hh] for hh in hs],
+                         'maps': [[R32(v) for v in r] for r in om.tolist()],
+                         'trig': [''.join(str(int(t)) for t in r) for r in trig]})
+    # the x edges at cs = 0.75 tell r / cs from r * (1 / cs) (at 0.3 the two put every edge on the same double)
+    for cs in (0.75,):
+        assert any(_om_x(r, cn, cs) != math.floor(r * (1.0 / cs) + cn / 2)
+                   for cn in range(1, 9) for k in range(cn + 1) if k != cn / 2 for e in [_om_edge(k, cn, cs)]
+                   for r in (np.nextafter(e, -np.inf), e)), cs
+    with gzip.open(os.path.join(OUT, 'om_edges.json.gz'), 'wt') as f:
+        json.dump({'rows': rows}, f, separators=(',', ':'))
+    print('om_edges rows', len(rows))
+
+
 def run_policy_decisions():
     """Greedy decisions of the reference's own CADRL and LSTM-RL policies (seed-0 weights, policy.config defaults, query_env):
     per-action values reward + gamma^(dt v_pref) * V and the chosen action on scenes a few steps into test episodes."""
@@ -932,6 +1085,7 @@ ONLY = {
     'rotate_envcfg': lambda: run_rotate('rotate_lookahead_envcfg', 'env_config', cases=(0, 3, 11), steps=16, every=4),
     'rotate_unicycle': run_rotate_unicycle,
     'rotate_edges': run_rotate_edges,
+    'om_edges': run_om_edges,
 }
 
 

@@ -263,11 +263,20 @@ def run_episodes(prm, N, seeds, rule='circle_crossing', gamma=0.9, robot_v_pref=
     return ep, st
 
 
+def _left_fold(xs):
+    s = 0.0
+    for x in xs:
+        s = s + x
+    return s
+
+
 def occupancy_maps(h_pos, h_vel, cell_num=4, cell_size=1.0, channels=3):
     """MultiHumanRL.build_occupancy_maps (crowd_nav/policy/multi_human_rl.py:109-163) restated for [B][N][2] float64
     position / velocity arrays -> [B][N][cell_num^2 * channels] float32. Plain float64 loops in the reference's
     expression order (rotation into the human's velocity frame :121-129, floor to cell indices :132-138, per-cell mean
-    of the occupants' rotated velocities :143-160)."""
+    of the occupants' rotated velocities :143-160). Each cell's sum is a plain left fold from 0.0 in ascending j, one
+    rounding per addition: the reference's sum() runs over numpy float64 scalars, which CPython 3.12 adds one by one,
+    while its sum() of exact floats is compensated (Neumaier) and can round a cell's mean to another float32."""
     import math
     h_pos = np.asarray(h_pos, dtype=np.float64); h_vel = np.asarray(h_vel, dtype=np.float64)
     B, N = h_pos.shape[:2]
@@ -295,8 +304,8 @@ def occupancy_maps(h_pos, h_vel, cell_num=4, cell_size=1.0, channels=3):
                 lists[cell_num * yi + xi][1].append(math.sin(vrot) * speed)
             for c, (lx, ly) in enumerate(lists):
                 occ = len(lx) > 0
-                mx = sum(lx) / len(lx) if occ else 0.0
-                my = sum(ly) / len(ly) if occ else 0.0
+                mx = _left_fold(lx) / len(lx) if occ else 0.0
+                my = _left_fold(ly) / len(ly) if occ else 0.0
                 if channels == 1:
                     out[e, i, c] = 1.0 if occ else 0.0
                 elif channels == 2:

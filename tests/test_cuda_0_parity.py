@@ -9,7 +9,8 @@ import torch
 
 from util import (SUITES, NON_DEFAULT, ORCA_TIGHT, PROFILE_SUITES, load_golden, scene_arrays, fill_host_state, pre_step_times,
                   profile, profile_env, profile_params, reset_kw, assert_same_bits, same_bits, assert_unicycle_step_within_bounds,
-                  assert_rotate_within_model, assert_rows_match, pack_inputs, lookahead_inputs)
+                  assert_rotate_within_model, assert_rows_match, pack_inputs, lookahead_inputs,
+                  assert_maps_within_model)
 
 pytestmark = pytest.mark.gpu
 
@@ -656,16 +657,17 @@ def test_lookahead_humans_matches_oracle(cuda_env, oracle):
 
 def test_occupancy_maps_match_reference_and_oracle(cuda_env, oracle):
     """crowdsim_occupancy_maps vs (a) the reference's own build_occupancy_maps outputs (fixtures), (b) the oracle on random
-    batches. Occupancy pattern identical, mean velocities to 1e-6 (float64 trig of CUDA vs glibc differs in the last ulp)."""
+    batches: both within the float64 model of tests/util.py (om_map_model; CUDA's double trig differs from glibc's in
+    the last ulps), the oracle's maps held to the same model."""
     rows = load_golden('occupancy_maps')['rows']
     for r in rows:
         h = np.array([[float(v) for v in hh] for hh in r['humans']])
         ref = np.array([[float(v) for v in m] for m in r['maps']], dtype=np.float32)
         env = cuda_env(1, h.shape[0])
         pos = torch.from_numpy(h[None, :, 0:2].copy()).to(env.device); vel = torch.from_numpy(h[None, :, 2:4].copy()).to(env.device)
-        got = env.occupancy_maps(pos, vel, r['cell_num'], float(r['cell_size']), r['channels'])[0].cpu().numpy()
-        assert same_bits(got != 0, ref != 0), r['tag']
-        assert np.abs(got - ref).max() <= 1e-6, r['tag']
+        got = env.occupancy_maps(pos, vel, r['cell_num'], float(r['cell_size']), r['channels']).cpu().numpy()
+        assert same_bits(got[0] != 0, ref != 0), r['tag']
+        assert_maps_within_model(got, h[None, :, 0:2], h[None, :, 2:4], r['cell_num'], float(r['cell_size']), r['channels'], r['tag'])
     rng = np.random.RandomState(3)
     for N in (2, 5, 20):
         B = 300
@@ -676,9 +678,8 @@ def test_occupancy_maps_match_reference_and_oracle(cuda_env, oracle):
             got = env.occupancy_maps(torch.from_numpy(pos).to(env.device), torch.from_numpy(vel).to(env.device), 4, 1.0, ch).cpu().numpy()
             ref = oracle.occupancy_maps(pos, vel, 4, 1.0, ch)
             assert (got != 0).sum() > 0                               # the maps are not empty
-            mism = (got != 0) != (ref != 0)
-            assert mism.sum() == 0, (N, ch, int(mism.sum()))
-            assert np.abs(got - ref).max() <= 1e-6
+            for m, what in ((got, 'kernel'), (ref, 'oracle')):
+                assert_maps_within_model(m, pos, vel, 4, 1.0, ch, '%s N=%d ch=%d' % (what, N, ch))
     env = cuda_env(4, 1)
     with pytest.raises(ValueError):
         env.occupancy_maps()                                          # the reference raises for a single human too

@@ -236,12 +236,17 @@ def _reference_il(N, k, robot_safety, multiagent, om=None):
     from crowd_sim.envs.policy.orca import ORCA
     from crowd_nav.utils.explorer import Explorer
 
+    humans = []
+
     class ListMemory(list):
+        """(state, value) pairs; `humans` gets the (px, py, vx, vy) of the human state each pair's rows were built from."""
         def push(self, item):
             self.append(item)
+            humans.append(target.last)
 
     class Target(object):
         def transform(self, state):
+            self.last = [(h.px, h.py, h.vx, h.vy) for h in state.human_states]
             rows = torch.cat([torch.Tensor([state.self_state + h]) for h in state.human_states], dim=0)
             rows = _torch_rotate(rows)
             if om is not None:
@@ -253,16 +258,23 @@ def _reference_il(N, k, robot_safety, multiagent, om=None):
     pol.multiagent_training = multiagent; pol.safety_space = robot_safety
     pol.set_phase('train'); pol.set_env(env1)
     ref_mem = ListMemory()
-    Explorer(env1, robot, torch.device('cpu'), memory=ref_mem, gamma=GAMMA, target_policy=Target()).run_k_episodes(
+    target = Target()
+    Explorer(env1, robot, torch.device('cpu'), memory=ref_mem, gamma=GAMMA, target_policy=target).run_k_episodes(
         k, 'train', update_memory=True, imitation_learning=True)
+    ref_mem.humans = np.array(humans, dtype=np.float64)                 # [pairs][N][4]
     return ref_mem
 
 
-def _assert_matches_reference(mem, ref_mem):
+def _assert_matches_reference(mem, ref_mem, om=None):
+    """The memory against the reference's pairs; with maps, both sides' map columns within the float64 model of the
+    reference's human state."""
     assert len(mem) == len(ref_mem) > 50
     ref_states = torch.stack([s for s, _ in ref_mem]); ref_values = torch.cat([v for _, v in ref_mem])
     assert torch.equal(mem.values[:len(mem), 0].cpu(), ref_values)
-    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, what='IL memory rows')
+    h = ref_mem.humans
+    maps = (h[..., 0:2], h[..., 2:4]) + tuple(om) if om else None
+    assert_rows_match(mem.states[:len(mem)].cpu().numpy(), ref_states.numpy(), False, turned_atol=2e-5, maps=maps,
+                      what='IL memory rows')
 
 
 def test_cadrl_il_matches_single_env_explorer(cuda_env):
@@ -292,7 +304,7 @@ def test_om_sarl_il_matches_single_env_explorer(cuda_env):
     target = types.SimpleNamespace(with_om=True, cell_num=4, cell_size=1.0, om_channel_size=3)
     BatchedExplorer(env, 'orca', memory=mem, gamma=GAMMA, target_policy=target).run_k_episodes(
         k, 'train', update_memory=True, imitation_learning=True, check_every=1)
-    _assert_matches_reference(mem, ref_mem)
+    _assert_matches_reference(mem, ref_mem, om)
 
 
 # ---- the explorer's choice of recorder --------------------------------------------------------------------------------------

@@ -321,7 +321,7 @@ def _shim_vs_oracle(oracle, N, prof):
 def test_occupancy_maps_match_reference(oracle):
     """oracle.occupancy_maps vs the reference's MultiHumanRL.build_occupancy_maps (multi_human_rl.py:109-163) on recorded
     scenes, lookahead states and random crowds, 3 grid configurations x 3 channel modes. The occupancy pattern must be
-    identical; mean velocities agree to float32 rounding (the reference sums Python floats, then casts to float32)."""
+    identical and every map bit for bit: the oracle sums each cell with the reference's plain left fold."""
     rows = load_golden('occupancy_maps')['rows']
     assert len(rows) > 100
     for r in rows:
@@ -330,7 +330,7 @@ def test_occupancy_maps_match_reference(oracle):
         got = oracle.occupancy_maps(h[None, :, 0:2], h[None, :, 2:4], r['cell_num'], float(r['cell_size']), r['channels'])[0]
         assert got.shape == ref.shape, r['tag']
         assert np.array_equal(got != 0, ref != 0), r['tag']
-        assert np.abs(got - ref).max() <= 1e-6, r['tag']
+        assert_same_bits(got, ref, r['tag'])
     assert any(np.array(r['maps'], dtype=np.float64).any() for r in rows)
 
 

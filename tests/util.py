@@ -273,15 +273,200 @@ def assert_rotate_within_model(rows, s, unicycle, robot_ulps=0, what=''):
         return float(np.nanmax(np.where(bound > 0, err / bound, 0.0)))
 
 
-def assert_rows_match(rows, ref, unicycle, robot_ulps=0, turned_atol=0.0, what=''):
-    """Rows [..., 13] against another implementation's rows of the same float32 inputs where the inputs are not at hand:
-    the exact columns bit for bit, the turned columns within turned_atol."""
+def assert_rows_match(rows, ref, unicycle, robot_ulps=0, turned_atol=0.0, maps=None, what=''):
+    """Rows [..., 13 (+ M)] against another implementation's rows of the same float32 inputs where the rotation's inputs
+    are not at hand: the exact columns bit for bit, the turned columns within turned_atol. Occupancy-map columns (13 on)
+    go to assert_maps_within_model when maps = (h_pos, h_vel, cell_num, cell_size, channels) gives the human state they
+    were built from (h_pos / h_vel [..., N, 2] over the rows' leading axes), and are held to turned_atol otherwise."""
     rows = np.asarray(rows, dtype=np.float32); ref = np.asarray(ref, dtype=np.float32)
+    assert rows.shape == ref.shape, '%s: %s vs %s' % (what, rows.shape, ref.shape)
     cols = exact_columns(unicycle, robot_ulps)
     assert_same_bits(rows[..., cols], ref[..., cols], '%s: exact columns %s' % (what, cols))
     turned = turned_columns(unicycle, robot_ulps)
     err = np.abs(rows[..., turned].astype(np.float64) - ref[..., turned])
     assert not (err > turned_atol).any(), '%s: turned columns %s differ by %r > %r' % (what, turned, float(err.max()), turned_atol)
+    if rows.shape[-1] == 13:
+        assert maps is None, what + ': map inputs given for rows without maps'
+        return
+    if maps is not None:
+        h_pos, h_vel, cell_num, cell_size, channels = maps
+        lead = rows.shape[:-2]
+        n = int(np.prod(lead))
+        N = rows.shape[-2]
+        pos = np.asarray(h_pos, dtype=np.float64).reshape(n, N, 2)
+        vel = np.asarray(h_vel, dtype=np.float64).reshape(n, N, 2)
+        for name, r in (('rows', rows), ('reference', ref)):
+            assert_maps_within_model(r[..., 13:].reshape(n, N, -1), pos, vel, cell_num, cell_size, channels,
+                                     what='%s: %s map columns' % (what, name))
+        return
+    err = np.abs(rows[..., 13:].astype(np.float64) - ref[..., 13:])
+    assert not (err > turned_atol).any(), '%s: map columns differ by %r > %r' % (what, float(err.max()), turned_atol)
+
+
+# Occupancy maps (MultiHumanRL.build_occupancy_maps, multi_human_rl.py:109-163; occupancy.cuh). For human i and occupant j:
+#   angle = atan2(vi.y, vi.x); ox, oy = pj - pi; rot = atan2(oy, ox) - angle; dist = sqrt(ox^2 + oy^2)
+#   rx, ry = cos(rot) dist, sin(rot) dist; cell = (floor(rx / cs + half), floor(ry / cs + half)), half = cell_num / 2
+#   vrot = atan2(vj.y, vj.x) - angle; speed = |vj|; (vx, vy) = (cos(vrot), sin(vrot)) speed
+# and each cell's mean is its occupants' sum, a plain left fold from 0.0 in ascending j, over their count, cast to float32.
+# Every operation is float64. ox, oy and the fold's order are the same on every side; atan2 / cos / sin are not correctly
+# rounded. Maximum errors in float64 ulps of the result: CUDA C Programming Guide, double-precision mathematical functions
+# (atan2 2, cos 2, sin 2); glibc's libm and numpy's vectorised loops are within 1 ulp (numpy's array arctan2 differs from
+# libm's atan2 on some inputs). Two sides are therefore at most 3 ulps apart at each such call.
+ULP_OM_TRIG_SIDES = 3
+# The doubles at which the maps call cos / sin when every atan2 argument lies on an axis: 0, +-pi/2 (atan2(y, 0)) and +-pi
+# (atan2(+-0, x < 0)). At +-0 every implementation returns cos = 1 and sin = +-0; at the other four the tests compare
+# CUDA's values with libm's before they treat them as exact.
+SPECIAL_ANGLES = (0.0, np.pi / 2, -np.pi / 2, np.pi, -np.pi)
+
+
+def _atan2_special(y, x):
+    """Whether atan2(y, x) is one of 0, +-pi/2, +-pi by IEEE 754's special cases (an argument is +-0)."""
+    return (y == 0) | (x == 0)
+
+
+def om_model(h_pos, h_vel, cell_num, cell_size):
+    """The occupancy-map computation evaluated in float64 on [B][N][2] position / velocity arrays, with a bound on how far
+    any implementation's intermediate values can be from it. Returns a dict of [B][N][N] arrays over (i, j):
+      xlo, xhi, ylo, yhi  the floor of the lowest and highest value rx / cs + half (ry likewise) can take on any side
+      cell                j's cell index in i's map when determined (xlo == xhi and ylo == yhi, or j out of the grid on
+                          either end), -1 outside the grid, -2 undetermined (j == i: -1)
+      vx, vy, dvx, dvy    j's rotated velocity in i's frame and its bound
+      trig                0: every atan2 result and every cos / sin argument is +-0; 1: they are SPECIAL_ANGLES; 2: other
+    Derivation (u = 2^-53, ulp = ulp64 of the value): angle and atan2(oy, ox) move by ULP_OM_TRIG_SIDES ulps; rot by
+    both plus one rounding on either side (ulp of rot); cos(rot + d) is within |sin| d of cos(rot), plus
+    ULP_OM_TRIG_SIDES ulps of its own; dist = sqrt(fl(ox^2) + fl(oy^2)) carries 2u relative per side (4u between two);
+    the product c dist rounds once per side (ulp); rx / cs and + half once more each (ulp of each result). The velocity
+    terms likewise with atan2(vj), |vj|. The bounds are widened by 1 % for the second-order terms."""
+    pos = np.asarray(h_pos, dtype=np.float64); vel = np.asarray(h_vel, dtype=np.float64)
+    B, N = pos.shape[:2]
+    T = ULP_OM_TRIG_SIDES
+    half = cell_num / 2
+    angle = np.arctan2(vel[..., 1], vel[..., 0])[:, :, None]                          # [B][N][1] over i
+    d_angle = T * ulp64(angle)
+    ox = pos[:, None, :, 0] - pos[:, :, None, 0]; oy = pos[:, None, :, 1] - pos[:, :, None, 1]   # [B][i][j]
+    t = np.arctan2(oy, ox)
+    rot = t - angle
+    d_rot = T * ulp64(t) + d_angle
+    d_rot = d_rot + ulp64(np.abs(rot) + d_rot)
+    dist = np.sqrt(ox * ox + oy * oy)
+    d_dist = 4 * U64 * dist
+    c, s = np.cos(rot), np.sin(rot)
+    dc = np.abs(s) * d_rot + T * ulp64(c)
+    ds = np.abs(c) * d_rot + T * ulp64(s)
+    rx, ry = c * dist, s * dist
+    d_rx = dist * dc + np.abs(c) * d_dist + ulp64(np.abs(rx) + dist * dc)
+    d_ry = dist * ds + np.abs(s) * d_dist + ulp64(np.abs(ry) + dist * ds)
+
+    def grid(r, d):
+        q = r / cell_size
+        d_q = d / cell_size + ulp64(np.abs(q) + d / cell_size)
+        v = q + half
+        d_v = 1.01 * (d_q + ulp64(np.abs(v) + d_q))
+        return np.floor(v - d_v), np.floor(v + d_v)
+
+    xlo, xhi = grid(rx, d_rx)
+    ylo, yhi = grid(ry, d_ry)
+    inside = lambda lo, hi: (lo >= 0) & (hi < cell_num)                              # noqa: E731
+    out = lambda lo, hi: (hi < 0) | (lo >= cell_num)                                  # noqa: E731
+    x_in, y_in = inside(xlo, xhi) & (xlo == xhi), inside(ylo, yhi) & (ylo == yhi)
+    outside = out(xlo, xhi) | out(ylo, yhi)
+    cell = np.where(outside, -1, np.where(x_in & y_in, cell_num * ylo + xlo, -2)).astype(np.int64)
+    eye = np.eye(N, dtype=bool)[None]
+    cell[np.broadcast_to(eye, cell.shape)] = -1
+    tv = np.arctan2(vel[..., 1], vel[..., 0])[:, None, :]                             # [B][1][N] over j
+    vrot = tv - angle
+    d_vrot = T * ulp64(tv) + d_angle
+    d_vrot = d_vrot + ulp64(np.abs(vrot) + d_vrot)
+    speed = np.sqrt(vel[..., 0] * vel[..., 0] + vel[..., 1] * vel[..., 1])[:, None, :]
+    d_speed = 4 * U64 * speed
+    cv, sv = np.cos(vrot), np.sin(vrot)
+    dcv = np.abs(sv) * d_vrot + T * ulp64(cv)
+    dsv = np.abs(cv) * d_vrot + T * ulp64(sv)
+    vx, vy = cv * speed, sv * speed
+    dvx = 1.01 * (speed * dcv + np.abs(cv) * d_speed + ulp64(np.abs(vx) + speed * dcv))
+    dvy = 1.01 * (speed * dsv + np.abs(sv) * d_speed + ulp64(np.abs(vy) + speed * dsv))
+    # the trig class of each (i, j): its atan2 calls' arguments and its cos / sin arguments
+    sp_a = _atan2_special(vel[..., 1], vel[..., 0])[:, :, None]
+    sp_t = _atan2_special(oy, ox)
+    sp_v = _atan2_special(vel[..., 1], vel[..., 0])[:, None, :]
+    special = sp_a & sp_t & sp_v & np.isin(rot, SPECIAL_ANGLES) & np.isin(vrot, SPECIAL_ANGLES)
+    zero = special & (angle == 0) & (t == 0) & (rot == 0) & (tv == 0) & (vrot == 0)
+    trig = np.where(zero, 0, np.where(special, 1, 2))
+    bc = lambda a: np.broadcast_to(a, (B, N, N))                                      # noqa: E731
+    return dict(xlo=xlo, xhi=xhi, ylo=ylo, yhi=yhi, cell=cell, vx=bc(vx), vy=bc(vy), dvx=bc(dvx), dvy=bc(dvy),
+                trig=bc(trig))
+
+
+def _candidates(m, cell_num):
+    """[B][N][N][cells] bool: the cells j can land in on some side (none where j is outside on every side)."""
+    B, N = m['cell'].shape[:2]
+    k = np.arange(cell_num)
+    xs = (k >= m['xlo'][..., None]) & (k <= m['xhi'][..., None])                       # [B][N][N][cell_num]
+    ys = (k >= m['ylo'][..., None]) & (k <= m['yhi'][..., None])
+    cand = (ys[..., :, None] & xs[..., None, :]).reshape(B, N, N, cell_num * cell_num)
+    cand &= (m['cell'] != -1)[..., None]
+    return cand
+
+
+def om_map_model(h_pos, h_vel, cell_num, cell_size, channels):
+    """What any implementation's maps [B][N][cell_num^2 * channels] may hold, from om_model:
+      sure      [B][N][cells] every occupant that can reach the cell is determined (then its occupancy is exact)
+      occupied  [B][N][cells] the model's occupancy where sure
+      lo, hi    [B][N][cells * channels] float32: the interval of float32 values each output can round to
+      trig      [B][N][cells] the largest trig class of any j that can reach the cell (0 when none can)
+    A sure cell's mean is its determined occupants' plain left fold in ascending j, bounded by the sum of their velocity
+    bounds and one rounding per addition on either side (ulp of the partial sum), then over the count (one rounding more
+    per side). An empty sure cell holds +0.0 exactly, and the occupancy channel holds 0.0 / 1.0 exactly."""
+    m = om_model(h_pos, h_vel, cell_num, cell_size)
+    B, N = m['cell'].shape[:2]
+    cells = cell_num * cell_num
+    cand = _candidates(m, cell_num)                                                    # [B][i][j][c]
+    undetermined = (m['cell'] == -2)[..., None] & cand
+    sure = ~undetermined.any(2)                                                        # [B][i][c]
+    trig = np.where(cand, m['trig'][..., None], 0).max(2)
+    onehot = (m['cell'][..., None] == np.arange(cells))                                # [B][i][j][c]
+    count = onehot.sum(2)
+    sums, bounds = [], []
+    for v, d in (('vx', 'dvx'), ('vy', 'dvy')):
+        S = np.zeros((B, N, cells)); D = np.zeros((B, N, cells))
+        for j in range(N):
+            add = onehot[:, :, j]
+            S_new = S + np.where(add, m[v][:, :, j, None], 0.0)
+            D = np.where(add, D + m[d][:, :, j, None] + ulp64(np.abs(S_new) + D + m[d][:, :, j, None]), D)
+            S = S_new
+        with np.errstate(invalid='ignore', divide='ignore'):
+            mean = np.where(count > 0, S / np.maximum(count, 1), 0.0)
+            dm = np.where(count > 0, D / np.maximum(count, 1), 0.0)
+        dm = np.where(count > 0, dm + ulp64(np.abs(mean) + dm), 0.0)
+        sums.append(mean); bounds.append(dm)
+    occ = (count > 0).astype(np.float64)
+    chans = {1: [occ], 2: sums, 3: [occ] + sums}[channels]
+    dchans = {1: [0 * occ], 2: bounds, 3: [0 * occ] + bounds}[channels]
+    val = np.stack(chans, -1).reshape(B, N, cells * channels)
+    dv = np.stack(dchans, -1).reshape(B, N, cells * channels)
+    lo = (val - dv).astype(np.float32); hi = (val + dv).astype(np.float32)
+    return dict(sure=sure, occupied=count > 0, lo=lo, hi=hi, trig=trig)
+
+
+def assert_maps_within_model(maps, h_pos, h_vel, cell_num, cell_size, channels, what=''):
+    """Maps [B][N][cell_num^2 * channels] of the state (h_pos, h_vel) [B][N][2] against om_map_model: on every sure cell
+    the occupancy channel equals the model's bit for bit and each mean lies in its interval of float32 values (an empty
+    cell's means are +0.0); cells an undetermined occupant can reach are skipped. Returns the number of skipped cells."""
+    maps = np.asarray(maps, dtype=np.float32)
+    B, N = np.asarray(h_pos).shape[:2]
+    cells = cell_num * cell_num
+    assert maps.shape == (B, N, cells * channels), '%s: maps %s, want %s' % (what, maps.shape, (B, N, cells * channels))
+    mm = om_map_model(h_pos, h_vel, cell_num, cell_size, channels)
+    sure = np.repeat(mm['sure'], channels, -1)
+    empty = np.repeat(mm['sure'] & ~mm['occupied'], channels, -1)
+    ok = (maps >= mm['lo']) & (maps <= mm['hi']) & ~np.isnan(maps)
+    ok &= ~(empty & (maps.view(np.uint32) != 0))                                       # +0.0, not -0.0
+    bad = sure & ~ok
+    if bad.any():
+        i = tuple(int(x) for x in np.argwhere(bad)[0])
+        raise AssertionError('%s: %d map entries outside the float64 model, first at %s: %r not in [%r, %r]' % (
+            what, int(bad.sum()), i, float(maps[i]), float(mm['lo'][i]), float(mm['hi'][i])))
+    return int((~mm['sure']).sum())
 
 
 def _tuples(rp, rv, ra, rg, th, hp, hv, hr):
