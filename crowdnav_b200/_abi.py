@@ -6,6 +6,11 @@ for its CPU library. No torch types cross the boundary.
 
 STRUCTS and FUNCTIONS describe the whole ABI once: load() applies FUNCTIONS to the product library, declare() to the
 oracle's restatement of some of its entry points, and tests/test_abi_cpu.py checks both tables against the header.
+SCENE_TABLE_STRUCTS / SCENE_TABLE_FUNCTIONS describe include/crowdsim_b200_scene_table.h, the additive header of the
+scene-table entry points, the same way (load() requires and declares them too). They are separate tables because
+tests/test_abi_cpu.py pins crowdsim_b200.h's entry points and structs (31 and 12) and requires STRUCTS / FUNCTIONS to mirror
+exactly that header; tests/test_scene_table_cpu.py checks these tables against the scene-table header and the test oracle's
+restatement (tests/native/scene_table_oracle.c).
 Structs are filled by field name (`Episodes(ep_case=..., ...)`): they have no instance __dict__, so a name that is not
 one of the C fields raises instead of being dropped.
 """
@@ -170,10 +175,31 @@ FUNCTIONS = {
 EXPORTS = tuple(FUNCTIONS)
 
 
+class SceneTableArgs(C.Structure):
+    """crowdsim_scene_table: k scenes of the caller's, handed out through a case queue (crowdsim_reset_table /
+    crowdsim_prefetch_table)."""
+    __slots__ = ()
+    _fields_ = [('h_pos', C.c_void_p), ('h_goal', C.c_void_p), ('h_attr', C.c_void_p), ('rows', C.c_int32),
+                ('case_counter', C.c_void_p), ('case_first', C.c_int32), ('case_total', C.c_int32),
+                ('circle_radius', C.c_double), ('robot_radius', C.c_double), ('robot_v_pref', C.c_double)]
+
+
+# include/crowdsim_b200_scene_table.h, the additive header of the scene-table entry points: described apart from STRUCTS /
+# FUNCTIONS, which must mirror include/crowdsim_b200.h whole (tests/test_abi_cpu.py), and checked against its own header
+# the same way (tests/test_scene_table_cpu.py).
+SCENE_TABLE_STRUCTS = {'crowdsim_scene_table': SceneTableArgs}
+SCENE_TABLE_FUNCTIONS = {
+    'crowdsim_reset_table': (_i, [_P(SceneTableArgs), _v, _i, _i, _P(State), _P(Episodes), STREAM]),
+    'crowdsim_prefetch_table': (_i, [_P(SceneTableArgs), _i, _i, _P(AutoReset), STREAM]),
+}
+SCENE_TABLE_EXPORTS = tuple(SCENE_TABLE_FUNCTIONS)
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
-    """Attach each FUNCTIONS entry's restype / argtypes to the symbol `prefix` + (its name after 'crowdsim_'), where `lib`
-    has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix 'oracle_crowdsim_')."""
-    for name, (restype, argtypes) in FUNCTIONS.items():
+    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
+    'crowdsim_'), where `lib` has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix
+    'oracle_crowdsim_')."""
+    for name, (restype, argtypes) in list(FUNCTIONS.items()) + list(SCENE_TABLE_FUNCTIONS.items()):
         sym = prefix + name[len('crowdsim_'):]
         if hasattr(lib, sym):
             f = getattr(lib, sym)
@@ -203,7 +229,7 @@ def load():
                 'libcrowdsim_b200.so is not built (%s). Run `python -m crowdnav_b200.build` '
                 '(needs nvcc); the product path has no CPU fallback.' % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
-        missing = [name for name in EXPORTS if not hasattr(lib, name)]
+        missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS if not hasattr(lib, name)]
         if missing:
             raise CudaLibraryMissing('%s lacks %s: not a library of ABI version %d' % (LIB_PATH, ', '.join(missing), ABI_VERSION))
         declare(lib)

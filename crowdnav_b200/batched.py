@@ -198,6 +198,97 @@ class ArrivalBuffers(object):
                              snap_h_attr=_ptr(self.snap_h_attr), snap_arrival=_ptr(self.snap_arrival))
 
 
+class SceneTable(object):
+    """k scenes of the caller's own (crowdsim_scene_table): each row holds the start positions, goals and (radius, v_pref)
+    of up to N humans; BatchedCrowdSim.reset_table / enable_autoreset(table=...) hand the rows to env slots through the
+    case queue, and the robot starts as every scene's does (crowd_sim.py:274).
+
+    h_pos, h_goal, h_attr: [k][N][2] float64 arrays; n_humans: [k] humans present per row (default N). Entries i >=
+    n_humans[j] are PARKED, as the `mixed` rule parks the humans a scene lacks: position = goal = (PARKED_X + 100 i,
+    PARKED_X), attributes parked_attr, so human_counts() counts the present ones. Refused (ValueError): arrays of other
+    shapes, N > MAX_HUMANS, non-finite values or a radius <= 0 among the present humans, and a present human whose
+    position or goal is on a parked coordinate (x >= PARKED_X / 2). A table is immutable: its arrays are read-only (the
+    device copy is made once per device); build a new table to change a scene."""
+
+    KEYS = ('h_pos', 'h_goal', 'h_attr', 'n_humans')
+
+    def __init__(self, h_pos, h_goal, h_attr, n_humans=None, parked_attr=(0.3, 1.0)):
+        arrs = [np.array(a, dtype=np.float64) for a in (h_pos, h_goal, h_attr)]
+        if arrs[0].ndim != 3 or arrs[0].shape[2] != 2 or arrs[0].shape[0] < 1:
+            raise ValueError('h_pos must be [k][N][2] with k >= 1, got %s' % (arrs[0].shape,))
+        k, N = arrs[0].shape[:2]
+        for name, a in zip(('h_goal', 'h_attr'), arrs[1:]):
+            if a.shape != (k, N, 2):
+                raise ValueError('%s must be [%d][%d][2] like h_pos, got %s' % (name, k, N, a.shape))
+        if N > _abi.MAX_HUMANS:
+            raise ValueError('%d humans per scene: at most %d' % (N, _abi.MAX_HUMANS))
+        n = np.full(k, N, dtype=np.int64) if n_humans is None else np.array(n_humans).astype(np.int64)
+        if n.shape != (k,) or (n < 0).any() or (n > N).any():
+            raise ValueError('n_humans must be [%d] integers in 0..%d' % (k, N))
+        present = np.arange(N)[None, :] < n[:, None]                               # [k][N]
+        if not all(np.isfinite(a[present]).all() for a in arrs):
+            raise ValueError('scene values must be finite')
+        if not (arrs[2][present][:, 0] > 0).all():
+            raise ValueError('every present human needs a radius > 0')
+        if (arrs[0][present][:, 0] >= _abi.PARKED_X / 2).any() or (arrs[1][present][:, 0] >= _abi.PARKED_X / 2).any():
+            raise ValueError('a present human lies on a parked coordinate (x >= %g)' % (_abi.PARKED_X / 2))
+        park = np.stack([_abi.PARKED_X + 100.0 * np.arange(N), np.full(N, _abi.PARKED_X)], -1)   # [N][2]
+        parked = ~present
+        arrs[0][parked] = np.broadcast_to(park, (k, N, 2))[parked]
+        arrs[1][parked] = np.broadcast_to(park, (k, N, 2))[parked]
+        arrs[2][parked] = np.asarray(parked_attr, dtype=np.float64)
+        self.h_pos, self.h_goal, self.h_attr = (np.ascontiguousarray(a) for a in arrs)
+        self.n_humans = n
+        for a in (self.h_pos, self.h_goal, self.h_attr, self.n_humans):
+            a.setflags(write=False)                 # the validated rows are what device_arrays() uploads, once
+        self.k, self.N = k, N
+        self._dev = {}
+
+    @classmethod
+    def from_scenes(cls, scenes, N, parked_attr=(0.3, 1.0)):
+        """A table from a list of scenes (h_pos, h_goal, h_attr), each [n_i][2] with n_i <= N."""
+        k = len(scenes)
+        h = np.zeros((3, k, N, 2))
+        n = np.zeros(k, dtype=np.int64)
+        for j, sc in enumerate(scenes):
+            rows = [np.asarray(a, dtype=np.float64).reshape(-1, 2) for a in sc]
+            n[j] = rows[0].shape[0]
+            if n[j] > N or any(r.shape[0] != n[j] for r in rows):
+                raise ValueError('scene %d: %s humans for N = %d' % (j, [r.shape[0] for r in rows], N))
+            for a, r in zip(h, rows):
+                a[j, :n[j]] = r
+        return cls(h[0], h[1], h[2], n, parked_attr)
+
+    def save(self, path):
+        """.npz with keys h_pos, h_goal, h_attr (the padded [k][N][2] arrays) and n_humans [k]."""
+        np.savez(path, h_pos=self.h_pos, h_goal=self.h_goal, h_attr=self.h_attr, n_humans=self.n_humans)
+
+    @classmethod
+    def load(cls, path):
+        with np.load(path) as f:
+            missing = [key for key in cls.KEYS if key not in f]
+            if missing:
+                raise ValueError('%s lacks %s' % (path, ', '.join(missing)))
+            h_pos, h_goal, h_attr, n = (f[key] for key in cls.KEYS)
+        parked_attr = (0.3, 1.0)
+        pad = np.arange(h_pos.shape[1])[None, :] >= np.asarray(n)[:, None] if h_pos.ndim == 3 else None
+        if pad is not None and pad.any():
+            parked_attr = tuple(h_attr[pad][0])                      # as saved
+        return cls(h_pos, h_goal, h_attr, n, parked_attr)
+
+    def has_parked(self, first=0, count=None):
+        """Whether any of rows first..first+count-1 lacks humans."""
+        count = self.k - first if count is None else count
+        return bool((self.n_humans[first:first + count] < self.N).any())
+
+    def device_arrays(self, device):
+        """(h_pos, h_goal, h_attr) as float64 tensors on `device`, uploaded once."""
+        device = torch.device(device)
+        if device not in self._dev:
+            self._dev[device] = tuple(torch.from_numpy(np.array(a)).to(device) for a in (self.h_pos, self.h_goal, self.h_attr))
+        return self._dev[device]
+
+
 class BatchedCrowdSim(object):
     def __init__(self, num_envs, device='cuda:0'):
         self.lib = _abi.load()
@@ -223,7 +314,9 @@ class BatchedCrowdSim(object):
         self.arrivals = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
-        self._scene_src = None                      # (rule, from the case queue?) of the scenes the envs now hold
+        self._table = None                          # the SceneTable the case queue counts rows of, or None (generated scenes)
+        self._table_rows = (0, 0)                   # the queue's (first row, rows) with a table
+        self._scene_src = None                      # (rule, from the case queue?) of the scenes the envs now hold; ('table', True) for table rows
         self._draw_bufs = None
 
     # ---- configuration -------------------------------------------------------------------------------------------
@@ -388,6 +481,12 @@ class BatchedCrowdSim(object):
         """crowdsim_reset for the envs selected by `mask` (uint8 device tensor, None = all) from the per-slot seeds.
         With seed_stride != 0 the slot's seed is advanced on device after use; with use_queue the seeds come from the
         shared case queue set up by set_case_queue()."""
+        if self._table is not None:
+            # generated scenes from here on: the table's queue counts rows, not cases, and prefetch() generates again
+            self.clear_table()
+            if use_queue:
+                raise ValueError('the case queue counted the rows of a scene table: set_case_queue over the phase\'s cases '
+                                 'before reset_seeds(use_queue=True)')
         if seeds is not None:
             self.set_seeds(seeds)
         if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
@@ -411,11 +510,24 @@ class BatchedCrowdSim(object):
                 self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
 
     # ---- auto-reset with prefetched scenes -------------------------------------------------------------------------
-    def set_case_queue(self, first_case, total, phase='test'):
+    def set_case_queue(self, first_case, total, phase=None):
         """Shared work queue of `total` cases starting at `first_case` of `phase` (seed = offset[phase] + case):
-        env slots pull the next case on device when their episode ends (Explorer.run_k_episodes with k > slots)."""
+        env slots pull the next case on device when their episode ends (Explorer.run_k_episodes with k > slots).
+        Without `phase`, while a scene table is in use (reset_table, enable_autoreset(table=...)), the queue counts the
+        table's rows instead: entry c is row first_case + c. A `phase` always means the phase's generated cases: a table
+        in use is let go (clear_table). Without either, the cases are the test phase's."""
+        if phase is not None:
+            self.clear_table()
+        elif self._table is None:
+            phase = 'test'
+        if self._table is not None and not (0 <= int(first_case) and int(total) >= 0 and int(first_case) + int(total) <= self._table.k):
+            raise ValueError('rows %d..%d of a table of %d' % (int(first_case), int(first_case) + int(total) - 1, self._table.k))
         self._case_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         self._case_total = int(total)
+        self._table_rows = (int(first_case), int(total))
+        if phase is None:                                    # table rows: no seeds
+            self._seed_base, self._case_first, self._case_wrap = 0, 0, 0
+            return
         size = self.case_size[phase] if self.case_size else 0
         if 0 < size < 2 ** 31:
             # the run may cross the end of the phase's case range: case numbers wrap like crowd_sim.py:283 does
@@ -423,20 +535,92 @@ class BatchedCrowdSim(object):
         else:                                                # train: 2**32 - 2001 cases, no wrap within int32 counters
             self._seed_base, self._case_first, self._case_wrap = (_PHASE_OFFSET[phase] + int(first_case)) % 2 ** 32, 0, 0
 
-    def enable_autoreset(self, rule='circle_crossing', seed_stride=0):
+    def enable_autoreset(self, rule='circle_crossing', seed_stride=0, table=None):
         """Allocate the per-slot next-scene buffers; step() then re-initialises finished envs in the same launch.
-        Call prefetch() (any stream) to (re)fill consumed slots."""
+        Call prefetch() (any stream) to (re)fill consumed slots. table: a SceneTable whose rows the refills copy, in case
+        queue order (set_case_queue then counts its rows; without a queue set yet, one over every row is set up)."""
         self.autoreset = AutoResetBuffers(self.B, self.human_num, self.device, self.circle_radius, self.robot_radius,
                                           self.robot_v_pref)
         self._ar_rule, self._ar_seed_stride = rule, seed_stride
+        if table is not None:
+            self._use_table(table)
+            if self._case_counter is None:
+                self.set_case_queue(0, table.k)
+            self._scene_src = ('table', True)
+            return self.autoreset
+        self.clear_table()                              # generated refills: a table's queue does not count their cases
         # installed scenes come from the case queue; per-slot prefetch seeds are not tracked (policy_draws refuses them)
         self._scene_src = (rule, True) if self._case_counter is not None else (rule, None)
         return self.autoreset
 
     def prefetch(self):
-        a = self._reset_args(None, self._ar_rule, self._ar_seed_stride, True)
         ar = self.autoreset.struct()
+        if self._table is not None:
+            t = self._table_args()
+            self._call('prefetch_table', C.byref(t), self.B, self.human_num, C.byref(ar))
+            return
+        a = self._reset_args(None, self._ar_rule, self._ar_seed_stride, True)
         self._call('prefetch_scenes', C.byref(a), self.B, self.human_num, C.byref(ar))
+
+    # ---- scenes from a table ----------------------------------------------------------------------------------------
+    def _use_table(self, table):
+        if not isinstance(table, SceneTable):
+            raise TypeError('a SceneTable is required, got %s' % type(table).__name__)
+        if table.N != self.human_num:
+            raise ValueError('the table has %d humans per scene, the env %d' % (table.N, self.human_num))
+        if self._table is not table:
+            self._case_counter = None                # a queue over another source's cases does not count these rows
+        self._table = table
+        table.device_arrays(self.device)
+
+    def _table_args(self):
+        """crowdsim_scene_table of the table in use and the case queue."""
+        hp, hg, ha = self._table.device_arrays(self.device)
+        first, total = self._table_rows
+        return _abi.SceneTableArgs(h_pos=_ptr(hp), h_goal=_ptr(hg), h_attr=_ptr(ha), rows=self._table.k,
+                                   case_counter=_ptr(self._case_counter), case_first=first, case_total=total,
+                                   circle_radius=self.circle_radius, robot_radius=self.robot_radius,
+                                   robot_v_pref=self.robot_v_pref)
+
+    def reset_table(self, table, rows=None, mask=None):
+        """crowdsim_reset_table: reset the envs selected by `mask` (uint8, None = all) to rows of `table`, handed out in
+        ascending slot order (with track_episodes; ep_case = the queue entry) from a new case queue over `rows` (a range of
+        consecutive rows or (first, count); None = every row). Slots the queue runs out for go idle. The robot, time,
+        velocities and accumulators are reset as reset() resets them. The table stays in use: set_case_queue counts its
+        rows and, after enable_autoreset(table=table), prefetch() refills from the same queue. When the queue already
+        counts the same rows of this table it starts over in place (a HostStepper's captured refill keeps its counter)."""
+        self._use_table(table)
+        if rows is None:
+            first, count = 0, table.k
+        elif isinstance(rows, range):
+            if rows.step != 1:
+                raise ValueError('rows must be consecutive')
+            first, count = rows.start, len(rows)
+        else:
+            first, count = (int(x) for x in rows)
+        if self._case_counter is not None and self._table_rows == (first, count):
+            self._case_counter.zero_()
+        else:
+            self.set_case_queue(first, count)
+        if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
+            mask = torch.as_tensor(mask).to(device=self.device, dtype=torch.uint8)
+        t = self._table_args()
+        st, ep = self.state.struct(), _struct(self.episodes)
+        self._call('reset_table', C.byref(t), _ptr(mask), self.B, self.human_num, C.byref(st), _ref(ep))
+        self._keep = (mask, t)
+        self._scene_src = ('table', True)
+        if self.arrivals is not None:                   # crowd_sim.py:263-265
+            if mask is None:
+                self.arrivals.h_arrival.zero_()
+            else:
+                self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
+        return self.observation()
+
+    def clear_table(self):
+        """Back to generated scenes: the table is no longer in use and its case queue is dropped (set_case_queue then
+        counts the phase's cases again). reset() / reset_seeds() and enable_autoreset() without a table do this too."""
+        if self._table is not None:
+            self._table, self._case_counter = None, None
 
     # ---- exploration draws from numpy's stream ---------------------------------------------------------------------
     def _stream_bufs(self):
@@ -463,6 +647,9 @@ class BatchedCrowdSim(object):
         if self._scene_src is None:
             raise ValueError('policy_draws needs the envs reset first')
         rule, use_queue = self._scene_src
+        if rule == 'table':
+            raise ValueError('policy_draws follows the seeded generator: scenes from a SceneTable have no seed, so numpy\'s '
+                             'stream after their reset is undefined')
         if use_queue is None:
             raise ValueError('policy_draws follows scenes of the case queue or of reset_seeds, not per-slot auto-reset')
         b = self._stream_bufs()
@@ -734,7 +921,9 @@ class HostStepper(object):
     transfer = 'direct': the kernels read the action from, and write the step's results to, the pinned host buffers
     themselves (unified addressing: the same pointers are valid on the device) -- the same bytes cross the link on every
     step, but as loads / stores of the step and decision kernels instead of two DMA transfers with their fixed set-up cost;
-    the results are visible to the host once the step's event has completed (wait())."""
+    the results are visible to the host once the step's event has completed (wait()).
+    With a scene table in use (env.enable_autoreset(table=...)) the refill branch copies the table's rows instead of
+    generating scenes (env.prefetch())."""
 
     def __init__(self, env, next_orca_action=True, obs='f32', prefetch_every=4, transfer='copy'):
         assert obs in ('f32', 'f64') and transfer in ('copy', 'direct')

@@ -8,8 +8,11 @@
 // without shared memory, a two-warp case assigner, and the multi-step kernel's shared-memory carve-out. The generator
 // (MT, scene.cuh) keeps the seeded MT19937 words it needs in registers and writes only the twisted words, to the slot's
 // column of a global [624][B] scratch (crowdsim_reset_args.scene_mt), so a scene reads no memory for its draws.
+// Scenes of the caller's own (include/crowdsim_b200_scene_table.h) go through the same case assigner and a copy kernel of
+// the scene kernel's shape (table_kernel).
 #include <limits.h>
 #include "scene.cuh"
+#include "../../include/crowdsim_b200_scene_table.h"
 
 namespace cs {
 
@@ -188,6 +191,118 @@ static int launch_scene_kernel(ResetKArgs A, int B, cudaStream_t stream)
     return (int)cudaGetLastError();
 }
 
+// ---- scenes from the caller's table (include/crowdsim_b200_scene_table.h) ----------------------------------------------
+// The same slot protocol and the same slot-order case assignment (assign_cases_kernel, launched on a ResetKArgs that carries
+// only the queue, the mask and the slot flags); the generator is replaced by a copy of the queue entry's table row.
+struct TableKArgs {
+    crowdsim_scene_table t;
+    crowdsim_state st;
+    crowdsim_episodes ep;
+    crowdsim_autoreset ar;
+    const uint8_t *mask;
+    int has_ep, B, N;
+    int *assigned;     // per-slot queue entry written by assign_cases_kernel (ep_case / n_case), or NULL
+};
+
+// The next queue entry of slot e; false when the queue is exhausted.
+__device__ __forceinline__ bool next_entry(const TableKArgs &A, int e, int &c)
+{
+    c = A.assigned ? A.assigned[e] : atomicAdd(A.t.case_counter, 1);
+    return c < A.t.case_total;
+}
+
+// Row case_first + c's humans to one slot's [N][2] arrays, one 16-byte load and store per two-vector.
+__device__ __forceinline__ void copy_row(const crowdsim_scene_table &t, int c, int N, double *hp, double *hg, double *ha)
+{
+    const size_t r = (size_t)(t.case_first + c) * N;
+    for (int i = 0; i < N; ++i) {
+        st2(hp, i, ld2(t.h_pos, r + i)); st2(hg, i, ld2(t.h_goal, r + i)); st2(ha, i, ld2(t.h_attr, r + i));
+    }
+}
+
+// Live-state reset of env e from its row: what reset_env writes, with the humans from the table.
+__device__ __forceinline__ void reset_row(const TableKArgs &A, int e)
+{
+    const crowdsim_scene_table &t = A.t;
+    const int N = A.N;
+    int c;
+    if (!next_entry(A, e, c)) {                              // case queue exhausted: the env goes idle
+        if (A.st.active) A.st.active[e] = 0;
+        if (A.has_ep) A.ep.ep_case[e] = -1;
+        return;
+    }
+    double *hp = A.st.h_pos + (size_t)e * N * 2, *hv = A.st.h_vel + (size_t)e * N * 2;
+    st2(A.st.r_pos, e, make_double2(0.0, -t.circle_radius)); st2(A.st.r_goal, e, make_double2(0.0, t.circle_radius));   // crowd_sim.py:274
+    st2(A.st.r_vel, e, make_double2(0, 0)); st2(A.st.r_attr, e, make_double2(t.robot_radius, t.robot_v_pref));
+    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
+    A.st.g_time[e] = 0.0;
+    copy_row(t, c, N, hp, A.st.h_goal + (size_t)e * N * 2, A.st.h_attr + (size_t)e * N * 2);
+    for (int i = 0; i < N; ++i) st2(hv, i, make_double2(0.0, 0.0));
+    if (A.st.active) A.st.active[e] = 1;
+    if (A.has_ep) {
+        A.ep.ep_steps[e] = 0; A.ep.ep_return[e] = 0.0; A.ep.ep_too_close[e] = 0; A.ep.ep_min_dist_sum[e] = 0.0;
+        A.ep.ep_case[e] = c;
+    }
+}
+
+// Generator side of the auto-reset protocol: fill a CLAIMED next-scene slot from its row, mark it READY (EXHAUSTED past the
+// queue's end).
+__device__ __forceinline__ void prefetch_row(const TableKArgs &A, int e)
+{
+    const crowdsim_autoreset &ar = A.ar;
+    const int N = A.N;
+    int c;
+    if (!next_entry(A, e, c)) {
+        ar.n_case[e] = -1;
+        st_release_u8(ar.n_state + e, CROWDSIM_SLOT_EXHAUSTED);
+        return;
+    }
+    copy_row(A.t, c, N, ar.n_h_pos + (size_t)e * N * 2, ar.n_h_goal + (size_t)e * N * 2, ar.n_h_attr + (size_t)e * N * 2);
+    ar.n_case[e] = c;
+    st_release_u8(ar.n_state + e, CROWDSIM_SLOT_READY);    // row visible before the flag (release at gpu scope)
+}
+
+// scene_kernel's shape (one warp per 32 slots, the k-th slot that needs a scene to lane k, no shared memory), so a table
+// refill fits beside five multi-step blocks per SM like a generated one (DESIGN §3.3).
+template <bool PREFETCH>
+__global__ void __launch_bounds__(32, 32) table_kernel(const __grid_constant__ TableKArgs A)
+{
+    CS_RES_BEGIN
+    const int lane = threadIdx.x, base = blockIdx.x * 32, e = base + lane;
+    // acquire: the consumer's reads of the previous scene happen-before the writes of the next one
+    const bool need = e < A.B && (PREFETCH ? ld_acquire_u8(A.ar.n_state + e) == CROWDSIM_SLOT_CLAIMED
+                                           : !(A.mask && !A.mask[e]));
+    const unsigned bal = __ballot_sync(0xffffffffu, need);
+    if (lane < __popc(bal)) {
+        const int slot = base + (int)__fns(bal, 0, lane + 1);
+        if (PREFETCH) prefetch_row(A, slot); else reset_row(A, slot);
+    }
+#ifdef CS_RESIDENCY_PROBE
+    __syncwarp();                                            // the block ends with its last lane
+#endif
+    CS_RES_END(CS_RES_SCENE);
+}
+
+template <bool PREFETCH>
+static int launch_table_kernel(TableKArgs A, cudaStream_t stream)
+{
+    cudaError_t err = set_carveout<table_kernel<PREFETCH>>();
+    if (err == cudaSuccess) err = set_carveout<assign_cases_kernel<PREFETCH>>();
+    if (err != cudaSuccess) return (int)err;
+    A.assigned = nullptr;
+    if (PREFETCH || A.has_ep) {
+        ResetKArgs Q;
+        memset(&Q, 0, sizeof(Q));
+        Q.a.mask = A.mask; Q.a.case_counter = A.t.case_counter; Q.ar = A.ar; Q.B = A.B; Q.N = A.N;
+        Q.assigned = A.assigned = PREFETCH ? A.ar.n_case : A.ep.ep_case;
+        assign_cases_kernel<PREFETCH><<<1, kAssignThreads, 0, stream>>>(Q);
+        ++g_launches;
+    }
+    table_kernel<PREFETCH><<<(A.B + 31) / 32, 32, 0, stream>>>(A);
+    ++g_launches;
+    return (int)cudaGetLastError();
+}
+
 }  // namespace cs
 
 #ifdef CS_RESIDENCY_PROBE
@@ -231,4 +346,39 @@ extern "C" int crowdsim_prefetch_scenes(const crowdsim_reset_args *args, int B, 
     cs::ResetKArgs A; A.a = *args; A.ar = *ar; A.has_ep = 0; A.B = B; A.N = N;
     memset(&A.st, 0, sizeof(A.st)); memset(&A.ep, 0, sizeof(A.ep));
     return cs::launch_scene_kernel<true>(A, B, (cudaStream_t)stream);
+}
+
+static int check_table(const crowdsim_scene_table *t, int B, int N)
+{
+    if (!t || B < 0 || N < 0) return CROWDSIM_EINVAL;
+    if (!t->h_pos || !t->h_goal || !t->h_attr || !t->case_counter) return CROWDSIM_EINVAL;
+    if (t->rows < 1 || t->case_first < 0 || t->case_total < 0 || (int64_t)t->case_first + t->case_total > t->rows) return CROWDSIM_EINVAL;
+    if (N > CROWDSIM_MAX_HUMANS) return CROWDSIM_EUNSUPPORTED;
+    return CROWDSIM_OK;
+}
+
+extern "C" int crowdsim_reset_table(const crowdsim_scene_table *t, const uint8_t *mask, int B, int N, crowdsim_state *st,
+                                    crowdsim_episodes *ep, void *stream)
+{
+    if (int rc = check_table(t, B, N)) return rc;
+    if (!st) return CROWDSIM_EINVAL;
+    if (N > 0 && (!st->h_pos || !st->h_vel || !st->h_goal || !st->h_attr)) return CROWDSIM_EINVAL;
+    if (!st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr || !st->g_time) return CROWDSIM_EINVAL;
+    if (ep && (!ep->ep_steps || !ep->ep_return || !ep->ep_too_close || !ep->ep_min_dist_sum || !ep->ep_case)) return CROWDSIM_EINVAL;
+    if (B == 0) return CROWDSIM_OK;
+    cs::TableKArgs A; A.t = *t; A.st = *st; A.mask = mask; A.has_ep = ep != nullptr; A.B = B; A.N = N;
+    if (ep) A.ep = *ep; else memset(&A.ep, 0, sizeof(A.ep));
+    memset(&A.ar, 0, sizeof(A.ar));
+    return cs::launch_table_kernel<false>(A, (cudaStream_t)stream);
+}
+
+extern "C" int crowdsim_prefetch_table(const crowdsim_scene_table *t, int B, int N, const crowdsim_autoreset *ar, void *stream)
+{
+    if (int rc = check_table(t, B, N)) return rc;
+    if (!ar) return CROWDSIM_EINVAL;
+    if (!ar->n_state || !ar->n_case || !ar->want || (N > 0 && (!ar->n_h_pos || !ar->n_h_goal || !ar->n_h_attr))) return CROWDSIM_EINVAL;
+    if (B == 0) return CROWDSIM_OK;
+    cs::TableKArgs A; A.t = *t; A.ar = *ar; A.mask = nullptr; A.has_ep = 0; A.B = B; A.N = N;
+    memset(&A.st, 0, sizeof(A.st)); memset(&A.ep, 0, sizeof(A.ep));
+    return cs::launch_table_kernel<true>(A, (cudaStream_t)stream);
 }

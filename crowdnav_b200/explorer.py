@@ -29,6 +29,10 @@ Multi-GPU (torchrun, one process per GPU): the k cases are split into contiguous
 collective; ONE gather of the per-case result rows (48 B per episode: 6 float64 columns; NCCL on GPU tensors, gloo in the CPU tests) brings
 them to rank 0, which prints the log lines.
 
+run_k_episodes(k, phase, scenes=table): the k cases are the rows of a batched.SceneTable (case i = row i) instead of the
+phase's generated scenes, streamed through the same queue and auto-reset (crowdsim_prefetch_table); human times are
+refused when a row parks humans, numpy-stream exploration always (a table scene has no seed).
+
 BatchedExplorer(..., human_times=True): the humans' time to goal after every successful episode (crowd_nav/test.py:105-107,
 "Average time for humans to reach goal"). The step kernels stamp the arrivals and keep each episode's end state
 (BatchedCrowdSim.track_arrivals); after the rollout CrowdSim.get_human_times runs once on device over every ReachGoal case
@@ -173,11 +177,26 @@ class BatchedExplorer(object):
         self.target_model = copy.deepcopy(target_model)
 
     def run_k_episodes(self, k, phase, update_memory=False, imitation_learning=False, episode=None,
-                       print_failure=False, prefetch_every=2, check_every=32, steps_per_launch=8):
+                       print_failure=False, prefetch_every=2, check_every=32, steps_per_launch=8, scenes=None):
+        """scenes: a batched.SceneTable whose rows 0..k-1 are the k cases (case i = row i; rank r of a multi-GPU run takes
+        its contiguous range of rows) instead of the phase's generated scenes; case_counter[phase] is left alone."""
         env = self.env
         if update_memory and (self.memory is None or self.gamma is None):
             raise ValueError('Memory or gamma value is not set!')            # explorer.py:93-94
         rule = env.test_sim if phase == 'test' else env.train_val_sim
+        if scenes is not None:
+            from .batched import SceneTable
+            if not isinstance(scenes, SceneTable):
+                raise TypeError('scenes must be a SceneTable, got %s' % type(scenes).__name__)
+            if not 0 <= k <= scenes.k:
+                raise ValueError('%d cases from a table of %d scenes' % (k, scenes.k))
+            if getattr(self.robot_policy, 'exploration', None) == 'numpy':
+                raise ValueError('exploration from numpy\'s stream follows the seeded generator\'s scenes: table scenes '
+                                 'have no seed')
+            rule = 'table'
+            if self.human_times and scenes.has_parked(0, k):
+                # humans a scene lacks are parked, as for rule mixed
+                raise ValueError('human times are not defined for scenes with parked humans')
         if self.human_times and rule == 'mixed':
             # the reference's own step raises IndexError there (crowd_sim.py:404-407 over a stale human_times, DESIGN §8)
             raise ValueError('human times are not defined for rule mixed')
@@ -187,7 +206,7 @@ class BatchedExplorer(object):
         start, n_local = shard_range(k, self.rank, self.world)
         gamma = self.gamma if self.gamma is not None else 0.9
         args = (env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
-                steps_per_launch, first_case, start, n_local, gamma, rule)
+                steps_per_launch, first_case, start, n_local, gamma, rule, scenes)
         if not self.human_times:
             return self._run(*args)
         prev_arrivals = env.arrivals                   # the caller's arrival tracking, back in place after the run
@@ -198,18 +217,25 @@ class BatchedExplorer(object):
             env.fit_arrival_snapshots()                # (the run replaced the episode rows)
 
     def _run(self, env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
-             steps_per_launch, first_case, start, n_local, gamma, rule):
+             steps_per_launch, first_case, start, n_local, gamma, rule, scenes):
         ep = env.track_episodes(max(n_local, 1), gamma)
         if self.human_times:
             env.track_arrivals(snapshots=True)
-        env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
-        env.enable_autoreset(rule)
+        if scenes is None:
+            env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
+            env.enable_autoreset(rule)
+        else:
+            env.enable_autoreset(table=scenes)
+            env.set_case_queue(start, n_local)         # this rank's rows
         unicycle = self.robot_policy != 'orca' and getattr(self.robot_policy, 'kinematics', 'holonomic') == 'unicycle'
         if self.robot_policy == 'orca':
             env.set_robot_policy('orca')
         else:
             env.set_robot_policy('external_rot' if unicycle else 'external_xy')
-        env.reset_seeds(rule=rule, use_queue=True)
+        if scenes is None:
+            env.reset_seeds(rule=rule, use_queue=True)
+        else:
+            env.reset_table(scenes, rows=(start, n_local))
         recorder = dev_rec = None
         chunk = max(1, int(steps_per_launch))
         if update_memory:
@@ -284,8 +310,11 @@ class BatchedExplorer(object):
             if ok.numel():
                 local_times[ok] = env.case_human_times(ok)[0]
         rows = gather_results(pack_results(ep, n_local, local_times), k, self.rank, self.world, self.group)
-        env.case_counter[phase] = (first_case + k) % env.case_size[phase]
+        if scenes is None:
+            env.case_counter[phase] = (first_case + k) % env.case_size[phase]
         env.autoreset = None
+        if scenes is not None:
+            env.clear_table()
         self.last_rows = rows
         if self.rank != 0:
             return None

@@ -5,7 +5,8 @@ else rl_model.pth), --square / --circle, ORCA's safety space and the run of run_
 print_failure=True), with every case streamed through --num_envs environments on device (BatchedExplorer) and the same
 log lines. --policy is orca (the robot's ORCA runs inside the step kernels) or one of the trainable policies of
 policy.policy_factory. --human_times adds the humans' average time to goal over the successful cases
-(BatchedExplorer(human_times=True)). Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
+(BatchedExplorer(human_times=True)). --scenes FILE.npz runs the scenes of a saved batched.SceneTable, one case per row,
+instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it). Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
 changes nothing: the run is always on cuda:0.
 """
 import argparse
@@ -34,6 +35,7 @@ def parse_args(argv=None):
     parser.add_argument('--traj', default=False, action='store_true')
     parser.add_argument('--num_envs', type=int, default=1024)
     parser.add_argument('--human_times', default=False, action='store_true')
+    parser.add_argument('--scenes', type=str, default=None)
     return parser, parser.parse_args(argv)
 
 
@@ -55,6 +57,8 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
     if args.visualize or args.traj or args.video_file is not None:
         parser.error('rendering (--visualize, --traj, --video_file) is not provided by the batched test driver; '
                      'run the reference\'s test.py for a single rendered case')
+    if args.scenes is not None and (args.square or args.circle):
+        parser.error('--scenes runs the scenes of its file: --square and --circle choose generated scenes')
     if args.policy != 'orca' and args.policy not in policy_factory:
         parser.error('unknown policy %s: orca or one of %s' % (args.policy, ', '.join(sorted(policy_factory))))
 
@@ -99,6 +103,10 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
         policy.set_device(device)
         fit_policy_to_env(policy, env)
         print_info(env, policy.kinematics)
+    if args.scenes is not None:
+        from .batched import SceneTable
+        scenes = SceneTable.load(args.scenes)
+        return explorer.run_k_episodes(scenes.k, args.phase, print_failure=True, scenes=scenes)
     return explorer.run_k_episodes(env.case_size[args.phase], args.phase, print_failure=True)
 
 
