@@ -10,7 +10,8 @@ SCENE_TABLE_STRUCTS / SCENE_TABLE_FUNCTIONS describe include/crowdsim_b200_scene
 scene-table entry points, the same way (load() requires and declares them too). They are separate tables because
 tests/test_abi_cpu.py pins crowdsim_b200.h's entry points and structs (31 and 12) and requires STRUCTS / FUNCTIONS to mirror
 exactly that header; tests/test_scene_table_cpu.py checks these tables against the scene-table header and the test oracle's
-restatement (tests/native/scene_table_oracle.c).
+restatement (tests/native/scene_table_oracle.c). METRICS_STRUCTS / METRICS_FUNCTIONS describe
+include/crowdsim_b200_metrics.h the same way.
 Structs are filled by field name (`Episodes(ep_case=..., ...)`): they have no instance __dict__, so a name that is not
 one of the C fields raises instead of being dropped.
 """
@@ -195,11 +196,29 @@ SCENE_TABLE_FUNCTIONS = {
 SCENE_TABLE_EXPORTS = tuple(SCENE_TABLE_FUNCTIONS)
 
 
+class Metrics(C.Structure):
+    """crowdsim_metrics: per-slot accumulators [B] and per-result-row outputs [k] of path length, closest approach and
+    human-human collisions (crowdsim_step_n_metrics)."""
+    __slots__ = ()
+    _fields_ = [('ep_path', C.c_void_p), ('ep_closest', C.c_void_p), ('ep_hh_steps', C.c_void_p), ('ep_hh_pairs', C.c_void_p),
+                ('res_path', C.c_void_p), ('res_closest', C.c_void_p), ('res_hh_steps', C.c_void_p),
+                ('res_hh_pairs', C.c_void_p)]
+
+
+# include/crowdsim_b200_metrics.h, the additive header of the episode metrics: described apart for the same reason as the
+# scene-table tables, and checked against its own header (tests/test_metrics_cpu.py).
+METRICS_STRUCTS = {'crowdsim_metrics': Metrics}
+METRICS_FUNCTIONS = {
+    'crowdsim_step_n_metrics': (_i, _STEP + [_i, _P(Arrivals), _P(Metrics), STREAM]),
+}
+METRICS_EXPORTS = tuple(METRICS_FUNCTIONS)
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
-    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
+    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
     'crowdsim_'), where `lib` has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix
     'oracle_crowdsim_')."""
-    for name, (restype, argtypes) in list(FUNCTIONS.items()) + list(SCENE_TABLE_FUNCTIONS.items()):
+    for name, (restype, argtypes) in list(FUNCTIONS.items()) + list(SCENE_TABLE_FUNCTIONS.items()) + list(METRICS_FUNCTIONS.items()):
         sym = prefix + name[len('crowdsim_'):]
         if hasattr(lib, sym):
             f = getattr(lib, sym)
@@ -229,7 +248,7 @@ def load():
                 'libcrowdsim_b200.so is not built (%s). Run `python -m crowdnav_b200.build` '
                 '(needs nvcc); the product path has no CPU fallback.' % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
-        missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS if not hasattr(lib, name)]
+        missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS + METRICS_EXPORTS if not hasattr(lib, name)]
         if missing:
             raise CudaLibraryMissing('%s lacks %s: not a library of ABI version %d' % (LIB_PATH, ', '.join(missing), ABI_VERSION))
         declare(lib)

@@ -11,6 +11,7 @@ Mirrors the reference environment's surface for a batch (paths relative to the r
 There is no CPU fallback: without the CUDA library / a GPU these calls raise.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -198,6 +199,37 @@ class ArrivalBuffers(object):
                              snap_h_attr=_ptr(self.snap_h_attr), snap_arrival=_ptr(self.snap_arrival))
 
 
+class MetricsBuffers(object):
+    """crowdsim_metrics (include/crowdsim_b200_metrics.h): each slot's running path length, closest approach and
+    human-human collision counts, and the same four per result row of k, written when an episode ends."""
+
+    COLUMNS = ('hh_steps', 'hh_pairs', 'path', 'closest')
+
+    def __init__(self, B, k, device):
+        f64 = lambda n: torch.zeros(n, dtype=torch.float64, device=device)  # noqa: E731
+        i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=device)  # noqa: E731
+        self.k = k
+        self.ep_path, self.ep_closest = f64(B), torch.full((B,), math.inf, dtype=torch.float64, device=device)
+        self.ep_hh_steps, self.ep_hh_pairs = i32(B), i32(B)
+        self.res_path, self.res_closest = f64(k), torch.full((k,), math.inf, dtype=torch.float64, device=device)
+        self.res_hh_steps, self.res_hh_pairs = i32(k), i32(k)
+
+    def clear(self, mask=None):
+        """A fresh episode's accumulators for the slots of `mask` (uint8, None = all), as a reset leaves them."""
+        sel = slice(None) if mask is None else (mask != 0)
+        for t, v in ((self.ep_path, 0.0), (self.ep_closest, math.inf), (self.ep_hh_steps, 0), (self.ep_hh_pairs, 0)):
+            if mask is None:
+                t.fill_(v)
+            else:
+                t.masked_fill_(sel, v)
+
+    def struct(self):
+        return _abi.Metrics(ep_path=_ptr(self.ep_path), ep_closest=_ptr(self.ep_closest), ep_hh_steps=_ptr(self.ep_hh_steps),
+                            ep_hh_pairs=_ptr(self.ep_hh_pairs), res_path=_ptr(self.res_path),
+                            res_closest=_ptr(self.res_closest), res_hh_steps=_ptr(self.res_hh_steps),
+                            res_hh_pairs=_ptr(self.res_hh_pairs))
+
+
 class SceneTable(object):
     """k scenes of the caller's own (crowdsim_scene_table): each row holds the start positions, goals and (radius, v_pref)
     of up to N humans; BatchedCrowdSim.reset_table / enable_autoreset(table=...) hand the rows to env slots through the
@@ -312,6 +344,7 @@ class BatchedCrowdSim(object):
         self.neighbor_dist = 10.0; self.max_neighbors = 10; self.time_horizon = 5.0
         self.state = None; self.episodes = None; self.autoreset = None
         self.arrivals = None
+        self.metrics = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
         self._table = None                          # the SceneTable the case queue counts rows of, or None (generated scenes)
@@ -368,6 +401,7 @@ class BatchedCrowdSim(object):
         # run on this batch's streams one after the other, so they share it
         self._scene_mt = torch.empty((624, B), dtype=torch.int32, device=self.device)
         self.arrivals = None
+        self.metrics = None
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -393,7 +427,39 @@ class BatchedCrowdSim(object):
         self.episodes = EpisodeBuffers(self.B, k, self.device, gamma, self.time_step, self.robot_v_pref,
                                        max_steps=max_episode_steps(self.time_limit, self.time_step))
         self.fit_arrival_snapshots()
+        if self.metrics is not None and self.metrics.k != k:
+            self.fit_metrics()
         return self.episodes
+
+    def fit_metrics(self):
+        """The metric rows of track_metrics are indexed by result row: after the episode rows change (track_episodes), give
+        them as many rows, keeping the slots' running accumulators."""
+        m = self.metrics
+        self.metrics = MetricsBuffers(self.B, self.episodes.k, self.device)
+        for f in ('ep_path', 'ep_closest', 'ep_hh_steps', 'ep_hh_pairs'):
+            getattr(self.metrics, f).copy_(getattr(m, f))
+
+    # ---- episode metrics ----------------------------------------------------------------------------------------------
+    def track_metrics(self):
+        """Measure every episode's robot path length, closest approach and human-human collisions from now on
+        (crowdsim_step_n_metrics, include/crowdsim_b200_metrics.h). Needs track_episodes: an episode's metrics go to its
+        result row (metrics.res_*). Every slot starts a fresh episode's accumulators; reset and auto-reset installs clear
+        them again. Recorded rollouts refuse tracked metrics."""
+        if self.episodes is None:
+            raise ValueError('metrics are kept per result row: track_episodes first')
+        self.metrics = MetricsBuffers(self.B, self.episodes.k, self.device)
+        return self.metrics
+
+    def _clear_slots(self, mask):
+        """What a reset clears beside the state and the episode accumulators: arrival stamps (crowd_sim.py:263-265) and
+        the metrics accumulators."""
+        if self.arrivals is not None:
+            if mask is None:
+                self.arrivals.h_arrival.zero_()
+            else:
+                self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
+        if self.metrics is not None:
+            self.metrics.clear(mask)
 
     def fit_arrival_snapshots(self):
         """The end snapshots of track_arrivals(snapshots=True) are indexed by result row: after the episode rows change
@@ -503,11 +569,7 @@ class BatchedCrowdSim(object):
         st, ep = self.state.struct(), _struct(self.episodes)
         self._call('reset', C.byref(a), self.B, self.human_num, C.byref(st), _ref(ep))
         self._keep = (mask, a)
-        if self.arrivals is not None:                   # crowd_sim.py:263-265
-            if mask is None:
-                self.arrivals.h_arrival.zero_()
-            else:
-                self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
+        self._clear_slots(mask)
 
     # ---- auto-reset with prefetched scenes -------------------------------------------------------------------------
     def set_case_queue(self, first_case, total, phase=None):
@@ -609,11 +671,7 @@ class BatchedCrowdSim(object):
         self._call('reset_table', C.byref(t), _ptr(mask), self.B, self.human_num, C.byref(st), _ref(ep))
         self._keep = (mask, t)
         self._scene_src = ('table', True)
-        if self.arrivals is not None:                   # crowd_sim.py:263-265
-            if mask is None:
-                self.arrivals.h_arrival.zero_()
-            else:
-                self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
+        self._clear_slots(mask)
         return self.observation()
 
     def clear_table(self):
@@ -695,6 +753,8 @@ class BatchedCrowdSim(object):
         (no actions); with an external robot one step with `actions` (n_steps = 1), booked around it by crowdsim_record_book
         and its rows staged by pack_joint (a recorder with sort_humans=True: LSTM-RL's sorted rows and, with maps, the
         sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full."""
+        if record is not None and self.metrics is not None:
+            raise ValueError('recorded rollouts do not measure episode metrics: track_metrics is for rollouts without a recorder')
         if record is not None and getattr(record, 'rl', False):
             return self._step_record_rl(actions, int(n_steps), record)
         if record is not None and self.arrivals is not None:
@@ -718,7 +778,14 @@ class BatchedCrowdSim(object):
         prm, st, io = self.params(), self.state.struct(), self._io()
         head = (C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(_struct(self.episodes)),
                 _ref(_struct(self.autoreset)), int(n_steps))
-        if self.arrivals is not None:
+        if self.metrics is not None:
+            if self.episodes is None or self.metrics.k != self.episodes.k:
+                # the kernels write row ep_case of arrays the C struct does not size: never past their end
+                raise ValueError('metric rows: %d, the episode results %s'
+                                 % (self.metrics.k, None if self.episodes is None else self.episodes.k))
+            arr = None if self.arrivals is None else C.byref(self.arrivals.struct())
+            self._call('step_n_metrics', *head, arr, C.byref(self.metrics.struct()))
+        elif self.arrivals is not None:
             self._call('step_n_arrivals', *head, C.byref(self.arrivals.struct()))
         else:
             self._call('step_n', *head)

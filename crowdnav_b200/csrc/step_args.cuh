@@ -3,6 +3,7 @@
 #pragma once
 #include <type_traits>
 #include "crowdsim_common.cuh"
+#include "../../include/crowdsim_b200_metrics.h"
 
 namespace cs {
 
@@ -46,10 +47,72 @@ struct StepArgs {
     crowdsim_arrivals arr;       // crowdsim_step_n_arrivals: read only by the ARR instantiations; last for the same reason
 };
 
+// crowdsim_step_n_metrics: the argument block of the MET instantiations. A struct of its own, not a StepArgs field, so that
+// the parameter block of every other kernel (and the offsets of the recording kernels' arguments after it) stays as it was.
+struct StepArgsMet : StepArgs {
+    crowdsim_metrics met;
+};
+template <bool MET>
+using StepArgsT = typename std::conditional<MET, StepArgsMet, StepArgs>::type;
+
+// ---- MET = true (include/crowdsim_b200_metrics.h): one env's running accumulators ----
+struct MetAcc {
+    double path, closest;
+    int hh_steps, hh_pairs;
+};
+__device__ __forceinline__ MetAcc met_load(const crowdsim_metrics &m, int e)
+{
+    return MetAcc{ m.ep_path[e], m.ep_closest[e], m.ep_hh_steps[e], m.ep_hh_pairs[e] };
+}
+__device__ __forceinline__ void met_store(const crowdsim_metrics &m, int e, const MetAcc &a)
+{
+    m.ep_path[e] = a.path; m.ep_closest[e] = a.closest; m.ep_hh_steps[e] = a.hh_steps; m.ep_hh_pairs[e] = a.hh_pairs;
+}
+__device__ __forceinline__ void met_result(const crowdsim_metrics &m, int c, const MetAcc &a)
+{
+    m.res_path[c] = a.path; m.res_closest[c] = a.closest; m.res_hh_steps[c] = a.hh_steps; m.res_hh_pairs[c] = a.hh_pairs;
+}
+__device__ __forceinline__ MetAcc met_fresh()
+{
+    return MetAcc{ 0.0, __longlong_as_double(0x7ff0000000000000LL), 0, 0 };
+}
+// One live step: the robot's displacement pos -> npos (test.py:92-97, numpy's 2-norm), the step's dmin, and the number of
+// overlapping human pairs.
+__device__ __forceinline__ void met_add(MetAcc &a, double2 pos, double2 npos, double dmin, int pairs)
+{
+    a.path = a.path + norm2(npos.x - pos.x, npos.y - pos.y);
+    if (dmin < a.closest) a.closest = dmin;
+    a.hh_steps += (pairs > 0) ? 1 : 0;
+    a.hh_pairs += pairs;
+}
+// MET = true: per env of the block, the step's count of overlapping human pairs (humans add, the robot reads) and, in the
+// multi-step kernel, the running accumulators. Declared only by the MET instantiations.
+template <int E>
+__device__ __forceinline__ int *met_hh_smem()
+{
+    __shared__ int s_hh[E];
+    return s_hh;
+}
+template <int E>
+__device__ __forceinline__ MetAcc *met_acc_smem()
+{
+    __shared__ MetAcc s_ma[E];
+    return s_ma;
+}
+// crowd_sim.py:353-362, the reference's pair test on pre-step positions, i < j (the library is built without FMA contraction,
+// so every product, sum and difference is rounded once). The reference writes (dx ** 2 + dy ** 2) ** (1 / 2), which is
+// glibc's pow: it is not x * x and sqrt bit for bit (the distance differs in about 0.13 % of the pairs of the reference
+// suites). There is no device pow, so within about an ulp of touching this decision can differ from the reference's.
+__device__ __forceinline__ bool hh_overlap(double2 pi, double ri, double2 pj, double rj)
+{
+    const double dx = pi.x - pj.x, dy = pi.y - pj.y;
+    return sqrt(dx * dx + dy * dy) - ri - rj < 0;
+}
+
 // Launch a multi-step kernel after setting its shared-memory carve-out (crowdsim_common.cuh). A carve-out error is
 // returned before anything is launched.
-template <auto Kernel>
-inline int launch_carved(const StepArgs &A, int blocks, int threads, cudaStream_t stream)
+template <auto Kernel, class Args>
+inline int launch_carved(const Args &A, int blocks, int threads, cudaStream_t stream)
 {
     if (const cudaError_t err = set_carveout<Kernel>()) return (int)err;
     Kernel<<<blocks, threads, 0, stream>>>(A);
@@ -117,6 +180,14 @@ static inline int check_arrivals(const crowdsim_arrivals *r, const crowdsim_epis
     if (!r->h_arrival) return CROWDSIM_EINVAL;
     const int snaps = !!r->snap_r_vel + !!r->snap_h_pos + !!r->snap_h_vel + !!r->snap_h_goal + !!r->snap_h_attr + !!r->snap_arrival;
     if (snaps != 0 && (snaps != 6 || !ep)) return CROWDSIM_EINVAL;
+    return CROWDSIM_OK;
+}
+
+// crowdsim_step_n_metrics' argument rules (include/crowdsim_b200_metrics.h).
+static inline int check_metrics(const crowdsim_metrics *m, const crowdsim_episodes *ep)
+{
+    if (!m || !ep || !m->ep_path || !m->ep_closest || !m->ep_hh_steps || !m->ep_hh_pairs || !m->res_path || !m->res_closest ||
+        !m->res_hh_steps || !m->res_hh_pairs) return CROWDSIM_EINVAL;
     return CROWDSIM_OK;
 }
 

@@ -44,6 +44,9 @@ namespace cs {
 // precision cos / sin / fmod code (12 % of the round-1 kernel's SASS) is only present in the kernels that execute it.
 // ARR: crowdsim_step_n_arrivals -- the humans stamp their arrivals and write the end snapshot of a finished episode
 // (step_args.cuh); ARR = false compiles to the SASS the kernel had before ARR.
+// MET: crowdsim_step_n_metrics -- the robot lane keeps its env's metrics accumulators (include/crowdsim_b200_metrics.h) in
+// registers; the human pairs (a, a + d) are tested on lane a, one ballot per d. MET = false compiles to the SASS the kernel
+// had before MET.
 #ifndef CS_FLAT_WPB
 #define CS_FLAT_WPB 4
 #endif
@@ -62,9 +65,9 @@ struct RobotRec {
     uint8_t want, o_done, any_live, dirty_ep, new_case;
 };
 
-template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false>
+template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false, bool MET = false>
 __global__ void __launch_bounds__(32 * CS_FLAT_WPB, CS_FLAT_MINBLOCKS * 4 / CS_FLAT_WPB)
-step_flat_kernel(const __grid_constant__ StepArgs A)
+step_flat_kernel(const __grid_constant__ StepArgsT<MET> A)
 {
     if constexpr (STAGE == 0) return;
     using namespace orca;
@@ -112,6 +115,8 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             rr = r0;
         }
     }
+    MetAcc ma = {};                                         // MET: robot lane of a valid env
+    if constexpr (MET) { if (env_ok && is_robot) ma = met_load(A.met, e); }
     if constexpr (STAGE == 1) {            // loads + stores only
         const bool live1 = env_ok && (act_flag != 0);
         if (live1 && !is_robot) { st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, make_double2(vel.x + goal.x * 0, vel.y + attr.x * 0)); }
@@ -261,6 +266,19 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         const double ci = __shfl_sync(CS_FULL, closest, ebase + i);
         if (!collision) { if (ci < 0) collision = true; else if (ci < dmin) dmin = ci; }
     }
+    // MET: the env's overlapping human pairs on the pre-step positions (crowd_sim.py:353-362), consumed by the robot lane
+    int hh_pairs = 0;
+    if constexpr (MET) {
+        const unsigned env_mask = ((1u << N) - 1u) << ebase;
+        #pragma unroll
+        for (int d = 1; d < N; ++d) {
+            const int src = (lane + d < 32) ? lane + d : lane;
+            const double qx = __shfl_sync(CS_FULL, pos.x, src), qy = __shfl_sync(CS_FULL, pos.y, src);
+            const double qr = __shfl_sync(CS_FULL, attr.x, src);
+            const bool hit = live && !is_robot && a + d < N && hh_overlap(pos, attr.x, make_double2(qx, qy), qr);
+            hh_pairs += __popc(__ballot_sync(CS_FULL, hit) & env_mask);
+        }
+    }
 
     // ---- robot lane: ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72);
     // decides about auto-reset ----
@@ -271,6 +289,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         if (live) {
             const double2 npos = robot_position(ROT, pos, theta, ax, ay, dt);
             const bool reaching_goal = norm2(npos.x - goal.x, npos.y - goal.y) < attr.x;
+            if constexpr (MET) met_add(ma, pos, npos, dmin, hh_pairs);
             const double gtime = rr.gtime;
             double reward;
             const int info = reward_ladder(gtime >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
@@ -290,9 +309,11 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                 if (info == CROWDSIM_INFO_DANGER) { ep_tc += 1; ep_mds += dmin; ep.ep_too_close[e] = ep_tc; ep.ep_min_dist_sum[e] = ep_mds; }
                 rr.ep_t = ep_t; rr.ep_tc = ep_tc; rr.ep_ret = ep_ret; rr.ep_mds = ep_mds;
                 ep.ep_return[e] = ep_ret; ep.ep_steps[e] = ep_t;
+                if constexpr (MET) met_store(A.met, e, ma);
                 if (done) {
                     const int ep_c = rr.ep_c;
                     if (ep_c >= 0) {
+                        if constexpr (MET) met_result(A.met, ep_c, ma);
                         ep.res_info[ep_c] = (uint8_t)info; ep.res_steps[ep_c] = ep_t;
                         ep.res_time[ep_c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
@@ -332,8 +353,10 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         install = __shfl_sync(CS_FULL, install, rl) && env_ok;
         // the scene goes straight from the slot to the live state (ar_install_*: acquire on the slot flag, copy)
         if (install) {
-            if (is_robot) ar_install_robot(A, e);
-            else {
+            if (is_robot) {
+                ar_install_robot(A, e);
+                if constexpr (MET) met_store(A.met, e, met_fresh());
+            } else {
                 ar_install_human(A, e, N, a);
                 if constexpr (ARR) A.arr.h_arrival[hi] = 0.0;                       // crowd_sim.py:263-265
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, hi); reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }

@@ -38,8 +38,11 @@ namespace cs {
 // MID = true: the crowd kernel for N > 5 (step_mid.cuh: register-resident lines, speculative LPs, compacted lp3).
 // ARR = true: crowdsim_step_n_arrivals (the humans stamp their arrivals and write a finished episode's end snapshot,
 // step_args.cuh); ARR = false compiles to the SASS the kernel had before ARR.
-template <bool MID, bool ARR = false>
-__global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgs A)
+// MET = true: crowdsim_step_n_metrics (include/crowdsim_b200_metrics.h): the env's human lanes test its pairs in N / 2 rounds,
+// counted with a ballot per round and added to a shared counter; the robot lane books them with the path length and dmin. MET = false compiles to
+// the SASS the kernel had before MET. (At most 128 envs per block: N = 0.)
+template <bool MID, bool ARR = false, bool MET = false>
+__global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgsT<MET> A)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_qcount;
@@ -54,6 +57,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
     const bool is_robot = (a == N);
     bool live = (e < A.B);
     if (live && A.st.active) live = (A.st.active[e] != 0);
+    if constexpr (MET) { if (is_robot) met_hh_smem<128>()[le] = 0; }
 
     // ---- load own agent (coalesced 16-byte loads) and stage it ----
     double2 pos = make_double2(0, 0), vel = pos, goal = pos, attr = pos;
@@ -99,6 +103,28 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
     // ---- human lanes: swept-segment clearance against the robot ----
     const double dt = k.time_step;
     if (live && !is_robot) s.closest[tid] = swept_clearance(pos, vel, s.pos64[le * L + N], s.act[le], attr.x, s.rad64[le * L + N], dt);
+    if constexpr (MET) {
+        // crowd_sim.py:353-362 on the pre-step positions. Round d pairs human a with human (a + d) mod N: rounds 1 .. N / 2
+        // cover every pair once (the last round of an even N only from a < N / 2), so every human lane tests at most
+        // N / 2 pairs. One ballot per round over the block's threads in this warp; the first lane of my env's humans in this
+        // warp adds their hits (an env may straddle two warps).
+        const int wbase = tid & ~31, wn = (T - wbase < 32) ? T - wbase : 32;
+        const unsigned wmask = (wn == 32) ? 0xffffffffu : (1u << wn) - 1u;
+        const int lo = max(le * L, wbase), hi = min(le * L + N, wbase + 32);       // my env's human threads in my warp
+        const unsigned envm = (hi <= lo) ? 0u : ((hi - lo == 32) ? 0xffffffffu : (((1u << (hi - lo)) - 1u) << (lo - wbase)));
+        int c = 0;
+        for (int d = 1; d <= N / 2; ++d) {
+            bool hit = false;
+            if (live && !is_robot && (2 * d < N || a < d)) {
+                const int j = (a + d < N) ? a + d : a + d - N;
+                const double2 pj = s.pos64[le * L + j];
+                const double rj = s.rad64[le * L + j];
+                hit = (a < j) ? hh_overlap(pos, attr.x, pj, rj) : hh_overlap(pj, rj, pos, attr.x);   // r_i, then r_j (i < j)
+            }
+            c += __popc(__ballot_sync(wmask, hit) & envm);
+        }
+        if (c && tid == lo) atomicAdd(&met_hh_smem<128>()[le], c);
+    }
     __syncthreads();
 
     // ---- robot lane: reduce clearances, ladder, update, bookkeeping; decides about auto-reset ----
@@ -117,6 +143,8 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
             const bool rot = k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT;
             const double2 npos = robot_position(rot, pos, theta, ax, ay, dt);
             const bool reaching_goal = norm2(npos.x - goal.x, npos.y - goal.y) < attr.x;    // crowd_sim.py:365-366
+            MetAcc ma = {};
+            if constexpr (MET) { ma = met_load(A.met, e); met_add(ma, pos, npos, dmin, met_hh_smem<128>()[le]); }
             double reward;
             const int info = reward_ladder(gtime >= k.time_limit - 1, collision, reaching_goal, dmin, k, dt, reward);
             done = ends_episode(info);
@@ -140,9 +168,11 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
                 int tc = ep.ep_too_close[e]; double mds = ep.ep_min_dist_sum[e];
                 if (info == CROWDSIM_INFO_DANGER) { tc += 1; mds += dmin; ep.ep_too_close[e] = tc; ep.ep_min_dist_sum[e] = mds; }
                 ep.ep_return[e] = ret; ep.ep_steps[e] = t + 1;
+                if constexpr (MET) met_store(A.met, e, ma);
                 if (done) {
                     const int c = ep.ep_case[e];
                     if (c >= 0) {
+                        if constexpr (MET) met_result(A.met, c, ma);
                         ep.res_info[c] = (uint8_t)info; ep.res_steps[c] = t + 1;
                         ep.res_time[c] = (info == CROWDSIM_INFO_TIMEOUT) ? k.time_limit : ntime;
                         ep.res_return[c] = ret; ep.res_too_close[c] = tc; ep.res_min_dist_sum[c] = mds;
@@ -171,8 +201,10 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
         __syncthreads();
         install = (s.closest[le * L + N] != 0.0) && env_ok;
         if (install) {
-            if (is_robot) ar_install_robot(A, e);
-            else {
+            if (is_robot) {
+                ar_install_robot(A, e);
+                if constexpr (MET) met_store(A.met, e, met_fresh());
+            } else {
                 ar_install_human(A, e, N, a);
                 if constexpr (ARR) A.arr.h_arrival[(size_t)e * N + a] = 0.0;      // crowd_sim.py:263-265
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, (size_t)e * N + a); reinterpret_cast<float4 *>(A.io.obs32)[(size_t)e * N + a] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
@@ -262,6 +294,7 @@ struct StepMode {
     bool act_only = false;                          // crowdsim_orca_act: the robot's ORCA decision only, nothing mutated
     double *la_pos = nullptr, *la_vel = nullptr;    // crowdsim_onestep_lookahead: the humans' next states go here
     const crowdsim_arrivals *arr = nullptr;         // crowdsim_step_n_arrivals: the ARR instantiations
+    const crowdsim_metrics *met = nullptr;          // crowdsim_step_n_metrics: the MET instantiations (arr optional)
     const crowdsim_record *rec = nullptr;           // crowdsim_step_n_record*: stage the steps for an IL recorder
     bool rec_any_route = false;                     // _ex / _rot: every N >= 1, through the launch loop off the multi route
     bool rec_rot = false;                           // _rot: the rows of a unicycle robot
@@ -274,6 +307,7 @@ static int check(const crowdsim_params *prm, int B, int N, const crowdsim_state 
 {
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
     if (m.arr) { const int rc = check_arrivals(m.arr, ep); if (rc != CROWDSIM_OK) return rc; }
+    if (m.met) { const int rc = check_metrics(m.met, ep); if (rc != CROWDSIM_OK) return rc; }
     if (const crowdsim_record *rec = m.rec) {
         // crowdsim_step_n_record: only the recording instantiation of the multi-step kernel records. crowdsim_step_n_record_ex
         // (rec_any_route): every N >= 1, through the launch loop where the multi-step kernel does not run
@@ -323,6 +357,14 @@ static Route route(const StepArgs &A, int n_steps, bool rec)
     return Route::flat;
 }
 
+// The argument block of a kernel instantiation: StepArgs, or StepArgsMet for the MET ones.
+template <bool MET>
+static const StepArgsT<MET> &args_for(const StepArgs &A, const StepArgsMet &AM)
+{
+    if constexpr (MET) return AM;
+    else return A;
+}
+
 // n_steps single-step launches, each staged and booked by the recording around it when m.rec is set.
 template <class StepOnce>
 static int launch_loop(const StepArgs &A, int n_steps, const StepMode &m, cudaStream_t stream, StepOnce &&step_once)
@@ -355,7 +397,9 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if (m.rec) A.rec = *m.rec; else memset(&A.rec, 0, sizeof(A.rec));
     if (m.recm) A.recm = *m.recm; else memset(&A.recm, 0, sizeof(A.recm));
     if (m.arr) A.arr = *m.arr; else memset(&A.arr, 0, sizeof(A.arr));
-    const bool arr = (m.arr != nullptr);
+    const bool arr = (m.arr != nullptr), met = (m.met != nullptr);
+    StepArgsMet AM;
+    if (met) { AM.met = *m.met; }
     switch (route(A, n_steps, m.rec != nullptr)) {
     case Route::act:
         with_int<1, 5>(N, [&](auto n) { orca_act_kernel<n><<<(B + 127) / 128, 128, 0, stream>>>(A); });
@@ -365,8 +409,10 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
         if (m.rec) { ++g_launches; return launch_multi_record(A, blocks, stream, m.rec_rot); }
+        if (met) static_cast<StepArgs &>(AM) = A;
         const int err = with_int<2, 5>(N, [&](auto n) { return with_bool(A.k.robot_visible, [&](auto vis) { return with_bool(arr, [&](auto ar_on) {
-            return launch_carved<step_multi_kernel<n, vis, false, false, ar_on>>(A, blocks, 32 * (n + 1), stream); }); }); });
+            return with_bool(met, [&](auto met_on) {
+                return launch_carved<step_multi_kernel<n, vis, false, false, ar_on, met_on>>(args_for<met_on>(A, AM), blocks, 32 * (n + 1), stream); }); }); }); });
         if (err != CROWDSIM_OK) return err;
         ++g_launches;
         return (int)cudaGetLastError();
@@ -381,23 +427,27 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         // The threshold scales with the device's SM count; scripts/latency_probe.cu times both. The unicycle robot's
         // kernel exists with the per-warp queue only.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        return launch_loop(A, n_steps, m, stream, [&] { with_int<1, 5>(N, [&](auto n) { with_bool(arr, [&](auto ar_on) {
-            if (rot) step_flat_kernel<n, 99, true, true, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
-            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
-            else step_flat_kernel<n, 99, false, false, ar_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); }); }); });
+        if (met) static_cast<StepArgs &>(AM) = A;
+        return launch_loop(A, n_steps, m, stream, [&] { with_int<1, 5>(N, [&](auto n) { with_bool(arr, [&](auto ar_on) { with_bool(met, [&](auto met_on) {
+            const auto &K = args_for<met_on>(A, AM);
+            if (rot) step_flat_kernel<n, 99, true, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K);
+            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K);
+            else step_flat_kernel<n, 99, false, false, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K); }); }); }); });
     }
     case Route::loop: {
         const int threads = A.EPB * A.L;
         const int blocks = (B + A.EPB - 1) / A.EPB;
         const bool mid = !g_force_generic && N > 5;          // (N = 0 and the forced A/B route stay on the generic kernel)
         const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
-        return with_bool(mid, [&](auto mid_) { return with_bool(arr, [&](auto ar_on) {
-            constexpr auto kernel = step_kernel<mid_, ar_on>;
+        if (met) static_cast<StepArgs &>(AM) = A;
+        return with_bool(mid, [&](auto mid_) { return with_bool(arr, [&](auto ar_on) { return with_bool(met, [&](auto met_on) {
+            constexpr auto kernel = step_kernel<mid_, ar_on, met_on>;
             if (smem > 48 * 1024) {                          // (a per-device attribute; setting it again is cheap)
                 const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 if (err != cudaSuccess) return (int)err;
             }
-            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(A); }); }); });
+            const auto &K = args_for<met_on>(A, AM);
+            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(K); }); }); }); });
     }
     }
     return CROWDSIM_EINVAL;   // (unreachable: route() returns one of the four)
@@ -423,6 +473,15 @@ extern "C" int crowdsim_step_n_arrivals(const crowdsim_params *prm, int B, int N
 {
     if (!arr) return CROWDSIM_EINVAL;
     cs::StepMode m; m.arr = arr;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
+}
+
+extern "C" int crowdsim_step_n_metrics(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                       crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps,
+                                       const crowdsim_arrivals *arr, const crowdsim_metrics *met, void *stream)
+{
+    if (!met) return CROWDSIM_EINVAL;
+    cs::StepMode m; m.arr = arr; m.met = met;
     return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 

@@ -180,12 +180,16 @@ __device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int
 // ARR = true (crowdsim_step_n_arrivals, not with REC): every human stamps its arrival (step_args.cuh) when it happens, from
 // one "arrived" bit kept across the steps, and writes its part of a finished episode's end snapshot before an install
 // replaces it; the robot writes its velocity's. ARR = false compiles to the SASS the kernel had before ARR.
-template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false>
+// MET = true (crowdsim_step_n_metrics, not with REC): each human tests its pairs (a, j > a) on the step's shared float64 view
+// and adds its env's overlaps to a shared counter before the clearance barrier; the robot books them with its path length
+// and dmin in its tail, its accumulators in shared memory beside RobotRec. MET = false compiles to the SASS it had before MET.
+template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false, bool MET = false>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
-step_multi_kernel(const __grid_constant__ StepArgs A)
+step_multi_kernel(const __grid_constant__ StepArgsT<MET> A)
 {
     static_assert(REC || !ROT, "unicycle rows are a recording variant");
     static_assert(!(REC && ARR), "arrivals are stamped by the rollout kernels only");
+    static_assert(!(REC && MET), "metrics are measured by the rollout kernels only");
     static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
     using namespace orca;
     CS_RES_BEGIN
@@ -246,8 +250,10 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             if (A.has_ar) r0.want = A.ar.want[e];
             s_rr[le] = r0;
             if constexpr (ROT) rec_theta_smem<E>()[le] = (float)A.st.r_theta[e];
+            if constexpr (MET) met_acc_smem<E>()[le] = met_load(A.met, e);
         }
     }
+    if constexpr (MET) { if (is_robot) met_hh_smem<E>()[le] = 0; }
     s_goal[tid] = goal;
     RobotRec &rr = s_rr[le];                                 // robot threads of valid envs only
     bool arrived = false;                                    // ARR: my h_arrival is non-zero
@@ -377,6 +383,13 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             const float2 rv = s_nv[rt];
             s_cl[tid] = swept_clearance(pos, vel, s_pos[rt], make_double2((double)rv.x, (double)rv.y), attr.x, s_rad[rt], dt);
             // agent.py:122-135 holonomic step with the ORCA action (float32 values widened); a scene installed below replaces it
+            if constexpr (MET) {
+                // crowd_sim.py:353-362 on the pre-step positions: my pairs (a, j > a)
+                int c = 0;
+                #pragma unroll
+                for (int j = 1; j < N; ++j) if (j > a) c += hh_overlap(pos, attr.x, s_pos[le * N + j], s_rad[le * N + j]) ? 1 : 0;
+                if (c) atomicAdd(&met_hh_smem<E>()[le], c);
+            }
             const double hx = (double)nv.x, hy = (double)nv.y;
             pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
             dirty_kin = true;
@@ -450,6 +463,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 }
                 // ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72)
                 const double npx = pos.x + ax * dt, npy = pos.y + ay * dt;
+                if constexpr (MET) {
+                    int &hh = met_hh_smem<E>()[le];
+                    met_add(met_acc_smem<E>()[le], pos, make_double2(npx, npy), dmin, hh);
+                    hh = 0;                                  // the next step's humans add after the loop-top barrier
+                }
                 const double gtime = rr.gtime;
                 const int t_rec = rr.ep_t;                   // REC: the episode step the row was recorded at
                 double reward;
@@ -475,6 +493,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                             ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
                             if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
                             if constexpr (ARR) { if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, ep_c, vel); }
+                            if constexpr (MET) met_result(A.met, ep_c, met_acc_smem<E>()[le]);
                         }
                         if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                     }
@@ -502,6 +521,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                         if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
                         if constexpr (ROT) rec_theta_smem<E>()[le] = (float)A.st.r_theta[e];     // the heading installed
                         if (A.has_ep) { rr.ep_t = 0; rr.ep_ret = 0.0; rr.ep_tc = 0; rr.ep_mds = 0.0; rr.ep_c = __ldcg(A.ar.n_case + e); rr.dirty_ep = 1; rr.new_case = 1; }
+                        if constexpr (MET) met_acc_smem<E>()[le] = met_fresh();
                         act_flag = 1; A.st.active[e] = 1; rr.want = 0; A.ar.want[e] = 0;
                         dirty_kin = true; dirty_scene = true; release = true;
                     } else {
@@ -534,6 +554,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             if (A.has_ep && rr.dirty_ep) {
                 A.ep.ep_steps[e] = rr.ep_t; A.ep.ep_return[e] = rr.ep_ret; A.ep.ep_too_close[e] = rr.ep_tc; A.ep.ep_min_dist_sum[e] = rr.ep_mds;
                 if (rr.new_case) A.ep.ep_case[e] = rr.ep_c;
+                if constexpr (MET) met_store(A.met, e, met_acc_smem<E>()[le]);
             }
         }
     }

@@ -37,8 +37,13 @@ BatchedExplorer(..., human_times=True): the humans' time to goal after every suc
 "Average time for humans to reach goal"). The step kernels stamp the arrivals and keep each episode's end state
 (BatchedCrowdSim.track_arrivals); after the rollout CrowdSim.get_human_times runs once on device over every ReachGoal case
 (BatchedCrowdSim.case_human_times). The result rows then carry N more columns, the case's human times (0 for other endings).
+
+BatchedExplorer(..., metrics=True): each episode's human-human collision steps and pairs, robot path length and closest
+approach, measured inside the step kernels (BatchedCrowdSim.track_metrics, include/crowdsim_b200_metrics.h). The result
+rows then end with 4 more columns (METRIC_COLUMNS) and summarize logs one more line after the reference's.
 """
 import logging
+import math
 
 import torch
 
@@ -62,15 +67,37 @@ def shard_range(k, rank, world):
     return start, base + (1 if rank < extra else 0)
 
 
-def pack_results(ep, n, human_times=None):
+RESULT_COLUMNS = ('info', 'steps', 'time', 'return', 'too_close', 'min_dist_sum')
+METRIC_COLUMNS = ('hh_steps', 'hh_pairs', 'path_length', 'closest_approach')
+
+
+def pack_results(ep, n, human_times=None, metrics=None):
     """Per-case result rows of an EpisodeBuffers as one [n][6] float64 tensor (exact for the integer columns); with
-    human_times ([n][N] float64) the rows are [n][6 + N]."""
+    human_times ([n][N] float64) the rows are [n][6 + N]; with metrics (batched.MetricsBuffers) 4 more columns follow,
+    METRIC_COLUMNS."""
     cols = [ep.res_info[:n].double(), ep.res_steps[:n].double(), ep.res_time[:n], ep.res_return[:n],
             ep.res_too_close[:n].double(), ep.res_min_dist_sum[:n]]
     rows = torch.stack(cols, dim=1)
     if human_times is not None:
         rows = torch.cat([rows, human_times[:n].to(rows.device, torch.float64)], dim=1)
+    if metrics is not None:
+        m = torch.stack([metrics.res_hh_steps[:n].double(), metrics.res_hh_pairs[:n].double(), metrics.res_path[:n],
+                         metrics.res_closest[:n]], dim=1)
+        rows = torch.cat([rows, m.to(rows.device)], dim=1)
     return rows.contiguous()
+
+
+def result_columns(rows, metrics=False):
+    """{column name: numpy array} of gathered result rows: RESULT_COLUMNS, 'human_times' [k][N] when the rows carry human
+    times, and METRIC_COLUMNS with metrics."""
+    a = rows.cpu().numpy()
+    out = {name: a[:, i] for i, name in enumerate(RESULT_COLUMNS)}
+    end = a.shape[1] - (len(METRIC_COLUMNS) if metrics else 0)
+    if end > len(RESULT_COLUMNS):
+        out['human_times'] = a[:, len(RESULT_COLUMNS):end]
+    if metrics:
+        out.update({name: a[:, end + i] for i, name in enumerate(METRIC_COLUMNS)})
+    return out
 
 
 def gather_results(local_rows, k, rank, world, group=None):
@@ -87,11 +114,16 @@ def gather_results(local_rows, k, rank, world, group=None):
     return torch.cat([out[r][:shard_range(k, r, world)[1]] for r in range(world)], dim=0)
 
 
-def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info):
+def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info, metrics=False):
     """explorer.py:52-90 on gathered per-case rows ([k][6]: info, steps, time, return, too_close, min_dist_sum; [k][6 + N]
     with the human times of BatchedExplorer(human_times=True)). Returns the statistics as a dict and emits the reference's
-    log lines through `log`."""
+    log lines through `log`. metrics=True: the rows end with METRIC_COLUMNS (BatchedExplorer(metrics=True)), and one more
+    line follows the reference's."""
     rows = rows.cpu().tolist()
+    met = None
+    if metrics:
+        met = [r[-len(METRIC_COLUMNS):] for r in rows]
+        rows = [r[:-len(METRIC_COLUMNS)] for r in rows]
     human_times = [list(r[6:]) if int(r[0]) == _abi.INFO_REACHGOAL else None for r in rows] if rows and len(rows[0]) > 6 else None
     rows = [r[:6] for r in rows]
     success_times, collision_times, timeout_times = [], [], []
@@ -138,6 +170,21 @@ def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure
     if print_failure:
         log('Collision cases: ' + ' '.join([str(x) for x in collision_cases]))
         log('Timeout cases: ' + ' '.join([str(x) for x in timeout_cases]))
+    if met is not None:
+        # what the reference computes and drops: crowd_sim.py:353-362's pair test, test.py:92-97's displacement, the
+        # minimum dmin (crowd_sim.py:331-351); an episode without humans has no closest approach (+inf) and is left out
+        hh_steps, hh_pairs, path, closest = ([r[i] for r in met] for i in range(len(METRIC_COLUMNS)))
+        finite = [c for c in closest if math.isfinite(c)]
+        stats['hh_collision_rate'] = sum(1 for x in hh_steps if x > 0) / k
+        stats['hh_pairs_per_episode'] = sum(hh_pairs) / k
+        stats['avg_path_length'] = average(path)
+        stats['avg_closest_approach'] = average(finite) if finite else math.inf
+        stats.update(hh_steps=[int(x) for x in hh_steps], hh_pairs=[int(x) for x in hh_pairs], path_length=path,
+                     closest_approach=closest)
+        log('{:<5} human-human collision rate: {:.2f}, pairs per episode: {:.2f}, average path length: {:.2f}, '
+            'average closest approach: {:.2f}'.format(phase.upper(), stats['hh_collision_rate'],
+                                                      stats['hh_pairs_per_episode'], stats['avg_path_length'],
+                                                      stats['avg_closest_approach']))
     return stats
 
 
@@ -159,9 +206,10 @@ def _unicycle_rows(policy):
 
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
-                 rank=0, world=1, group=None, human_times=False):
+                 rank=0, world=1, group=None, human_times=False, metrics=False):
         self.env = env
         self.human_times = bool(human_times)
+        self.metrics = bool(metrics)
         self.robot_policy = robot_policy
         self.device = device or env.device
         self.memory = memory
@@ -202,25 +250,34 @@ class BatchedExplorer(object):
             raise ValueError('human times are not defined for rule mixed')
         if self.human_times and update_memory:
             raise ValueError('human times are measured by rollouts that do not record (update_memory=False)')
+        if self.metrics and update_memory:
+            raise ValueError('episode metrics are measured by rollouts that do not record (update_memory=False)')
         first_case = env.case_counter[phase]
         start, n_local = shard_range(k, self.rank, self.world)
         gamma = self.gamma if self.gamma is not None else 0.9
         args = (env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
                 steps_per_launch, first_case, start, n_local, gamma, rule, scenes)
-        if not self.human_times:
+        if not (self.human_times or self.metrics):
             return self._run(*args)
-        prev_arrivals = env.arrivals                   # the caller's arrival tracking, back in place after the run
+        prev_arrivals, prev_metrics = env.arrivals, env.metrics     # the caller's tracking, back in place after the run
         try:
             return self._run(*args)
         finally:
-            env.arrivals = prev_arrivals
-            env.fit_arrival_snapshots()                # (the run replaced the episode rows)
+            if self.human_times:
+                env.arrivals = prev_arrivals
+                env.fit_arrival_snapshots()            # (the run replaced the episode rows)
+            if self.metrics:
+                env.metrics = prev_metrics
+                if prev_metrics is not None and env.episodes is not None and prev_metrics.k != env.episodes.k:
+                    env.fit_metrics()
 
     def _run(self, env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
              steps_per_launch, first_case, start, n_local, gamma, rule, scenes):
         ep = env.track_episodes(max(n_local, 1), gamma)
         if self.human_times:
             env.track_arrivals(snapshots=True)
+        if self.metrics:
+            env.track_metrics()
         if scenes is None:
             env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
             env.enable_autoreset(rule)
@@ -309,7 +366,8 @@ class BatchedExplorer(object):
             ok = torch.nonzero(ep.res_info[:n_local] == _abi.INFO_REACHGOAL).flatten()
             if ok.numel():
                 local_times[ok] = env.case_human_times(ok)[0]
-        rows = gather_results(pack_results(ep, n_local, local_times), k, self.rank, self.world, self.group)
+        rows = gather_results(pack_results(ep, n_local, local_times, env.metrics if self.metrics else None), k, self.rank,
+                              self.world, self.group)
         if scenes is None:
             env.case_counter[phase] = (first_case + k) % env.case_size[phase]
         env.autoreset = None
@@ -318,6 +376,6 @@ class BatchedExplorer(object):
         self.last_rows = rows
         if self.rank != 0:
             return None
-        stats = summarize(rows, k, phase, env.time_limit, env.time_step, episode, print_failure)
+        stats = summarize(rows, k, phase, env.time_limit, env.time_step, episode, print_failure, metrics=self.metrics)
         self.last_env_steps = stats['env_steps']
         return stats

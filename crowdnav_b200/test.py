@@ -6,7 +6,11 @@ print_failure=True), with every case streamed through --num_envs environments on
 log lines. --policy is orca (the robot's ORCA runs inside the step kernels) or one of the trainable policies of
 policy.policy_factory. --human_times adds the humans' average time to goal over the successful cases
 (BatchedExplorer(human_times=True)). --scenes FILE.npz runs the scenes of a saved batched.SceneTable, one case per row,
-instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it). Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
+instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it). --metrics adds
+one line: the rate of episodes with a human-human collision, the overlapping pairs per episode, the robot's average path
+length and closest approach (BatchedExplorer(metrics=True)). --results FILE.npz saves every case's result row, one array per
+column (explorer.result_columns: the reference's columns, then human_times and the metric columns when asked for), so two
+checkpoints can be compared case by case. Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
 changes nothing: the run is always on cuda:0.
 """
 import argparse
@@ -36,6 +40,8 @@ def parse_args(argv=None):
     parser.add_argument('--num_envs', type=int, default=1024)
     parser.add_argument('--human_times', default=False, action='store_true')
     parser.add_argument('--scenes', type=str, default=None)
+    parser.add_argument('--metrics', default=False, action='store_true')
+    parser.add_argument('--results', type=str, default=None)
     return parser, parser.parse_args(argv)
 
 
@@ -91,7 +97,8 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
         env.test_sim = 'square_crossing'
     if args.circle:
         env.test_sim = 'circle_crossing'
-    explorer = explorer_class(env, policy, device, gamma=0.9, human_times=args.human_times)
+    explorer = explorer_class(env, policy, device, gamma=0.9, human_times=args.human_times,
+                              **({'metrics': True} if args.metrics else {}))
 
     if policy == 'orca':
         # test.py:77-85: no safety space for ORCA, visible robot or not
@@ -106,8 +113,19 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
     if args.scenes is not None:
         from .batched import SceneTable
         scenes = SceneTable.load(args.scenes)
-        return explorer.run_k_episodes(scenes.k, args.phase, print_failure=True, scenes=scenes)
-    return explorer.run_k_episodes(env.case_size[args.phase], args.phase, print_failure=True)
+        stats = explorer.run_k_episodes(scenes.k, args.phase, print_failure=True, scenes=scenes)
+    else:
+        stats = explorer.run_k_episodes(env.case_size[args.phase], args.phase, print_failure=True)
+    if args.results is not None:
+        save_results(args.results, explorer.last_rows, args.metrics)
+    return stats
+
+
+def save_results(path, rows, metrics=False):
+    """--results: every case's result row as an .npz of one array per column (explorer.result_columns)."""
+    import numpy as np
+    from .explorer import result_columns
+    np.savez(path, **result_columns(rows, metrics))
 
 
 if __name__ == '__main__':
