@@ -450,6 +450,12 @@ class BatchedCrowdSim(object):
         self.metrics = MetricsBuffers(self.B, self.episodes.k, self.device)
         return self.metrics
 
+    def _device_mask(self, mask):
+        """A reset's `mask` as the uint8 tensor on this batch's device that the kernels read (None stays None)."""
+        if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
+            mask = torch.as_tensor(mask).to(device=self.device, dtype=torch.uint8)
+        return mask
+
     def _clear_slots(self, mask):
         """What a reset clears beside the state and the episode accumulators: arrival stamps (crowd_sim.py:263-265) and
         the metrics accumulators."""
@@ -555,8 +561,7 @@ class BatchedCrowdSim(object):
                                  'before reset_seeds(use_queue=True)')
         if seeds is not None:
             self.set_seeds(seeds)
-        if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
-            mask = torch.as_tensor(mask).to(device=self.device, dtype=torch.uint8)
+        mask = self._device_mask(mask)
         a = self._reset_args(mask, rule, seed_stride, use_queue)
         q = use_queue and self._case_counter is not None
         self._scene_src = (rule, q)
@@ -664,8 +669,7 @@ class BatchedCrowdSim(object):
             self._case_counter.zero_()
         else:
             self.set_case_queue(first, count)
-        if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
-            mask = torch.as_tensor(mask).to(device=self.device, dtype=torch.uint8)
+        mask = self._device_mask(mask)
         t = self._table_args()
         st, ep = self.state.struct(), _struct(self.episodes)
         self._call('reset_table', C.byref(t), _ptr(mask), self.B, self.human_num, C.byref(st), _ref(ep))

@@ -93,6 +93,37 @@ __device__ __forceinline__ double2 ld2(const double *p, size_t i) { return reint
 __device__ __forceinline__ void st2(double *p, size_t i, double2 v) { reinterpret_cast<double2 *>(p)[i] = v; }
 __device__ __forceinline__ double2 ld2_cg(const double *p, size_t i) { return __ldcg(reinterpret_cast<const double2 *>(p) + i); }
 
+// A fresh episode of env e, as the resets and the single-step kernels' auto-reset install write it (the multi-step kernel
+// keeps its robot in registers and writes its own): global_time = 0 and robot.set(0, -R, 0, R, 0, 0, pi / 2)
+// (crowd_sim.py:262,274), and the running episode accumulators of Explorer.run_k_episodes cleared (explorer.py:41-50).
+__device__ __forceinline__ void fresh_robot(const crowdsim_state &st, int e, double R, double radius, double v_pref)
+{
+    st2(st.r_pos, e, make_double2(0.0, -R)); st2(st.r_goal, e, make_double2(0.0, R));
+    st2(st.r_vel, e, make_double2(0, 0)); st2(st.r_attr, e, make_double2(radius, v_pref));
+    if (st.r_theta) st.r_theta[e] = CS_PI / 2;
+    st.g_time[e] = 0.0;
+}
+__device__ __forceinline__ void clear_episode(const crowdsim_episodes &ep, int e)
+{
+    ep.ep_steps[e] = 0; ep.ep_return[e] = 0.0; ep.ep_too_close[e] = 0; ep.ep_min_dist_sum[e] = 0.0;
+}
+
+// Argument rules the reset and step entry points share (include/crowdsim_b200.h): the state arrays a reset or a step
+// writes, the slot arrays of an episodes buffer, and the slot arrays of an auto-reset.
+inline bool has_state_arrays(const crowdsim_state &st, int N)
+{
+    if (N > 0 && (!st.h_pos || !st.h_vel || !st.h_goal || !st.h_attr)) return false;
+    return st.r_pos && st.r_vel && st.r_goal && st.r_attr && st.g_time;
+}
+inline bool has_episode_slots(const crowdsim_episodes &ep)
+{
+    return ep.ep_steps && ep.ep_return && ep.ep_too_close && ep.ep_min_dist_sum && ep.ep_case;
+}
+inline bool has_autoreset_slots(const crowdsim_autoreset &ar, int N)
+{
+    return ar.n_state && ar.n_case && ar.want && !(N > 0 && (!ar.n_h_pos || !ar.n_h_goal || !ar.n_h_attr));
+}
+
 // Slot flags of the auto-reset protocol (include/crowdsim_b200.h: crowdsim_autoreset). The generator and the step kernels may
 // run concurrently on different streams, so the hand-over is a formal release / acquire pair at gpu scope:
 //   generator:  ld.acquire(flag) == EMPTY  ->  write the scene  ->  st.release(flag, READY)

@@ -45,15 +45,8 @@ struct StepArgs {
     crowdsim_record_maps recm;   // crowdsim_step_n_record_ex with occupancy-map rows (h_pos == NULL: none); after rec for
                                  // the same reason
     crowdsim_arrivals arr;       // crowdsim_step_n_arrivals: read only by the ARR instantiations; last for the same reason
+    crowdsim_metrics met;        // crowdsim_step_n_metrics: read only by the MET instantiations; last for the same reason
 };
-
-// crowdsim_step_n_metrics: the argument block of the MET instantiations. A struct of its own, not a StepArgs field, so that
-// the parameter block of every other kernel (and the offsets of the recording kernels' arguments after it) stays as it was.
-struct StepArgsMet : StepArgs {
-    crowdsim_metrics met;
-};
-template <bool MET>
-using StepArgsT = typename std::conditional<MET, StepArgsMet, StepArgs>::type;
 
 // ---- MET = true (include/crowdsim_b200_metrics.h): one env's running accumulators ----
 struct MetAcc {
@@ -163,12 +156,9 @@ __device__ __forceinline__ void ar_install_human(const StepArgs &A, int e, int N
 __device__ __forceinline__ void ar_install_robot(const StepArgs &A, int e)
 {
     (void)ld_acquire_u8(A.ar.n_state + e);
-    st2(A.st.r_pos, e, make_double2(0.0, -A.ar.circle_radius)); st2(A.st.r_goal, e, make_double2(0.0, A.ar.circle_radius));
-    st2(A.st.r_vel, e, make_double2(0, 0)); st2(A.st.r_attr, e, make_double2(A.ar.robot_radius, A.ar.robot_v_pref));
-    if (A.st.r_theta) A.st.r_theta[e] = CS_PI / 2;
-    A.st.g_time[e] = 0.0;
+    fresh_robot(A.st, e, A.ar.circle_radius, A.ar.robot_radius, A.ar.robot_v_pref);
     if (A.has_ep) {
-        A.ep.ep_steps[e] = 0; A.ep.ep_return[e] = 0.0; A.ep.ep_too_close[e] = 0; A.ep.ep_min_dist_sum[e] = 0.0;
+        clear_episode(A.ep, e);
         A.ep.ep_case[e] = __ldcg(A.ar.n_case + e);
     }
     A.st.active[e] = 1; A.ar.want[e] = 0;

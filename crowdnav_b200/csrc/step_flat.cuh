@@ -67,7 +67,7 @@ struct RobotRec {
 
 template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false, bool MET = false>
 __global__ void __launch_bounds__(32 * CS_FLAT_WPB, CS_FLAT_MINBLOCKS * 4 / CS_FLAT_WPB)
-step_flat_kernel(const __grid_constant__ StepArgsT<MET> A)
+step_flat_kernel(const __grid_constant__ StepArgs A)
 {
     if constexpr (STAGE == 0) return;
     using namespace orca;

@@ -42,7 +42,7 @@ namespace cs {
 // counted with a ballot per round and added to a shared counter; the robot lane books them with the path length and dmin. MET = false compiles to
 // the SASS the kernel had before MET. (At most 128 envs per block: N = 0.)
 template <bool MID, bool ARR = false, bool MET = false>
-__global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgsT<MET> A)
+__global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgs A)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_qcount;
@@ -319,20 +319,16 @@ static int check(const crowdsim_params *prm, int B, int N, const crowdsim_state 
         if (rc != CROWDSIM_OK) return rc;
     }
     if (N > CROWDSIM_MAX_HUMANS || prm->max_neighbors > CROWDSIM_MAX_NEIGHBORS) return CROWDSIM_EUNSUPPORTED;
-    if (N > 0 && (!st->h_pos || !st->h_vel || !st->h_goal || !st->h_attr)) return CROWDSIM_EINVAL;
-    if (!st->r_pos || !st->r_vel || !st->r_goal || !st->r_attr || !st->g_time) return CROWDSIM_EINVAL;
+    if (!has_state_arrays(*st, N)) return CROWDSIM_EINVAL;
     if (prm->robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT && !st->r_theta) return CROWDSIM_EINVAL;
     if (m.act_only) { if (!io->action_out) return CROWDSIM_EINVAL; }
     else {
         if (!io->reward || !io->dmin || !io->done || !io->info) return CROWDSIM_EINVAL;
         if (prm->robot_policy != CROWDSIM_ROBOT_ORCA && !io->action) return CROWDSIM_EINVAL;
     }
-    if (ep && !m.act_only && (!ep->ep_case || !ep->ep_steps || !ep->ep_return || !ep->ep_too_close || !ep->ep_min_dist_sum ||
-                              !ep->discount || !ep->res_info || !ep->res_steps || !ep->res_time || !ep->res_return ||
-                              !ep->res_too_close || !ep->res_min_dist_sum)) return CROWDSIM_EINVAL;
-    if (ar && !m.act_only) {
-        if (!st->active || !ar->n_state || !ar->n_case || !ar->want || (N > 0 && (!ar->n_h_pos || !ar->n_h_goal || !ar->n_h_attr))) return CROWDSIM_EINVAL;
-    }
+    if (ep && !m.act_only && (!has_episode_slots(*ep) || !ep->discount || !ep->res_info || !ep->res_steps || !ep->res_time ||
+                              !ep->res_return || !ep->res_too_close || !ep->res_min_dist_sum)) return CROWDSIM_EINVAL;
+    if (ar && !m.act_only && (!st->active || !has_autoreset_slots(*ar, N))) return CROWDSIM_EINVAL;
     return CROWDSIM_OK;
 }
 
@@ -355,14 +351,6 @@ static Route route(const StepArgs &A, int n_steps, bool rec)
     if (!small || A.lookahead) return Route::loop;
     if ((n_steps > 1 || rec) && A.N >= 2 && A.k.robot_policy == CROWDSIM_ROBOT_ORCA) return Route::multi;
     return Route::flat;
-}
-
-// The argument block of a kernel instantiation: StepArgs, or StepArgsMet for the MET ones.
-template <bool MET>
-static const StepArgsT<MET> &args_for(const StepArgs &A, const StepArgsMet &AM)
-{
-    if constexpr (MET) return AM;
-    else return A;
 }
 
 // n_steps single-step launches, each staged and booked by the recording around it when m.rec is set.
@@ -397,9 +385,8 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if (m.rec) A.rec = *m.rec; else memset(&A.rec, 0, sizeof(A.rec));
     if (m.recm) A.recm = *m.recm; else memset(&A.recm, 0, sizeof(A.recm));
     if (m.arr) A.arr = *m.arr; else memset(&A.arr, 0, sizeof(A.arr));
+    if (m.met) A.met = *m.met; else memset(&A.met, 0, sizeof(A.met));
     const bool arr = (m.arr != nullptr), met = (m.met != nullptr);
-    StepArgsMet AM;
-    if (met) { AM.met = *m.met; }
     switch (route(A, n_steps, m.rec != nullptr)) {
     case Route::act:
         with_int<1, 5>(N, [&](auto n) { orca_act_kernel<n><<<(B + 127) / 128, 128, 0, stream>>>(A); });
@@ -409,10 +396,9 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         const int blocks = (B + 31) / 32;                    // 32 envs per block, N + 1 warps
         A.n_steps = n_steps;
         if (m.rec) { ++g_launches; return launch_multi_record(A, blocks, stream, m.rec_rot); }
-        if (met) static_cast<StepArgs &>(AM) = A;
         const int err = with_int<2, 5>(N, [&](auto n) { return with_bool(A.k.robot_visible, [&](auto vis) { return with_bool(arr, [&](auto ar_on) {
             return with_bool(met, [&](auto met_on) {
-                return launch_carved<step_multi_kernel<n, vis, false, false, ar_on, met_on>>(args_for<met_on>(A, AM), blocks, 32 * (n + 1), stream); }); }); }); });
+                return launch_carved<step_multi_kernel<n, vis, false, false, ar_on, met_on>>(A, blocks, 32 * (n + 1), stream); }); }); }); });
         if (err != CROWDSIM_OK) return err;
         ++g_launches;
         return (int)cudaGetLastError();
@@ -427,27 +413,23 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         // The threshold scales with the device's SM count; scripts/latency_probe.cu times both. The unicycle robot's
         // kernel exists with the per-warp queue only.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
-        if (met) static_cast<StepArgs &>(AM) = A;
         return launch_loop(A, n_steps, m, stream, [&] { with_int<1, 5>(N, [&](auto n) { with_bool(arr, [&](auto ar_on) { with_bool(met, [&](auto met_on) {
-            const auto &K = args_for<met_on>(A, AM);
-            if (rot) step_flat_kernel<n, 99, true, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K);
-            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K);
-            else step_flat_kernel<n, 99, false, false, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(K); }); }); }); });
+            if (rot) step_flat_kernel<n, 99, true, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else step_flat_kernel<n, 99, false, false, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); }); }); }); });
     }
     case Route::loop: {
         const int threads = A.EPB * A.L;
         const int blocks = (B + A.EPB - 1) / A.EPB;
         const bool mid = !g_force_generic && N > 5;          // (N = 0 and the forced A/B route stay on the generic kernel)
         const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
-        if (met) static_cast<StepArgs &>(AM) = A;
         return with_bool(mid, [&](auto mid_) { return with_bool(arr, [&](auto ar_on) { return with_bool(met, [&](auto met_on) {
             constexpr auto kernel = step_kernel<mid_, ar_on, met_on>;
             if (smem > 48 * 1024) {                          // (a per-device attribute; setting it again is cheap)
                 const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 if (err != cudaSuccess) return (int)err;
             }
-            const auto &K = args_for<met_on>(A, AM);
-            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(K); }); }); }); });
+            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(A); }); }); }); });
     }
     }
     return CROWDSIM_EINVAL;   // (unreachable: route() returns one of the four)

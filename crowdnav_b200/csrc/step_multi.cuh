@@ -185,7 +185,7 @@ __device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int
 // and dmin in its tail, its accumulators in shared memory beside RobotRec. MET = false compiles to the SASS it had before MET.
 template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false, bool MET = false>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
-step_multi_kernel(const __grid_constant__ StepArgsT<MET> A)
+step_multi_kernel(const __grid_constant__ StepArgs A)
 {
     static_assert(REC || !ROT, "unicycle rows are a recording variant");
     static_assert(!(REC && ARR), "arrivals are stamped by the rollout kernels only");
