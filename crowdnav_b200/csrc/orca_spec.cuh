@@ -106,6 +106,81 @@ ORCA_HD __forceinline__ void make_line_sel(V2 p, V2 v, float r, V2 po, V2 vo, fl
     point = v + 0.5f * u;
 }
 
+// Bit casts of the integer fields of a queued item and of a pair core's flags (__int_as_float / __float_as_int have no
+// host version).
+ORCA_HD __forceinline__ float int_bits(int i) { float f; __builtin_memcpy(&f, &i, sizeof f); return f; }
+ORCA_HD __forceinline__ int bits_int(float f) { int i; __builtin_memcpy(&i, &f, sizeof i); return i; }
+
+// make_line_sel split in two for a pair of agents that build each other's half-plane with the same radii (the multi-step
+// kernel's humans): pair_core computes, once per pair, the part that is bit-identical in both orders, and line_from_core
+// finishes one agent's line from it with that agent's own operands.
+// Why the core is the same in both orders (round to nearest): fl(x - y) = -fl(y - x) unless x == y, where both are +0, so
+// the two orders' rel_pos and rel_vel agree componentwise in magnitude; so does k * rel_pos for k > 0 (k * -0 = -0). A
+// component of w = rel_vel - k * rel_pos is a - b with |a'| = |a|, |b'| = |b|: both non-zero gives w' = -w, or +0 on both
+// sides when a == b; a zero gives w = -b, w' = -b' (or a, a'), the same magnitude. Every product term of dot1 and of
+// det(rel_pos, w) is then identical or a zero of either sign, so their values agree up to the sign of a zero result and
+// their comparisons with 0 agree, and dist_sq, w_len_sq and comb_r (commutative) agree bit for bit. Hence the overlap test,
+// the cut-off test, the left-leg test, w_len = sqrt(w_len_sq) and its reciprocal, leg = sqrt(dist_sq - comb_r_sq) and
+// 1 / dist_sq are the pair's. Everything that carries a sign (unit_w, the legs' numerators, dir, u, point) is recomputed
+// by each agent from its own operands with make_line_sel's operations.
+// A line needs either (w_len, 1 / w_len) (overlap: w from inv_dt; cut-off circle: w from inv_th) or (leg, 1 / dist_sq), so
+// the core holds those two non-negative floats (one IEEE sqrt and one reciprocal per pair instead of two of each per line)
+// with the case in their sign bits: x < 0 (sign bit) = circle (overlap or cut-off); then y's sign bit = overlap, else left.
+ORCA_HD __forceinline__ V2 pair_core(V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_th, float inv_dt)
+{
+    const V2 rel_pos = po - p;
+    const V2 rel_vel = v - vo;
+    const float dist_sq = abssq(rel_pos);
+    const float comb_r = r + ro;
+    const float comb_r_sq = sqr(comb_r);
+    const bool overlap = !(dist_sq > comb_r_sq);
+    const V2 w = rel_vel - (overlap ? inv_dt : inv_th) * rel_pos;
+    const float w_len_sq = abssq(w);
+    const float dot1 = dot(w, rel_pos);
+    const bool circle = overlap || (dot1 < 0.0f && sqr(dot1) > comb_r_sq * w_len_sq);
+    const bool left = det(rel_pos, w) > 0.0f;
+    const float len = sqrtf(circle ? w_len_sq : dist_sq - comb_r_sq);      // w_len or leg
+    const float inv = 1.0f / (circle ? len : dist_sq);                       // vdiv's reciprocals
+    return mk(circle ? -len : len, (circle ? overlap : left) ? -inv : inv);
+}
+
+// Agent (p, v, r)'s line against (po, vo, ro) from their pair's core c (pair_core in either order); bit for bit
+// make_line_sel(p, v, r, po, vo, ro, ...), in its operation order.
+ORCA_HD __forceinline__ void line_from_core(V2 c, V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_th, float inv_dt,
+                                            V2 &point, V2 &dir)
+{
+    const bool circle = bits_int(c.x) < 0, flag = bits_int(c.y) < 0;
+    const float len = fabsf(c.x), inv = fabsf(c.y);
+    const V2 rel_pos = po - p;
+    const V2 rel_vel = v - vo;
+    const float comb_r = r + ro;
+    const float k = (circle && flag) ? inv_dt : inv_th;
+    // circle: overlap or cut-off
+    const V2 w = rel_vel - k * rel_pos;
+    const V2 unit_w = mk(w.x * inv, w.y * inv);
+    const V2 dir_c = mk(unit_w.y, -unit_w.x);
+    const V2 u_c = (comb_r * k - len) * unit_w;
+    // legs
+    const V2 num_l = mk(rel_pos.x * len - rel_pos.y * comb_r, rel_pos.x * comb_r + rel_pos.y * len);
+    const V2 num_r = mk(rel_pos.x * len + rel_pos.y * comb_r, -rel_pos.x * comb_r + rel_pos.y * len);
+    const V2 n = flag ? num_l : num_r;
+    const V2 q = mk(n.x * inv, n.y * inv);
+    const V2 dir_l = flag ? q : -q;
+    const float dot2 = dot(rel_vel, dir_l);
+    const V2 u_l = dot2 * dir_l - rel_vel;
+    dir = circle ? dir_c : dir_l;
+    const V2 u = circle ? u_c : u_l;
+    point = v + 0.5f * u;
+}
+
+// make_line_sel bit for bit with one IEEE sqrt and one reciprocal instead of two of each: the core of the line's own pair,
+// finished at once (lines nobody else shares, such as the robot's against a human).
+ORCA_HD __forceinline__ void make_line_core(V2 p, V2 v, float r, V2 po, V2 vo, float ro, float inv_th, float inv_dt,
+                                            V2 &point, V2 &dir)
+{
+    line_from_core(pair_core(p, v, r, po, vo, ro, inv_th, inv_dt), p, v, r, po, vo, ro, inv_th, inv_dt, point, dir);
+}
+
 // lp1 candidates of every position (speculative). valid[i]: position i holds a line (absent positions never constrain).
 // CNT = number of leading positions to evaluate (compile time, <= M).
 template <int M, int CNT>
@@ -169,10 +244,6 @@ ORCA_HD __forceinline__ V2 lp2_init(V2 opt, float radius)
     if (abssq(opt) > sqr(radius)) { const V2 nv = normalize(opt); return mk(nv.x * radius, nv.y * radius); }
     return opt;
 }
-
-// Bit casts of the integer fields of a queued item (__int_as_float / __float_as_int have no host version).
-ORCA_HD __forceinline__ float int_bits(int i) { float f; __builtin_memcpy(&f, &i, sizeof f); return f; }
-ORCA_HD __forceinline__ int bits_int(float f) { int i; __builtin_memcpy(&i, &f, sizeof i); return i; }
 
 // The linearProgram3 queue of the step kernels (step_flat.cuh, step_multi.cuh, step_mid.cuh): a solve that needs
 // linearProgram3 is put in one column of a [rows][stride] float array in shared memory, its M lines first (line k in rows

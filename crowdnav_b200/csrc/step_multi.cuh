@@ -22,10 +22,14 @@
 //   1. every agent publishes its float32 view (position, velocity, the radius seen by a human and by the robot) and its
 //      float64 position, velocity and radius; the barrier that ends the step loop when no env of the block has work left
 //      (__syncthreads_or) makes them visible.
-//   2. every human builds the robot's line against itself and arrives at named barrier 1; every thread solves (flat solver
-//      of orca_spec.cuh, lines in registers; the robot waits on barrier 1 and reads its lines instead of building them)
-//      and publishes its lp2 result; the solves that need linearProgram3 go to a block queue of T / (N - 1) items (the
-//      step kernels' orca::Lp3Queue item, sized for N lines, plus the owner thread), one pass. The pass writes each result
+//   2. every human builds the robot's line against itself (orca::make_line_core: make_line_sel bit for bit with one sqrt
+//      and one reciprocal) and arrives at named barrier 1; then it computes the
+//      orca::pair_core of its human pairs (a, a + d mod N), each pair of a live env once, into the pair table, and the
+//      human warps sync on named barrier 2; every thread solves (flat solver of orca_spec.cuh, lines in registers: a
+//      human finishes its human-human lines from the table with orca::line_from_core, bit for bit make_line_sel; the
+//      robot waits on barrier 1 and reads its lines instead of building them) and publishes its lp2 result; the solves
+//      that need linearProgram3 go to a block queue of T / (N - 1) items (the step kernels' orca::Lp3Queue item, sized for
+//      N lines, plus the owner thread), one pass. The pass writes each result
 //      over its owner's lp2 result, so that after it the humans read their robot's velocity without a barrier.
 //   3. humans compute their swept-segment clearance against that velocity, publish it and integrate; meanwhile the robot
 //      publishes the rest of what the env's ending depends on (timeout, goal reached, its slot's state, read after its
@@ -44,7 +48,7 @@
 namespace cs {
 
 // Resident warps per SM the multi-step kernel is compiled for: blocks per SM = CS_MULTI_WARPS / (N + 1). N = 5: 5 blocks of
-// 6 warps (64 registers; CUDA 12.9 spills 86 B, 34.6 KB of shared memory per block); 3 blocks (18 warps) measured 16 %
+// 6 warps (64 registers; CUDA 12.9 spills 50 B, 34.6 KB of shared memory per block); 3 blocks (18 warps) measured 16 %
 // slower with 16 batches in flight (DESIGN §3.6, §10). A -D knob for A/B builds.
 #ifndef CS_MULTI_WARPS
 #define CS_MULTI_WARPS 30
@@ -69,15 +73,28 @@ static __device__ unsigned long long g_phase[2][CS_PHASES + 1];
 #define CS_PROBE_FLUSH(robot, steps) do { } while (0)
 #endif
 
+// The pair table: the orca::pair_core of every human pair of every env of the block, one row of N per human thread t
+// (entry b of row t = le * N + a: the core of the pair (a, b); the diagonal is not used). Each core is computed once and
+// stored in both of its humans' rows, so that a solve finds its line's core at the index of the partner, as it finds the
+// partner's view (a triangular table indexed by the pair spilled 44 B more at N = 5). At N = 5 and N = 2 it lives in s_pv's
+// dead rows; N = 3 and N = 4, whose s_pv has no room for it, declare this array instead.
+template <int S>
+__device__ __forceinline__ float2 *pair_table_smem()
+{
+    __shared__ float2 s_pt[S];
+    return s_pt;
+}
+
 // One solve of the multi-step kernel: agent a of the env whose float32 views start at slot ebase (robot: a = N). M lines
-// (candidates in the reference's order: the other humans, then the robot iff VIS; the robot sees all humans). Returns the
-// lp2 result, and what a linearProgram3 item needs (fail < nl): the lines in rank order (R, zero beyond M), nl, fail and
-// the maximum speed.
+// (candidates in the reference's order: the other humans, then the robot iff VIS; the robot sees all humans). A human
+// finishes its line against human b from their pair's core, entry b of its row s_pt of the pair table, and builds its line
+// against a visible robot whole (orca::make_line_core). Returns the lp2 result, and what a linearProgram3 item needs (fail < nl): the lines
+// in rank order (R, zero beyond M), nl, fail and the maximum speed.
 template <int N, int M, bool ROBOT>
 __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *s_view, const float *s_rview, int ebase, int a,
                                                 bool solves, double2 pos, double2 goal, double v_pref, orca::V2 p, orca::V2 v,
-                                                float r, const float *s_rl, orca::RegLines<N> &Rq, int &nl_out, int &fail_out,
-                                                float &max_speed_out)
+                                                float r, const float *s_rl, const float2 *s_pt, orca::RegLines<N> &Rq,
+                                                int &nl_out, int &fail_out, float &max_speed_out)
 {
     using namespace orca;
     const V2 pref = pref_velocity(pos, goal);
@@ -110,9 +127,15 @@ __device__ __forceinline__ orca::V2 multi_solve(const KParams &k, const float4 *
                 const int c = (ebase / (N + 1)) * N + src[kk];
                 R.p[kk] = mk(s_rl[0 * T + c], s_rl[1 * T + c]); R.d[kk] = mk(s_rl[2 * T + c], s_rl[3 * T + c]);
             } else {
-                const int sl = ebase + src[kk];
+                const int b = src[kk], sl = ebase + b;
                 const float4 q = s_view[sl];
-                make_line_sel(p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
+                if (M == N && b == N) {
+                    make_line_core(p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon, k.inv_time_step, R.p[kk], R.d[kk]);
+                } else {
+                    const float2 c = s_pt[b];
+                    line_from_core(mk(c.x, c.y), p, v, r, mk(q.x, q.y), mk(q.z, q.w), s_rview[sl], k.inv_time_horizon,
+                                   k.inv_time_step, R.p[kk], R.d[kk]);
+                }
             }
         }
     }
@@ -204,10 +227,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     // the float32 views (rows 0-3: position and velocity of slot le * L + a as a float4; rows 4, 5: radius as seen by a
     // human / by the robot) and the robot's lines (rows 6-9, column = the human thread that built it) are dead once the
     // lines are built; the projected lines of the lp3 pass (4 * SUB rows) are only live inside the pass: one array serves
-    // all of them
-    __shared__ __align__(16) float s_pv[PV][T];
-    // per-thread sub-problem result (x, y, ok) inside the lp3 pass; after it, the humans' clearances (one double each)
-    __shared__ __align__(16) float s_r2[3][T];
+    // all of them. Rows PV .. PV + 2 (s_r2): per-thread sub-problem result (x, y, ok) inside the lp3 pass; after it, the
+    // humans' clearances (one double each). Rows 10 .. PV + 2 are dead from the loop-top barrier to the queue barrier: the
+    // pair table's window.
+    __shared__ __align__(16) float s_pv[PV + 3][T];
+    float (*const s_r2)[T] = s_pv + PV;
     // float64 position and velocity of every agent at the start of the step (threads 0 .. 32N-1 humans, then the robots):
     // the humans' view for the robot's swept-segment test, and each thread's own copy, re-read after the solve, so that
     // they hold no registers across it
@@ -221,6 +245,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     constexpr unsigned PRE_TIMEOUT = 1, PRE_GOAL = 2, PRE_READY = 4, PRE_WANT = 8;   // timeout, goal reached, slot READY, parked
     float4 *const s_view = reinterpret_cast<float4 *>(&s_pv[0][0]);
     float *const s_radh = s_pv[4], *const s_radr = s_pv[5];
+    // the pair table (pair_table_smem): written after the loop-top barrier and read by the human solves, so at N = 5 and
+    // N = 2 it lives in s_pv's rows 10 .. PV + 2
+    float2 *s_pt;
+    if constexpr ((PV + 3 - 10) * T >= 2 * E * N * N) s_pt = reinterpret_cast<float2 *>(&s_pv[10][0]);
+    else s_pt = pair_table_smem<E * N * N>();
     const Lp3Queue<N> Q = { &s_q[0][0], QC };
 
     const KParams &k = A.k;
@@ -304,17 +333,36 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     if (!is_robot) {
         // the robot's half-plane against me, as the robot's solve would build it (the robot's view and radius as p, v, r;
         // mine as seen by the robot as po, vo, ro): it shortens the robot warp, the critical path of every step. Every
-        // human thread arrives, inactive envs' included, so that the robot warp's barrier.sync completes.
+        // human thread arrives, inactive envs' included, so that the robot warp's barrier.sync completes. make_line_core, not
+        // make_line_sel: the same bits with half the IEEE square roots and reciprocals, on the robot's critical path.
         const int rs = le * L + N;
         const float4 q = s_view[rs];
         V2 lp, ld;
-        make_line_sel(mk(q.x, q.y), mk(q.z, q.w), s_radr[rs], p, v, frr, k.inv_time_horizon, k.inv_time_step, lp, ld);
+        make_line_core(mk(q.x, q.y), mk(q.z, q.w), s_radr[rs], p, v, frr, k.inv_time_horizon, k.inv_time_step, lp, ld);
         s_pv[6][tid] = lp.x; s_pv[7][tid] = lp.y; s_pv[8][tid] = ld.x; s_pv[9][tid] = ld.y;
         asm volatile("barrier.arrive 1, %0;" :: "r"(T) : "memory");
+        // then, while the robot solves, the cores of my pairs (a, (a + d) mod N), d = 1 .. N / 2, the d = N / 2 pairs of an
+        // even N from a < N / 2 only: every pair of a live env once (orca::pair_core, bit-identical in both orders), into
+        // both rows. Not live: no solve reads them. Not unrolled: the unrolled loop's two cores overlap and the kernel spills
+        // 72 B more at N = 5. (Computed before the robot's line, they hold the robot warp at barrier 1 longer; the bench
+        // did not tell the two orders apart.)
+        if (live) {
+            #pragma unroll 1
+            for (int d = 1; d <= N / 2; ++d) {
+                if (2 * d < N || a < d) {
+                    const int b = (a + d < N) ? a + d : a + d - N, sl = le * L + b;
+                    const float4 qb = s_view[sl];
+                    const V2 c = pair_core(p, v, frh, mk(qb.x, qb.y), mk(qb.z, qb.w), s_radh[sl], k.inv_time_horizon, k.inv_time_step);
+                    s_pt[tid * N + b] = make_float2(c.x, c.y); s_pt[(le * N + b) * N + a] = make_float2(c.x, c.y);
+                }
+            }
+        }
+        // the pair table is complete (an env's humans may straddle two warps): named barrier 2, the human warps only
+        asm volatile("barrier.sync 2, %0;" :: "r"(32 * N) : "memory");
     }
     RegLines<N> R; int nl, fail; float max_speed;
-    V2 nv = is_robot ? multi_solve<N, N, true>(k, s_view, s_radr, le * L, N, live, pos, s_goal[tid], attr.y, p, v, frr, s_pv[6], R, nl, fail, max_speed)
-                     : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, s_pv[6], R, nl, fail, max_speed);
+    V2 nv = is_robot ? multi_solve<N, N, true>(k, s_view, s_radr, le * L, N, live, pos, s_goal[tid], attr.y, p, v, frr, s_pv[6], s_pt, R, nl, fail, max_speed)
+                     : multi_solve<N, MH, false>(k, s_view, s_radh, le * L, a, live, pos, s_goal[tid], attr.y, p, v, frh, s_pv[6], s_pt + tid * N, R, nl, fail, max_speed);
 
     // ---- linearProgram3 of the solves that need it: a block queue of QC items, one pass. The sub-problems of an item run
     // on SUB lanes of one warp in parallel (sequential shared-memory LP code of orca_device.cuh), the item's first lane finishes
