@@ -11,7 +11,8 @@ scene-table entry points, the same way (load() requires and declares them too). 
 tests/test_abi_cpu.py pins crowdsim_b200.h's entry points and structs (31 and 12) and requires STRUCTS / FUNCTIONS to mirror
 exactly that header; tests/test_scene_table_cpu.py checks these tables against the scene-table header and the test oracle's
 restatement (tests/native/scene_table_oracle.c). METRICS_STRUCTS / METRICS_FUNCTIONS describe
-include/crowdsim_b200_metrics.h the same way.
+include/crowdsim_b200_metrics.h the same way, and TABLE_ROBOT_STRUCTS / TABLE_ROBOT_FUNCTIONS
+include/crowdsim_b200_table_robots.h.
 Structs are filled by field name (`Episodes(ep_case=..., ...)`): they have no instance __dict__, so a name that is not
 one of the C fields raises instead of being dropped.
 """
@@ -214,11 +215,28 @@ METRICS_FUNCTIONS = {
 METRICS_EXPORTS = tuple(METRICS_FUNCTIONS)
 
 
+class TableRobots(C.Structure):
+    """crowdsim_table_robots: the robot start, goal and heading of every scene-table row (crowdsim_place_table_robots)."""
+    __slots__ = ()
+    _fields_ = [('r_pos', C.c_void_p), ('r_goal', C.c_void_p), ('r_theta', C.c_void_p), ('rows', C.c_int32),
+                ('case_first', C.c_int32)]
+
+
+# include/crowdsim_b200_table_robots.h, the additive header of the table rows' robots: described apart for the same reason
+# as the scene-table tables, and checked against its own header (tests/test_table_robots_cpu.py).
+TABLE_ROBOT_STRUCTS = {'crowdsim_table_robots': TableRobots}
+TABLE_ROBOT_FUNCTIONS = {
+    'crowdsim_place_table_robots': (_i, [_P(TableRobots), _i, _P(State), _P(Episodes), STREAM]),
+}
+TABLE_ROBOT_EXPORTS = tuple(TABLE_ROBOT_FUNCTIONS)
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
-    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
+    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
     'crowdsim_'), where `lib` has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix
     'oracle_crowdsim_')."""
-    for name, (restype, argtypes) in list(FUNCTIONS.items()) + list(SCENE_TABLE_FUNCTIONS.items()) + list(METRICS_FUNCTIONS.items()):
+    tables = (FUNCTIONS, SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS)
+    for name, (restype, argtypes) in [item for t in tables for item in t.items()]:
         sym = prefix + name[len('crowdsim_'):]
         if hasattr(lib, sym):
             f = getattr(lib, sym)
@@ -248,7 +266,8 @@ def load():
                 'libcrowdsim_b200.so is not built (%s). Run `python -m crowdnav_b200.build` '
                 '(needs nvcc); the product path has no CPU fallback.' % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
-        missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS + METRICS_EXPORTS if not hasattr(lib, name)]
+        missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS + METRICS_EXPORTS + TABLE_ROBOT_EXPORTS
+                   if not hasattr(lib, name)]
         if missing:
             raise CudaLibraryMissing('%s lacks %s: not a library of ABI version %d' % (LIB_PATH, ', '.join(missing), ABI_VERSION))
         declare(lib)

@@ -233,18 +233,25 @@ class MetricsBuffers(object):
 class SceneTable(object):
     """k scenes of the caller's own (crowdsim_scene_table): each row holds the start positions, goals and (radius, v_pref)
     of up to N humans; BatchedCrowdSim.reset_table / enable_autoreset(table=...) hand the rows to env slots through the
-    case queue, and the robot starts as every scene's does (crowd_sim.py:274).
+    case queue. Without robot columns the robot starts as every scene's does (crowd_sim.py:274); with them every row
+    has its own robot (include/crowdsim_b200_table_robots.h).
 
     h_pos, h_goal, h_attr: [k][N][2] float64 arrays; n_humans: [k] humans present per row (default N). Entries i >=
     n_humans[j] are PARKED, as the `mixed` rule parks the humans a scene lacks: position = goal = (PARKED_X + 100 i,
-    PARKED_X), attributes parked_attr, so human_counts() counts the present ones. Refused (ValueError): arrays of other
-    shapes, N > MAX_HUMANS, non-finite values or a radius <= 0 among the present humans, and a present human whose
-    position or goal is on a parked coordinate (x >= PARKED_X / 2). A table is immutable: its arrays are read-only (the
-    device copy is made once per device); build a new table to change a scene."""
+    PARKED_X), attributes parked_attr, so human_counts() counts the present ones.
+    r_pos, r_goal: [k][2] float64, optional and together: the robot's start and goal of each row; r_theta: [k] its heading
+    (default pi / 2, the heading crowd_sim.py:274 gives; only with r_pos and r_goal). The robot's radius and v_pref stay
+    env.config's. BatchedCrowdSim places a row's robot after the reset or install that starts the row's episode and
+    before its first step, so a robot table steps one env-step per launch (BatchedCrowdSim.step).
+    Refused (ValueError): arrays of other shapes, N > MAX_HUMANS, non-finite values or a radius <= 0 among the present
+    humans, a present human whose position or goal is on a parked coordinate (x >= PARKED_X / 2), non-finite robot
+    values, a robot start or goal on a parked coordinate, and r_theta without r_pos / r_goal. A table is immutable: its
+    arrays are read-only (the device copy is made once per device); build a new table to change a scene."""
 
     KEYS = ('h_pos', 'h_goal', 'h_attr', 'n_humans')
+    ROBOT_KEYS = ('r_pos', 'r_goal', 'r_theta')     # saved only by a table with robots
 
-    def __init__(self, h_pos, h_goal, h_attr, n_humans=None, parked_attr=(0.3, 1.0)):
+    def __init__(self, h_pos, h_goal, h_attr, n_humans=None, parked_attr=(0.3, 1.0), r_pos=None, r_goal=None, r_theta=None):
         arrs = [np.array(a, dtype=np.float64) for a in (h_pos, h_goal, h_attr)]
         if arrs[0].ndim != 3 or arrs[0].shape[2] != 2 or arrs[0].shape[0] < 1:
             raise ValueError('h_pos must be [k][N][2] with k >= 1, got %s' % (arrs[0].shape,))
@@ -271,29 +278,70 @@ class SceneTable(object):
         arrs[2][parked] = np.asarray(parked_attr, dtype=np.float64)
         self.h_pos, self.h_goal, self.h_attr = (np.ascontiguousarray(a) for a in arrs)
         self.n_humans = n
-        for a in (self.h_pos, self.h_goal, self.h_attr, self.n_humans):
-            a.setflags(write=False)                 # the validated rows are what device_arrays() uploads, once
+        self.r_pos, self.r_goal, self.r_theta = self._robots(k, r_pos, r_goal, r_theta)
+        for a in (self.h_pos, self.h_goal, self.h_attr, self.n_humans, self.r_pos, self.r_goal, self.r_theta):
+            if a is not None:
+                a.setflags(write=False)             # the validated rows are what device_arrays() uploads, once
         self.k, self.N = k, N
         self._dev = {}
 
+    @staticmethod
+    def _robots(k, r_pos, r_goal, r_theta):
+        """The validated robot columns (r_pos [k][2], r_goal [k][2], r_theta [k]), or three Nones."""
+        if r_pos is None and r_goal is None:
+            if r_theta is not None:
+                raise ValueError('r_theta needs r_pos and r_goal')
+            return None, None, None
+        if r_pos is None or r_goal is None:
+            raise ValueError('a robot table needs both r_pos and r_goal')
+        pos, goal = (np.array(a, dtype=np.float64) for a in (r_pos, r_goal))
+        theta = np.full(k, np.pi / 2) if r_theta is None else np.array(r_theta, dtype=np.float64)
+        for name, a, shape in (('r_pos', pos, (k, 2)), ('r_goal', goal, (k, 2)), ('r_theta', theta, (k,))):
+            if a.shape != shape:
+                raise ValueError('%s must be %s, got %s' % (name, list(shape), a.shape))
+        if not all(np.isfinite(a).all() for a in (pos, goal, theta)):
+            raise ValueError('robot values must be finite')
+        if (pos[:, 0] >= _abi.PARKED_X / 2).any() or (goal[:, 0] >= _abi.PARKED_X / 2).any():
+            raise ValueError('a robot start or goal lies on a parked coordinate (x >= %g)' % (_abi.PARKED_X / 2))
+        return tuple(np.ascontiguousarray(a) for a in (pos, goal, theta))
+
+    @property
+    def has_robots(self):
+        """Whether every row has its own robot (r_pos, r_goal, r_theta)."""
+        return self.r_pos is not None
+
     @classmethod
     def from_scenes(cls, scenes, N, parked_attr=(0.3, 1.0)):
-        """A table from a list of scenes (h_pos, h_goal, h_attr), each [n_i][2] with n_i <= N."""
+        """A table from a list of scenes (h_pos, h_goal, h_attr), each [n_i][2] with n_i <= N, or (h_pos, h_goal, h_attr,
+        robot) with robot = (r_pos, r_goal) or (r_pos, r_goal, r_theta) of that scene. Either every scene has a robot or
+        none has."""
         k = len(scenes)
         h = np.zeros((3, k, N, 2))
         n = np.zeros(k, dtype=np.int64)
+        robots = [sc[3] if len(sc) > 3 else None for sc in scenes]
+        if any(r is None for r in robots) and any(r is not None for r in robots):
+            raise ValueError('either every scene has a robot or none has')
         for j, sc in enumerate(scenes):
-            rows = [np.asarray(a, dtype=np.float64).reshape(-1, 2) for a in sc]
+            rows = [np.asarray(a, dtype=np.float64).reshape(-1, 2) for a in sc[:3]]
             n[j] = rows[0].shape[0]
             if n[j] > N or any(r.shape[0] != n[j] for r in rows):
                 raise ValueError('scene %d: %s humans for N = %d' % (j, [r.shape[0] for r in rows], N))
             for a, r in zip(h, rows):
                 a[j, :n[j]] = r
-        return cls(h[0], h[1], h[2], n, parked_attr)
+        if k == 0 or robots[0] is None:
+            return cls(h[0], h[1], h[2], n, parked_attr)
+        for j, r in enumerate(robots):
+            if len(r) not in (2, 3):
+                raise ValueError('scene %d: a robot is (r_pos, r_goal) or (r_pos, r_goal, r_theta)' % j)
+        r_theta = [r[2] if len(r) == 3 else np.pi / 2 for r in robots]
+        return cls(h[0], h[1], h[2], n, parked_attr, r_pos=[r[0] for r in robots], r_goal=[r[1] for r in robots],
+                   r_theta=r_theta)
 
     def save(self, path):
-        """.npz with keys h_pos, h_goal, h_attr (the padded [k][N][2] arrays) and n_humans [k]."""
-        np.savez(path, h_pos=self.h_pos, h_goal=self.h_goal, h_attr=self.h_attr, n_humans=self.n_humans)
+        """.npz with keys h_pos, h_goal, h_attr (the padded [k][N][2] arrays) and n_humans [k]; a table with robots also
+        r_pos, r_goal [k][2] and r_theta [k]."""
+        robots = dict(r_pos=self.r_pos, r_goal=self.r_goal, r_theta=self.r_theta) if self.has_robots else {}
+        np.savez(path, h_pos=self.h_pos, h_goal=self.h_goal, h_attr=self.h_attr, n_humans=self.n_humans, **robots)
 
     @classmethod
     def load(cls, path):
@@ -302,11 +350,12 @@ class SceneTable(object):
             if missing:
                 raise ValueError('%s lacks %s' % (path, ', '.join(missing)))
             h_pos, h_goal, h_attr, n = (f[key] for key in cls.KEYS)
+            robots = {key: f[key] for key in cls.ROBOT_KEYS if key in f}
         parked_attr = (0.3, 1.0)
         pad = np.arange(h_pos.shape[1])[None, :] >= np.asarray(n)[:, None] if h_pos.ndim == 3 else None
         if pad is not None and pad.any():
             parked_attr = tuple(h_attr[pad][0])                      # as saved
-        return cls(h_pos, h_goal, h_attr, n, parked_attr)
+        return cls(h_pos, h_goal, h_attr, n, parked_attr, **robots)
 
     def has_parked(self, first=0, count=None):
         """Whether any of rows first..first+count-1 lacks humans."""
@@ -314,11 +363,20 @@ class SceneTable(object):
         return bool((self.n_humans[first:first + count] < self.N).any())
 
     def device_arrays(self, device):
-        """(h_pos, h_goal, h_attr) as float64 tensors on `device`, uploaded once."""
+        """(h_pos, h_goal, h_attr) as float64 tensors on `device`, uploaded once, with the robot columns of a robot table
+        (robot_device_arrays)."""
         device = torch.device(device)
         if device not in self._dev:
-            self._dev[device] = tuple(torch.from_numpy(np.array(a)).to(device) for a in (self.h_pos, self.h_goal, self.h_attr))
-        return self._dev[device]
+            up = lambda arrs: tuple(torch.from_numpy(np.array(a)).to(device) for a in arrs)  # noqa: E731
+            self._dev[device] = (up((self.h_pos, self.h_goal, self.h_attr)),
+                                 up((self.r_pos, self.r_goal, self.r_theta)) if self.has_robots else None)
+        return self._dev[device][0]
+
+    def robot_device_arrays(self, device):
+        """(r_pos, r_goal, r_theta) as float64 tensors on `device` (uploaded once by device_arrays), or None without
+        robots."""
+        self.device_arrays(device)
+        return self._dev[torch.device(device)][1]
 
 
 class BatchedCrowdSim(object):
@@ -350,6 +408,7 @@ class BatchedCrowdSim(object):
         self._table = None                          # the SceneTable the case queue counts rows of, or None (generated scenes)
         self._table_rows = (0, 0)                   # the queue's (first row, rows) with a table
         self._scene_src = None                      # (rule, from the case queue?) of the scenes the envs now hold; ('table', True) for table rows
+        self._host_stepped = False                  # a HostStepper captured step(): its graph places no table robots
         self._draw_bufs = None
 
     # ---- configuration -------------------------------------------------------------------------------------------
@@ -495,7 +554,8 @@ class BatchedCrowdSim(object):
         """CrowdSim.get_human_times (crowdsim_human_times) from the end snapshots of the given result rows (episodes that
         ended at the goal; track_arrivals(snapshots=True)): (human_times [k][N], global_time [k], final positions [k][N+1][2]
         robot first). The robot's position and time are the rows' res_final_rpos / res_time, its goal and attributes those
-        every episode starts with (crowd_sim.py:274)."""
+        every episode starts with (crowd_sim.py:274); while a table with robots is in use, the goal is that of the result
+        row's table row (the queue's first row + the result row)."""
         arr, ep = self.arrivals, self.episodes
         if arr is None or arr.k == 0 or ep is None:
             raise ValueError('case_human_times needs track_arrivals(snapshots=True)')
@@ -510,13 +570,20 @@ class BatchedCrowdSim(object):
         snap = dict(h_pos=arr.snap_h_pos[idx].contiguous(), h_vel=arr.snap_h_vel[idx].contiguous(),
                     h_goal=arr.snap_h_goal[idx].contiguous(), h_attr=arr.snap_h_attr[idx].contiguous(),
                     r_pos=ep.res_final_rpos[idx].contiguous(), r_vel=arr.snap_r_vel[idx].contiguous(),
-                    r_goal=f64([0.0, self.circle_radius]), r_attr=f64([self.robot_radius, self.robot_v_pref]),
+                    r_goal=self._case_goals(idx), r_attr=f64([self.robot_radius, self.robot_v_pref]),
                     r_theta=torch.full((k,), np.pi / 2, dtype=torch.float64, device=self.device),
                     g_time=ep.res_time[idx].contiguous())
         st = _abi.State(**{f: _ptr(t) for f, t in snap.items()})
         prm = self.params()
         self._call('human_times', C.byref(prm), k, N, C.byref(st), _ptr(ht), _ptr(gt), _ptr(fp), int(max_steps))
         return ht, gt, fp
+
+    def _case_goals(self, idx):
+        """[k][2] robot goals of the result rows `idx`: the table rows' with a robot table in use, else (0, circle_radius)."""
+        robots = self._robot_table()
+        if robots is None:
+            return torch.tensor([0.0, self.circle_radius], dtype=torch.float64, device=self.device).expand(idx.numel(), 2).contiguous()
+        return robots.robot_device_arrays(self.device)[1][idx + self._table_rows[0]].contiguous()
 
     # ---- reset ---------------------------------------------------------------------------------------------------
     def reset(self, phase='test', cases=None, mask=None, rule=None):
@@ -635,6 +702,10 @@ class BatchedCrowdSim(object):
             raise TypeError('a SceneTable is required, got %s' % type(table).__name__)
         if table.N != self.human_num:
             raise ValueError('the table has %d humans per scene, the env %d' % (table.N, self.human_num))
+        if table.has_robots and self.episodes is None:
+            raise ValueError('a row\'s robot is placed by its episode\'s case: track_episodes before using a table with robots')
+        if table.has_robots and self._host_stepped:
+            raise ValueError('a HostStepper\'s captured step places no table robots: tables with robots are stepped by step()')
         if self._table is not table:
             self._case_counter = None                # a queue over another source's cases does not count these rows
         self._table = table
@@ -674,9 +745,27 @@ class BatchedCrowdSim(object):
         st, ep = self.state.struct(), _struct(self.episodes)
         self._call('reset_table', C.byref(t), _ptr(mask), self.B, self.human_num, C.byref(st), _ref(ep))
         self._keep = (mask, t)
+        self.place_table_robots()
         self._scene_src = ('table', True)
         self._clear_slots(mask)
         return self.observation()
+
+    def _robot_table(self):
+        """The table in use when its rows have robots, else None."""
+        return self._table if self._table is not None and self._table.has_robots else None
+
+    def place_table_robots(self):
+        """crowdsim_place_table_robots (include/crowdsim_b200_table_robots.h): every live env that has not stepped yet gets
+        the robot of its table row (the queue's first row + ep_case): start, goal, heading and zero velocity. reset_table()
+        and step() call it while a table with robots is in use; without one it does nothing."""
+        table = self._robot_table()
+        if table is None:
+            return
+        r_pos, r_goal, r_theta = table.robot_device_arrays(self.device)
+        r = _abi.TableRobots(r_pos=_ptr(r_pos), r_goal=_ptr(r_goal), r_theta=_ptr(r_theta), rows=table.k,
+                             case_first=self._table_rows[0])
+        st, ep = self.state.struct(), self.episodes.struct()
+        self._call('place_table_robots', C.byref(r), self.B, C.byref(st), C.byref(ep))
 
     def clear_table(self):
         """Back to generated scenes: the table is no longer in use and its case queue is dropped (set_case_queue then
@@ -756,7 +845,16 @@ class BatchedCrowdSim(object):
         record: a memory.DeviceRLRecorder -- with an ORCA robot the same n_steps steps through crowdsim_step_n_record_ex
         (no actions); with an external robot one step with `actions` (n_steps = 1), booked around it by crowdsim_record_book
         and its rows staged by pack_joint (a recorder with sort_humans=True: LSTM-RL's sorted rows and, with maps, the
-        sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full."""
+        sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full.
+        With a table whose rows have robots in use (SceneTable r_pos / r_goal), every env-step is a launch of its own
+        (n_steps of them) followed by place_table_robots(), so an episode the step's auto-reset installs gets its row's robot
+        before its first step; such rollouts record nothing (ValueError with `record`)."""
+        robots = self._robot_table()
+        if robots is not None:
+            if record is not None:
+                raise ValueError('rollouts from a table with robots record nothing: step() without a recorder')
+            if self.episodes is None:
+                raise ValueError('a row\'s robot is placed by its episode\'s case: track_episodes before stepping a table with robots')
         if record is not None and self.metrics is not None:
             raise ValueError('recorded rollouts do not measure episode metrics: track_metrics is for rollouts without a recorder')
         if record is not None and getattr(record, 'rl', False):
@@ -780,19 +878,25 @@ class BatchedCrowdSim(object):
             if actions.data_ptr() != self.action.data_ptr():
                 self.action.copy_(actions, non_blocking=True)
         prm, st, io = self.params(), self.state.struct(), self._io()
+        # a robot table: n_steps launches of one env-step, each followed by the placement
+        per_launch, launches = (1, int(n_steps)) if robots is not None else (int(n_steps), 1)
         head = (C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(_struct(self.episodes)),
-                _ref(_struct(self.autoreset)), int(n_steps))
+                _ref(_struct(self.autoreset)), per_launch)
         if self.metrics is not None:
             if self.episodes is None or self.metrics.k != self.episodes.k:
                 # the kernels write row ep_case of arrays the C struct does not size: never past their end
                 raise ValueError('metric rows: %d, the episode results %s'
                                  % (self.metrics.k, None if self.episodes is None else self.episodes.k))
             arr = None if self.arrivals is None else C.byref(self.arrivals.struct())
-            self._call('step_n_metrics', *head, arr, C.byref(self.metrics.struct()))
+            name, tail = 'step_n_metrics', (arr, C.byref(self.metrics.struct()))
         elif self.arrivals is not None:
-            self._call('step_n_arrivals', *head, C.byref(self.arrivals.struct()))
+            name, tail = 'step_n_arrivals', (C.byref(self.arrivals.struct()),)
         else:
-            self._call('step_n', *head)
+            name, tail = 'step_n', ()
+        for _ in range(launches):
+            self._call(name, *head, *tail)
+            if robots is not None:
+                self.place_table_robots()
         return self.observation(), self.reward, self.done, self.info
 
     def _io(self, obs32=True):
@@ -997,6 +1101,11 @@ class HostStepper(object):
     generating scenes (env.prefetch())."""
 
     def __init__(self, env, next_orca_action=True, obs='f32', prefetch_every=4, transfer='copy'):
+        if env._robot_table() is not None:
+            # the captured step would install fresh episodes whose robots nothing places before the next-action kernel
+            # and the next step read them
+            raise ValueError('HostStepper does not place the robots of a scene table: step tables with robots with env.step()')
+        env._host_stepped = True
         assert obs in ('f32', 'f64') and transfer in ('copy', 'direct')
         assert transfer == 'copy' or obs == 'f32', "transfer='direct' serves the float32 observation"
         self.env, self.obs, self.transfer = env, obs, transfer

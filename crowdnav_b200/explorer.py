@@ -31,7 +31,10 @@ them to rank 0, which prints the log lines.
 
 run_k_episodes(k, phase, scenes=table): the k cases are the rows of a batched.SceneTable (case i = row i) instead of the
 phase's generated scenes, streamed through the same queue and auto-reset (crowdsim_prefetch_table); human times are
-refused when a row parks humans, numpy-stream exploration always (a table scene has no seed).
+refused when a row parks humans, numpy-stream exploration always (a table scene has no seed). A table whose rows have
+robots (SceneTable r_pos / r_goal) runs one env-step per launch, each followed by the placement of the robots of episodes
+that have not stepped yet (BatchedCrowdSim.place_table_robots), so the ORCA robot's several steps per launch become one;
+such a rollout records nothing (update_memory=True is refused).
 
 BatchedExplorer(..., human_times=True): the humans' time to goal after every successful episode (crowd_nav/test.py:105-107,
 "Average time for humans to reach goal"). The step kernels stamp the arrivals and keep each episode's end state
@@ -227,7 +230,8 @@ class BatchedExplorer(object):
     def run_k_episodes(self, k, phase, update_memory=False, imitation_learning=False, episode=None,
                        print_failure=False, prefetch_every=2, check_every=32, steps_per_launch=8, scenes=None):
         """scenes: a batched.SceneTable whose rows 0..k-1 are the k cases (case i = row i; rank r of a multi-GPU run takes
-        its contiguous range of rows) instead of the phase's generated scenes; case_counter[phase] is left alone."""
+        its contiguous range of rows) instead of the phase's generated scenes; case_counter[phase] is left alone. With
+        robot columns each case's robot starts, heads for its goal and faces as its row says."""
         env = self.env
         if update_memory and (self.memory is None or self.gamma is None):
             raise ValueError('Memory or gamma value is not set!')            # explorer.py:93-94
@@ -242,6 +246,8 @@ class BatchedExplorer(object):
                 raise ValueError('exploration from numpy\'s stream follows the seeded generator\'s scenes: table scenes '
                                  'have no seed')
             rule = 'table'
+            if scenes.has_robots and update_memory:
+                raise ValueError('rollouts from a table with robots record nothing: update_memory=False')
             if self.human_times and scenes.has_parked(0, k):
                 # humans a scene lacks are parked, as for rule mixed
                 raise ValueError('human times are not defined for scenes with parked humans')
@@ -327,8 +333,8 @@ class BatchedExplorer(object):
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per
         # launch (crowdsim_step_n, or crowdsim_step_n_record_ex when it also records); a step-by-step recorder or a host-side
         # policy needs every step
-        if not (self.robot_policy == 'orca' and recorder is None):
-            chunk = 1
+        if not (self.robot_policy == 'orca' and recorder is None) or (scenes is not None and scenes.has_robots):
+            chunk = 1                                  # (a robot table: placed between launches of one env-step each)
         if chunk > 1:
             prefetch_every, check_every = 1, max(1, check_every // chunk)
         from .batched import max_episode_steps

@@ -6,7 +6,8 @@ print_failure=True), with every case streamed through --num_envs environments on
 log lines. --policy is orca (the robot's ORCA runs inside the step kernels) or one of the trainable policies of
 policy.policy_factory. --human_times adds the humans' average time to goal over the successful cases
 (BatchedExplorer(human_times=True)). --scenes FILE.npz runs the scenes of a saved batched.SceneTable, one case per row,
-instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it). --metrics adds
+instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it); a file saved
+with robot columns (r_pos, r_goal, r_theta) also gives every case its own robot start, goal and heading. --metrics adds
 one line: the rate of episodes with a human-human collision, the overlapping pairs per episode, the robot's average path
 length and closest approach (BatchedExplorer(metrics=True)). --results FILE.npz saves every case's result row, one array per
 column (explorer.result_columns: the reference's columns, then human_times and the metric columns when asked for), so two

@@ -14,7 +14,8 @@
  * the humans of each scene from a table of `rows` scenes instead -- a scenario of the caller's own, a fixed evaluation set,
  * or the reference's own scenes bit for bit -- and hand them out through the same case queue in the same slot order, so
  * Explorer.run_k_episodes-style runs stream k table rows through B <= k env slots with the step kernels' auto-reset
- * install unchanged. The robot is reset as crowd_sim.py:274 resets it (per-scene robots are not part of a table).
+ * install unchanged. The robot is reset as crowd_sim.py:274 resets it; a robot of each row's own is placed afterwards by
+ * crowdsim_place_table_robots (include/crowdsim_b200_table_robots.h), which this header's entry points do not read.
  */
 #ifndef CROWDSIM_B200_SCENE_TABLE_H
 #define CROWDSIM_B200_SCENE_TABLE_H
