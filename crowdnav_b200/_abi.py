@@ -11,8 +11,8 @@ scene-table entry points, the same way (load() requires and declares them too). 
 tests/test_abi_cpu.py pins crowdsim_b200.h's entry points and structs (31 and 12) and requires STRUCTS / FUNCTIONS to mirror
 exactly that header; tests/test_scene_table_cpu.py checks these tables against the scene-table header and the test oracle's
 restatement (tests/native/scene_table_oracle.c). METRICS_STRUCTS / METRICS_FUNCTIONS describe
-include/crowdsim_b200_metrics.h the same way, and TABLE_ROBOT_STRUCTS / TABLE_ROBOT_FUNCTIONS
-include/crowdsim_b200_table_robots.h.
+include/crowdsim_b200_metrics.h the same way, TABLE_ROBOT_STRUCTS / TABLE_ROBOT_FUNCTIONS
+include/crowdsim_b200_table_robots.h, and HUMAN_METRICS_STRUCTS / HUMAN_METRICS_FUNCTIONS include/crowdsim_b200_human_metrics.h.
 Structs are filled by field name (`Episodes(ep_case=..., ...)`): they have no instance __dict__, so a name that is not
 one of the C fields raises instead of being dropped.
 """
@@ -215,6 +215,23 @@ METRICS_FUNCTIONS = {
 METRICS_EXPORTS = tuple(METRICS_FUNCTIONS)
 
 
+class HumanMetrics(C.Structure):
+    """crowdsim_human_metrics: per-slot-and-human accumulators [B][N], per-result-row outputs [k][N] of each human's closest
+    approach and danger steps, and each result row's colliding human [k] (crowdsim_step_n_human_metrics)."""
+    __slots__ = ()
+    _fields_ = [('ep_h_closest', C.c_void_p), ('ep_h_danger', C.c_void_p), ('res_h_closest', C.c_void_p),
+                ('res_h_danger', C.c_void_p), ('res_collider', C.c_void_p)]
+
+
+# include/crowdsim_b200_human_metrics.h, the additive header of the per-human metrics: described apart for the same reason
+# as the scene-table tables, and checked against its own header (tests/test_human_metrics_cpu.py).
+HUMAN_METRICS_STRUCTS = {'crowdsim_human_metrics': HumanMetrics}
+HUMAN_METRICS_FUNCTIONS = {
+    'crowdsim_step_n_human_metrics': (_i, _STEP + [_i, _P(Arrivals), _P(Metrics), _P(HumanMetrics), STREAM]),
+}
+HUMAN_METRICS_EXPORTS = tuple(HUMAN_METRICS_FUNCTIONS)
+
+
 class TableRobots(C.Structure):
     """crowdsim_table_robots: the robot start, goal and heading of every scene-table row (crowdsim_place_table_robots)."""
     __slots__ = ()
@@ -232,10 +249,10 @@ TABLE_ROBOT_EXPORTS = tuple(TABLE_ROBOT_FUNCTIONS)
 
 
 def declare(lib, prefix='crowdsim_', with_stream=True):
-    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
+    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
     'crowdsim_'), where `lib` has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix
     'oracle_crowdsim_')."""
-    tables = (FUNCTIONS, SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS)
+    tables = (FUNCTIONS, SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS)
     for name, (restype, argtypes) in [item for t in tables for item in t.items()]:
         sym = prefix + name[len('crowdsim_'):]
         if hasattr(lib, sym):
@@ -267,7 +284,7 @@ def load():
                 '(needs nvcc); the product path has no CPU fallback.' % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
         missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS + METRICS_EXPORTS + TABLE_ROBOT_EXPORTS
-                   if not hasattr(lib, name)]
+                   + HUMAN_METRICS_EXPORTS if not hasattr(lib, name)]
         if missing:
             raise CudaLibraryMissing('%s lacks %s: not a library of ABI version %d' % (LIB_PATH, ', '.join(missing), ABI_VERSION))
         declare(lib)

@@ -230,6 +230,33 @@ class MetricsBuffers(object):
                             res_hh_pairs=_ptr(self.res_hh_pairs))
 
 
+class HumanMetricsBuffers(object):
+    """crowdsim_human_metrics (include/crowdsim_b200_human_metrics.h): each slot's running per-human closest approach and
+    danger-step count [B][N], the same two per result row of k [k][N], and each row's colliding human [k] (-1: the episode
+    did not end in a collision), written when an episode ends."""
+
+    def __init__(self, B, N, k, device):
+        self.k = k
+        self.ep_h_closest = torch.full((B, N), math.inf, dtype=torch.float64, device=device)
+        self.ep_h_danger = torch.zeros((B, N), dtype=torch.int32, device=device)
+        self.res_h_closest = torch.full((k, N), math.inf, dtype=torch.float64, device=device)
+        self.res_h_danger = torch.zeros((k, N), dtype=torch.int32, device=device)
+        self.res_collider = torch.full((k,), -1, dtype=torch.int32, device=device)
+
+    def clear(self, mask=None):
+        """A fresh episode's accumulators for the slots of `mask` (uint8, None = all), as a reset leaves them."""
+        for t, v in ((self.ep_h_closest, math.inf), (self.ep_h_danger, 0)):
+            if mask is None:
+                t.fill_(v)
+            else:
+                t.masked_fill_((mask != 0)[:, None], v)
+
+    def struct(self):
+        return _abi.HumanMetrics(ep_h_closest=_ptr(self.ep_h_closest), ep_h_danger=_ptr(self.ep_h_danger),
+                                 res_h_closest=_ptr(self.res_h_closest), res_h_danger=_ptr(self.res_h_danger),
+                                 res_collider=_ptr(self.res_collider))
+
+
 class SceneTable(object):
     """k scenes of the caller's own (crowdsim_scene_table): each row holds the start positions, goals and (radius, v_pref)
     of up to N humans; BatchedCrowdSim.reset_table / enable_autoreset(table=...) hand the rows to env slots through the
@@ -403,6 +430,7 @@ class BatchedCrowdSim(object):
         self.state = None; self.episodes = None; self.autoreset = None
         self.arrivals = None
         self.metrics = None
+        self.human_metrics = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
         self._table = None                          # the SceneTable the case queue counts rows of, or None (generated scenes)
@@ -461,6 +489,7 @@ class BatchedCrowdSim(object):
         self._scene_mt = torch.empty((624, B), dtype=torch.int32, device=self.device)
         self.arrivals = None
         self.metrics = None
+        self.human_metrics = None
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -488,6 +517,8 @@ class BatchedCrowdSim(object):
         self.fit_arrival_snapshots()
         if self.metrics is not None and self.metrics.k != k:
             self.fit_metrics()
+        if self.human_metrics is not None and self.human_metrics.k != k:
+            self.fit_human_metrics()
         return self.episodes
 
     def fit_metrics(self):
@@ -497,6 +528,13 @@ class BatchedCrowdSim(object):
         self.metrics = MetricsBuffers(self.B, self.episodes.k, self.device)
         for f in ('ep_path', 'ep_closest', 'ep_hh_steps', 'ep_hh_pairs'):
             getattr(self.metrics, f).copy_(getattr(m, f))
+
+    def fit_human_metrics(self):
+        """fit_metrics for the per-human rows of track_human_metrics."""
+        h = self.human_metrics
+        self.human_metrics = HumanMetricsBuffers(self.B, self.human_num, self.episodes.k, self.device)
+        for f in ('ep_h_closest', 'ep_h_danger'):
+            getattr(self.human_metrics, f).copy_(getattr(h, f))
 
     # ---- episode metrics ----------------------------------------------------------------------------------------------
     def track_metrics(self):
@@ -509,6 +547,17 @@ class BatchedCrowdSim(object):
         self.metrics = MetricsBuffers(self.B, self.episodes.k, self.device)
         return self.metrics
 
+    def track_human_metrics(self):
+        """Measure every episode's per-human closest approach and danger steps (clearance < discomfort_dist), and which human
+        a collision hits, from now on (crowdsim_step_n_human_metrics, include/crowdsim_b200_human_metrics.h). Needs
+        track_episodes: an episode's rows go to its result row (human_metrics.res_*). Parked humans never update. Every slot
+        starts a fresh episode's accumulators; reset and auto-reset installs clear them again. Recorded rollouts refuse
+        tracked per-human metrics."""
+        if self.episodes is None:
+            raise ValueError('per-human metrics are kept per result row: track_episodes first')
+        self.human_metrics = HumanMetricsBuffers(self.B, self.human_num, self.episodes.k, self.device)
+        return self.human_metrics
+
     def _device_mask(self, mask):
         """A reset's `mask` as the uint8 tensor on this batch's device that the kernels read (None stays None)."""
         if mask is not None and not (isinstance(mask, torch.Tensor) and mask.dtype == torch.uint8 and mask.device == self.device):
@@ -517,7 +566,7 @@ class BatchedCrowdSim(object):
 
     def _clear_slots(self, mask):
         """What a reset clears beside the state and the episode accumulators: arrival stamps (crowd_sim.py:263-265) and
-        the metrics accumulators."""
+        the metrics and per-human metrics accumulators."""
         if self.arrivals is not None:
             if mask is None:
                 self.arrivals.h_arrival.zero_()
@@ -525,6 +574,8 @@ class BatchedCrowdSim(object):
                 self.arrivals.h_arrival.masked_fill_((mask != 0)[:, None], 0.0)
         if self.metrics is not None:
             self.metrics.clear(mask)
+        if self.human_metrics is not None:
+            self.human_metrics.clear(mask)
 
     def fit_arrival_snapshots(self):
         """The end snapshots of track_arrivals(snapshots=True) are indexed by result row: after the episode rows change
@@ -857,6 +908,9 @@ class BatchedCrowdSim(object):
                 raise ValueError('a row\'s robot is placed by its episode\'s case: track_episodes before stepping a table with robots')
         if record is not None and self.metrics is not None:
             raise ValueError('recorded rollouts do not measure episode metrics: track_metrics is for rollouts without a recorder')
+        if record is not None and self.human_metrics is not None:
+            raise ValueError('recorded rollouts do not measure per-human metrics: track_human_metrics is for rollouts without a '
+                             'recorder')
         if record is not None and getattr(record, 'rl', False):
             return self._step_record_rl(actions, int(n_steps), record)
         if record is not None and self.arrivals is not None:
@@ -887,6 +941,14 @@ class BatchedCrowdSim(object):
                 # the kernels write row ep_case of arrays the C struct does not size: never past their end
                 raise ValueError('metric rows: %d, the episode results %s'
                                  % (self.metrics.k, None if self.episodes is None else self.episodes.k))
+        if self.human_metrics is not None:
+            if self.episodes is None or self.human_metrics.k != self.episodes.k:
+                raise ValueError('per-human metric rows: %d, the episode results %s'
+                                 % (self.human_metrics.k, None if self.episodes is None else self.episodes.k))
+            arr = None if self.arrivals is None else C.byref(self.arrivals.struct())
+            met = None if self.metrics is None else C.byref(self.metrics.struct())
+            name, tail = 'step_n_human_metrics', (arr, met, C.byref(self.human_metrics.struct()))
+        elif self.metrics is not None:
             arr = None if self.arrivals is None else C.byref(self.arrivals.struct())
             name, tail = 'step_n_metrics', (arr, C.byref(self.metrics.struct()))
         elif self.arrivals is not None:

@@ -4,6 +4,7 @@
 #include <type_traits>
 #include "crowdsim_common.cuh"
 #include "../../include/crowdsim_b200_metrics.h"
+#include "../../include/crowdsim_b200_human_metrics.h"
 
 namespace cs {
 
@@ -46,6 +47,7 @@ struct StepArgs {
                                  // the same reason
     crowdsim_arrivals arr;       // crowdsim_step_n_arrivals: read only by the ARR instantiations; last for the same reason
     crowdsim_metrics met;        // crowdsim_step_n_metrics: read only by the MET instantiations; last for the same reason
+    crowdsim_human_metrics hm;   // crowdsim_step_n_human_metrics: read only by the HM instantiations; last for the same reason
 };
 
 // ---- MET = true (include/crowdsim_b200_metrics.h): one env's running accumulators ----
@@ -100,6 +102,39 @@ __device__ __forceinline__ bool hh_overlap(double2 pi, double ri, double2 pj, do
 {
     const double dx = pi.x - pj.x, dy = pi.y - pj.y;
     return sqrt(dx * dx + dy * dy) - ri - rj < 0;
+}
+
+// ---- HM = true (include/crowdsim_b200_human_metrics.h): one human's running accumulators, on the lane that computes its
+// clearance ----
+struct HumAcc {
+    double closest;
+    int danger;
+};
+__device__ __forceinline__ HumAcc hm_fresh()
+{
+    return HumAcc{ __longlong_as_double(0x7ff0000000000000LL), 0 };
+}
+__device__ __forceinline__ HumAcc hm_load(const crowdsim_human_metrics &h, size_t hi)
+{
+    return HumAcc{ h.ep_h_closest[hi], h.ep_h_danger[hi] };
+}
+__device__ __forceinline__ void hm_store(const crowdsim_human_metrics &h, size_t hi, const HumAcc &a)
+{
+    h.ep_h_closest[hi] = a.closest; h.ep_h_danger[hi] = a.danger;
+}
+// Human a's part of the result row c of the episode that ended.
+__device__ __forceinline__ void hm_result(const crowdsim_human_metrics &h, int c, int N, int a, const HumAcc &acc)
+{
+    const size_t j = (size_t)c * N + a;
+    h.res_h_closest[j] = acc.closest; h.res_h_danger[j] = acc.danger;
+}
+// One live step of a human with pre-step x = px and clearance cl. A parked human (the `mixed` rule's and the scene tables'
+// absent humans, include/crowdsim_b200.h) never updates.
+__device__ __forceinline__ void hm_add(HumAcc &a, double px, double cl, double discomfort_dist)
+{
+    if (!(px < CROWDSIM_PARKED_X / 2)) return;
+    if (cl < a.closest) a.closest = cl;
+    a.danger += (cl < discomfort_dist) ? 1 : 0;
 }
 
 // Launch a multi-step kernel after setting its shared-memory carve-out (crowdsim_common.cuh). A carve-out error is
@@ -178,6 +213,15 @@ static inline int check_metrics(const crowdsim_metrics *m, const crowdsim_episod
 {
     if (!m || !ep || !m->ep_path || !m->ep_closest || !m->ep_hh_steps || !m->ep_hh_pairs || !m->res_path || !m->res_closest ||
         !m->res_hh_steps || !m->res_hh_pairs) return CROWDSIM_EINVAL;
+    return CROWDSIM_OK;
+}
+
+// crowdsim_step_n_human_metrics' argument rules (include/crowdsim_b200_human_metrics.h): at N = 0 the [.][N] arrays are
+// empty, and only res_collider is required.
+static inline int check_human_metrics(const crowdsim_human_metrics *h, const crowdsim_episodes *ep, int N)
+{
+    if (!h || !ep || !h->res_collider) return CROWDSIM_EINVAL;
+    if (N > 0 && (!h->ep_h_closest || !h->ep_h_danger || !h->res_h_closest || !h->res_h_danger)) return CROWDSIM_EINVAL;
     return CROWDSIM_OK;
 }
 

@@ -47,6 +47,9 @@ namespace cs {
 // MET: crowdsim_step_n_metrics -- the robot lane keeps its env's metrics accumulators (include/crowdsim_b200_metrics.h) in
 // registers; the human pairs (a, a + d) are tested on lane a, one ballot per d. MET = false compiles to the SASS the kernel
 // had before MET.
+// HM: crowdsim_step_n_human_metrics -- each human lane keeps its accumulators (include/crowdsim_b200_human_metrics.h) in
+// registers and writes its part of a finished episode's row; the robot lane's clearance fold names the colliding human.
+// HM = false compiles to the SASS the kernel had before HM.
 #ifndef CS_FLAT_WPB
 #define CS_FLAT_WPB 4
 #endif
@@ -65,7 +68,7 @@ struct RobotRec {
     uint8_t want, o_done, any_live, dirty_ep, new_case;
 };
 
-template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false, bool MET = false>
+template <int N, int STAGE = 99, bool ROT = false, bool WARPQ = false, bool ARR = false, bool MET = false, bool HM = false>
 __global__ void __launch_bounds__(32 * CS_FLAT_WPB, CS_FLAT_MINBLOCKS * 4 / CS_FLAT_WPB)
 step_flat_kernel(const __grid_constant__ StepArgs A)
 {
@@ -117,6 +120,8 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     }
     MetAcc ma = {};                                         // MET: robot lane of a valid env
     if constexpr (MET) { if (env_ok && is_robot) ma = met_load(A.met, e); }
+    HumAcc ha = {};                                         // HM: human lanes of valid envs
+    if constexpr (HM) { if (env_ok && !is_robot) ha = hm_load(A.hm, hi); }
     if constexpr (STAGE == 1) {            // loads + stores only
         const bool live1 = env_ok && (act_flag != 0);
         if (live1 && !is_robot) { st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, make_double2(vel.x + goal.x * 0, vel.y + attr.x * 0)); }
@@ -259,12 +264,14 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
     // ---- human lanes: swept-segment clearance ----
     double closest = 0.0;
     if (live && !is_robot) closest = swept_clearance(pos, vel, make_double2(Rpx, Rpy), make_double2(Rvx, Rvy), attr.x, Rrad, dt);
+    if constexpr (HM) { if (live && !is_robot) hm_add(ha, pos.x, closest, k.discomfort_dist); }
     // ordered fold over the env's humans (first collision breaks, crowd_sim.py:346-351); consumed by the robot lane
     double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
+    int collider = -1;                                       // HM: the human the fold breaks at
     #pragma unroll
     for (int i = 0; i < N; ++i) {
         const double ci = __shfl_sync(CS_FULL, closest, ebase + i);
-        if (!collision) { if (ci < 0) collision = true; else if (ci < dmin) dmin = ci; }
+        if (!collision) { if (ci < 0) { collision = true; if constexpr (HM) collider = i; } else if (ci < dmin) dmin = ci; }
     }
     // MET: the env's overlapping human pairs on the pre-step positions (crowd_sim.py:353-362), consumed by the robot lane
     int hh_pairs = 0;
@@ -319,6 +326,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
                         ep.res_return[ep_c] = ep_ret; ep.res_too_close[ep_c] = ep_tc; ep.res_min_dist_sum[ep_c] = ep_mds;
                         if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
                         if constexpr (ARR) { snap_c = ep_c; if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, ep_c, vel); }
+                        if constexpr (HM) { snap_c = ep_c; A.hm.res_collider[ep_c] = (info == CROWDSIM_INFO_COLLISION) ? collider : -1; }
                     }
                     if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                 }
@@ -349,6 +357,11 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             if (snap >= 0) arr_snap_human(A, snap, N, a, np_, make_double2((double)nv.x, (double)nv.y), goal, attr, t);
         }
     }
+    if constexpr (HM) {
+        // the humans' part of the row of the episode that ended this step, before an install clears the accumulators
+        const int snap = __shfl_sync(CS_FULL, snap_c, rl);
+        if (live && !is_robot && snap >= 0) hm_result(A.hm, snap, N, a, ha);
+    }
     if (A.has_ar) {                                          // warp-uniform
         install = __shfl_sync(CS_FULL, install, rl) && env_ok;
         // the scene goes straight from the slot to the live state (ar_install_*: acquire on the slot flag, copy)
@@ -359,6 +372,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
             } else {
                 ar_install_human(A, e, N, a);
                 if constexpr (ARR) A.arr.h_arrival[hi] = 0.0;                       // crowd_sim.py:263-265
+                if constexpr (HM) hm_store(A.hm, hi, hm_fresh());
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, hi); reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
             }
         }
@@ -371,6 +385,7 @@ step_flat_kernel(const __grid_constant__ StepArgs A)
         pos = make_double2(pos.x + hx * dt, pos.y + hy * dt); vel = make_double2(hx, hy);
         st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
         if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, nv.x, nv.y);
+        if constexpr (HM) hm_store(A.hm, hi, ha);
     }
 }
 

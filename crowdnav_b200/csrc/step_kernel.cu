@@ -41,7 +41,10 @@ namespace cs {
 // MET = true: crowdsim_step_n_metrics (include/crowdsim_b200_metrics.h): the env's human lanes test its pairs in N / 2 rounds,
 // counted with a ballot per round and added to a shared counter; the robot lane books them with the path length and dmin. MET = false compiles to
 // the SASS the kernel had before MET. (At most 128 envs per block: N = 0.)
-template <bool MID, bool ARR = false, bool MET = false>
+// HM = true: crowdsim_step_n_human_metrics (include/crowdsim_b200_human_metrics.h): each human lane keeps its accumulators
+// and writes its part of a finished episode's row; the robot lane's clearance fold names the colliding human. HM = false
+// compiles to the SASS the kernel had before HM.
+template <bool MID, bool ARR = false, bool MET = false, bool HM = false>
 __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) step_kernel(const __grid_constant__ StepArgs A)
 {
     extern __shared__ __align__(16) unsigned char smem[];
@@ -103,6 +106,10 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
     // ---- human lanes: swept-segment clearance against the robot ----
     const double dt = k.time_step;
     if (live && !is_robot) s.closest[tid] = swept_clearance(pos, vel, s.pos64[le * L + N], s.act[le], attr.x, s.rad64[le * L + N], dt);
+    HumAcc ha = {};                                          // HM: human lanes of live envs
+    if constexpr (HM) {
+        if (live && !is_robot) { ha = hm_load(A.hm, (size_t)e * N + a); hm_add(ha, pos.x, s.closest[tid], k.discomfort_dist); }
+    }
     if constexpr (MET) {
         // crowd_sim.py:353-362 on the pre-step positions. Round d pairs human a with human (a + d) mod N: rounds 1 .. N / 2
         // cover every pair once (the last round of an even N only from a < N / 2), so every human lane tests at most
@@ -135,9 +142,10 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
         bool done = false;
         if (live) {
             double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
+            int collider = -1;                      // HM: the human the loop breaks at
             for (int i = 0; i < N; ++i) {           // crowd_sim.py:346-351 (first collision breaks; dmin only matters without one)
                 const double c = s.closest[le * L + i];
-                if (c < 0) { collision = true; break; }
+                if (c < 0) { collision = true; if constexpr (HM) collider = i; break; }
                 else if (c < dmin) dmin = c;
             }
             const bool rot = k.robot_policy == CROWDSIM_ROBOT_EXTERNAL_ROT;
@@ -178,22 +186,27 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
                         ep.res_return[c] = ret; ep.res_too_close[c] = tc; ep.res_min_dist_sum[c] = mds;
                         if (ep.res_final_rpos) st2(ep.res_final_rpos, c, npos);
                         if constexpr (ARR) { snap_c = c; if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, c, nvel); }
+                        if constexpr (HM) { snap_c = c; A.hm.res_collider[c] = (info == CROWDSIM_INFO_COLLISION) ? collider : -1; }
                     }
                     if (A.st.active && !A.has_ar) A.st.active[e] = 0;
                 }
             }
-            if constexpr (ARR) s.act[le] = make_double2(ntime, (double)snap_c);   // (the humans read s.act[le] before the last barrier)
+            if constexpr (ARR || HM) s.act[le] = make_double2(ntime, (double)snap_c);   // (the humans read s.act[le] before the last barrier)
         }
         if (A.has_ar) install = ar_decide(A, e, ld_relaxed_u8(A.ar.n_state + e), live && done, !live && A.ar.want[e] != 0);
     }
-    if constexpr (ARR) {
-        // the humans' post-step positions, stamped and, when the episode ended, snapshotted before an install replaces them
+    if constexpr (ARR || HM) {
+        // ARR: the humans' post-step positions, stamped and, when the episode ended, snapshotted before an install replaces
+        // them; HM: the humans' part of the ended episode's row
         __syncthreads();
         if (live && !is_robot) {
             const double2 tc = s.act[le];                            // (post-step global_time, result row or -1)
-            const double2 np_ = make_double2(pos.x + (double)nv.x * dt, pos.y + (double)nv.y * dt);
-            const double t = arr_stamp(A, (size_t)e * N + a, np_, goal, attr.x, tc.x);
-            if (tc.y >= 0) arr_snap_human(A, (int)tc.y, N, a, np_, make_double2((double)nv.x, (double)nv.y), goal, attr, t);
+            if constexpr (ARR) {
+                const double2 np_ = make_double2(pos.x + (double)nv.x * dt, pos.y + (double)nv.y * dt);
+                const double t = arr_stamp(A, (size_t)e * N + a, np_, goal, attr.x, tc.x);
+                if (tc.y >= 0) arr_snap_human(A, (int)tc.y, N, a, np_, make_double2((double)nv.x, (double)nv.y), goal, attr, t);
+            }
+            if constexpr (HM) { if (tc.y >= 0) hm_result(A.hm, (int)tc.y, N, a, ha); }
         }
     }
     if (A.has_ar) {
@@ -207,6 +220,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
             } else {
                 ar_install_human(A, e, N, a);
                 if constexpr (ARR) A.arr.h_arrival[(size_t)e * N + a] = 0.0;      // crowd_sim.py:263-265
+                if constexpr (HM) hm_store(A.hm, (size_t)e * N + a, hm_fresh());
                 if (A.io.obs32) { const double2 np_ = ld2_cg(A.ar.n_h_pos, (size_t)e * N + a); reinterpret_cast<float4 *>(A.io.obs32)[(size_t)e * N + a] = make_float4((float)np_.x, (float)np_.y, 0.f, 0.f); }
             }
         }
@@ -222,6 +236,7 @@ __global__ void __launch_bounds__(MID ? 128 : 256, MID ? CS_MID_MINBLOCKS : 1) s
         st2(A.st.h_pos, i, np_);
         st2(A.st.h_vel, i, make_double2(hx, hy));
         if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[i] = make_float4((float)np_.x, (float)np_.y, nv.x, nv.y);
+        if constexpr (HM) hm_store(A.hm, i, ha);
     }
 }
 
@@ -295,6 +310,7 @@ struct StepMode {
     double *la_pos = nullptr, *la_vel = nullptr;    // crowdsim_onestep_lookahead: the humans' next states go here
     const crowdsim_arrivals *arr = nullptr;         // crowdsim_step_n_arrivals: the ARR instantiations
     const crowdsim_metrics *met = nullptr;          // crowdsim_step_n_metrics: the MET instantiations (arr optional)
+    const crowdsim_human_metrics *hm = nullptr;     // crowdsim_step_n_human_metrics: the HM instantiations (arr, met optional)
     const crowdsim_record *rec = nullptr;           // crowdsim_step_n_record*: stage the steps for an IL recorder
     bool rec_any_route = false;                     // _ex / _rot: every N >= 1, through the launch loop off the multi route
     bool rec_rot = false;                           // _rot: the rows of a unicycle robot
@@ -308,6 +324,7 @@ static int check(const crowdsim_params *prm, int B, int N, const crowdsim_state 
     if (!prm || !st || !io || B < 0 || N < 0 || n_steps < 1) return CROWDSIM_EINVAL;
     if (m.arr) { const int rc = check_arrivals(m.arr, ep); if (rc != CROWDSIM_OK) return rc; }
     if (m.met) { const int rc = check_metrics(m.met, ep); if (rc != CROWDSIM_OK) return rc; }
+    if (m.hm) { const int rc = check_human_metrics(m.hm, ep, N); if (rc != CROWDSIM_OK) return rc; }
     if (const crowdsim_record *rec = m.rec) {
         // crowdsim_step_n_record: only the recording instantiation of the multi-step kernel records. crowdsim_step_n_record_ex
         // (rec_any_route): every N >= 1, through the launch loop where the multi-step kernel does not run
@@ -386,7 +403,8 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
     if (m.recm) A.recm = *m.recm; else memset(&A.recm, 0, sizeof(A.recm));
     if (m.arr) A.arr = *m.arr; else memset(&A.arr, 0, sizeof(A.arr));
     if (m.met) A.met = *m.met; else memset(&A.met, 0, sizeof(A.met));
-    const bool arr = (m.arr != nullptr), met = (m.met != nullptr);
+    if (m.hm) A.hm = *m.hm; else memset(&A.hm, 0, sizeof(A.hm));
+    const bool arr = (m.arr != nullptr), met = (m.met != nullptr), hm = (m.hm != nullptr);
     switch (route(A, n_steps, m.rec != nullptr)) {
     case Route::act:
         with_int<1, 5>(N, [&](auto n) { orca_act_kernel<n><<<(B + 127) / 128, 128, 0, stream>>>(A); });
@@ -397,8 +415,8 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         A.n_steps = n_steps;
         if (m.rec) { ++g_launches; return launch_multi_record(A, blocks, stream, m.rec_rot); }
         const int err = with_int<2, 5>(N, [&](auto n) { return with_bool(A.k.robot_visible, [&](auto vis) { return with_bool(arr, [&](auto ar_on) {
-            return with_bool(met, [&](auto met_on) {
-                return launch_carved<step_multi_kernel<n, vis, false, false, ar_on, met_on>>(A, blocks, 32 * (n + 1), stream); }); }); }); });
+            return with_bool(met, [&](auto met_on) { return with_bool(hm, [&](auto hm_on) {
+                return launch_carved<step_multi_kernel<n, vis, false, false, ar_on, met_on, hm_on>>(A, blocks, 32 * (n + 1), stream); }); }); }); }); });
         if (err != CROWDSIM_OK) return err;
         ++g_launches;
         return (int)cudaGetLastError();
@@ -414,9 +432,10 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         // kernel exists with the per-warp queue only.
         const bool warpq = blocks * CS_FLAT_WPB <= 12 * sm_count();
         return launch_loop(A, n_steps, m, stream, [&] { with_int<1, 5>(N, [&](auto n) { with_bool(arr, [&](auto ar_on) { with_bool(met, [&](auto met_on) {
-            if (rot) step_flat_kernel<n, 99, true, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
-            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
-            else step_flat_kernel<n, 99, false, false, ar_on, met_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); }); }); }); });
+            with_bool(hm, [&](auto hm_on) {
+            if (rot) step_flat_kernel<n, 99, true, true, ar_on, met_on, hm_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else if (warpq) step_flat_kernel<n, 99, false, true, ar_on, met_on, hm_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A);
+            else step_flat_kernel<n, 99, false, false, ar_on, met_on, hm_on><<<blocks, 32 * CS_FLAT_WPB, 0, stream>>>(A); }); }); }); }); });
     }
     case Route::loop: {
         const int threads = A.EPB * A.L;
@@ -424,12 +443,13 @@ static int launch(const crowdsim_params *prm, int B, int N, const crowdsim_state
         const bool mid = !g_force_generic && N > 5;          // (N = 0 and the forced A/B route stay on the generic kernel)
         const size_t smem = mid ? stage_bytes_mid(A.EPB, A.L, mid_lp3_floats()) : stage_bytes(A.EPB, A.L, A.k.nb_alloc, threads);
         return with_bool(mid, [&](auto mid_) { return with_bool(arr, [&](auto ar_on) { return with_bool(met, [&](auto met_on) {
-            constexpr auto kernel = step_kernel<mid_, ar_on, met_on>;
+          return with_bool(hm, [&](auto hm_on) {
+            constexpr auto kernel = step_kernel<mid_, ar_on, met_on, hm_on>;
             if (smem > 48 * 1024) {                          // (a per-device attribute; setting it again is cheap)
                 const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 if (err != cudaSuccess) return (int)err;
             }
-            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(A); }); }); }); });
+            return launch_loop(A, n_steps, m, stream, [&] { kernel<<<blocks, threads, smem, stream>>>(A); }); }); }); }); });
     }
     }
     return CROWDSIM_EINVAL;   // (unreachable: route() returns one of the four)
@@ -464,6 +484,16 @@ extern "C" int crowdsim_step_n_metrics(const crowdsim_params *prm, int B, int N,
 {
     if (!met) return CROWDSIM_EINVAL;
     cs::StepMode m; m.arr = arr; m.met = met;
+    return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
+}
+
+extern "C" int crowdsim_step_n_human_metrics(const crowdsim_params *prm, int B, int N, crowdsim_state *st, crowdsim_step_io *io,
+                                             crowdsim_episodes *ep, const crowdsim_autoreset *ar, int n_steps,
+                                             const crowdsim_arrivals *arr, const crowdsim_metrics *met,
+                                             const crowdsim_human_metrics *hm, void *stream)
+{
+    if (!hm) return CROWDSIM_EINVAL;
+    cs::StepMode m; m.arr = arr; m.met = met; m.hm = hm;
     return cs::launch(prm, B, N, st, io, ep, ar, n_steps, stream, m);
 }
 

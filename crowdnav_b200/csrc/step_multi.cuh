@@ -206,13 +206,17 @@ __device__ __forceinline__ void rec_map_state(const crowdsim_record_maps &m, int
 // MET = true (crowdsim_step_n_metrics, not with REC): each human tests its pairs (a, j > a) on the step's shared float64 view
 // and adds its env's overlaps to a shared counter before the clearance barrier; the robot books them with its path length
 // and dmin in its tail, its accumulators in shared memory beside RobotRec. MET = false compiles to the SASS it had before MET.
-template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false, bool MET = false>
+// HM = true (crowdsim_step_n_human_metrics, not with REC): each human keeps its accumulators in registers across the steps,
+// updates them from its clearance, writes its part of a finished episode's row where it decides the ending and stores them
+// once at the end; the robot's clearance fold names the colliding human. HM = false compiles to the SASS it had before HM.
+template <int N, bool VIS, bool REC, bool ROT = false, bool ARR = false, bool MET = false, bool HM = false>
 __global__ void __launch_bounds__(32 * (N + 1), CS_MULTI_WARPS / (N + 1))
 step_multi_kernel(const __grid_constant__ StepArgs A)
 {
     static_assert(REC || !ROT, "unicycle rows are a recording variant");
     static_assert(!(REC && ARR), "arrivals are stamped by the rollout kernels only");
     static_assert(!(REC && MET), "metrics are measured by the rollout kernels only");
+    static_assert(!(REC && HM), "per-human metrics are measured by the rollout kernels only");
     static_assert(N >= 2 && N <= 5, "small crowds with at least two humans (N = 1 runs n single-step launches)");
     using namespace orca;
     CS_RES_BEGIN
@@ -287,6 +291,8 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     RobotRec &rr = s_rr[le];                                 // robot threads of valid envs only
     bool arrived = false;                                    // ARR: my h_arrival is non-zero
     if constexpr (ARR) { if (env_ok && !is_robot) arrived = A.arr.h_arrival[hi] != 0.0; }
+    HumAcc ha = {};                                          // HM: human threads of valid envs
+    if constexpr (HM) { if (env_ok && !is_robot) ha = hm_load(A.hm, hi); }
 
     // what this launch changed on this thread (decides the stores at the end)
     bool dirty_kin = false, dirty_scene = false;
@@ -423,13 +429,14 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
     // read their env's clearances after the barrier below without another one
     double *const s_cl = reinterpret_cast<double *>(&s_r2[0][0]);     // [E * N]: the humans' clearances
     bool timeout = false, reaching_goal = false;                       // robot lanes of live envs
-    int arr_c = -1;                                                    // ARR: my env's result row, read before the robot's tail
+    int arr_c = -1;                                                    // ARR, HM: my env's result row, read before the robot's tail
     if (!is_robot) {
         if (live) {
             // swept-segment clearance against the robot's velocity of this step
             const int rt = 32 * N + le;
             const float2 rv = s_nv[rt];
             s_cl[tid] = swept_clearance(pos, vel, s_pos[rt], make_double2((double)rv.x, (double)rv.y), attr.x, s_rad[rt], dt);
+            if constexpr (HM) { hm_add(ha, pos.x, s_cl[tid], k.discomfort_dist); arr_c = rr.ep_c; }
             // agent.py:122-135 holonomic step with the ORCA action (float32 values widened); a scene installed below replaces it
             if constexpr (MET) {
                 // crowd_sim.py:353-362 on the pre-step positions: my pairs (a, j > a)
@@ -485,6 +492,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 if constexpr (ARR) {
                     if (done && arr_c >= 0) arr_snap_human(A, arr_c, N, a, pos, vel, s_goal[tid], attr, arrived ? A.arr.h_arrival[hi] : 0.0);
                 }
+                if constexpr (HM) { if (done && arr_c >= 0) hm_result(A.hm, arr_c, N, a, ha); }
             }
             if (A.has_ar && ((live && done) || (!live && (pf & PRE_WANT)))) {
                 act_flag = (pf & PRE_READY) ? 1 : 0;                                      // install, or park
@@ -493,6 +501,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                     pos = ld2_cg(A.ar.n_h_pos, hi); vel = make_double2(0, 0); s_goal[tid] = ld2_cg(A.ar.n_h_goal, hi); attr = ld2_cg(A.ar.n_h_attr, hi);
                     dirty_kin = true; dirty_scene = true;
                     if constexpr (ARR) { A.arr.h_arrival[hi] = 0.0; arrived = false; }       // crowd_sim.py:263-265
+                    if constexpr (HM) ha = hm_fresh();
                 }
             }
         }
@@ -504,10 +513,11 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                 const double ax = (double)nv.x, ay = (double)nv.y;
                 // ordered fold of the humans' clearances (first collision breaks, crowd_sim.py:346-351)
                 double dmin = __longlong_as_double(0x7ff0000000000000LL); bool collision = false;
+                int collider = -1;                           // HM: the human the fold breaks at
                 #pragma unroll
                 for (int i = 0; i < N; ++i) {
                     const double ci = s_cl[le * N + i];
-                    if (!collision) { if (ci < 0) collision = true; else if (ci < dmin) dmin = ci; }
+                    if (!collision) { if (ci < 0) { collision = true; if constexpr (HM) collider = i; } else if (ci < dmin) dmin = ci; }
                 }
                 // ladder (crowd_sim.py:365-389), update (agent.py:110-135), bookkeeping (explorer.py:41-72)
                 const double npx = pos.x + ax * dt, npy = pos.y + ay * dt;
@@ -542,6 +552,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
                             if (ep.res_final_rpos) st2(ep.res_final_rpos, ep_c, pos);
                             if constexpr (ARR) { if (A.arr.snap_r_vel) st2(A.arr.snap_r_vel, ep_c, vel); }
                             if constexpr (MET) met_result(A.met, ep_c, met_acc_smem<E>()[le]);
+                            if constexpr (HM) A.hm.res_collider[ep_c] = (info == CROWDSIM_INFO_COLLISION) ? collider : -1;
                         }
                         if (A.st.active && !A.has_ar) { A.st.active[e] = 0; act_flag = 0; }
                     }
@@ -590,6 +601,7 @@ step_multi_kernel(const __grid_constant__ StepArgs A)
             if (dirty_kin) {
                 st2(A.st.h_pos, hi, pos); st2(A.st.h_vel, hi, vel);
                 if (A.io.obs32) reinterpret_cast<float4 *>(A.io.obs32)[hi] = make_float4((float)pos.x, (float)pos.y, (float)vel.x, (float)vel.y);
+                if constexpr (HM) hm_store(A.hm, hi, ha);
             }
             if (dirty_scene) { st2(A.st.h_goal, hi, s_goal[tid]); st2(A.st.h_attr, hi, attr); }
         } else {

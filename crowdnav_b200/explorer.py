@@ -44,10 +44,16 @@ BatchedExplorer(..., human_times=True): the humans' time to goal after every suc
 BatchedExplorer(..., metrics=True): each episode's human-human collision steps and pairs, robot path length and closest
 approach, measured inside the step kernels (BatchedCrowdSim.track_metrics, include/crowdsim_b200_metrics.h). The result
 rows then end with 4 more columns (METRIC_COLUMNS) and summarize logs one more line after the reference's.
+
+BatchedExplorer(..., human_metrics=True): each episode's per-human closest approach and danger steps (clearance below
+discomfort_dist), and the human a collision hit, measured inside the step kernels (BatchedCrowdSim.track_human_metrics,
+include/crowdsim_b200_human_metrics.h). The result rows then end with 2 N + 1 more columns (HUMAN_METRIC_COLUMNS: N closest
+approaches, N danger counts, the colliding human or -1) and summarize logs one more line after the others.
 """
 import logging
 import math
 
+import numpy as np
 import torch
 
 from . import _abi
@@ -72,12 +78,13 @@ def shard_range(k, rank, world):
 
 RESULT_COLUMNS = ('info', 'steps', 'time', 'return', 'too_close', 'min_dist_sum')
 METRIC_COLUMNS = ('hh_steps', 'hh_pairs', 'path_length', 'closest_approach')
+HUMAN_METRIC_COLUMNS = ('h_closest', 'h_danger', 'collider')     # [N], [N] and 1 column
 
 
-def pack_results(ep, n, human_times=None, metrics=None):
+def pack_results(ep, n, human_times=None, metrics=None, human_metrics=None):
     """Per-case result rows of an EpisodeBuffers as one [n][6] float64 tensor (exact for the integer columns); with
     human_times ([n][N] float64) the rows are [n][6 + N]; with metrics (batched.MetricsBuffers) 4 more columns follow,
-    METRIC_COLUMNS."""
+    METRIC_COLUMNS; with human_metrics (batched.HumanMetricsBuffers) 2 N + 1 more, HUMAN_METRIC_COLUMNS."""
     cols = [ep.res_info[:n].double(), ep.res_steps[:n].double(), ep.res_time[:n], ep.res_return[:n],
             ep.res_too_close[:n].double(), ep.res_min_dist_sum[:n]]
     rows = torch.stack(cols, dim=1)
@@ -87,19 +94,36 @@ def pack_results(ep, n, human_times=None, metrics=None):
         m = torch.stack([metrics.res_hh_steps[:n].double(), metrics.res_hh_pairs[:n].double(), metrics.res_path[:n],
                          metrics.res_closest[:n]], dim=1)
         rows = torch.cat([rows, m.to(rows.device)], dim=1)
+    if human_metrics is not None:
+        h = human_metrics
+        m = torch.cat([h.res_h_closest[:n], h.res_h_danger[:n].double(), h.res_collider[:n, None].double()], dim=1)
+        rows = torch.cat([rows, m.to(rows.device)], dim=1)
     return rows.contiguous()
 
 
-def result_columns(rows, metrics=False):
+def split_human_metrics(a, human_metrics):
+    """(rows without the per-human columns, {HUMAN_METRIC_COLUMNS name: [k][N] / [k][N] / [k]}) of result rows `a` (a numpy
+    array or nested lists) that end with the per-human columns of human_metrics = N humans."""
+    N = int(human_metrics)
+    a = np.asarray(a, dtype=np.float64).reshape(len(a), -1)
+    cut = a.shape[1] - (2 * N + 1)
+    return a[:, :cut], {'h_closest': a[:, cut:cut + N], 'h_danger': a[:, cut + N:cut + 2 * N], 'collider': a[:, cut + 2 * N]}
+
+
+def result_columns(rows, metrics=False, human_metrics=None):
     """{column name: numpy array} of gathered result rows: RESULT_COLUMNS, 'human_times' [k][N] when the rows carry human
-    times, and METRIC_COLUMNS with metrics."""
+    times, METRIC_COLUMNS with metrics, and HUMAN_METRIC_COLUMNS with human_metrics = N, the rows' number of humans."""
     a = rows.cpu().numpy()
+    hm = {}
+    if human_metrics is not None:
+        a, hm = split_human_metrics(a, human_metrics)
     out = {name: a[:, i] for i, name in enumerate(RESULT_COLUMNS)}
     end = a.shape[1] - (len(METRIC_COLUMNS) if metrics else 0)
     if end > len(RESULT_COLUMNS):
         out['human_times'] = a[:, len(RESULT_COLUMNS):end]
     if metrics:
         out.update({name: a[:, end + i] for i, name in enumerate(METRIC_COLUMNS)})
+    out.update(hm)
     return out
 
 
@@ -117,12 +141,18 @@ def gather_results(local_rows, k, rank, world, group=None):
     return torch.cat([out[r][:shard_range(k, r, world)[1]] for r in range(world)], dim=0)
 
 
-def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info, metrics=False):
+def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info, metrics=False,
+              human_metrics=None):
     """explorer.py:52-90 on gathered per-case rows ([k][6]: info, steps, time, return, too_close, min_dist_sum; [k][6 + N]
     with the human times of BatchedExplorer(human_times=True)). Returns the statistics as a dict and emits the reference's
     log lines through `log`. metrics=True: the rows end with METRIC_COLUMNS (BatchedExplorer(metrics=True)), and one more
-    line follows the reference's."""
+    line follows the reference's. human_metrics = N: the rows end with the HUMAN_METRIC_COLUMNS of N humans
+    (BatchedExplorer(human_metrics=True)), and one more line follows all the others."""
     rows = rows.cpu().tolist()
+    hm = None
+    if human_metrics is not None:
+        a, hm = split_human_metrics(rows, human_metrics)
+        rows = a.tolist()
     met = None
     if metrics:
         met = [r[-len(METRIC_COLUMNS):] for r in rows]
@@ -188,6 +218,21 @@ def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure
             'average closest approach: {:.2f}'.format(phase.upper(), stats['hh_collision_rate'],
                                                       stats['hh_pairs_per_episode'], stats['avg_path_length'],
                                                       stats['avg_closest_approach']))
+    if hm is not None:
+        # what the reference computes and drops: each human's clearance of crowd_sim.py:331-345 and the human its collision
+        # loop breaks at. A parked human keeps +inf and 0 and is left out: the present humans are those with a finite
+        # closest approach
+        closest, danger, collider = hm['h_closest'], hm['h_danger'], hm['collider']
+        present = np.isfinite(closest)
+        stats['h_closest'] = closest.tolist()
+        stats['h_danger'] = danger.astype(np.int64).tolist()
+        stats['collider'] = collider.astype(np.int64).tolist()
+        stats['avg_h_closest'] = float(closest[present].mean()) if present.any() else math.inf
+        stats['h_discomfort_per_episode'] = float(((danger > 0) & present).sum()) / k
+        stats['collisions_by_human'] = [int((collider == i).sum()) for i in range(int(human_metrics))]
+        log('{:<5} per-human closest approach: {:.2f}, humans entered discomfort per episode: {:.2f}, collisions by human: '
+            '{}'.format(phase.upper(), stats['avg_h_closest'], stats['h_discomfort_per_episode'],
+                        stats['collisions_by_human']))
     return stats
 
 
@@ -209,10 +254,11 @@ def _unicycle_rows(policy):
 
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
-                 rank=0, world=1, group=None, human_times=False, metrics=False):
+                 rank=0, world=1, group=None, human_times=False, metrics=False, human_metrics=False):
         self.env = env
         self.human_times = bool(human_times)
         self.metrics = bool(metrics)
+        self.human_metrics = bool(human_metrics)
         self.robot_policy = robot_policy
         self.device = device or env.device
         self.memory = memory
@@ -258,14 +304,17 @@ class BatchedExplorer(object):
             raise ValueError('human times are measured by rollouts that do not record (update_memory=False)')
         if self.metrics and update_memory:
             raise ValueError('episode metrics are measured by rollouts that do not record (update_memory=False)')
+        if self.human_metrics and update_memory:
+            raise ValueError('per-human metrics are measured by rollouts that do not record (update_memory=False)')
         first_case = env.case_counter[phase]
         start, n_local = shard_range(k, self.rank, self.world)
         gamma = self.gamma if self.gamma is not None else 0.9
         args = (env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
                 steps_per_launch, first_case, start, n_local, gamma, rule, scenes)
-        if not (self.human_times or self.metrics):
+        if not (self.human_times or self.metrics or self.human_metrics):
             return self._run(*args)
         prev_arrivals, prev_metrics = env.arrivals, env.metrics     # the caller's tracking, back in place after the run
+        prev_human_metrics = env.human_metrics
         try:
             return self._run(*args)
         finally:
@@ -276,6 +325,10 @@ class BatchedExplorer(object):
                 env.metrics = prev_metrics
                 if prev_metrics is not None and env.episodes is not None and prev_metrics.k != env.episodes.k:
                     env.fit_metrics()
+            if self.human_metrics:
+                env.human_metrics = prev_human_metrics
+                if prev_human_metrics is not None and env.episodes is not None and prev_human_metrics.k != env.episodes.k:
+                    env.fit_human_metrics()
 
     def _run(self, env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
              steps_per_launch, first_case, start, n_local, gamma, rule, scenes):
@@ -284,6 +337,8 @@ class BatchedExplorer(object):
             env.track_arrivals(snapshots=True)
         if self.metrics:
             env.track_metrics()
+        if self.human_metrics:
+            env.track_human_metrics()
         if scenes is None:
             env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
             env.enable_autoreset(rule)
@@ -372,7 +427,8 @@ class BatchedExplorer(object):
             ok = torch.nonzero(ep.res_info[:n_local] == _abi.INFO_REACHGOAL).flatten()
             if ok.numel():
                 local_times[ok] = env.case_human_times(ok)[0]
-        rows = gather_results(pack_results(ep, n_local, local_times, env.metrics if self.metrics else None), k, self.rank,
+        rows = gather_results(pack_results(ep, n_local, local_times, env.metrics if self.metrics else None,
+                                           env.human_metrics if self.human_metrics else None), k, self.rank,
                               self.world, self.group)
         if scenes is None:
             env.case_counter[phase] = (first_case + k) % env.case_size[phase]
@@ -382,6 +438,7 @@ class BatchedExplorer(object):
         self.last_rows = rows
         if self.rank != 0:
             return None
-        stats = summarize(rows, k, phase, env.time_limit, env.time_step, episode, print_failure, metrics=self.metrics)
+        stats = summarize(rows, k, phase, env.time_limit, env.time_step, episode, print_failure, metrics=self.metrics,
+                          **({'human_metrics': env.human_num} if self.human_metrics else {}))
         self.last_env_steps = stats['env_steps']
         return stats

@@ -9,9 +9,11 @@ policy.policy_factory. --human_times adds the humans' average time to goal over 
 instead of the phase's generated ones (k = its number of rows; --square / --circle do not combine with it); a file saved
 with robot columns (r_pos, r_goal, r_theta) also gives every case its own robot start, goal and heading. --metrics adds
 one line: the rate of episodes with a human-human collision, the overlapping pairs per episode, the robot's average path
-length and closest approach (BatchedExplorer(metrics=True)). --results FILE.npz saves every case's result row, one array per
-column (explorer.result_columns: the reference's columns, then human_times and the metric columns when asked for), so two
-checkpoints can be compared case by case. Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
+length and closest approach (BatchedExplorer(metrics=True)). --human_metrics adds one line: the present humans' average
+closest approach, how many humans entered the discomfort distance per episode and how many collisions hit each human index
+(BatchedExplorer(human_metrics=True)). --results FILE.npz saves every case's result row, one array per column
+(explorer.result_columns: the reference's columns, then human_times, the metric columns and h_closest [k][N], h_danger
+[k][N] and collider [k] when asked for), so two checkpoints can be compared case by case. Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
 changes nothing: the run is always on cuda:0.
 """
 import argparse
@@ -43,6 +45,7 @@ def parse_args(argv=None):
     parser.add_argument('--scenes', type=str, default=None)
     parser.add_argument('--metrics', default=False, action='store_true')
     parser.add_argument('--results', type=str, default=None)
+    parser.add_argument('--human_metrics', default=False, action='store_true')
     return parser, parser.parse_args(argv)
 
 
@@ -99,7 +102,8 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
     if args.circle:
         env.test_sim = 'circle_crossing'
     explorer = explorer_class(env, policy, device, gamma=0.9, human_times=args.human_times,
-                              **({'metrics': True} if args.metrics else {}))
+                              **({'metrics': True} if args.metrics else {}),
+                              **({'human_metrics': True} if args.human_metrics else {}))
 
     if policy == 'orca':
         # test.py:77-85: no safety space for ORCA, visible robot or not
@@ -118,15 +122,17 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
     else:
         stats = explorer.run_k_episodes(env.case_size[args.phase], args.phase, print_failure=True)
     if args.results is not None:
-        save_results(args.results, explorer.last_rows, args.metrics)
+        save_results(args.results, explorer.last_rows, args.metrics,
+                     **({'human_metrics': env.human_num} if args.human_metrics else {}))
     return stats
 
 
-def save_results(path, rows, metrics=False):
-    """--results: every case's result row as an .npz of one array per column (explorer.result_columns)."""
+def save_results(path, rows, metrics=False, human_metrics=None):
+    """--results: every case's result row as an .npz of one array per column (explorer.result_columns; human_metrics = N,
+    the rows' number of humans, when they carry the per-human columns)."""
     import numpy as np
     from .explorer import result_columns
-    np.savez(path, **result_columns(rows, metrics))
+    np.savez(path, **result_columns(rows, metrics, human_metrics))
 
 
 if __name__ == '__main__':
