@@ -12,7 +12,8 @@ tests/test_abi_cpu.py pins crowdsim_b200.h's entry points and structs (31 and 12
 exactly that header; tests/test_scene_table_cpu.py checks these tables against the scene-table header and the test oracle's
 restatement (tests/native/scene_table_oracle.c). METRICS_STRUCTS / METRICS_FUNCTIONS describe
 include/crowdsim_b200_metrics.h the same way, TABLE_ROBOT_STRUCTS / TABLE_ROBOT_FUNCTIONS
-include/crowdsim_b200_table_robots.h, and HUMAN_METRICS_STRUCTS / HUMAN_METRICS_FUNCTIONS include/crowdsim_b200_human_metrics.h.
+include/crowdsim_b200_table_robots.h, HUMAN_METRICS_STRUCTS / HUMAN_METRICS_FUNCTIONS include/crowdsim_b200_human_metrics.h,
+and TRAJECTORY_STRUCTS / TRAJECTORY_FUNCTIONS include/crowdsim_b200_trajectories.h.
 Structs are filled by field name (`Episodes(ep_case=..., ...)`): they have no instance __dict__, so a name that is not
 one of the C fields raises instead of being dropped.
 """
@@ -248,11 +249,29 @@ TABLE_ROBOT_FUNCTIONS = {
 TABLE_ROBOT_EXPORTS = tuple(TABLE_ROBOT_FUNCTIONS)
 
 
+class Trajectories(C.Structure):
+    """crowdsim_trajectories: every result row's robot [k][T][9] and human [k][T][N][8] states before each step
+    (crowdsim_capture_states)."""
+    __slots__ = ()
+    _fields_ = [('r_traj', C.c_void_p), ('h_traj', C.c_void_p), ('k', C.c_int32), ('T', C.c_int32)]
+
+
+# include/crowdsim_b200_trajectories.h, the additive header of the per-step states: described apart for the same reason as
+# the scene-table tables, and checked against its own header (tests/test_trajectories_cpu.py).
+TRAJECTORY_STRUCTS = {'crowdsim_trajectories': Trajectories}
+TRAJECTORY_FUNCTIONS = {
+    'crowdsim_capture_states': (_i, [_P(Trajectories), _i, _i, _P(State), _P(Episodes), STREAM]),
+}
+TRAJECTORY_EXPORTS = tuple(TRAJECTORY_FUNCTIONS)
+
+
 def declare(lib, prefix='crowdsim_', with_stream=True):
-    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
+    """Attach each FUNCTIONS (and SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS,
+    TRAJECTORY_FUNCTIONS) entry's restype / argtypes to the symbol `prefix` + (its name after
     'crowdsim_'), where `lib` has one; with_stream=False drops the trailing stream (the oracle's host restatements: prefix
     'oracle_crowdsim_')."""
-    tables = (FUNCTIONS, SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS)
+    tables = (FUNCTIONS, SCENE_TABLE_FUNCTIONS, METRICS_FUNCTIONS, TABLE_ROBOT_FUNCTIONS, HUMAN_METRICS_FUNCTIONS,
+              TRAJECTORY_FUNCTIONS)
     for name, (restype, argtypes) in [item for t in tables for item in t.items()]:
         sym = prefix + name[len('crowdsim_'):]
         if hasattr(lib, sym):
@@ -284,7 +303,7 @@ def load():
                 '(needs nvcc); the product path has no CPU fallback.' % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
         missing = [name for name in EXPORTS + SCENE_TABLE_EXPORTS + METRICS_EXPORTS + TABLE_ROBOT_EXPORTS
-                   + HUMAN_METRICS_EXPORTS if not hasattr(lib, name)]
+                   + HUMAN_METRICS_EXPORTS + TRAJECTORY_EXPORTS if not hasattr(lib, name)]
         if missing:
             raise CudaLibraryMissing('%s lacks %s: not a library of ABI version %d' % (LIB_PATH, ', '.join(missing), ABI_VERSION))
         declare(lib)

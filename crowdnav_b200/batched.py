@@ -257,6 +257,20 @@ class HumanMetricsBuffers(object):
                                  res_collider=_ptr(self.res_collider))
 
 
+class TrajectoryBuffers(object):
+    """crowdsim_trajectories (include/crowdsim_b200_trajectories.h): every result row's robot state [k][T][9] (px py vx vy
+    gx gy radius v_pref theta) and human states [k][T][N][8] (px py vx vy gx gy radius v_pref) before each of its steps,
+    NaN where no step was captured."""
+
+    def __init__(self, k, T, N, device):
+        self.k, self.T, self.N = k, T, N
+        self.r_traj = torch.full((k, T, 9), math.nan, dtype=torch.float64, device=device)
+        self.h_traj = torch.full((k, T, N, 8), math.nan, dtype=torch.float64, device=device)
+
+    def struct(self):
+        return _abi.Trajectories(r_traj=_ptr(self.r_traj), h_traj=_ptr(self.h_traj), k=self.k, T=self.T)
+
+
 class SceneTable(object):
     """k scenes of the caller's own (crowdsim_scene_table): each row holds the start positions, goals and (radius, v_pref)
     of up to N humans; BatchedCrowdSim.reset_table / enable_autoreset(table=...) hand the rows to env slots through the
@@ -431,6 +445,7 @@ class BatchedCrowdSim(object):
         self.arrivals = None
         self.metrics = None
         self.human_metrics = None
+        self.trajectories = None
         self._case_counter = None; self._case_total = 0; self._seed_base = 0; self._case_first = 0; self._case_wrap = 0
         self._ar_rule = None; self._ar_seed_stride = 0
         self._table = None                          # the SceneTable the case queue counts rows of, or None (generated scenes)
@@ -490,6 +505,7 @@ class BatchedCrowdSim(object):
         self.arrivals = None
         self.metrics = None
         self.human_metrics = None
+        self.trajectories = None
 
     def set_robot_policy(self, kind):
         self.robot_policy = {'orca': _abi.ROBOT_ORCA, 'external_xy': _abi.ROBOT_EXTERNAL_XY, 'holonomic': _abi.ROBOT_EXTERNAL_XY,
@@ -519,6 +535,8 @@ class BatchedCrowdSim(object):
             self.fit_metrics()
         if self.human_metrics is not None and self.human_metrics.k != k:
             self.fit_human_metrics()
+        if self.trajectories is not None and self.trajectories.k != k:
+            self.track_trajectories()
         return self.episodes
 
     def fit_metrics(self):
@@ -557,6 +575,33 @@ class BatchedCrowdSim(object):
             raise ValueError('per-human metrics are kept per result row: track_episodes first')
         self.human_metrics = HumanMetricsBuffers(self.B, self.human_num, self.episodes.k, self.device)
         return self.human_metrics
+
+    # ---- per-step states ------------------------------------------------------------------------------------------------
+    def track_trajectories(self):
+        """Keep every result row's states before each of its steps from now on: the reference's env.states
+        (crowd_sim.py:391-393). Allocates TrajectoryBuffers(k, T = max_episode_steps, N), NaN-filled so rows no step reached
+        stay visible; track_episodes with another k allocates new ones. step() then runs one env-step per launch, each
+        preceded by capture_states(), so row t of a case is its state before step t. Needs track_episodes. Recorded rollouts
+        and a HostStepper refuse it."""
+        if self.episodes is None:
+            raise ValueError('trajectories are kept per result row: track_episodes first')
+        if self._host_stepped:
+            raise ValueError('a HostStepper\'s captured step captures no states: trajectories are stepped by step()')
+        self.trajectories = TrajectoryBuffers(self.episodes.k, max_episode_steps(self.time_limit, self.time_step),
+                                              self.human_num, self.device)
+        return self.trajectories
+
+    def capture_states(self):
+        """crowdsim_capture_states (include/crowdsim_b200_trajectories.h): every live env with a result row writes its
+        current state to row (ep_case, ep_steps) of the trajectory buffers. step() calls it before every env-step while
+        trajectories are tracked."""
+        tr = self.trajectories
+        if self.episodes is None or tr.k != self.episodes.k:
+            # the kernel writes row ep_case of arrays the C struct sizes: never rows of another episode buffer
+            raise ValueError('trajectory rows: %d, the episode results %s'
+                             % (tr.k, None if self.episodes is None else self.episodes.k))
+        t, st, ep = tr.struct(), self.state.struct(), self.episodes.struct()
+        self._call('capture_states', C.byref(t), self.B, self.human_num, C.byref(st), C.byref(ep))
 
     def _device_mask(self, mask):
         """A reset's `mask` as the uint8 tensor on this batch's device that the kernels read (None stays None)."""
@@ -899,7 +944,9 @@ class BatchedCrowdSim(object):
         sorted human state, crowdsim_pack_joint_sorted). The recorder flushes its reinforcement-learning pairs when its staging is full.
         With a table whose rows have robots in use (SceneTable r_pos / r_goal), every env-step is a launch of its own
         (n_steps of them) followed by place_table_robots(), so an episode the step's auto-reset installs gets its row's robot
-        before its first step; such rollouts record nothing (ValueError with `record`)."""
+        before its first step; such rollouts record nothing (ValueError with `record`).
+        With trajectories tracked (track_trajectories) every env-step is a launch of its own too, preceded by
+        capture_states(): place -> capture -> step; recorded rollouts refuse it."""
         robots = self._robot_table()
         if robots is not None:
             if record is not None:
@@ -910,6 +957,9 @@ class BatchedCrowdSim(object):
             raise ValueError('recorded rollouts do not measure episode metrics: track_metrics is for rollouts without a recorder')
         if record is not None and self.human_metrics is not None:
             raise ValueError('recorded rollouts do not measure per-human metrics: track_human_metrics is for rollouts without a '
+                             'recorder')
+        if record is not None and self.trajectories is not None:
+            raise ValueError('recorded rollouts do not capture trajectories: track_trajectories is for rollouts without a '
                              'recorder')
         if record is not None and getattr(record, 'rl', False):
             return self._step_record_rl(actions, int(n_steps), record)
@@ -932,8 +982,10 @@ class BatchedCrowdSim(object):
             if actions.data_ptr() != self.action.data_ptr():
                 self.action.copy_(actions, non_blocking=True)
         prm, st, io = self.params(), self.state.struct(), self._io()
-        # a robot table: n_steps launches of one env-step, each followed by the placement
-        per_launch, launches = (1, int(n_steps)) if robots is not None else (int(n_steps), 1)
+        # a robot table or trajectories: n_steps launches of one env-step, each followed by the placement and preceded by
+        # the capture
+        traj = self.trajectories is not None
+        per_launch, launches = (1, int(n_steps)) if robots is not None or traj else (int(n_steps), 1)
         head = (C.byref(prm), self.B, self.human_num, C.byref(st), C.byref(io), _ref(_struct(self.episodes)),
                 _ref(_struct(self.autoreset)), per_launch)
         if self.metrics is not None:
@@ -956,6 +1008,8 @@ class BatchedCrowdSim(object):
         else:
             name, tail = 'step_n', ()
         for _ in range(launches):
+            if traj:
+                self.capture_states()
             self._call(name, *head, *tail)
             if robots is not None:
                 self.place_table_robots()
@@ -1167,6 +1221,8 @@ class HostStepper(object):
             # the captured step would install fresh episodes whose robots nothing places before the next-action kernel
             # and the next step read them
             raise ValueError('HostStepper does not place the robots of a scene table: step tables with robots with env.step()')
+        if env.trajectories is not None:
+            raise ValueError('HostStepper does not capture trajectories: step an env that tracks them with env.step()')
         env._host_stepped = True
         assert obs in ('f32', 'f64') and transfer in ('copy', 'direct')
         assert transfer == 'copy' or obs == 'f32', "transfer='direct' serves the float32 observation"

@@ -19,8 +19,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 TARGET = os.path.join(CSRC, 'libcrowdsim_b200.so')
 SOURCES = ['step_kernel.cu', 'reset_kernel.cu', 'pack_kernel.cu', 'times_kernel.cu', 'record_kernel.cu', 'draws_kernel.cu',
-           'table_robot_kernel.cu']
-HEADERS = ['crowdsim_common.cuh', 'orca_device.cuh', 'step_flat.cuh', 'step_multi.cuh', 'step_mid.cuh', 'orca_spec.cuh', 'rotate.cuh', 'step_args.cuh', 'occupancy.cuh', 'scene.cuh', os.path.join('..', '..', 'include', 'crowdsim_b200.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_scene_table.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_metrics.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_table_robots.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_human_metrics.h')]
+           'table_robot_kernel.cu', 'trajectory_kernel.cu']
+HEADERS = ['crowdsim_common.cuh', 'orca_device.cuh', 'step_flat.cuh', 'step_multi.cuh', 'step_mid.cuh', 'orca_spec.cuh', 'rotate.cuh', 'step_args.cuh', 'occupancy.cuh', 'scene.cuh', os.path.join('..', '..', 'include', 'crowdsim_b200.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_scene_table.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_metrics.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_table_robots.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_human_metrics.h'), os.path.join('..', '..', 'include', 'crowdsim_b200_trajectories.h')]
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '--fmad=false',
               '-prec-div=true', '-prec-sqrt=true', '-ftz=false', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared', '-cudart', 'shared', '--threads', '4']

@@ -49,6 +49,12 @@ BatchedExplorer(..., human_metrics=True): each episode's per-human closest appro
 discomfort_dist), and the human a collision hit, measured inside the step kernels (BatchedCrowdSim.track_human_metrics,
 include/crowdsim_b200_human_metrics.h). The result rows then end with 2 N + 1 more columns (HUMAN_METRIC_COLUMNS: N closest
 approaches, N danger counts, the colliding human or -1) and summarize logs one more line after the others.
+
+BatchedExplorer(..., trajectories=True): every case's states before each of its steps, the reference's env.states
+(crowd_sim.py:391-393), captured on device before every env-step (BatchedCrowdSim.track_trajectories,
+include/crowdsim_b200_trajectories.h). Every env-step is then a launch of its own, the ORCA robot's included. After the
+rollout rank 0 holds last_trajectories = {'r_states': [k][T][9], 'h_states': [k][T][N][8], 'steps': [k]} as numpy arrays:
+rows t < steps[c] of case c are its states, the others NaN. Such a rollout records nothing (update_memory=True is refused).
 """
 import logging
 import math
@@ -139,6 +145,18 @@ def gather_results(local_rows, k, rank, world, group=None):
     out = [torch.empty_like(pad) for _ in range(world)]
     dist.all_gather(out, pad, group=group)
     return torch.cat([out[r][:shard_range(k, r, world)[1]] for r in range(world)], dim=0)
+
+
+def gather_trajectories(tr, n, k, rank, world, group=None):
+    """The first n rows of this rank's batched.TrajectoryBuffers from every rank, in case order: (r_states [k][T][9],
+    h_states [k][T][N][8]) on every rank. One gather_results of the rows flattened to one line per case; a rank whose shard
+    is empty (k < world) sends none."""
+    if world == 1:
+        return tr.r_traj[:n], tr.h_traj[:n]
+    cut = tr.T * 9
+    flat = torch.cat([tr.r_traj[:n].reshape(n, cut), tr.h_traj[:n].reshape(n, tr.T * tr.N * 8)], dim=1)
+    rows = gather_results(flat, k, rank, world, group)
+    return rows[:, :cut].reshape(k, tr.T, 9), rows[:, cut:].reshape(k, tr.T, tr.N, 8)
 
 
 def summarize(rows, k, phase, time_limit, time_step, episode=None, print_failure=False, log=logging.info, metrics=False,
@@ -254,11 +272,12 @@ def _unicycle_rows(policy):
 
 class BatchedExplorer(object):
     def __init__(self, env, robot_policy='orca', device=None, memory=None, gamma=None, target_policy=None,
-                 rank=0, world=1, group=None, human_times=False, metrics=False, human_metrics=False):
+                 rank=0, world=1, group=None, human_times=False, metrics=False, human_metrics=False, trajectories=False):
         self.env = env
         self.human_times = bool(human_times)
         self.metrics = bool(metrics)
         self.human_metrics = bool(human_metrics)
+        self.trajectories = bool(trajectories)
         self.robot_policy = robot_policy
         self.device = device or env.device
         self.memory = memory
@@ -267,6 +286,7 @@ class BatchedExplorer(object):
         self.target_model = None
         self.rank, self.world, self.group = rank, world, group
         self.last_rows = None
+        self.last_trajectories = None
         self.last_env_steps = 0
 
     def update_target_model(self, target_model):
@@ -306,15 +326,17 @@ class BatchedExplorer(object):
             raise ValueError('episode metrics are measured by rollouts that do not record (update_memory=False)')
         if self.human_metrics and update_memory:
             raise ValueError('per-human metrics are measured by rollouts that do not record (update_memory=False)')
+        if self.trajectories and update_memory:
+            raise ValueError('trajectories are captured by rollouts that do not record (update_memory=False)')
         first_case = env.case_counter[phase]
         start, n_local = shard_range(k, self.rank, self.world)
         gamma = self.gamma if self.gamma is not None else 0.9
         args = (env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
                 steps_per_launch, first_case, start, n_local, gamma, rule, scenes)
-        if not (self.human_times or self.metrics or self.human_metrics):
+        if not (self.human_times or self.metrics or self.human_metrics or self.trajectories):
             return self._run(*args)
         prev_arrivals, prev_metrics = env.arrivals, env.metrics     # the caller's tracking, back in place after the run
-        prev_human_metrics = env.human_metrics
+        prev_human_metrics, prev_trajectories = env.human_metrics, env.trajectories
         try:
             return self._run(*args)
         finally:
@@ -329,6 +351,10 @@ class BatchedExplorer(object):
                 env.human_metrics = prev_human_metrics
                 if prev_human_metrics is not None and env.episodes is not None and prev_human_metrics.k != env.episodes.k:
                     env.fit_human_metrics()
+            if self.trajectories:
+                env.trajectories = prev_trajectories
+                if prev_trajectories is not None and env.episodes is not None and prev_trajectories.k != env.episodes.k:
+                    env.track_trajectories()
 
     def _run(self, env, k, phase, update_memory, imitation_learning, episode, print_failure, prefetch_every, check_every,
              steps_per_launch, first_case, start, n_local, gamma, rule, scenes):
@@ -339,6 +365,8 @@ class BatchedExplorer(object):
             env.track_metrics()
         if self.human_metrics:
             env.track_human_metrics()
+        if self.trajectories:
+            env.track_trajectories()
         if scenes is None:
             env.set_case_queue((first_case + start) % env.case_size[phase], n_local, phase)    # wraps inside the phase like crowd_sim.py:283
             env.enable_autoreset(rule)
@@ -388,8 +416,10 @@ class BatchedExplorer(object):
         # an ORCA robot decides on device: the episode loop of explorer.py:41-43 closes inside the kernel, several steps per
         # launch (crowdsim_step_n, or crowdsim_step_n_record_ex when it also records); a step-by-step recorder or a host-side
         # policy needs every step
-        if not (self.robot_policy == 'orca' and recorder is None) or (scenes is not None and scenes.has_robots):
-            chunk = 1                                  # (a robot table: placed between launches of one env-step each)
+        if (not (self.robot_policy == 'orca' and recorder is None) or (scenes is not None and scenes.has_robots)
+                or self.trajectories):
+            chunk = 1                                  # (a robot table: placed between launches of one env-step each;
+            #                                            trajectories: captured before each of them)
         if chunk > 1:
             prefetch_every, check_every = 1, max(1, check_every // chunk)
         from .batched import max_episode_steps
@@ -430,6 +460,12 @@ class BatchedExplorer(object):
         rows = gather_results(pack_results(ep, n_local, local_times, env.metrics if self.metrics else None,
                                            env.human_metrics if self.human_metrics else None), k, self.rank,
                               self.world, self.group)
+        self.last_trajectories = None
+        if self.trajectories:
+            r_states, h_states = gather_trajectories(env.trajectories, n_local, k, self.rank, self.world, self.group)
+            if self.rank == 0:
+                self.last_trajectories = {'r_states': r_states.cpu().numpy(), 'h_states': h_states.cpu().numpy(),
+                                          'steps': rows[:, 1].cpu().numpy().astype(np.int32)}
         if scenes is None:
             env.case_counter[phase] = (first_case + k) % env.case_size[phase]
         env.autoreset = None

@@ -13,7 +13,10 @@ length and closest approach (BatchedExplorer(metrics=True)). --human_metrics add
 closest approach, how many humans entered the discomfort distance per episode and how many collisions hit each human index
 (BatchedExplorer(human_metrics=True)). --results FILE.npz saves every case's result row, one array per column
 (explorer.result_columns: the reference's columns, then human_times, the metric columns and h_closest [k][N], h_danger
-[k][N] and collider [k] when asked for), so two checkpoints can be compared case by case. Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
+[k][N] and collider [k] when asked for), so two checkpoints can be compared case by case. --trajectories FILE.npz saves
+every case's states before each of its steps, the reference's env.states (BatchedExplorer(trajectories=True)): r_states
+[k][T][9] (px, py, vx, vy, gx, gy, radius, v_pref, theta), h_states [k][T][N][8] (px, py, vx, vy, gx, gy, radius, v_pref),
+NaN past each case's end, and steps [k]. Rendering (--visualize, --traj, --video_file) is not provided. --gpu is accepted and
 changes nothing: the run is always on cuda:0.
 """
 import argparse
@@ -46,6 +49,7 @@ def parse_args(argv=None):
     parser.add_argument('--metrics', default=False, action='store_true')
     parser.add_argument('--results', type=str, default=None)
     parser.add_argument('--human_metrics', default=False, action='store_true')
+    parser.add_argument('--trajectories', type=str, default=None)
     return parser, parser.parse_args(argv)
 
 
@@ -103,7 +107,8 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
         env.test_sim = 'circle_crossing'
     explorer = explorer_class(env, policy, device, gamma=0.9, human_times=args.human_times,
                               **({'metrics': True} if args.metrics else {}),
-                              **({'human_metrics': True} if args.human_metrics else {}))
+                              **({'human_metrics': True} if args.human_metrics else {}),
+                              **({'trajectories': True} if args.trajectories is not None else {}))
 
     if policy == 'orca':
         # test.py:77-85: no safety space for ORCA, visible robot or not
@@ -124,6 +129,8 @@ def main(argv=None, make_env=make_env, explorer_class=None, device=None):
     if args.results is not None:
         save_results(args.results, explorer.last_rows, args.metrics,
                      **({'human_metrics': env.human_num} if args.human_metrics else {}))
+    if args.trajectories is not None:
+        save_trajectories(args.trajectories, explorer.last_trajectories)
     return stats
 
 
@@ -133,6 +140,12 @@ def save_results(path, rows, metrics=False, human_metrics=None):
     import numpy as np
     from .explorer import result_columns
     np.savez(path, **result_columns(rows, metrics, human_metrics))
+
+
+def save_trajectories(path, trajectories):
+    """--trajectories: BatchedExplorer.last_trajectories (r_states, h_states, steps) as an .npz."""
+    import numpy as np
+    np.savez(path, **trajectories)
 
 
 if __name__ == '__main__':
